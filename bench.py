@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py - crops/s of the MeTRAbs crop-model hot path (BASELINE.json metric) on N B200s of one node.
+"""bench.py - crops/s of the MeTRAbs crop-model hot path (BASELINE.json metric) on N H100s of one node.
 
   python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path (one rank per GPU under torchrun)
   python bench.py --impl reference --steps K --warmup W    # the reference's CPU path (oracle port, torch-cpu)
@@ -7,7 +7,9 @@
 One JSON line on rank 0.  `value`: whole-job crops/s with the crops already resident in HBM.  `e2e`: the same metric
 through the reference-facing host-buffer call (mtb_forward_host: pinned host crops -> H2D -> forward -> D2H joints).
 `roofline`: the dominant kernel class, timed live with CUDA events on the launching stream inside the timed region.
-`cpu_baseline`: the oracle port on the box's host cores on a bounded sample (rank 0, N=1 only)."""
+`cpu_baseline`: the oracle port on the box's host cores on a bounded sample (rank 0, N=1 only).
+`--dump-outputs DIR`: after the timed steps, the joints the last timed step returned (DIR/poses3d.npy, float32
+[batch, joints, 3]); inputs and weights are seeded, so two builds run with the same arguments compare output for output."""
 import argparse
 import json
 import os
@@ -48,6 +50,8 @@ def parse():
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--graph', type=int, default=int(os.environ.get('MTB_BENCH_GRAPH', '0')),
                     help='1: replay the forward from a CUDA graph in the `value` region (mtb_forward never syncs or allocates)')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write what the last timed step computed (rank 0) as DIR/<name>.npy')
     return ap.parse_args()
 
 
@@ -58,11 +62,11 @@ def peaks():
             p = json.load(f)
         return dict(hbm_gbs=p['hbm_gbs'], tflops=p.get('bf16_tflops_sustained', p['bf16_tflops']),
                     tflops_burst=p['bf16_tflops'], source='measured (MEASURED_PEAKS.json)')
-    return dict(hbm_gbs=6650.0, tflops=1400.0, tflops_burst=1590.0, source='fallback (B200_PROFILING.md)')
+    return dict(hbm_gbs=3350.0, tflops=989.0, tflops_burst=989.0, source='data sheet (H100 SXM, dense bf16, 700 W)')
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons DURING the timed region."""
     Q = ('index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,'
          'clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,'
          'clocks_event_reasons.sw_power_cap')
@@ -348,7 +352,7 @@ def frames_leg(args, model, device, iters=5):
             'poses3d_finite': bool(all(torch.isfinite(p).all() for p in res['poses3d']))}
 
 
-def time_mode(args, eng, world, rank, device, dist, sharded_inputs):
+def time_mode(args, eng, world, rank, device, dist, sharded_inputs, dump_dir=None):
     """Warm-up + timed loop of one precision mode.  -> dict(elapsed_ms, launches, prof_all (last warm-up step, warm),
     prof_dom, dom_name, clocks, e2e_ms, e2e_mode, graph_ms)."""
     crops_h, k_h, k_all_h, crops_d, k_d, k_all_d, out_d = sharded_inputs
@@ -409,6 +413,10 @@ def time_mode(args, eng, world, rank, device, dist, sharded_inputs):
     t_end = sampler.mark()
     elapsed_ms = ev0.elapsed_time(ev1)
     prof_dom = eng.profile_end()[dom_name]
+    if dump_dir and rank == 0:  # out_d still holds what the last timed step returned
+        import numpy as np
+        os.makedirs(dump_dir, exist_ok=True)
+        np.save(os.path.join(dump_dir, 'poses3d.npy'), out_d.float().cpu().numpy())
     clocks = sampler.stop(t_begin, t_end) if rank == 0 else None
 
     # ---- end to end through the host-buffer entry points: pinned host crops in, host joints out, EVERY step
@@ -516,7 +524,7 @@ def run_b200(args):
     inputs = (crops_h, k_h, k_all_h, crops_d, k_d, k_all_d, out_d)
 
     a_main, model, eng = make_engine(args.precision)
-    r = time_mode(a_main, eng, world, rank, device, dist, inputs)
+    r = time_mode(a_main, eng, world, rank, device, dist, inputs, dump_dir=args.dump_outputs)
     elapsed_ms, e2e_ms = r['elapsed_ms'], r['e2e_ms']
     if world > 1:
         t = torch.tensor([elapsed_ms, e2e_ms], device=device, dtype=torch.float64)
@@ -567,9 +575,8 @@ def run_b200(args):
                 'avg_launch_us': prof_dom['ms'] * 1e3 / prof_dom['launches'],
                 'share_of_step': prof_all[dom_name]['ms'] / total_ms_all,
                 'class_ms_warm_step': {n: round(v['ms'], 3) for n, v in prof_all.items()}}
-        # the other tcgen05 conv kernel of the step (fused FusedMBConv blocks) and both together: the dominant CLASS holds the
-        # layers that were not fused, so its fraction alone understates what the tensor-core kernels of the step achieve
-        tc_names = [n for n in ('tc_conv_kernel', 'fmb_kernel', 'tc32_conv_kernel') if n in prof_all and prof_all[n]['flops'] > 0]
+        # every tensor-core conv kernel class of the step and all of them together
+        tc_names = [n for n in ('tc_conv_kernel', 'tc32_conv_kernel') if n in prof_all and prof_all[n]['flops'] > 0]
         if bound == 'tensor' and len(tc_names) > 1:
             fl = sum(prof_all[n]['flops'] for n in tc_names)
             ms = sum(prof_all[n]['ms'] for n in tc_names)
@@ -594,8 +601,8 @@ def run_b200(args):
         'config': {'workload': workload_name(args), 'global_batch': B_total, 'crops_per_gpu': B, 'parallelism': f'dp{world}',
                    'precision_mode': args.precision, 'weights': 'conditioned random init (metrabs_b200/init.py)',
                    'l2_policy': f'inputs larger than L2: {B * 3 * S * S * 4 / 1e6:.0f} MB of crops per step'
-                                if B * 3 * S * S * 4 > 126e6 else
-                                f'{B * 3 * S * S * 4 / 1e6:.0f} MB of crops per step; every step streams > 1 GB of activations through L2 (126 MB)',
+                                if B * 3 * S * S * 4 > 50e6 else
+                                f'{B * 3 * S * S * 4 / 1e6:.0f} MB of crops per step; every step streams > 1 GB of activations through L2 (50 MB)',
                    'multi_gpu_step': ('mtb_forward_sharded: local backbone + head decode, one ncclAllGather of [c2d|c3d], full-batch '
                                       'reconstruction on every rank') if world > 1 else None,
                    'backbone_gflop_per_crop': flops_crop / 1e9,
@@ -615,7 +622,7 @@ def run_b200(args):
         pv = B_total * sibling['steps'] / (sibling['elapsed_ms'] / 1e3)
         line['parity_mode'] = {
             'precision_mode': 'tf32x3', 'what': 'the SAME workload in the mode that meets the 1e-3 joint tolerance on tensor cores '
-            '(tcgen05 kind::tf32, three split products, fp32 accumulation outside the tensor core)',
+            '(wgmma tf32, three split products, fp32 accumulation outside the tensor core)',
             'value': pv, 'unit': 'crops/s', 'steps': sibling['steps'], 'ms_per_step': sibling['elapsed_ms'] / sibling['steps'],
             'e2e': {'value': B_total * sibling['steps'] / (sibling['e2e_ms'] / 1e3), 'unit': 'crops/s', 'mode': rp['e2e_mode']},
             'gpu_launches': rp['launches'], 'clocks': rp['clocks'], 'roofline': roofline_of(rp, 'tf32x3'),

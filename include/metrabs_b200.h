@@ -1,5 +1,5 @@
 /*
- * metrabs_b200.h - C ABI of libmetrabs_b200.so: the B200 (sm_100a) implementation of the MeTRAbs per-crop
+ * metrabs_b200.h - C ABI of libmetrabs_b200.so: the H100 (sm_90a) implementation of the MeTRAbs per-crop
  * inference hot path   crops -> CNN backbone -> 1x1-conv head -> 2D + volumetric soft-argmax -> metric scaling
  * -> reconstruct_absolute -> joints [B,J,3].
  *
@@ -48,14 +48,14 @@ typedef enum { MTB_ARCH_EFFNET = 0, MTB_ARCH_RESNET50 = 1, MTB_ARCH_MOBILENETV3_
                MTB_ARCH_HEAD_ONLY = 3 } mtb_arch;
 
 /* Arithmetic of the conv/GEMM kernels.  FP32: CUDA-core fp32 FMA everywhere (the 1e-3 parity mode).
- * BF16_TC: bf16 operands on tcgen05 tensor cores with fp32 accumulation in TMEM, bf16 activations in HBM
+ * BF16_TC: bf16 operands on wgmma tensor cores with fp32 accumulation in registers, bf16 activations in HBM
  * (the throughput mode; the reference itself deploys under fp16 autocast, multiperson_model.py:241). */
 typedef enum { MTB_PRECISION_FP32 = 0, MTB_PRECISION_BF16_TC = 1,
                /* verification mode: same bf16 storage and bf16-rounded weights as BF16_TC, but every conv on CUDA
                 * cores (fp32 FMA) - lets tests separate tensor-core kernel bugs from bf16 rounding effects */
                MTB_PRECISION_BF16_SIMT = 2,
-               /* the 1e-3 parity mode ON TENSOR CORES: fp32 storage, every conv/GEMM as three tcgen05 kind::tf32
-                * products of hi/lo-split operands (a_hi*b_hi + a_lo*b_hi + a_hi*b_lo) with fp32 accumulation in TMEM;
+               /* the 1e-3 parity mode ON TENSOR CORES: fp32 storage, every conv/GEMM as three wgmma tf32
+                * products of hi/lo-split operands (a_hi*b_hi + a_lo*b_hi + a_hi*b_lo) with fp32 accumulation in registers;
                 * conv outputs agree with the fp32 FMA chain to ~1e-6 */
                MTB_PRECISION_TF32X3 = 3 } mtb_precision;
 
@@ -277,7 +277,7 @@ int mtb_op_input_shape(const mtb_handle* h, int op, int* height, int* width, int
                        int* has_scale);
 /* Runs ONE backbone op in isolation on caller-provided fp32 NHWC device tensors (converted to the handle's
  * storage type): in [B,Hin,Win,Cin] (the stem takes NCHW crops), optional residual [B,Hout,Wout,Cout] and
- * squeeze-excitation scale [B,Cin]; out receives [B,Hout,Wout,Cout] as fp32.  Lets tests compare the tcgen05
+ * squeeze-excitation scale [B,Cin]; out receives [B,Hout,Wout,Cout] as fp32.  Lets tests compare the tensor-core
  * kernels with the CUDA-core kernels on identical inputs. */
 int mtb_debug_run_op(mtb_handle* h, int op_index, const float* in, const float* res, const float* scale, int batch,
                      float* out, size_t out_floats, void* workspace, size_t workspace_bytes, void* stream);
@@ -310,12 +310,6 @@ double mtb_backbone_flops_per_crop(const mtb_handle* h);
  * rows per item, row bands per crop (= SE pooling slices) and bytes of one shared-memory stage; all 0 when the shape falls
  * back to the strip kernel. */
 int mtb_debug_dw_plan(int height, int width, int* crops_per_item, int* rows_per_item, int* row_bands, int* stage_bytes);
-
-/* Host-side plan and weight re-pack of the fused FusedMBConv kernel (no device needed; tests/test_host_plans.py): the shared-memory
- * plan for a block shape (all outputs 0 when the shape is not covered) and the stage images of the two weight matrices
- * (w1 [cexp][9*cin], w2 [cout][cexp], any 16-bit element type; pair = 1: the half-per-CTA images of the cta_group::2 kernel). */
-int mtb_debug_fmb_plan(int cin, int cexp, int cout, int pair, int* nstages, int* npatch, int* stage_bytes, int* smem_bytes);
-int mtb_debug_fmb_pack(const uint16_t* w1, const uint16_t* w2, int cin, int cexp, int cout, int pair, uint16_t* img1, uint16_t* img2);
 
 #ifdef __cplusplus
 }

@@ -123,9 +123,6 @@ _SIGNATURES = {
     'mtb_backbone_flops_per_crop': (C.c_double, [C.c_void_p]),
     'mtb_debug_dw_plan': (C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int),
                                     C.POINTER(C.c_int)]),
-    'mtb_debug_fmb_plan': (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int),
-                                     C.POINTER(C.c_int)]),
-    'mtb_debug_fmb_pack': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -1,4 +1,4 @@
-"""EfficientNetV2 backbones for the B200 engine.
+"""EfficientNetV2 backbones for the H100 engine.
 
 Mirrors the constructor surface of /root/reference/metrabs_pytorch/backbones/efficientnet.py
 (``efficientnet_v2_{s,m,l}()`` returning an object whose ``.features`` is used, and ``PreprocLayer``; model

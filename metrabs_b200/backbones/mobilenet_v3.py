@@ -1,4 +1,4 @@
-"""MobileNetV3-Small parameter holder for the B200 engine.
+"""MobileNetV3-Small parameter holder for the H100 engine.
 
 Keras-only in the reference (/root/reference/metrabs_tf/backbones/mobilenet_v3.py:258-296, :348-384, :465-553); key schema
 defined by this build from the Keras layer names with '/' -> '.': ``backbone.Conv.weight``,

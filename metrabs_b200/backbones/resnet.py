@@ -1,4 +1,4 @@
-"""ResNet-50 (V1, MeTRAbs stride/dilation switching) parameter holder for the B200 engine.
+"""ResNet-50 (V1, MeTRAbs stride/dilation switching) parameter holder for the H100 engine.
 
 The reference has this backbone only as Keras code (/root/reference/metrabs_tf/backbones/resnet.py:239-319, :601-666,
 :764-770); there is no PyTorch key schema for it, so this build defines one from the Keras layer names:

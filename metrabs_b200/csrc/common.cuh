@@ -1,4 +1,4 @@
-// Shared helpers for the metrabs_b200 CUDA sources (sm_100a only).
+// Shared helpers for the metrabs_b200 CUDA sources (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -19,9 +19,8 @@ enum Act : int { ACT_NONE = 0, ACT_SILU = 1, ACT_RELU = 2, ACT_HSWISH = 3, ACT_S
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
-// Measured on B200 (EfficientNetV2-L, 256 crops/step): 8.41 k crops/s without the attribute, 8.01 k with it (dependents
-// that launch early hold SM slots while spinning in griddepcontrol.wait), so PDL is OFF unless MTB_ENABLE_PDL=1; without
-// the launch attribute griddepcontrol.* are no-ops.
+// Dependents that launch early hold SM slots while spinning in griddepcontrol.wait, so PDL is OFF unless MTB_ENABLE_PDL=1;
+// without the launch attribute griddepcontrol.* are no-ops.
 inline bool pdl_enabled() {
   static int v = -1;
   if (v < 0) {
@@ -32,7 +31,7 @@ inline bool pdl_enabled() {
 }
 
 // Scoped PDL for a chain of tiny dependent launches (the squeeze-excitation FCs): their launch latency, not their work, is
-// what the step pays for, and a small early-launched grid does not hold the SM slots a 210 KB tensor-core CTA would.
+// what the step pays for, and a small early-launched grid does not hold the SM slots a tensor-core CTA would.
 inline int& pdl_force_depth() {
   static thread_local int d = 0;
   return d;
@@ -56,6 +55,17 @@ inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, siz
   cfg.attrs = attr;
   cfg.numAttrs = (pdl_enabled() || pdl_force_depth() > 0) ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kernel, KArgs(std::forward<Args>(args))...);
+}
+
+// streaming multiprocessors of the current device (grid sizes of the persistent / grid-stride kernels)
+inline int num_sms() {
+  static int n = 0;
+  if (n == 0) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
+      n = 132;
+  }
+  return n;
 }
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + __expf(-x)); }
@@ -143,31 +153,15 @@ __device__ __forceinline__ void store1<float>(float* p, float v) { *p = v; }
 template <>
 __device__ __forceinline__ void store1<__nv_bfloat16>(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
 
-// Packed fp32 pairs (sm_100 FFMA2 / FMUL2 / FADD2): two IEEE fp32 operations per issued instruction, bit-identical to the
-// scalar fmaf / fmul / fadd.  The kernel is issue-bound (ncu: 56 % issue-active with 2 warps per scheduler), so halving
-// the FMA instruction count is worth more than any memory-side change.
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 f2_pack(float lo, float hi) {
-  f32x2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void f2_unpack(f32x2 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ f32x2 f2_fma(f32x2 a, f32x2 b, f32x2 c) {
-  f32x2 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ f32x2 f2_mul(f32x2 a, f32x2 b) {
-  f32x2 d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ f32x2 f2_add(f32x2 a, f32x2 b) {
-  f32x2 d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
+// fp32 pairs: kernels written against two-wide arithmetic (f2_fma / f2_mul / f2_add).  Each half is the scalar IEEE
+// fma / mul / add with round-to-nearest (__fmaf_rn etc. are never contracted or reassociated), so a kernel using them is
+// bit-identical to its scalar formulation.
+typedef float2 f32x2;
+__device__ __forceinline__ f32x2 f2_pack(float lo, float hi) { return make_float2(lo, hi); }
+__device__ __forceinline__ void f2_unpack(f32x2 v, float& lo, float& hi) { lo = v.x; hi = v.y; }
+__device__ __forceinline__ f32x2 f2_fma(f32x2 a, f32x2 b, f32x2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ f32x2 f2_mul(f32x2 a, f32x2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ f32x2 f2_add(f32x2 a, f32x2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

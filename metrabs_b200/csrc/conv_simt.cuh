@@ -744,10 +744,10 @@ __global__ void __launch_bounds__(256) maxpool_kernel(ConvParams p) {
 template <typename TIn, typename TOut>
 inline cudaError_t launch_conv_igemm(const ConvParams& p, cudaStream_t st) {
   const int M = p.B * p.Hout * p.Wout;
-  if (p.Cout > 64 && M >= 128 * 148) {
+  if (p.Cout > 64 && M >= 128 * (size_t)num_sms()) {
     dim3 grid((M + 127) / 128, (p.Cout + 127) / 128);
     launch_k(conv_igemm_kernel<128, 128, 8, 8, TIn, TOut>, dim3(grid), dim3(256), 0, st, p);
-  } else if (M >= 128 * 148) {
+  } else if (M >= 128 * (size_t)num_sms()) {
     dim3 grid((M + 127) / 128, (p.Cout + 63) / 64);
     launch_k(conv_igemm_kernel<128, 64, 8, 4, TIn, TOut>, dim3(grid), dim3(256), 0, st, p);
   } else {
@@ -759,7 +759,7 @@ inline cudaError_t launch_conv_igemm(const ConvParams& p, cudaStream_t st) {
 
 inline int grid_for(size_t total, int block) {
   size_t g = (total + block - 1) / block;
-  size_t cap = 148 * 16;
+  size_t cap = (size_t)num_sms() * 16;
   return (int)(g < cap ? (g ? g : 1) : cap);
 }
 

@@ -84,30 +84,14 @@ struct Vec16<__half> {
   }
 };
 
-// packed fp32 pairs (FFMA2 / FADD2 / FMUL2 on sm_100): the 16-bit-logit soft-argmax spends 8 elements per 16-byte load and
-// is issue-bound, not bandwidth-bound, with scalar math (r1: 0.42-0.45 of the HBM peak)
-typedef unsigned long long sa_f2;
-__device__ __forceinline__ sa_f2 sa_pack(float lo, float hi) {
-  sa_f2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void sa_unpack(sa_f2 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ sa_f2 sa_fma(sa_f2 a, sa_f2 b, sa_f2 c) {
-  sa_f2 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ sa_f2 sa_mul(sa_f2 a, sa_f2 b) {
-  sa_f2 d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ sa_f2 sa_add(sa_f2 a, sa_f2 b) {
-  sa_f2 d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
+// fp32 pairs for the 16-bit-logit soft-argmax (8 elements per 16-byte load); each operation is the scalar IEEE fma / mul / add
+// per half, so results do not depend on how the compiler schedules the pair
+typedef float2 sa_f2;
+__device__ __forceinline__ sa_f2 sa_pack(float lo, float hi) { return make_float2(lo, hi); }
+__device__ __forceinline__ void sa_unpack(sa_f2 v, float& lo, float& hi) { lo = v.x; hi = v.y; }
+__device__ __forceinline__ sa_f2 sa_fma(sa_f2 a, sa_f2 b, sa_f2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ sa_f2 sa_mul(sa_f2 a, sa_f2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ sa_f2 sa_add(sa_f2 a, sa_f2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 
 __device__ __forceinline__ float ex2_fast(float x) {  // one MUFU op; inputs here are <= 0
   float y;

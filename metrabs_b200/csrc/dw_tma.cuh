@@ -269,8 +269,8 @@ dw3x3s1_tma_kernel(const __grid_constant__ CUtensorMap tmIn, const DwTmaParams p
       }
       if (p.pooled) {
         // fixed-order reduction of this pass: strip slots -> (crop, channel) owner threads
-        *reinterpret_cast<ulonglong2*>(&red[sidx][j * CPT]) = make_ulonglong2(psum[0], psum[1]);
-        if constexpr (!F32) *reinterpret_cast<ulonglong2*>(&red[sidx][j * CPT + 4]) = make_ulonglong2(psum[2], psum[3]);
+        *reinterpret_cast<float4*>(&red[sidx][j * CPT]) = make_float4(psum[0].x, psum[0].y, psum[1].x, psum[1].y);
+        if constexpr (!F32) *reinterpret_cast<float4*>(&red[sidx][j * CPT + 4]) = make_float4(psum[2].x, psum[2].y, psum[3].x, psum[3].y);
         __syncthreads();
         for (int g = own_g0; g < p.G; g += GSTEP) {
           // strip slots of crop g in this pass: [g * strips_per_crop, (g + 1) * strips_per_crop) - s0, clipped
@@ -334,7 +334,7 @@ inline const char* dw_tma_launch(DwTmaCache& cache, const DwTmaPlan& plan, const
   }
   // + one pixel row of slack: the last strip of a ragged row may read (never use) a few pixels past the patch
   const size_t smem = (size_t)DWT_STAGES * p.stage_bytes + 128 + 8 * 128;
-  const int grid = p.items < 2 * 148 ? p.items : 2 * 148;
+  const int grid = std::min(p.items, 2 * num_sms());
 #define MTB_DWT_LAUNCH_T(A, T)                                                                                             \
   {                                                                                                                        \
     static bool attr_set = false;                                                                                          \

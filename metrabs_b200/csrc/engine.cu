@@ -68,8 +68,8 @@ struct Op {
   float bn_eps = 1e-3f;
   float* d_w = nullptr;     // fp32 [R*S*Cin][Cout]  (dw: [R*S][C])
   float* d_bias = nullptr;  // fp32 [Cout]
-  TcWeights tc;             // bf16 K-major copy + TMA descriptor state for the tcgen05 path
-  Tc32Weights tc32;         // fp32 K-major copy + TMA descriptor state for the 3xTF32 tcgen05 path (MTB_PRECISION_TF32X3)
+  TcWeights tc;             // bf16 K-major copy + TMA descriptor state for the wgmma path
+  Tc32Weights tc32;         // fp32 K-major copy + TMA descriptor state for the 3xTF32 wgmma path (MTB_PRECISION_TF32X3)
   FmbWeights fmb;           // bf16 mode: this 3x3 expand conv and the NEXT op (1x1 projection) run as one fmb_kernel launch
   mutable DwTmaCache dw_cache;  // input tensor map of the TMA-staged depthwise kernel
   double flops = 0;         // 2*MACs per crop
@@ -589,7 +589,7 @@ int prepare_op_weights(mtb_handle* h, Op& op) {
   if (rc) return rc;
   if (h->cfg.precision == MTB_PRECISION_BF16_TC && tc_like && !tc_disabled()) {
     const char* e = tc_prepare_weights(op.tc, wk.data(), bias.data(), K, op.Cout, op.R, op.S, op.Cin, h->dev_allocs);
-    if (e) return fail(h, MTB_ERR_CUDA, "tcgen05 weight prep for '%s': %s", op.name.c_str(), e);
+    if (e) return fail(h, MTB_ERR_CUDA, "tensor-core weight prep for '%s': %s", op.name.c_str(), e);
   }
   if (h->cfg.precision == MTB_PRECISION_TF32X3 && !tc_disabled() &&
       tc32_eligible(op.type == OP_CONV, op.depthwise, op.small_io, op.R, op.stride, op.Cin, op.Cout)) {
@@ -771,9 +771,8 @@ template <typename T>
 int run_op_t(mtb_handle* h, const Op& op, const float* crops, int B, const Workspace& ws, void* features,
              cudaStream_t st) {
   PdlScope pdl_scope(pdl_se_enabled() && op.small_io);
-  if (op.type == OP_CONV && op.tc.ready && op.scale_buf != BUF_NONE && !tc_can_fuse_se(op.R, op.stride, op.Cin, op.act)) {
-    // squeeze-excitation scale applied in place ahead of a tensor-core conv that cannot fuse it (1x1 stride-1 projections
-    // apply it to the A tiles in shared memory inside tc_conv_kernel)
+  if (op.type == OP_CONV && op.tc.ready && op.scale_buf != BUF_NONE) {
+    // squeeze-excitation scale applied in place ahead of the bf16 tensor-core conv
     void* x = act_ptr(h, ws, op.in_buf, features, op.Hin, op.Win, op.Cin);
     const double bytes = 2.0 * B * op.Hin * op.Win * op.Cin * elem_size(h);
     ProfScope ps(h, KC_SE_SCALE, 0.0, bytes, st, false);
@@ -883,7 +882,7 @@ int run_op_t(mtb_handle* h, const Op& op, const float* crops, int B, const Works
         if (e != cudaSuccess) return fail(h, MTB_ERR_CUDA, "launch %s: %s", op.name.c_str(), cudaGetErrorString(e));
       } else if (op.tc.ready) {
         const char* e = tc_conv_launch(op.tc, p, op.res_first, st);
-        if (e) return fail(h, MTB_ERR_CUDA, "tcgen05 launch %s: %s", op.name.c_str(), e);
+        if (e) return fail(h, MTB_ERR_CUDA, "tensor-core launch %s: %s", op.name.c_str(), e);
       } else if (op.tc32.ready) {
         const char* e = tc32_conv_launch(op.tc32, p, op.res_first, st);  // SE scale (p.a_scale) applied by the splitter warps
         if (e) return fail(h, MTB_ERR_CUDA, "3xTF32 launch %s: %s", op.name.c_str(), e);
@@ -913,9 +912,8 @@ int run_op(mtb_handle* h, const Op& op, const float* crops, int B, const Workspa
   return run_op_t<float>(h, op, crops, B, ws, features, st);
 }
 
-// Crop chunking (running a stage chunk by chunk so that its intermediates stay in the 126 MB L2) was built and measured
-// in round 1: 29.5 ms vs 22.7 ms per 256 crops - these kernels are latency / issue bound at 32-128 crops, not bandwidth
-// bound, so smaller launches lose more than L2 residency wins.  The executor therefore runs every op on the whole batch.
+// The executor runs every op on the whole batch: running a stage crop chunk by crop chunk (intermediates resident in L2)
+// makes smaller launches, and these kernels are latency / issue bound at small batches rather than bandwidth bound.
 // one fmb_kernel launch for the FusedMBConv block (a = 3x3 expand, b = 1x1 projection [+ residual = a's input])
 int run_fused_block(mtb_handle* h, const Op& a, const Op& b, int B, const Workspace& ws, void* features, cudaStream_t st) {
   const void* in = act_ptr(h, ws, a.in_buf, features, a.Hin, a.Win, a.Cin);
@@ -998,7 +996,7 @@ int head_decode_impl(mtb_handle* h, const void* features, int B, float* c2d, flo
   const double feat_bytes = (double)B * P * op.Cin * elem_size(h);
   const double out_bytes = (double)B * c.n_joints * 5 * 4;
   if (op.tc.ready) {
-    // fused: 1x1-conv GEMM on tcgen05 with the soft-argmax reduction in the epilogue; logits never reach HBM
+    // fused: 1x1-conv GEMM on the tensor cores with the soft-argmax reduction in the epilogue; logits never reach HBM
     ProfScope prof(h, KC_HEAD_FUSED, op.flops * B, feat_bytes + (double)op.Cin * op.Cout * 2 + out_bytes, st);
     const char* e = tc_head_launch(op.tc, features, B, h->feat_side, h->feat_side, c.n_joints, c.depth, make_scale(c),
                                    c2d, c3d, ws.base + ws.off_logits, st);
@@ -1106,7 +1104,7 @@ struct DeviceGuard {
 // =================================================================================================== C ABI
 extern "C" {
 
-const char* mtb_version(void) { return "metrabs_b200 0.1 (sm_100a)"; }
+const char* mtb_version(void) { return "metrabs_b200 0.1 (sm_90a)"; }
 
 const char* mtb_last_error(const mtb_handle* h) { return h ? h->err.c_str() : g_error.c_str(); }
 
@@ -1128,8 +1126,8 @@ int mtb_create(const mtb_config* cfg, mtb_handle** out) {
     return fail(nullptr, MTB_ERR_CUDA, "no CUDA device: this library has no CPU fallback");
   if (cfg->device < 0 || cfg->device >= ndev) return fail(nullptr, MTB_ERR_INVALID_ARG, "device %d out of range", cfg->device);
   cudaDeviceProp prop;
-  if (cudaGetDeviceProperties(&prop, cfg->device) != cudaSuccess || prop.major != 10)
-    return fail(nullptr, MTB_ERR_CUDA, "device %d is not sm_100 (compute capability %d.%d)", cfg->device, prop.major, prop.minor);
+  if (cudaGetDeviceProperties(&prop, cfg->device) != cudaSuccess || prop.major != 9 || prop.minor != 0)
+    return fail(nullptr, MTB_ERR_CUDA, "device %d is not sm_90 (compute capability %d.%d)", cfg->device, prop.major, prop.minor);
   mtb_handle* h = new mtb_handle();
   h->cfg = *cfg;
   int rc = plan(h);
@@ -1253,7 +1251,7 @@ int mtb_finalize_weights(mtb_handle* h) {
     if (b.R != 1 || b.stride != 1 || b.act != ACT_NONE || b.scale_buf != BUF_NONE || b.res_first || b.in_buf != a.out_buf) continue;
     if (b.res_buf != BUF_NONE && b.res_buf != a.in_buf) continue;
     if (a.Hin != a.Hout || a.Win != a.Wout || b.out_buf == a.in_buf) continue;
-    const char* e = fmb_prepare(a.fmb, a.tc, b.tc, h->dev_allocs);
+    const char* e = fmb_prepare(a.fmb, a.tc, b.tc);
     if (e) return fail(h, MTB_ERR_CUDA, "fused FusedMBConv weight prep for '%s': %s", a.name.c_str(), e);
   }
   {
@@ -1287,7 +1285,7 @@ int mtb_finalize_weights(mtb_handle* h) {
           for (int cc = 0; cc < hd.Cin; ++cc) w0[(size_t)n * hd.Cin + cc] = w->data[(size_t)n * hd.Cin + cc];
         }
         const char* e = tc_prepare_head(hd.tc, w0.data(), b0.data(), hd.Cin, n_real, h->dev_allocs);
-        if (e) return fail(h, MTB_ERR_CUDA, "tcgen05 head weight prep: %s", e);
+        if (e) return fail(h, MTB_ERR_CUDA, "tensor-core head weight prep: %s", e);
       }
     }
   }
@@ -1982,7 +1980,7 @@ int mtb_debug_run_fused_block(mtb_handle* h, int op_index, const float* in, int 
   launch_k(from_float_kernel, dim3(grid_for(n_in, 256)), dim3(256), 0, st, in, (__nv_bfloat16*)buf_ptr(ws, 0, nullptr), n_in);
   a.in_buf = 0; a.out_buf = 1; b.in_buf = 1; b.out_buf = 2;
   if (b.res_buf != BUF_NONE) b.res_buf = 0;
-  a.fmb.cached_out = nullptr;  // the copy must not reuse a tensor map encoded for other buffers
+  a.fmb.cached_in = nullptr;  // the copy must not reuse a tensor map encoded for other buffers
   rc = run_fused_block(h, a, b, batch, ws, nullptr, st);
   if (rc) return rc;
   launch_k(to_float_kernel, dim3(grid_for(n_out, 256)), dim3(256), 0, st, (const __nv_bfloat16*)buf_ptr(ws, 2, nullptr), out, n_out);
@@ -1991,22 +1989,6 @@ int mtb_debug_run_fused_block(mtb_handle* h, int op_index, const float* in, int 
 
 int64_t mtb_last_launch_count(const mtb_handle* h) { return h ? h->launches : 0; }
 double mtb_backbone_flops_per_crop(const mtb_handle* h) { return h ? h->flops_per_crop : 0.0; }
-
-int mtb_debug_fmb_plan(int cin, int cexp, int cout, int pair, int* nstages, int* npatch, int* stage_bytes, int* smem_bytes) {
-  if (!nstages || !npatch || !stage_bytes || !smem_bytes) return fail(nullptr, MTB_ERR_INVALID_ARG, "invalid arguments");
-  *nstages = *npatch = *stage_bytes = *smem_bytes = 0;
-  if (!fmb_shape_ok(cin, cexp, cout) || (pair && (cexp % FMB_NC != 0 || cin != cout))) return MTB_OK;
-  const FmbPlan pl = fmb_plan(cin, cexp, cout, pair != 0);
-  if (!pl.ok) return MTB_OK;
-  *nstages = pl.nstages; *npatch = pl.npatch; *stage_bytes = pl.stage_bytes; *smem_bytes = pl.smem_bytes;
-  return MTB_OK;
-}
-
-int mtb_debug_fmb_pack(const uint16_t* w1, const uint16_t* w2, int cin, int cexp, int cout, int pair, uint16_t* img1, uint16_t* img2) {
-  if (!w1 || !w2 || !img1 || !img2 || !fmb_shape_ok(cin, cexp, cout)) return fail(nullptr, MTB_ERR_INVALID_ARG, "invalid arguments");
-  fmb_pack_images(w1, w2, cin, cexp, cout, pair ? 2 : 1, img1, img2);
-  return MTB_OK;
-}
 
 int mtb_debug_dw_plan(int height, int width, int* crops_per_item, int* rows_per_item, int* row_bands, int* stage_bytes) {
   if (height <= 0 || width <= 0 || !crops_per_item || !rows_per_item || !row_bands || !stage_bytes)

@@ -2,536 +2,200 @@
 //
 //     y = x + BN2(conv1x1( SiLU(BN1(conv3x3(x))) ))            x: [B,H,W,Cin] bf16 NHWC, expanded width Cexp = 4*Cin
 //
-// as ONE persistent tcgen05 kernel: the 128-pixel x Cexp expanded tile never leaves the SM.
-//
-//   GEMM-1  (3x3 expand, implicit GEMM)   A = resident (8+2) x (16+2) x Cin input patch (chunk-planar, no-swizzle UMMA
-//           descriptors shifted per tap, as mode 2 of tc_conv_kernel), B = one (tap, 128-channel chunk) weight block per ring
-//           stage, D = TMEM accumulator acc1[g & 1] (128 lanes x 128 columns), 9 * Cin/16 MMAs per chunk.
-//   epilogue-1 (8 warps)  acc1 -> + folded-BN bias -> SiLU -> bf16 -> shared memory, written directly in the canonical K-major
-//           no-swizzle operand layout [channel chunk of 8][128 rows][16 B]: it IS the A operand of GEMM-2.
-//   GEMM-2  (1x1 projection)  acc2[tile & 1] += A2(chunk) * W2[:, chunk]^T, 8 MMAs of N = Cout per chunk; the W2 slice of the
-//           chunk travels through the same ring (one stage).
-//   epilogue-2  acc2 -> + bias -> + residual x (re-read from L2: the patch loader fetched it two tiles ago) -> bf16 ->
-//           dense per-warp slab -> one TMA store per warp (box: Cout/2 channels x 8 x 4 pixels).
-//
-// The MMA issuer software-pipelines by one chunk:  G1(g), G2(g-1), G1(g+1), G2(g), ...  so the tensor pipe always has the
-// next chunk's GEMM-1 queued while the epilogue warps convert the previous accumulator.  HBM traffic per block = input
-// (1.4x with the halo, mostly L2 hits) + output; the expanded tensor (4x the input) is never written or re-read.
-//
-// Weights are re-packed on the host into the exact shared-memory images of the ring stages, so a stage is ONE 1-D bulk copy
-// (cp.async.bulk) with no tensor map.
+// as ONE kernel: the 128-pixel x Cexp expanded tile never leaves the SM.  Per output tile (16 x 8 pixels, as mode 1 of
+// tc_conv_kernel) and per chunk of 128 expanded channels:
+//   GEMM-1  (3x3 expand, implicit GEMM)   acc1[128 x 128] = shifted input boxes (4D TMA per tap) x W1[chunk rows]^T
+//   epilogue-1  acc1 -> + folded-BN bias -> SiLU -> bf16 -> shared memory in the 128B-swizzled K-major operand layout:
+//           it IS the A operand of GEMM-2 (channels >= Cexp are written as zeros)
+//   GEMM-2  (1x1 projection)  acc2[128 x Cout] += A2 x W2[:, chunk]^T, the W2 slice travelling through the same TMA ring
+// and after the last chunk epilogue-2: acc2 -> + bias -> + residual x -> bf16 store.  Each consumer warpgroup owns 64 rows
+// of the tile in both GEMMs, so the A2 hand-over needs only a warpgroup barrier.  The MMA sequence of every output element
+// (tap-major K of GEMM-1, chunk-major K of GEMM-2, K = 16 per wgmma) and every rounding are those of the two-launch path
+// (tc_conv_kernel twice), so the fused block reproduces it.
 #pragma once
 #include "tc_gemm.cuh"
 
 namespace mtb {
 
 constexpr int FMB_NC = 128;                       // expanded channels per chunk (N of GEMM-1, K of GEMM-2)
-constexpr int FMB_A2_BYTES = 128 * FMB_NC * 2;    // one GEMM-2 A operand buffer
-constexpr int FMB_MAX_STAGES = 8;
-constexpr int FMB_SMEM_BUDGET = 226 * 1024;       // + 1 KB alignment slack = the 227 KB opt-in limit
+constexpr int FMB_STAGES = 4;
+constexpr int FMB_STAGE_BYTES = TC_A_BYTES + FMB_NC * TC_BK * 2;   // 32 KB: [A 16 KB | W1 block 16 KB] or [W2 slice <= 32 KB]
+constexpr int FMB_A2_OFF = FMB_STAGES * FMB_STAGE_BYTES;
+constexpr int FMB_A2_BYTES = TC_BM * FMB_NC * 2;  // two 16 KB swizzle tiles (expanded channels 0-63, 64-127 of the chunk)
+constexpr int FMB_BAR_OFF = FMB_A2_OFF + FMB_A2_BYTES;
+constexpr int FMB_SMEM_BYTES = FMB_BAR_OFF + 256 + 1024 /*align slack*/;
 
 struct FmbParams {
-  const __nv_bfloat16* in;  // [B][H][W][Cin]; also the residual
-  const uint8_t* w1;        // chunk-major images: (chunk c, tap) -> [Cin/8][wc][8] bf16
-  const uint8_t* w2;        // chunk c -> [wc/8][Cout][8] bf16
+  TcConvParams g;           // geometry of the 3x3 expand conv (mode 1); g.res = x (residual), g.out = block output
   const float* bias1;       // [Cexp]
-  const float* bias2;       // [Cout]
-  int H, W, Cin, Cexp, Cout;
-  int tiles_w, tiles_h, total_tiles;
-  int nch;                  // ceil(Cexp / 128)
-  int pad_t, pad_l;
-  int has_res;
-  int npatch, patch_bytes, patch_off;
-  int nstages, stage_bytes;  // ring at offset 0
-  int na2, a2_off, slab_off, bias_off, bar_off;
-  long long* trace;          // MTB_FMB_TRACE=<Cin>: CTA 0 writes (code, clock64) pairs: [0,256) MMA warp, [256,512) epilogue warp 0,
-                             // [512,768) weight producer, [768,1024) patch loader warp 8
-  int debug;                 // MTB_FMB_DEBUG bits (perf experiments): 1 skip TMA store, 2 skip epilogue-1 math, 4 skip residual,
-                             // 8 skip the weight copies, 16 skip the patch copies, 32 skip the MMAs
+  int Cexp, nch, has_res;
 };
 
-__device__ __forceinline__ void bulk_load_1d(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src),
-               "r"(bytes), "r"(bar)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld8_issue(uint32_t taddr, uint32_t* r) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
-}
-
-#define FMB_TRACE(base, code)                                                     \
-  do {                                                                            \
-    if (trace_on && tr < 127) {                                                   \
-      p.trace[(base) + 2 * tr] = (code);                                          \
-      p.trace[(base) + 2 * tr + 1] = clock64();                                   \
-      ++tr;                                                                       \
-    }                                                                             \
-  } while (0)
-
-// Warp roles: 0-7 epilogue; 8, 11, 12 patch loaders; 9 and 13 weight producers (alternate ring stages: one bulk-copy issue
-// costs a thread ~350 cycles, a 16 KB stage is consumed in 256); 10 TMEM allocator + MMA issuer; 14 idle.
-// K1 = Cin / 16: MMAs (K = 16) per tap, compile-time so that the issue loop is straight-line code.
-//
-// PAIR: two CTAs of a cluster (the two SMs of a TPC) work on two tiles in lockstep with ONE stream of tcgen05.mma.cta_group::2
-// instructions (M = 256) issued by the leader: each CTA stages only HALF of every weight block (the tensor core reads the other
-// half from the peer's shared memory), which halves the weight bytes written to and read from each SM's shared memory - the
-// pipe that bounds the single-CTA kernel (ncu: shared-memory pipe 79 %, tensor pipe 48 %).  Barriers the leader's issuer
-// waits on (patch / A2 / accumulator hand-overs) collect the arrivals of both CTAs; its commits are multicast to both.
-template <int K1, bool PAIR>
-__global__ void __launch_bounds__(TC_THREADS, 1) fmb_kernel(const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmW1, const __grid_constant__ CUtensorMap tmW2,
+template <int BN2>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+fmb_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW1, const __grid_constant__ CUtensorMap tmW2,
            const FmbParams p) {
   extern __shared__ uint8_t tc_smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)tc_smem_raw + 1023) & ~(uintptr_t)1023);
-  uint64_t* bars = (uint64_t*)(smem + p.bar_off);
-  uint64_t* full = bars;                       // [8]  ring stage landed (expect_tx)
-  uint64_t* empty = bars + 8;                  // [8]  ring stage consumed (tcgen05.commit)
-  uint64_t* patch_full = bars + 16;            // [4]
-  uint64_t* patch_empty = bars + 20;           // [4]
-  uint64_t* acc1_full = bars + 24;             // [2]
-  uint64_t* acc1_unused = bars + 26;           // [2]  (acc1 hand-back is implied by a2_full, see the MMA issuer)
-  uint64_t* a2_full = bars + 28;               // [2]
-  uint64_t* a2_empty = bars + 30;              // [2]
-  uint64_t* acc2_full = bars + 32;             // [2]
-  uint64_t* acc2_empty = bars + 34;            // [2]
-  uint64_t* fullp = bars + 36;                 // [8]  (unused)
-  uint32_t* tmem_slot = (uint32_t*)(bars + 44);
-  float* bias1_s = (float*)(smem + p.bias_off);
-  float* bias2_s = bias1_s + p.Cexp;
+  uint64_t* full = (uint64_t*)(smem + FMB_BAR_OFF);
+  uint64_t* empty = full + FMB_STAGES;
+  const TcConvParams& g = p.g;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 8 && lane == 0) tma_prefetch_desc(&tmO);
-  if (warp == 9 && lane == 0) {
-    constexpr int NC = PAIR ? 2 : 1;  // CTAs whose warps arrive on the leader's hand-over barriers
-    for (int i = 0; i < 8; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); mbar_init(&fullp[i], 1); }
-    // a patch slot is free again once the tile's GEMM-1 MMAs (commit) AND its epilogue-2 (residual read, 8 warps) are done with it
-    for (int i = 0; i < 4; ++i) { mbar_init(&patch_full[i], 3 * NC); mbar_init(&patch_empty[i], 1 + TCV_EPI_WARPS); }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&acc1_full[i], 1); mbar_init(&acc1_unused[i], 1);
-      mbar_init(&a2_full[i], TCV_EPI_WARPS * NC); mbar_init(&a2_empty[i], 1);
-      mbar_init(&acc2_full[i], 1); mbar_init(&acc2_empty[i], TCV_EPI_WARPS * NC);
+  if (threadIdx.x == TC_CONSUMER_WARPS * 32) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmW1);
+    tma_prefetch_desc(&tmW2);
+    for (int i = 0; i < FMB_STAGES; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], TC_CONSUMER_WARPS);
     }
     fence_barrier_init();
   }
-  if (warp == 10) {
-    if constexpr (PAIR) {  // same logical warp in both CTAs (Allocator2Sm contract)
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512u) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      tmem_alloc(tmem_slot, 512);
-    }
-  }
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
-  const bool leader = rank == 0;
+  __syncthreads();
   pdl_trigger();
   pdl_wait();
-  // bias1 is staged HALVED: SiLU(v + b) = h + h * tanh(h) with h = 0.5 v + 0.5 b (one FMA; scaling by 0.5 is exact)
-  for (int i = threadIdx.x; i < p.Cexp + p.Cout; i += blockDim.x) bias1_s[i] = i < p.Cexp ? 0.5f * p.bias1[i] : p.bias2[i - p.Cexp];
-  tc_fence_before();
-  if constexpr (PAIR) cluster_sync_all();  // barriers of both CTAs initialised, TMEM allocated, before any cross-CTA traffic
-  else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);
 
-  // tile walk: single CTA: t = blockIdx.x + i * grid; pair u = blockIdx.x / 2: t = 2 * (u + i * npairs) + rank (a pair whose
-  // second tile does not exist still runs it: zero patch, no stores)
-  const int walk_first = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int walk_step = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-  const int walk_total = PAIR ? (p.total_tiles + 1) / 2 : p.total_tiles;
-  auto tile_of = [&](int i) { return PAIR ? 2 * (walk_first + i * walk_step) + (int)rank : walk_first + i * walk_step; };
-  const int ntl = (walk_first < walk_total) ? (walk_total - walk_first + walk_step - 1) / walk_step : 0;
-  const int nch = p.nch;
-  const int G = ntl * nch;                      // chunk jobs of this CTA
-  const uint32_t smem_base = smem_u32(smem);
-  const uint32_t full0 = smem_u32(full), empty0 = smem_u32(empty);
-  const int nstages = p.nstages;
-  const uint32_t stage_bytes = (uint32_t)p.stage_bytes;
-  const int planes = p.Cin >> 3;
-  const bool trace_on = p.trace != nullptr && blockIdx.x == 0 && lane == 0;
-  int tr = 0;
-
-  if (warp == 9 || warp == 13) {
-    // ===== weight producers: per chunk job g the nine (tap) blocks of W1, then the W2 slice of job g-1; ring use n is issued by
-    // warp 9 when n is even and by warp 13 when n is odd =====
-    const uint32_t mine = warp == 9 ? 0u : 1u;
-    uint32_t stage = 0, phase = 0, n = 0;
-    const uint32_t cin2 = (uint32_t)p.Cin * 2, cout2 = (uint32_t)p.Cout * 2;
-    // PAIR: the images are addressed as [rows of 128 B] matrices through a tensor map (box = one half block) so that the copy
-    // can complete on the LEADER's barrier (cta_group::2 form); `src` then only carries the byte offset into the image
-    auto put = [&](const CUtensorMap* map, const uint8_t* base, const uint8_t* src, uint32_t bytes) {
-      if ((n & 1u) == mine) {
-        mbar_wait_a(empty0 + stage * 8, phase ^ 1);
-        if (elect_one()) {
-          if constexpr (PAIR) {
-            if (leader) mbar_expect_tx_a(full0 + stage * 8, 2u * bytes);  // both CTAs' halves
-            tma_load_2d_2sm(smem_base + stage * stage_bytes, map, full0 + stage * 8, 0, (int)((size_t)(src - base) >> 7));
-          } else if (p.debug & 8) {  // perf experiment: no weight traffic
-            mbar_arrive((uint64_t*)(smem + p.bar_off) + stage);
+  const int m_blk = blockIdx.x;
+  const int num_kb = g.taps * g.kchunks;
+  if (warp == TC_CONSUMER_WARPS) {
+    // ===== TMA producer: per chunk, num_kb (input box, W1 block) stages, then one W2 stage =====
+    if (lane == 0) {
+      int it = 0;
+      for (int c = 0; c < p.nch; ++c) {
+        for (int kb = 0; kb <= num_kb; ++kb, ++it) {
+          const int s = it % FMB_STAGES;
+          mbar_wait(&empty[s], ((it / FMB_STAGES) & 1) ^ 1);
+          uint8_t* st = smem + s * FMB_STAGE_BYTES;
+          if (kb < num_kb) {
+            const int tap = kb / g.kchunks, kc = kb - tap * g.kchunks;
+            mbar_expect_tx(&full[s], FMB_STAGE_BYTES);
+            tma_load_a_tile<TC_BK>(st, &tmA, &full[s], g, m_blk, kb);
+            tma_load_2d(st + TC_A_BYTES, &tmW1, &full[s], tap * g.Cin + kc * TC_BK, c * FMB_NC);
           } else {
-            mbar_expect_tx_a(full0 + stage * 8, bytes);
-            bulk_load_1d(smem_base + stage * stage_bytes, src, bytes, full0 + stage * 8);
+            mbar_expect_tx(&full[s], 2 * BN2 * TC_BK * 2);
+            tma_load_2d(st, &tmW2, &full[s], c * FMB_NC, 0);
+            tma_load_2d(st + BN2 * TC_BK * 2, &tmW2, &full[s], c * FMB_NC + TC_BK, 0);
           }
         }
-        __syncwarp();
-        if (warp == 9) FMB_TRACE(512, 1);
       }
-      ++n;
-      if (++stage == (uint32_t)nstages) { stage = 0; phase ^= 1; }
-    };
-    int c = 0, cprev = 0;
-    for (int g = 0; g <= G; ++g) {
-      if (g < G) {
-        const int wc = min(FMB_NC, p.Cexp - c * FMB_NC);
-        const uint8_t* src = p.w1 + (size_t)c * FMB_NC * 9 * cin2;
-        // PAIR: the image of a (chunk, tap) block is [half][Cin/8][wc/2][8]; this CTA stages half `rank`
-        const uint32_t blk = (uint32_t)wc * cin2, mine_b = PAIR ? blk / 2 : blk;
-#pragma unroll 1
-        for (int tap = 0; tap < 9; ++tap) put(&tmW1, p.w1, src + (size_t)tap * blk + (size_t)rank * mine_b, mine_b);
-      }
-      if (g >= 1) {
-        const int wc = min(FMB_NC, p.Cexp - cprev * FMB_NC);
-        const uint32_t blk = (uint32_t)wc * cout2, mine_b = PAIR ? blk / 2 : blk;
-        put(&tmW2, p.w2, p.w2 + (size_t)cprev * FMB_NC * cout2 + (size_t)rank * mine_b, mine_b);
-      }
-      cprev = c;
-      if (++c == nch) c = 0;
     }
-  } else if (warp == 10 && !leader) {
-    // PAIR, peer CTA: this warp only allocates / frees tensor memory
-  } else if (warp == 10) {
-    // ===== MMA issuer (PAIR: leader CTA only, cta_group::2 instructions, commits multicast to both CTAs) =====
-    auto mma = [&](uint32_t d, uint64_t ad, uint64_t bd, uint32_t idesc, uint32_t accum) {
-      if constexpr (PAIR) umma_bf16_2sm(d, ad, bd, idesc, accum);
-      else umma_bf16(d, ad, bd, idesc, accum);
-    };
-    auto commit = [&](uint32_t bar) {
-      if constexpr (PAIR) umma_commit_2sm(bar);
-      else umma_commit_a(bar);
-    };
-    auto wait_x = [&](uint32_t bar, uint32_t parity) {  // barriers that also collect the peer's arrivals
-      if constexpr (PAIR) mbar_wait_cl(bar, parity);
-      else mbar_wait_a(bar, parity);
-    };
-    constexpr uint32_t hi_patch = (uint32_t)((TC_PATCH_W * 16) >> 4) | (1u << 14);  // SBO = one patch row
-    constexpr uint32_t hi_8 = 8u | (1u << 14);                                      // SBO = 8 rows x 16 B
-    constexpr uint32_t plane16 = TC_PLANE_BYTES >> 4;
-    const uint32_t base16 = smem_base >> 4, stage16 = stage_bytes >> 4;
-    const uint32_t patch0_16 = base16 + ((uint32_t)p.patch_off >> 4), patch_b16 = (uint32_t)p.patch_bytes >> 4;
-    const uint32_t a2_16 = base16 + ((uint32_t)p.a2_off >> 4);
-    const uint32_t acc1_full0 = smem_u32(acc1_full);
-    const uint32_t a2_full0 = smem_u32(a2_full), a2_empty0 = smem_u32(a2_empty);
-    const uint32_t acc2_full0 = smem_u32(acc2_full), acc2_empty0 = smem_u32(acc2_empty);
-    const uint32_t patch_full0 = smem_u32(patch_full), patch_empty0 = smem_u32(patch_empty);
-    const uint32_t Cout = (uint32_t)p.Cout;
-    const uint32_t idesc2 = PAIR ? umma_idesc_bf16_m256(p.Cout) : umma_idesc_bf16(p.Cout);
-    uint32_t stage = 0, phase = 0, s16 = base16;
-    uint32_t pb = 0, pb_phase = 0;
-    uint32_t a2b = 0, a2_phase = 0;    // A2 buffer of the NEXT G2
-    int c = 0, cprev = 0, tl_prev = 0;
-    for (int g = 0; g <= G; ++g) {
-      if (g < G) {
-        const uint32_t ab = (uint32_t)g & 1u;
-        const uint32_t wc = (uint32_t)min(FMB_NC, p.Cexp - c * FMB_NC);
-        // acc1[ab] is free: its previous user is chunk job g - 2, and GEMM-2 of g - 2 (issued before this point) waited for
-        // a2_full(g - 2), which the epilogue warps signal only after their last TMEM read of that job
-        FMB_TRACE(0, 10);
-        if (c == 0) wait_x(patch_full0 + pb * 8, pb_phase);
-        FMB_TRACE(0, 11);   // patch ready: G1 issue starts
-        tc_fence_after();
-        const uint32_t idesc1 = PAIR ? umma_idesc_bf16_m256((int)wc) : umma_idesc_bf16((int)wc);
-        const uint32_t d1 = tmem_base + ab * FMB_NC;
-        const uint32_t patch16 = patch0_16 + pb * patch_b16;
-        const uint32_t wrows = PAIR ? wc >> 1 : wc;  // weight rows of a block held by THIS CTA
-        const uint32_t lbo_b = wrows << 16;  // B planes are wrows rows x 16 B apart
-        const uint32_t wc2 = 2u * wrows;
-        // one kernel row (3 taps = 3 ring stages) per elected issue block: the per-block costs of the single-thread issue
-        // path (barrier polls, fence, elect, warp re-convergence) are paid once per 3 * K1 MMAs
-#pragma unroll 1
-        for (int r = 0; r < 3; ++r) {
-          uint32_t st[3], sb[3];
-#pragma unroll
-          for (int i = 0; i < 3; ++i) {
-            st[i] = stage;
-            sb[i] = s16;
-            mbar_wait_a(full0 + stage * 8, phase);
-            s16 += stage16;
-            if (++stage == (uint32_t)nstages) { stage = 0; phase ^= 1; s16 = base16; }
-          }
-          tc_fence_after();
-          if (elect_one()) {
-            const uint32_t a_row = (patch16 + (uint32_t)(r * TC_PATCH_W)) | (plane16 << 16);
-#pragma unroll
-            for (int i = 0; i < 3; ++i) {
-              const uint32_t b_lo = sb[i] | lbo_b;
-#pragma unroll
-              for (int k = 0; k < K1; ++k)
-                if (!(p.debug & 32))
-                  mma(d1, make_desc(a_row + (uint32_t)i + (uint32_t)(2 * k) * plane16, hi_patch),
-                      make_desc(b_lo + (uint32_t)k * wc2, hi_8), idesc1, (uint32_t)(r | i | k));
-              commit(empty0 + st[i] * 8);
-            }
-          }
-          __syncwarp();
-        }
-        if (elect_one()) {
-          commit(acc1_full0 + ab * 8);
-          if (c == nch - 1) commit(patch_empty0 + pb * 8);
-        }
-        __syncwarp();
-        FMB_TRACE(0, 12);   // G1 issued
-        if (c == nch - 1 && ++pb == (uint32_t)p.npatch) { pb = 0; pb_phase ^= 1; }
-      }
-      if (g >= 1) {
-        // GEMM-2 of chunk job g-1
-        const uint32_t wc = (uint32_t)min(FMB_NC, p.Cexp - cprev * FMB_NC);
-        const uint32_t acc = (uint32_t)tl_prev & 1u;
-        wait_x(a2_full0 + a2b * 8, a2_phase);
-        FMB_TRACE(0, 20);   // A2 ready
-        if (cprev == 0) wait_x(acc2_empty0 + acc * 8, (((uint32_t)tl_prev >> 1) & 1u) ^ 1u);
-        mbar_wait_a(full0 + stage * 8, phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t d2 = tmem_base + 2 * FMB_NC + acc * FMB_NC;
-          const uint32_t a16 = a2_16 + a2b * (FMB_A2_BYTES >> 4);
-          const int k2 = (int)(wc >> 4);
-          const uint32_t orows = PAIR ? Cout >> 1 : Cout;  // W2 rows (output channels) held by THIS CTA
-          const uint32_t a_lo = a16 | (128u << 16), b_lo = s16 | (orows << 16), cout2 = 2u * orows;
-#pragma unroll
-          for (int k = 0; k < FMB_NC / 16; ++k)
-            if (k < k2)
-              mma(d2, make_desc(a_lo + (uint32_t)(2 * k) * 128u, hi_8), make_desc(b_lo + (uint32_t)k * cout2, hi_8), idesc2,
-                  (uint32_t)(cprev | k));
-          commit(empty0 + stage * 8);
-          commit(a2_empty0 + a2b * 8);
-          if (cprev == nch - 1) commit(acc2_full0 + acc * 8);
-        }
-        __syncwarp();
-        FMB_TRACE(0, 21);   // G2 issued
-        s16 += stage16;
-        if (++stage == (uint32_t)nstages) { stage = 0; phase ^= 1; s16 = base16; }
-        if (++a2b == (uint32_t)p.na2) { a2b = 0; a2_phase ^= 1; }
-        if (cprev == nch - 1) ++tl_prev;
-      }
-      cprev = c;
-      if (++c == nch) c = 0;
-    }
-  } else if (warp == 8 || warp == 11 || warp == 12) {
-    // ===== patch loaders: the (16+2) x (8+2) x Cin input patch of a tile, chunk-planar [plane][patch row][patch col][16 B];
-    // out-of-image pixels (the reference's explicit zero padding, efficientnet.py:1127-1161) are zero-filled =====
-    const int lt = (warp == 8 ? 0 : warp == 11 ? 32 : 64) + lane;
-    const int items = TC_PATCH_H * TC_PATCH_W * planes;
-    uint32_t pb = 0, pb_phase = 0;
-    for (int i = 0; i < ntl; ++i) {
-      const int t = tile_of(i);
-      const bool tile_ok = t < p.total_tiles;  // PAIR: the second tile of the last pair may not exist (zero patch)
-      const int tw = t % p.tiles_w, th = (t / p.tiles_w) % p.tiles_h, b = t / (p.tiles_w * p.tiles_h);
-      const int ih0 = th * TC_PT_H - p.pad_t, iw0 = tw * TC_PT_W - p.pad_l;
-      mbar_wait_a(smem_u32(&patch_empty[pb]), pb_phase ^ 1);
-      if (warp == 8) FMB_TRACE(768, 30);  // patch slot free
-      uint8_t* patch = smem + p.patch_off + pb * p.patch_bytes;
-      for (int it = lt; it < items && !(p.debug & 16); it += 96) {
-        const int j = it % planes, pix = it / planes;
-        const int ph = pix / TC_PATCH_W, pw = pix - ph * TC_PATCH_W;
-        const int ih = ih0 + ph, iw = iw0 + pw;
-        const bool ok = tile_ok && ih >= 0 && ih < p.H && iw >= 0 && iw < p.W;
-        const __nv_bfloat16* src = ok ? p.in + ((size_t)(b * p.H + ih) * p.W + iw) * p.Cin + j * 8 : p.in;
-        cp_async_16(patch + j * TC_PLANE_BYTES + pix * 16, src, ok ? 16u : 0u);
-      }
-      cp_async_wait_all();
-      fence_proxy_async();  // generic-proxy writes -> visible to the tensor core (async proxy)
-      __syncwarp();
-      if (lane == 0) {
-        if constexpr (PAIR) mbar_arrive_leader(smem_u32(&patch_full[pb]), leader);
-        else mbar_arrive(&patch_full[pb]);
-      }
-      if (warp == 8) FMB_TRACE(768, 31);  // patch staged
-      if (++pb == (uint32_t)p.npatch) { pb = 0; pb_phase ^= 1; }
-    }
-  } else if (warp < TCV_EPI_WARPS) {
-    // ===== epilogue warps: epilogue-1 of every chunk job, epilogue-2 of tile t after epilogue-1 of (t+1, chunk 0) =====
-    const int q = warp & 3, hh = warp >> 2;
-    const int row = q * 32 + lane;
-    const int half = p.Cout >> 1;               // output channels per warp in epilogue-2 (multiple of 8)
-    const int n8 = half >> 3;
-    uint8_t* slab = smem + p.slab_off + warp * (32 * half * 2);
-    const uint32_t lane_taddr = tmem_base + ((uint32_t)(q * 32) << 16);
-    uint32_t a2b = 0, a2_phase = 0;
-
-    auto epi2 = [&](int tl) {
-      const int t = tile_of(tl);
-      const bool tile_ok = t < p.total_tiles;
-      const int tw = t % p.tiles_w, th = (t / p.tiles_w) % p.tiles_h, b = t / (p.tiles_w * p.tiles_h);
-      const int oh = th * TC_PT_H + (row >> 3), ow = tw * TC_PT_W + (row & 7);
-      const bool valid = tile_ok && oh < p.H && ow < p.W;
-      const uint32_t acc = (uint32_t)tl & 1u;
-      // residual (= the block input): the centre of the tile's input patch, still resident in shared memory (the patch slot is
-      // handed back to the loaders below, not by the MMA commit alone) - no second trip to L2 (the first version re-read it from
-      // global memory: ~1000 exposed cycles per tile, the epilogue warps being the critical path by then)
-      const uint32_t pslot = (uint32_t)tl % (uint32_t)p.npatch;
-      const uint8_t* pcell = smem + p.patch_off + pslot * p.patch_bytes + (((row >> 3) + 1) * TC_PATCH_W + (row & 7) + 1) * 16;
-      uint4 rv[6];
-#pragma unroll
-      for (int i = 0; i < 6; ++i) {
-        rv[i] = make_uint4(0u, 0u, 0u, 0u);
-        if (i < n8 && p.has_res && !(p.debug & 4)) rv[i] = *reinterpret_cast<const uint4*>(pcell + (hh * n8 + i) * TC_PLANE_BYTES);
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&patch_empty[pslot]);
-      if (warp == 0) FMB_TRACE(256, 50);
-      mbar_wait_a(smem_u32(&acc2_full[acc]), ((uint32_t)tl >> 1) & 1u);
-      if (warp == 0) FMB_TRACE(256, 51);
-      tc_fence_after();
-      const uint32_t taddr = lane_taddr + 2 * FMB_NC + acc * FMB_NC + (uint32_t)(hh * half);
-      uint32_t v[6][8];
-#pragma unroll
-      for (int i = 0; i < 6; ++i)
-        if (i < n8) tmem_ld8_issue(taddr + i * 8, v[i]);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (warp == 0) FMB_TRACE(256, 53);
-      if (lane == 0) tma_store_wait_read<0>();  // the previous store of this warp has read the slab
-      __syncwarp();
-      if (warp == 0) FMB_TRACE(256, 54);
-#pragma unroll
-      for (int i = 0; i < 6; ++i) {
-        if (i < n8) {
-          const float4 bl = *reinterpret_cast<const float4*>(bias2_s + hh * half + i * 8);
-          const float4 bh = *reinterpret_cast<const float4*>(bias2_s + hh * half + i * 8 + 4);
-          const float bs[8] = {bl.x, bl.y, bl.z, bl.w, bh.x, bh.y, bh.z, bh.w};
-          const unsigned wd[4] = {rv[i].x, rv[i].y, rv[i].z, rv[i].w};
-          uint4 ov;
-          __nv_bfloat162* o2 = reinterpret_cast<__nv_bfloat162*>(&ov);
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float x0 = __uint_as_float(v[i][2 * e]) + bs[2 * e] + __uint_as_float(wd[e] << 16);
-            const float x1 = __uint_as_float(v[i][2 * e + 1]) + bs[2 * e + 1] + __uint_as_float(wd[e] & 0xffff0000u);
-            o2[e] = __floats2bfloat162_rn(x0, x1);
-          }
-          *reinterpret_cast<uint4*>(slab + lane * (half * 2) + i * 16) = ov;
-        }
-      }
-      if (warp == 0) FMB_TRACE(256, 55);
-      fence_proxy_async();
-      __syncwarp();
-      if (warp == 0) FMB_TRACE(256, 56);
-      if (lane == 0) {
-        if (tile_ok && !(p.debug & 1)) {
-          tma_store_4d(&tmO, slab, hh * half, tw * TC_PT_W, th * TC_PT_H + q * 4, b);
-          tma_store_commit();
-        }
-        // accumulator hand-back (its TMEM reads completed above); last, so that a remote arrive does not stall the warp
-        if constexpr (PAIR) mbar_arrive_leader(smem_u32(&acc2_empty[acc]), leader);
-        else mbar_arrive(&acc2_empty[acc]);
-      }
-      if (warp == 0) FMB_TRACE(256, 52);
-    };
-
-    int c = 0, tl = 0;
-    for (int g = 0; g < G; ++g) {
-      const uint32_t ab = (uint32_t)g & 1u;
-      const int wc = min(FMB_NC, p.Cexp - c * FMB_NC);
-      mbar_wait_a(smem_u32(&acc1_full[ab]), ((uint32_t)g >> 1) & 1u);
-      if (warp == 0) FMB_TRACE(256, 40);
-      mbar_wait_a(smem_u32(&a2_empty[a2b]), a2_phase ^ 1);
-      if (warp == 0) FMB_TRACE(256, 41);
-      tc_fence_after();
-      const int col0 = hh * 64;
-      const uint32_t taddr = lane_taddr + ab * FMB_NC + (uint32_t)col0;
-      uint8_t* a2 = smem + p.a2_off + a2b * FMB_A2_BYTES + row * 16;
-      const float* b1 = bias1_s + c * FMB_NC + col0;
-#pragma unroll
-      for (int hf = 0; hf < 2; ++hf) {
-        const int cb = hf * 32;
-        if (col0 + cb < wc) {
-          uint32_t v[32];
-          tmem_ld16_issue(taddr + cb, v);
-          if (col0 + cb + 16 < wc) tmem_ld16_issue(taddr + cb + 16, v + 16);
-          tmem_ld_wait();
-#pragma unroll
-          for (int gq = 0; gq < 4; ++gq) {
-            if (col0 + cb + gq * 8 < wc) {
-              uint4 ov = make_uint4(0u, 0u, 0u, 0u);
-              if (!(p.debug & 2)) {
-                __nv_bfloat162* o2 = reinterpret_cast<__nv_bfloat162*>(&ov);
-                const float4 bl = *reinterpret_cast<const float4*>(b1 + cb + gq * 8);      // broadcast reads (0.5 * bias)
-                const float4 bh = *reinterpret_cast<const float4*>(b1 + cb + gq * 8 + 4);
-                const f32x2 hb[4] = {f2_pack(bl.x, bl.y), f2_pack(bl.z, bl.w), f2_pack(bh.x, bh.y), f2_pack(bh.z, bh.w)};
-                const f32x2 half2 = f2_pack(0.5f, 0.5f);
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  // SiLU(x) = h + h * tanh(h), h = x / 2 (the arithmetic of tc_act<ACT_SILU>, two elements per FFMA2)
-                  const f32x2 h = f2_fma(f2_pack(__uint_as_float(v[gq * 8 + 2 * e]), __uint_as_float(v[gq * 8 + 2 * e + 1])), half2, hb[e]);
-                  float h0, h1, x0, x1;
-                  f2_unpack(h, h0, h1);
-                  f2_unpack(f2_fma(h, f2_pack(tanh_approx(h0), tanh_approx(h1)), h), x0, x1);
-                  o2[e] = __floats2bfloat162_rn(x0, x1);
-                }
-              }
-              *reinterpret_cast<uint4*>(a2 + ((col0 + cb) / 8 + gq) * 2048) = ov;
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      fence_proxy_async();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
-      __syncwarp();
-      if (lane == 0) {
-        if constexpr (PAIR) mbar_arrive_leader(smem_u32(&a2_full[a2b]), leader);
-        else mbar_arrive(&a2_full[a2b]);
-      }
-      if (warp == 0) FMB_TRACE(256, 42);
-      if (++a2b == (uint32_t)p.na2) { a2b = 0; a2_phase ^= 1; }
-      if (c == 0 && tl >= 1) epi2(tl - 1);
-      if (++c == nch) { c = 0; ++tl; }
-    }
-    if (ntl > 0) epi2(ntl - 1);
-    if (lane == 0) tma_store_wait_all();
+    return;
   }
-  tc_fence_before();
-  if constexpr (PAIR) cluster_sync_all();  // neither CTA leaves while the pair's MMAs / remote arrivals may still touch it
-  else __syncthreads();
-  if (warp == 10) {
-    tc_fence_after();
-    if constexpr (PAIR) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
-    else tmem_dealloc(tmem_base, 512);
+  const int wg = warp >> 2;
+  const uint32_t a2 = smem_u32(smem + FMB_A2_OFF);
+  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // fragment rows r0, r0 + 8; columns 8 j + 2 (lane % 4) + {0, 1}
+  float acc2[BN2 / 2];
+#pragma unroll
+  for (int i = 0; i < BN2 / 2; ++i) acc2[i] = 0.f;
+  int it = 0;
+  for (int c = 0; c < p.nch; ++c) {
+    // ---- GEMM-1 ----
+    float acc1[FMB_NC / 2];
+#pragma unroll
+    for (int i = 0; i < FMB_NC / 2; ++i) acc1[i] = 0.f;
+    int prev = -1;
+    for (int kb = 0; kb < num_kb; ++kb, ++it) {
+      const int s = it % FMB_STAGES;
+      mbar_wait(&full[s], (it / FMB_STAGES) & 1);
+      const uint32_t a = smem_u32(smem + s * FMB_STAGE_BYTES) + wg * 64 * 128;
+      const uint32_t b = smem_u32(smem + s * FMB_STAGE_BYTES + TC_A_BYTES);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < TC_BK / 16; ++k)
+        wgmma_bf16<FMB_NC>(acc1, gmma_desc<128>(a + 32 * k), gmma_desc<128>(b + 32 * k), (uint32_t)(kb | k));
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[prev]);
+      }
+      prev = s;
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs<FMB_NC / 2>(acc1);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[prev]);
+    // ---- epilogue-1: + bias, SiLU, bf16 -> A2 (this warpgroup's rows; 16-byte chunk j of row r at j ^ (r & 7)) ----
+#pragma unroll
+    for (int j = 0; j < FMB_NC / 8; ++j) {
+      const int cc = 8 * j + 2 * (lane & 3);  // column within the chunk
+      const int col = c * FMB_NC + cc;
+      float2 bv = make_float2(0.f, 0.f);
+      if (col < p.Cexp) bv = __ldg(reinterpret_cast<const float2*>(p.bias1 + col));  // Cexp % 16 == 0: col + 1 valid with col
+      const uint32_t sub = (uint32_t)(cc >> 6) * (TC_BM * 128), kc = (uint32_t)(cc & 63);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = r0 + 8 * h;
+        __nv_bfloat162 v = __floats2bfloat162_rn(0.f, 0.f);
+        if (col < p.Cexp)
+          v = __floats2bfloat162_rn(tc_act<ACT_SILU>(acc1[4 * j + 2 * h] + bv.x), tc_act<ACT_SILU>(acc1[4 * j + 2 * h + 1] + bv.y));
+        const uint32_t off = sub + (uint32_t)r * 128 + ((((kc >> 3) ^ (uint32_t)(r & 7))) << 4) + (kc & 7) * 2;
+        *reinterpret_cast<__nv_bfloat162*>(smem + FMB_A2_OFF + off) = v;
+      }
+    }
+    fence_proxy_async();  // generic-proxy writes -> visible to the tensor core (async proxy)
+    wg_sync(wg);
+    // ---- GEMM-2: acc2 += A2 x W2[:, chunk]^T ----
+    {
+      const int s = it % FMB_STAGES;
+      mbar_wait(&full[s], (it / FMB_STAGES) & 1);
+      const uint32_t b = smem_u32(smem + s * FMB_STAGE_BYTES);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < FMB_NC / 16; ++k) {
+        const uint32_t sub = (uint32_t)(k >> 2), ko = (uint32_t)(k & 3) * 32;
+        wgmma_bf16<BN2>(acc2, gmma_desc<128>(a2 + sub * (TC_BM * 128) + wg * 64 * 128 + ko), gmma_desc<128>(b + sub * (BN2 * 128) + ko),
+                        (uint32_t)(c | k));
+      }
+      wgmma_commit();
+      wgmma_wait<0>();  // A2 is rewritten by the next chunk's epilogue-1
+      wgmma_fence_regs<BN2 / 2>(acc2);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[s]);
+      ++it;
+    }
+  }
+  // ---- epilogue-2: + bias, + residual x, bf16 store ----
+  const __nv_bfloat16* __restrict__ res = (const __nv_bfloat16*)g.res;
+  __nv_bfloat16* __restrict__ out = (__nv_bfloat16*)g.out;
+  const int c0 = 2 * (lane & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    size_t off;
+    if (!tile_row_offset(1, m_blk, r0 + 8 * h, g.M, g.Cout, g.tiles_w, g.tiles_h, g.Hout, g.Wout, off)) continue;
+#pragma unroll
+    for (int j = 0; j < BN2 / 8; ++j) {
+      const int cidx = c0 + 8 * j;
+      if (cidx >= g.Cout) break;
+      const float2 bv = __ldg(reinterpret_cast<const float2*>(g.bias + cidx));
+      float o0 = acc2[4 * j + 2 * h] + bv.x, o1 = acc2[4 * j + 2 * h + 1] + bv.y;
+      if (p.has_res) {
+        const float2 rv = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(res + off + cidx));
+        o0 += rv.x;
+        o1 += rv.y;
+      }
+      *reinterpret_cast<__nv_bfloat162*>(out + off + cidx) = __floats2bfloat162_rn(o0, o1);
+    }
   }
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-struct FmbPlan {  // shared-memory plan (byte offsets from the 1024-aligned base; the weight ring sits at offset 0)
-  int npatch = 0, patch_bytes = 0, patch_off = 0, nstages = 0, stage_bytes = 0, na2 = 1, a2_off = 0, slab_off = 0, bias_off = 0,
-      bar_off = 0, smem_bytes = 0;
-  bool ok = false;
-};
 struct FmbWeights {
   bool ready = false;
-  uint8_t* d_w1[2] = {nullptr, nullptr};  // [0] single-CTA images, [1] CTA-pair images (each block split in two halves)
-  uint8_t* d_w2[2] = {nullptr, nullptr};
-  const float* d_b1 = nullptr;
-  const float* d_b2 = nullptr;
-  int Cin = 0, Cexp = 0, Cout = 0;
-  FmbPlan plan[2];                         // [0] single CTA, [1] CTA pair (half-size ring stages)
-  CUtensorMap mapW1, mapW2;                // pair images as [rows of 128 B] matrices, box = one half block
-  bool pair_ok = false;
-  mutable CUtensorMap mapO;
-  mutable const void* cached_out = nullptr;
+  const TcWeights* w1 = nullptr;  // the expand conv's bf16 K-major weights [Cexp][9*Cin] + bias
+  const TcWeights* w2 = nullptr;  // the projection's [Cout][Cexp] + bias
+  int Cin = 0, Cexp = 0, Cout = 0, bn2 = 0;
+  CUtensorMap mapW1, mapW2;
+  mutable CUtensorMap mapA;
+  mutable const void* cached_in = nullptr;
   mutable int cached_B = -1;
 };
 
-inline bool fmb_enabled() {  // MTB_FMB=0: FusedMBConv blocks run as two tc_conv_kernel launches (A/B runs, tests)
+inline bool fmb_enabled() {  // MTB_FMB=0: FusedMBConv blocks run as two tc_conv_kernel launches (A/B runs)
   static int v = -1;
   if (v < 0) {
     const char* e = getenv("MTB_FMB");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
-}
-inline bool fmb_pair_enabled() {  // MTB_FMB_PAIR=0: the single-CTA kernel (A/B runs)
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("MTB_FMB_PAIR");
     v = (e && e[0] == '0') ? 0 : 1;
   }
   return v == 1;
@@ -542,213 +206,65 @@ inline bool fmb_shape_ok(int cin, int cexp, int cout) {
   return cin % 16 == 0 && cin >= 16 && cin <= 96 && cout == cin && cexp % 16 == 0 && cexp >= 32 && cexp <= 512;
 }
 
-inline FmbPlan fmb_plan(int Cin, int Cexp, int Cout, bool pair) {
-  FmbPlan f;
-  const int planes = Cin / 8;
-  f.patch_bytes = (planes * TC_PLANE_BYTES + 1023) / 1024 * 1024;
-  f.stage_bytes = (FMB_NC * std::max(Cin, Cout) * 2 / (pair ? 2 : 1) + 1023) / 1024 * 1024;
-  const int slab = 8 * 32 * (Cout / 2) * 2;
-  const int bias = ((Cexp + Cout) * 4 + 127) / 128 * 128;
-  f.na2 = 1;  // one GEMM-2 operand buffer: a second one measured 2.5 % faster on Cin = 64 but does not fit next to the Cin = 96 ring
-  for (int np = 3; np >= 2; --np) {
-    const int fixed = f.na2 * FMB_A2_BYTES + slab + bias + 512 + np * f.patch_bytes;
-    const int ns = std::min((FMB_SMEM_BUDGET - fixed) / f.stage_bytes, FMB_MAX_STAGES);
-    if (ns >= 4 || (np == 2 && ns >= 3)) {
-      f.npatch = np;
-      f.nstages = ns;
-      f.patch_off = ns * f.stage_bytes;
-      f.a2_off = f.patch_off + np * f.patch_bytes;
-      f.slab_off = f.a2_off + f.na2 * FMB_A2_BYTES;
-      f.bias_off = f.slab_off + slab;
-      f.bar_off = f.bias_off + bias;
-      f.smem_bytes = f.bar_off + 512 + 1024;
-      f.ok = true;
-      return f;
-    }
-  }
-  return f;
-}
-
-// rank-2 bf16 matrix [rows][64] (128-byte rows), box = [box_rows][64], no swizzle: a dense copy of box_rows * 128 bytes
-inline const char* make_tmap_2d_dense(CUtensorMap* m, const void* ptr, uint64_t rows, uint32_t box_rows) {
-  tmap_encode_fn enc = get_tmap_encode();
-  if (!enc) return "cuTensorMapEncodeTiled unavailable";
-  cuuint64_t dims[2] = {64, rows};
-  cuuint64_t strides[1] = {128};
-  cuuint32_t box[2] = {64, box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? nullptr : "cuTensorMapEncodeTiled(2d dense) failed";
-}
-
-// Host-side re-pack of the two weight matrices into the shared-memory images of the ring stages (any 16-bit element type):
-//   h1 [Cexp][9*Cin] (k = tap*Cin + c)  ->  i1: for chunk c, tap t, half h: [Cin/8 planes][rows/halves][8]   (rows = chunk width)
-//   h2 [Cout][Cexp]                     ->  i2: for chunk c,        half h: [rows/8 planes][Cout/halves][8]
-// halves = 1: single-CTA kernel; halves = 2: one half per CTA of a pair (each half is one contiguous TMA box).
-template <typename E>
-inline void fmb_pack_images(const E* h1, const E* h2, int Cin, int Cexp, int Cout, int halves, E* i1, E* i2) {
-  const int K1 = 9 * Cin;
-  const int nch = (Cexp + FMB_NC - 1) / FMB_NC;
-  size_t o1 = 0, o2 = 0;
-  for (int c = 0; c < nch; ++c) {
-    const int wc = std::min(FMB_NC, Cexp - c * FMB_NC);
-    for (int tap = 0; tap < 9; ++tap)
-      for (int hf = 0; hf < halves; ++hf)
-        for (int j = 0; j < Cin / 8; ++j)
-          for (int n = hf * (wc / halves); n < (hf + 1) * (wc / halves); ++n)
-            for (int e = 0; e < 8; ++e) i1[o1++] = h1[(size_t)(c * FMB_NC + n) * K1 + tap * Cin + j * 8 + e];
-    for (int hf = 0; hf < halves; ++hf)
-      for (int j = 0; j < wc / 8; ++j)
-        for (int n = hf * (Cout / halves); n < (hf + 1) * (Cout / halves); ++n)
-          for (int e = 0; e < 8; ++e) i2[o2++] = h2[(size_t)n * Cexp + c * FMB_NC + j * 8 + e];
-  }
-}
-
-// w1: bf16 [Cexp][9*Cin] (k = tap*Cin + c), w2: bf16 [Cout][Cexp] (device copies of the two convs' tensor-core weights)
-inline const char* fmb_prepare(FmbWeights& f, const TcWeights& w1, const TcWeights& w2, std::vector<void*>& allocs) {
+inline const char* fmb_prepare(FmbWeights& f, const TcWeights& w1, const TcWeights& w2) {
   f.ready = false;
+  if (!fmb_shape_ok(w1.Cin, w1.Cout, w2.Cout) || w2.Cin != w1.Cout || w1.taps != 9) return nullptr;
+  f.w1 = &w1; f.w2 = &w2;
   f.Cin = w1.Cin; f.Cexp = w1.Cout; f.Cout = w2.Cout;
-  if (!fmb_shape_ok(f.Cin, f.Cexp, f.Cout) || w2.Cin != f.Cexp || w1.taps != 9 || w2.taps != 1) return nullptr;
-  f.plan[0] = fmb_plan(f.Cin, f.Cexp, f.Cout, false);
-  f.plan[1] = fmb_plan(f.Cin, f.Cexp, f.Cout, true);
-  if (!f.plan[0].ok) return nullptr;
-  const int K1 = 9 * f.Cin;
-  std::vector<__nv_bfloat16> h1((size_t)f.Cexp * K1), h2((size_t)f.Cout * f.Cexp);
-  if (cudaMemcpy(h1.data(), w1.d_w, h1.size() * 2, cudaMemcpyDeviceToHost) != cudaSuccess) return "cudaMemcpy failed";
-  if (cudaMemcpy(h2.data(), w2.d_w, h2.size() * 2, cudaMemcpyDeviceToHost) != cudaSuccess) return "cudaMemcpy failed";
-  for (int v = 0; v < 2; ++v) {
-    std::vector<__nv_bfloat16> i1(h1.size()), i2(h2.size());
-    fmb_pack_images(h1.data(), h2.data(), f.Cin, f.Cexp, f.Cout, v + 1, i1.data(), i2.data());
-    if (cudaMalloc((void**)&f.d_w1[v], i1.size() * 2) != cudaSuccess) return "cudaMalloc failed";
-    allocs.push_back(f.d_w1[v]);
-    if (cudaMalloc((void**)&f.d_w2[v], i2.size() * 2) != cudaSuccess) return "cudaMalloc failed";
-    allocs.push_back(f.d_w2[v]);
-    if (cudaMemcpy(f.d_w1[v], i1.data(), i1.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess) return "cudaMemcpy failed";
-    if (cudaMemcpy(f.d_w2[v], i2.data(), i2.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess) return "cudaMemcpy failed";
-  }
-  f.d_b1 = w1.d_bias; f.d_b2 = w2.d_bias;
-  f.cached_out = nullptr; f.cached_B = -1;
-  // pair mode: every block is a full 128-channel chunk (all half blocks have the same size = one TMA box of Cin rows x 128 B)
-  f.pair_ok = false;
-  memset(&f.mapW1, 0, sizeof(f.mapW1));
-  memset(&f.mapW2, 0, sizeof(f.mapW2));
-  if (f.plan[1].ok && f.Cexp % FMB_NC == 0 && f.Cin == f.Cout) {
-    const char* e1 = make_tmap_2d_dense(&f.mapW1, f.d_w1[1], (uint64_t)f.Cexp * K1 * 2 / 128, (uint32_t)f.Cin);
-    const char* e2 = make_tmap_2d_dense(&f.mapW2, f.d_w2[1], (uint64_t)f.Cout * f.Cexp * 2 / 128, (uint32_t)f.Cin);
-    if (e1 || e2) return e1 ? e1 : e2;
-    f.pair_ok = true;
-  }
+  f.bn2 = tc_pick_bn(f.Cout);
+  const char* e = make_tmap_2d(&f.mapW1, w1.d_w, (uint64_t)f.Cexp, (uint64_t)9 * f.Cin, FMB_NC);
+  if (e) return e;
+  e = make_tmap_2d(&f.mapW2, w2.d_w, (uint64_t)f.Cout, (uint64_t)f.Cexp, (uint32_t)f.bn2);
+  if (e) return e;
+  f.cached_in = nullptr;
+  f.cached_B = -1;
   f.ready = true;
   return nullptr;
 }
 
-// rank-4 bf16 NHWC output, box = (box_c channels) x 8 x 4 pixels, dense (no swizzle) rows in shared memory
-inline const char* make_tmap_nhwc_dense(CUtensorMap* m, const void* ptr, uint64_t B, uint64_t H, uint64_t W, uint64_t C, uint32_t box_c) {
-  tmap_encode_fn enc = get_tmap_encode();
-  if (!enc) return "cuTensorMapEncodeTiled unavailable";
-  cuuint64_t dims[4] = {C, W, H, B};
-  cuuint64_t strides[3] = {C * 2, W * C * 2, H * W * C * 2};
-  cuuint32_t box[4] = {box_c, TC_PT_W, 4, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? nullptr : "cuTensorMapEncodeTiled(4d dense) failed";
-}
-
-template <int K1, bool PAIR>
-inline cudaError_t fmb_launch_k(int grid, int smem_bytes, const CUtensorMap& mapO, const CUtensorMap& w1, const CUtensorMap& w2,
-                                const FmbParams& p, cudaStream_t st) {
+template <int BN2>
+inline const char* fmb_launch_k(int grid, const FmbWeights& f, const FmbParams& q, cudaStream_t st) {
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(fmb_kernel<K1, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize, FMB_SMEM_BUDGET + 1024);
-    if (e != cudaSuccess) return e;
+    if (cudaFuncSetAttribute(fmb_kernel<BN2>, cudaFuncAttributeMaxDynamicSharedMemorySize, FMB_SMEM_BYTES) != cudaSuccess)
+      return "cannot raise dynamic shared memory for fmb_kernel";
     attr_set = true;
   }
-  if constexpr (PAIR) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(TC_THREADS);
-    cfg.dynamicSmemBytes = (size_t)smem_bytes;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, fmb_kernel<K1, PAIR>, mapO, w1, w2, p);
-  } else {
-    launch_k(fmb_kernel<K1, PAIR>, dim3(grid), dim3(TC_THREADS), (size_t)smem_bytes, st, mapO, w1, w2, p);
-    return cudaGetLastError();
-  }
-}
-template <bool PAIR>
-inline cudaError_t fmb_launch_p(int k1, int grid, int smem_bytes, const CUtensorMap& mapO, const CUtensorMap& w1, const CUtensorMap& w2,
-                                const FmbParams& p, cudaStream_t st) {
-  switch (k1) {
-    case 1: return fmb_launch_k<1, PAIR>(grid, smem_bytes, mapO, w1, w2, p, st);
-    case 2: return fmb_launch_k<2, PAIR>(grid, smem_bytes, mapO, w1, w2, p, st);
-    case 3: return fmb_launch_k<3, PAIR>(grid, smem_bytes, mapO, w1, w2, p, st);
-    case 4: return fmb_launch_k<4, PAIR>(grid, smem_bytes, mapO, w1, w2, p, st);
-    case 5: return fmb_launch_k<5, PAIR>(grid, smem_bytes, mapO, w1, w2, p, st);
-    default: return fmb_launch_k<6, PAIR>(grid, smem_bytes, mapO, w1, w2, p, st);
-  }
+  launch_k(fmb_kernel<BN2>, dim3(grid), dim3(TC_THREADS), FMB_SMEM_BYTES, st, f.mapA, f.mapW1, f.mapW2, q);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 
 inline const char* fmb_launch(const FmbWeights& f, const void* in, void* out, int B, int H, int W, int pad_t, int pad_l, bool has_res,
                               cudaStream_t st) {
-  if (f.cached_out != out || f.cached_B != B) {
-    const char* e = make_tmap_nhwc_dense(&f.mapO, out, B, H, W, f.Cout, (uint32_t)(f.Cout / 2));
+  if (!f.ready) return "fused FusedMBConv block not prepared";
+  FmbParams q;
+  TcConvParams& g = q.g;
+  g.res = in; g.bias = f.w2->d_bias; g.out = out;
+  g.mode = 1;
+  g.Hin = H; g.Win = W; g.Hout = H; g.Wout = W;
+  g.Cin = f.Cin; g.Cout = f.Cout;
+  g.taps = 9; g.S = 3; g.stride = 1; g.dil = 1; g.pad_t = pad_t; g.pad_l = pad_l;
+  g.kchunks = (f.Cin + TC_BK - 1) / TC_BK;
+  g.tiles_w = (W + TC_TILE_W - 1) / TC_TILE_W;
+  g.tiles_h = (H + TC_TILE_H - 1) / TC_TILE_H;
+  g.M = B * H * W;
+  q.bias1 = f.w1->d_bias;
+  q.Cexp = f.Cexp;
+  q.nch = (f.Cexp + FMB_NC - 1) / FMB_NC;
+  q.has_res = has_res ? 1 : 0;
+  if (f.cached_in != in || f.cached_B != B) {
+    const char* e = make_tmap_nhwc(&f.mapA, in, B, H, W, f.Cin, 1);
     if (e) return e;
-    f.cached_out = out; f.cached_B = B;
+    f.cached_in = in;
+    f.cached_B = B;
   }
-  FmbParams p;
-  p.tiles_w = (W + TC_PT_W - 1) / TC_PT_W; p.tiles_h = (H + TC_PT_H - 1) / TC_PT_H;
-  p.total_tiles = B * p.tiles_w * p.tiles_h;
-  const bool pair = fmb_pair_enabled() && f.pair_ok && p.total_tiles >= 2;
-  const FmbPlan& pl = f.plan[pair ? 1 : 0];
-  p.in = (const __nv_bfloat16*)in; p.w1 = f.d_w1[pair ? 1 : 0]; p.w2 = f.d_w2[pair ? 1 : 0]; p.bias1 = f.d_b1; p.bias2 = f.d_b2;
-  p.H = H; p.W = W; p.Cin = f.Cin; p.Cexp = f.Cexp; p.Cout = f.Cout;
-  p.nch = (f.Cexp + FMB_NC - 1) / FMB_NC;
-  p.pad_t = pad_t; p.pad_l = pad_l; p.has_res = has_res ? 1 : 0;
-  p.npatch = pl.npatch; p.patch_bytes = pl.patch_bytes; p.patch_off = pl.patch_off;
-  p.nstages = pl.nstages; p.stage_bytes = pl.stage_bytes;
-  p.na2 = pl.na2; p.a2_off = pl.a2_off; p.slab_off = pl.slab_off; p.bias_off = pl.bias_off; p.bar_off = pl.bar_off;
-  { static int dbg = -1; if (dbg < 0) { const char* e = getenv("MTB_FMB_DEBUG"); dbg = e ? atoi(e) : 0; } p.debug = dbg; }
-  int grid = p.total_tiles < 148 ? p.total_tiles : 148;
-  if (pair) grid = std::min(148, (p.total_tiles + 1) / 2 * 2);  // whole pairs
-  p.trace = nullptr;
-  static const char* trace_env = getenv("MTB_FMB_TRACE");  // "<Cin>": trace the first launch with that input width
-  static long long* trace_buf = nullptr;
-  static bool traced = false;
-  bool dump = false;
-  if (trace_env && !traced && atoi(trace_env) == f.Cin) {
-    if (!trace_buf) cudaMalloc(&trace_buf, 1024 * sizeof(long long));
-    cudaMemsetAsync(trace_buf, 0, 1024 * sizeof(long long), st);
-    p.trace = trace_buf;
-    dump = traced = true;
+  const int grid = B * g.tiles_w * g.tiles_h;
+  switch (f.bn2) {
+    case 32: return fmb_launch_k<32>(grid, f, q, st);
+    case 64: return fmb_launch_k<64>(grid, f, q, st);
+    default: return fmb_launch_k<128>(grid, f, q, st);
   }
-  cudaError_t e = pair ? fmb_launch_p<true>(f.Cin / 16, grid, pl.smem_bytes, f.mapO, f.mapW1, f.mapW2, p, st)
-                       : fmb_launch_p<false>(f.Cin / 16, grid, pl.smem_bytes, f.mapO, f.mapW1, f.mapW2, p, st);
-  if (dump && e == cudaSuccess) {
-    std::vector<long long> hb(1024);
-    cudaStreamSynchronize(st);
-    cudaMemcpy(hb.data(), trace_buf, 1024 * sizeof(long long), cudaMemcpyDeviceToHost);
-    long long t0 = 1LL << 62;
-    for (int r = 0; r < 4; ++r)
-      if (hb[r * 256] && hb[r * 256 + 1] < t0) t0 = hb[r * 256 + 1];
-    fprintf(stderr, "MTB_FMB_TRACE Cin=%d Cexp=%d H=%d W=%d tiles=%d grid=%d pair=%d nstages=%d npatch=%d na2=%d (code:cycles since first event)\n",
-            f.Cin, f.Cexp, H, W, p.total_tiles, grid, (int)pair, pl.nstages, pl.npatch, pl.na2);
-    const char* names[4] = {"mma (10 acc1 free, 11 patch ready, 12 G1 issued, 20 A2 ready, 21 G2 issued)",
-                            "epilogue warp 0 (40 acc1 full, 41 A2 free, 42 epi1 done, 50 epi2 start, 51 acc2 full, 52 epi2 done)",
-                            "weight producer (1 stage issued)", "patch loader (30 slot free, 31 staged)"};
-    for (int r = 0; r < 4; ++r) {
-      fprintf(stderr, "  %s:", names[r]);
-      for (int i = 0; i < 127 && hb[r * 256 + 2 * i]; ++i) fprintf(stderr, " %lld:%lld", hb[r * 256 + 2 * i], hb[r * 256 + 2 * i + 1] - t0);
-      fprintf(stderr, "\n");
-    }
-  }
-  return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 
 }  // namespace mtb

@@ -1,16 +1,18 @@
-// tcgen05 tensor-core path (sm_100a): bf16 operands staged by TMA into 128B-swizzled shared memory, fp32
-// accumulators in TMEM, warp-specialised persistent kernels.
+// Tensor-core path (sm_90a): bf16 operands staged by TMA into 128B-swizzled shared memory, fp32 accumulators in registers of
+// two consumer warpgroups (wgmma.mma_async), an mbarrier ring between one TMA producer warp and the consumers.
 //
 //   tc_conv_kernel   1x1 conv == GEMM  D[pixels, Cout] = A[pixels, Cin] * W[Cout, Cin]^T          (mode 0, 2D TMA)
-//                    3x3 stride-1 conv as implicit GEMM: per tap (r,s) the A tile is a shifted [8 x 16] pixel box
+//                    RxS conv (stride 1/2, dilation) as implicit GEMM: per tap (r,s) the A tile is a shifted [8 x 16] pixel box
 //                    of the NHWC input fetched by a 4D TMA (out-of-bounds = the reference's explicit zero padding,
-//                    backbones/efficientnet.py:1127-1161)                                            (mode 1)
-//                    epilogue: TMEM -> registers, + folded-BN bias, SiLU, + residual, bf16 NHWC store.
-//   tc_head_kernel   MetrabsHeads (models/metrabs.py:75-85): swapped operands, D[channel, pixel] = W[N, C] * F^T,
-//                    so every epilogue thread owns one (d,j) channel and reduces its pixels in registers: the
-//                    J x D x H x W logits never leave the SM.
+//                    backbones/efficientnet.py:1127-1161)                                             (mode 1)
+//                    epilogue: registers -> + folded-BN bias, activation, + residual, bf16 NHWC store.
+//   tc_head_kernel   MetrabsHeads (models/metrabs.py:75-85): swapped operands, D[channel, pixel] = W[N, C] * F^T, so every
+//                    epilogue thread owns one (d,j) channel and reduces its pixels in registers: the J x D x H x W logits
+//                    never leave the SM.
 //
-// Descriptor encodings follow the sm_100 UMMA formats (cute/arch/mma_sm100_desc.hpp in the vendored CUTLASS tree).
+// One CTA per output tile of 128 rows (64 per consumer warpgroup) x BN columns; the 1-2 CTAs an SM holds overlap one tile's
+// epilogue with another's main loop.  Descriptor encodings: the sm_90 GMMA shared-memory descriptor (PTX ISA, "Matrix
+// Descriptor Format" of wgmma).
 #pragma once
 #include <cuda.h>
 
@@ -23,6 +25,7 @@
 #include "common.cuh"
 #include "conv_simt.cuh"
 #include "decode.cuh"
+#include "wgmma.cuh"
 
 namespace mtb {
 
@@ -51,21 +54,18 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a pipeline bug (wrong expect_tx bytes, missing commit) traps after ~seconds instead of hanging the GPU.
+// Bounded wait: a pipeline bug (wrong expect_tx bytes, missing arrive) traps after ~seconds instead of hanging the GPU.  Kept
+// inline and free of calls: a call between wgmma instructions makes ptxas serialise the whole wgmma pipeline.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
-  while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 8000000000LL) {  // ~4 s at 2 GHz
-      printf("metrabs_b200: mbarrier wait timed out (block %d thread %d)\n", (int)blockIdx.x, (int)threadIdx.x);
-      __trap();
-    }
-  }
+  while (!mbar_try_wait(bar, parity))
+    if (clock64() - t0 > 8000000000LL) __trap();  // ~4 s at 2 GHz
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// named barrier of one consumer warpgroup (ids 1, 2; id 0 is __syncthreads)
+__device__ __forceinline__ void wg_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
 
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
   asm volatile(
@@ -85,213 +85,43 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], bf16 x bf16 -> fp32, issued by ONE thread for the CTA.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// 32 lanes x 16 consecutive 32-bit columns: thread i of the warp gets TMEM lane (base_lane + i).
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// K-major, 128B-swizzled operand tile: rows of 64 bf16 (128 B); 8-row groups are 1024 B apart (SBO); LBO unused.
-__device__ __forceinline__ uint64_t umma_smem_desc(uint32_t smem_addr) {
+// K-major operand tile with rows of RB bytes (128: SWIZZLE_128B, 64: SWIZZLE_64B), 8-row groups 8 * RB bytes apart (SBO);
+// LBO is unused for swizzled K-major layouts.  Advancing along K inside the swizzle atom = advancing the start address.
+template <int RB>
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t smem_addr) {
   uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);   // start address, bits [0,14)
-  d |= (uint64_t)(1024 >> 4) << 32;             // stride byte offset, bits [32,46)
-  d |= (uint64_t)1 << 46;                       // descriptor version (sm_100)
-  d |= (uint64_t)2 << 61;                       // layout type: SWIZZLE_128B
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);    // start address, bits [0,14)
+  d |= (uint64_t)1 << 16;                         // leading byte offset (ignored)
+  d |= (uint64_t)((8 * RB) >> 4) << 32;           // stride byte offset, bits [32,46)
+  d |= (uint64_t)(RB == 128 ? 1 : 2) << 62;       // layout type: 1 = SWIZZLE_128B, 2 = SWIZZLE_64B
   return d;
-}
-// same for rows of BK bf16: BK = 64 -> 128 B rows / SWIZZLE_128B (type 2), BK = 32 -> 64 B rows / SWIZZLE_64B (type 4);
-// 8-row groups are 8*row_bytes apart
-template <int BK>
-__device__ __forceinline__ uint64_t umma_smem_desc_k(uint32_t smem_addr) {
-  constexpr uint64_t sbo = (8 * BK * 2) >> 4;
-  constexpr uint64_t layout = BK == 64 ? 2 : 4;
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= sbo << 32;
-  d |= (uint64_t)1 << 46;
-  d |= layout << 61;
-  return d;
-}
-// K-major, NO swizzle ("interleave"): 8-row x 16-byte core matrices; LBO = byte distance between the two K core matrices
-// of one MMA (K = 16 bf16), SBO = byte distance between consecutive 8-row groups  (canonical layout ((8,n),2):((1,SBO),LBO)
-// in 16-byte units, cute/atom/mma_traits_sm100.hpp)
-__device__ __forceinline__ uint64_t umma_smem_desc_nosw(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  return d;
-}
-// kind::f16 instruction descriptor: D fp32, A/B bf16, both K-major, M = 128, N = n.
-__host__ __device__ inline uint32_t umma_idesc_bf16(int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
-
-// ---- CTA-pair (cta_group::2) helpers: PTX forms of the CUTLASS sm100 2-SM recipes (cute/arch/mma_sm100_umma.hpp
-// SM100_MMA_F16BF16_2x1SM_SS, cutlass/arch/barrier.h umma_arrive_multicast_2x1SM, cute/arch/tmem_allocator_sm100.hpp Allocator2Sm)
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// D[tmem, both CTAs] (+)= A[smem of each CTA: its 128 rows] * B[smem: N/2 rows from each CTA], issued by ONE thread of the leader
-__device__ __forceinline__ void umma_bf16_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive (once all prior tcgen05.mma of this thread have completed) on the mbarrier at this offset in BOTH CTAs of the pair
-__device__ __forceinline__ void umma_commit_2sm(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-               "h"((uint16_t)3)
-               : "memory");
-}
-// arrive on the mbarrier at this offset in the LEADER CTA (rank 0 of the pair), from either CTA
-__device__ __forceinline__ void mbar_arrive_leader(uint32_t bar, bool is_leader) {
-  if (is_leader) {  // own barrier: the plain CTA-local arrive
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-    return;
-  }
-  uint32_t remote;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, 0;" : "=r"(remote) : "r"(bar));
-  // relaxed: the data the barrier guards was written to THIS CTA's shared memory and made visible to the async proxy
-  // (fence.proxy.async) before the arrive is issued; a release.cluster arrive cost ~800 cycles per call (measured)
-  asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
-}
-// 2-SM TMA load of a [rows][64 bf16] box: data into THIS CTA's shared memory, transaction bytes onto the mbarrier at the same
-// offset in the LEADER CTA (CUTLASS SM100_TMA_2SM_LOAD: the CTA-rank bit of the shared::cluster barrier address is cleared)
-__device__ __forceinline__ void tma_load_2d_2sm(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
-      "l"(map), "r"(bar & 0xFEFFFFFFu), "r"(c0), "r"(c1)
-      : "memory");
-}
-// wait with cluster-scope acquire (the barrier receives arrivals from the peer CTA)
-__device__ __forceinline__ bool mbar_try_wait_cl(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n"
-      ".reg .pred P1;\n"
-      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 P1, [%1], %2;\n"
-      "selp.u32 %0, 1, 0, P1;\n"
-      "}\n"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait_cl(uint32_t bar, uint32_t parity) {
-  if (mbar_try_wait_cl(bar, parity)) return;
-  const long long t0 = clock64();
-  while (!mbar_try_wait_cl(bar, parity)) {
-    if (clock64() - t0 > 8000000000LL) {
-      printf("metrabs_b200: cluster mbarrier wait timed out (block %d thread %d)\n", (int)blockIdx.x, (int)threadIdx.x);
-      __trap();
-    }
-  }
-}
-// kind::f16 instruction descriptor for a pair: D fp32, A/B bf16, both K-major, M = 256, N = n
-__host__ __device__ inline uint32_t umma_idesc_bf16_m256(int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
 }
 
 // ------------------------------------------------------------------------------------------- conv/GEMM kernel
-// constants shared with the fused head kernel (fixed 4-stage ring of [A 16 KB | B 32 KB] stages)
-constexpr int TC_BM = 128, TC_BK = 64, TC_STAGES = 4, TC_MAX_BN = 256;
+constexpr int TC_BM = 128, TC_BK = 64;
 constexpr int TC_A_BYTES = TC_BM * TC_BK * 2;       // 16 KB
-constexpr int TC_B_BYTES = TC_MAX_BN * TC_BK * 2;   // 32 KB
-constexpr int TC_STAGE_BYTES = TC_A_BYTES + TC_B_BYTES;
-constexpr int TC_SMEM_BYTES = TC_STAGES * TC_STAGE_BYTES + 32768 + 1024 /*align slack*/ + 256 /*barriers*/;
-
-// conv kernel: shared-memory plan (bytes from the 1024-aligned base)
-//   [0, RING)            operand ring: `nstages` stages of (A tile | B tile); in mode 2 the ring holds B tiles only and
-//                        the two resident input patches live at its tail
-//   [RING, RING+64K)     epilogue staging: 8 warps x 2 slabs of [32 rows x 128 B] (one TMA-store box each)
-//   then                 per-warp bias staging (8 x 256 B), mbarriers, TMEM slot
-constexpr int TCV_RING_BYTES = 144 * 1024;
-constexpr int TCV_MAX_STAGES = 12;
-constexpr int TCV_SLAB_BYTES = 32 * 128;
-constexpr int TCV_EPI_OFF = TCV_RING_BYTES;
-constexpr int TCV_BIAS_OFF = TCV_EPI_OFF + 8 * 2 * TCV_SLAB_BYTES;
-constexpr int TCV_BAR_OFF = TCV_BIAS_OFF + 8 * 256;
-constexpr int TCV_SMEM_BYTES = TCV_BAR_OFF + 512 + 1024 /*align slack*/;
+constexpr int TC_THREADS = 288;                     // warps 0-7: two consumer warpgroups; warp 8: TMA producer
+constexpr int TC_CONSUMER_WARPS = 8;
 constexpr int TC_TILE_W = 16, TC_TILE_H = 8;        // spatial M tile of mode 1 (16 x 8 = 128 output pixels)
-// mode 2 (resident patch): 8 x 16 pixel tile, patch (8+2) x (16+2) pixels, planes of 16-byte channel chunks
-constexpr int TC_PT_W = 8, TC_PT_H = 16, TC_PATCH_W = TC_PT_W + 2, TC_PATCH_H = TC_PT_H + 2;
-constexpr int TC_PLANE_BYTES = TC_PATCH_W * TC_PATCH_H * 16;   // 2880
-constexpr int TC_PATCH_MAX_PLANES = 12;                          // Cin <= 96
-constexpr int TC_THREADS = 480;  // warps 0-7 epilogue; 8 A producer / patch loader; 9 B producer; 10 MMA + TMEM; 11 patch loader /
-                                 // SE scaler; 12-14 SE scalers
-constexpr int TCV_EPI_WARPS = 8;
+
+// ring depth per N tile: 96 KB of stages at BN = 128 (two CTAs per SM), four stages below
+template <int BN>
+struct TcRing {
+  static constexpr int stages = BN >= 128 ? 3 : 4;
+  static constexpr int stage_bytes = TC_A_BYTES + BN * TC_BK * 2;
+  static constexpr int smem_bytes = stages * stage_bytes + 1024 /*align slack*/ + 256 /*barriers*/;
+};
 
 struct TcConvParams {
   const void* res;
-  const void* res_in;  // mode 2: the NHWC input tensor, read by the patch loader warps
   const float* bias;
-  const float* a_scale;  // mode 0 only: squeeze-excitation scale [B][Cin] (fp32) applied to the A tiles in shared memory
-  int a_scale_P;         // pixels per crop (row / P = crop index)
-  int mode;     // 0: flat 1x1 stride 1 (rows = B*H*W, 2D maps); 1: spatial tiles, A tile per tap by 4D TMA (any RxS, stride
-                // 1/2, dilation); 2: 3x3 stride 1 with a RESIDENT input patch: the (tile+halo) x Cin patch is staged once per
-                // tile in a channel-chunk-planar layout and every tap's A operand is a no-swizzle UMMA descriptor into it
-  int tile_w, tile_h, tile_w_log2;  // spatial M tile: 16x8 (mode 1) or 8x16 (mode 2)
+  void* out;
+  int mode;     // 0: flat 1x1 stride 1 (rows = B*H*W, 2D maps); 1: spatial 16x8 tiles, A tile per tap by 4D TMA
   int Hin, Win;
   int M;        // mode 0: number of rows
   int Cout, Cin;
-  int bn;       // N-tile stride, multiple of 64 (the MMA N of a tile is its valid width rounded up to 16)
-  int b_rows;   // rows of the weight TMA box: bn, or Cout rounded up to 16 when one N tile covers Cout (no zero-fill rows)
-  int npatch;   // mode 2: resident patch buffers (2..4)
-  int n_tiles, m_tiles, kchunks, taps;
-  int nstages, stage_stride;  // operand ring depth and stage size in bytes (A at +0, B at +a_bytes)
-  int patch_off, patch_bytes; // mode 2: the two resident patches sit at the tail of the ring region
-  int b_resident;             // mode 2, one N tile, all k-blocks of the weights fit the ring: loaded once per CTA
-  int Hout, Wout, tiles_w, tiles_h, pad_t, pad_l, R, S, stride, dil;
-  long long* trace;  // MTB_TC_TRACE: CTA 0 writes clock64 timestamps [role][event] (0 A/B producer, 1 MMA, 2 epilogue warp 0)
-  int debug;    // MTB_TC_DEBUG bits (perf experiments only): 1 = skip the TMA store, 2 = skip the epilogue math + staging,
-                // 4 = skip the residual load, 8 = skip the patch loads (mode 2)
-  int bk;       // K elements per ring stage (host-side copy of the BK template argument)
-  int trace_cta; // the CTA that writes the clock64 trace
-  int rot;       // modes 0 / 1: rotate the start of each CTA's K loop (see the A producer); 0 with the fused SE scalers
-  int pair;        // flat GEMM run by CTA pairs (PAIRM kernel): b_rows = HALF the weight rows of a tile
-  int epi_single;  // mode 0, long K: ONE epilogue slab per warp; the freed 32 KB extend the operand ring to 176 KB
+  int kchunks, taps;
+  int Hout, Wout, tiles_w, tiles_h, pad_t, pad_l, S, stride, dil;
 };
 
 __device__ __forceinline__ float tanh_approx(float x) {
@@ -315,840 +145,136 @@ __device__ __forceinline__ float tc_act(float x) {
     return x;
   }
 }
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map), "r"(smem_u32(src)),
-               "r"(c0), "r"(c1)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, const void* src, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(map),
-               "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void tma_store_wait_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-__device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-// 16-byte async copy global -> shared; src_bytes = 0 zero-fills (out-of-image halo)
-__device__ __forceinline__ void cp_async_16(void* dst, const void* src, uint32_t src_bytes) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst)), "l"(src), "r"(src_bytes) : "memory");
-}
-__device__ __forceinline__ void cp_async_wait_all() {
-  asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 0;" ::: "memory");
-}
-// four TMEM loads in flight, one wait
-__device__ __forceinline__ void tmem_ld16_issue(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ uint64_t make_desc(uint32_t lo, uint32_t hi) {
-  uint64_t d;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "r"(lo), "r"(hi));
-  return d;
+// Output row r (0..127) of a tile -> (valid, element offset of channel 0) in the NHWC output
+__device__ __forceinline__ bool tile_row_offset(int mode, int m_blk, int r, int M, int Cout, int tiles_w, int tiles_h, int Hout, int Wout,
+                                                size_t& off) {
+  if (mode == 0) {
+    const int m = m_blk * TC_BM + r;
+    off = (size_t)m * Cout;
+    return m < M;
+  }
+  const int tw = m_blk % tiles_w, th = (m_blk / tiles_w) % tiles_h, b = m_blk / (tiles_w * tiles_h);
+  const int oh = th * TC_TILE_H + (r >> 4), ow = tw * TC_TILE_W + (r & 15);
+  off = ((size_t)(b * Hout + oh) * Wout + ow) * Cout;
+  return oh < Hout && ow < Wout;
 }
 
-// variants taking shared-window byte addresses (the issuer loops keep barrier / tile addresses as plain 32-bit offsets)
-__device__ __forceinline__ bool mbar_try_wait_a(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n"
-      ".reg .pred P1;\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 P1, [%1], %2;\n"
-      "selp.u32 %0, 1, 0, P1;\n"
-      "}\n"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-__device__ __noinline__ void mbar_wait_slow(uint32_t bar, uint32_t parity) {
-  const long long t0 = clock64();
-  while (!mbar_try_wait_a(bar, parity)) {
-    if (clock64() - t0 > 8000000000LL) {  // ~4 s at 2 GHz
-      printf("metrabs_b200: mbarrier wait timed out (block %d thread %d)\n", (int)blockIdx.x, (int)threadIdx.x);
-      __trap();
-    }
+// The A tile of k-block kb (tap = kb / kchunks, channel chunk kc = kb % kchunks) for output tile m_blk: 2D box of 128 rows
+// (mode 0) or the shifted 16 x 8 pixel box of tap (r, s) (mode 1).  BKE: channels per k-block.
+template <int BKE, typename P>
+__device__ __forceinline__ void tma_load_a_tile(void* dst, const CUtensorMap* map, uint64_t* bar, const P& p, int m_blk, int kb) {
+  const int tap = kb / p.kchunks, kc = kb - tap * p.kchunks;
+  if (p.mode == 0) {
+    tma_load_2d(dst, map, bar, kc * BKE, m_blk * TC_BM);
+  } else {
+    const int tw = m_blk % p.tiles_w, th = (m_blk / p.tiles_w) % p.tiles_h, b = m_blk / (p.tiles_w * p.tiles_h);
+    const int r = tap / p.S, s = tap - r * p.S;
+    tma_load_4d(dst, map, bar, kc * BKE, tw * TC_TILE_W * p.stride - p.pad_l + s * p.dil, th * TC_TILE_H * p.stride - p.pad_t + r * p.dil, b);
   }
 }
-__device__ __forceinline__ void mbar_wait_a(uint32_t bar, uint32_t parity) {
-  if (!mbar_try_wait_a(bar, parity)) mbar_wait_slow(bar, parity);
-}
-__device__ __forceinline__ void mbar_arrive_a(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx_a(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_a(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
-               "l"(map), "r"(bar), "r"(c0), "r"(c1)
-               : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_a(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(dst),
-      "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_a(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// keeps a loop-invariant value in a register (opaque to the optimiser, so it is not rematerialised from the constant bank)
-__device__ __forceinline__ int pin(int v) {
-  asm volatile("" : "+r"(v));
-  return v;
-}
-__device__ __forceinline__ uint32_t pin(uint32_t v) {
-  asm volatile("" : "+r"(v));
-  return v;
-}
-// one lane of a converged warp (elect.sync): the issue idiom that keeps operands in uniform registers
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n.reg .pred px;\nelect.sync _|px, 0xffffffff;\nselp.u32 %0, 1, 0, px;\n}\n" : "=r"(pred));
-  return pred != 0;
-}
-// persistent tile walk t = first, first + step, ...: (m_blk, n_blk) = (t / n_tiles, t % n_tiles) without a division per tile
-struct TileWalk {
-  int m_blk, n_blk, dm, dn, n_tiles;
-  __device__ __forceinline__ TileWalk(int first, int step, int nt) : m_blk(first / nt), n_blk(first % nt), dm(step / nt), dn(step % nt), n_tiles(nt) {}
-  __device__ __forceinline__ void next() {
-    m_blk += dm;
-    n_blk += dn;
-    if (n_blk >= n_tiles) { n_blk -= n_tiles; ++m_blk; }
-  }
-};
 
 // ACT: epilogue activation; RES: 0 no residual, 1 residual added AFTER the activation (EfficientNet), 2 BEFORE (ResNet);
-// BK: K elements per ring stage: 64 (128B-swizzled rows) or 32 (64B-swizzled rows).
-//
-// Warp roles (higher warp ids win issue arbitration on Blackwell, so the single-thread issuers sit on top):
-//   warps 0-7  epilogue: warp w owns TMEM lanes / tile rows [32(w&3), +32) and the 64-column chunks ch = (w>>2) mod 2;
-//              TMEM -> registers -> +bias -> act -> (+residual) -> bf16 -> private 128B-swizzled [32 x 64] slab -> its own
-//              TMA store.  No cross-warp synchronisation in the epilogue.
-//   warp 8     A-operand TMA producer (modes 0/1) / patch loader (mode 2)
-//   warp 9     B-operand (weights) TMA producer
-//   warp 10    TMEM allocator + single-thread tcgen05.mma issuer
-//   warp 11    second patch loader (mode 2)
-//
-// SCALE (flat 1x1 GEMMs with a squeeze-excitation scale on their input, BK = 64): the A operand does NOT travel by TMA.  Eight
-// loader warps (4-7, 11-14; the epilogue runs on warps 0-3 only - one tile's epilogue per >= 8 k-blocks leaves them idle most
-// of the time) read the activations from global memory into registers three k-blocks ahead, multiply by s[crop(row)][k] and
-// store the bf16 products straight into 128B-swizzled A slots; only the weights use the TMA ring.  The in-flight A bytes
-// live in registers instead of ring stages, and there is no second barrier hop between "landed" and "scaled".
-//
-// PAIRM (flat 1x1 GEMMs, BK = 64): two CTAs of a cluster compute a 256-row x bn tile with tcgen05.mma.cta_group::2 issued by
-// the leader: each CTA loads its own 128 rows of A and HALF of the weight tile (the tensor core reads the other half from the
-// peer's shared memory), so a ring stage is 16 KB + bn x 64 B instead of 16 KB + bn x 128 B and the weight bytes that cross the
-// L2 -> SM port - what bounds the MBConv expand / projection GEMMs - halve.
-template <int ACT, int RES, int BK, bool PATCH, bool SCALE = false, bool PAIRM = false>
+// BN: output channels per tile (wgmma N).
+template <int ACT, int RES, int BN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
-tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const __grid_constant__ CUtensorMap tmO, const TcConvParams p) {
+tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcConvParams p) {
+  using Ring = TcRing<BN>;
+  constexpr int STAGES = Ring::stages;
   extern __shared__ uint8_t tc_smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)tc_smem_raw + 1023) & ~(uintptr_t)1023);  // SWIZZLE_128B needs 1024 B alignment
-  uint64_t* bars = (uint64_t*)(smem + TCV_BAR_OFF);
-  uint64_t* full = bars;                              // [8]
-  uint64_t* empty = bars + TCV_MAX_STAGES;            // [8]
-  uint64_t* tmem_full = bars + 2 * TCV_MAX_STAGES;    // [2]
-  uint64_t* tmem_empty = tmem_full + 2;               // [2]
-  uint64_t* patch_full = tmem_empty + 2;              // [4]
-  uint64_t* patch_empty = patch_full + 4;             // [4]
-  uint64_t* scaled = patch_empty + 4;                 // [12] mode 0 + SE: A tile of the stage multiplied by the SE scale
-  uint32_t* tmem_slot = (uint32_t*)(scaled + TCV_MAX_STAGES);
+  uint64_t* full = (uint64_t*)(smem + STAGES * Ring::stage_bytes);
+  uint64_t* empty = full + STAGES;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr bool patch_mode = PATCH;  // compile-time: each kernel carries one operand pipeline (smaller hot code)
-  if (warp == 8 && lane == 0) {
+  if (threadIdx.x == TC_CONSUMER_WARPS * 32) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    tma_prefetch_desc(&tmO);
-  }
-  if (warp == 9 && lane == 0) {
-    for (int i = 0; i < TCV_MAX_STAGES; ++i) {
-      mbar_init(&full[i], (patch_mode || SCALE) ? 1 : 2);  // one arrive.expect_tx per TMA producer
-      mbar_init(&empty[i], 1);                  // tcgen05.commit
-      mbar_init(&scaled[i], 8);                 // one arrive per scaler warp
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      // one-chunk tiles (Cout <= 64, e.g. the 32->32 stage-1 convs) alternate between the two epilogue warp groups, and each
-      // accumulator buffer is only ever read by ONE group: its hand-back must not wait for the other group, which is still busy
-      // with the previous tile (it did until round 2: the groups ran strictly one after the other, 3400 cycles per tile)
-      mbar_init(&tmem_empty[i], PAIRM ? 2 * TCV_EPI_WARPS : (SCALE || (p.n_tiles == 1 && p.Cout <= 64)) ? 4 : TCV_EPI_WARPS);  // (the host never pairs Cout <= 64)
-    }
-    for (int i = 0; i < 4; ++i) {
-      mbar_init(&patch_full[i], p.b_resident ? 3 : 2);   // one arrive per loader warp
-      mbar_init(&patch_empty[i], 1);  // tcgen05.commit
+    for (int i = 0; i < STAGES; ++i) {
+      mbar_init(&full[i], 1);                  // the producer's arrive.expect_tx
+      mbar_init(&empty[i], TC_CONSUMER_WARPS); // one arrive per consumer warp
     }
     fence_barrier_init();
   }
-  if (warp == 10) {
-    if constexpr (PAIRM) {  // same logical warp in both CTAs (Allocator2Sm contract)
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512u) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      tmem_alloc(tmem_slot, 512);
-    }
-  }
-  const uint32_t rank = PAIRM ? cluster_ctarank() : 0u;
-  const bool leader = rank == 0;
-  tc_fence_before();
-  if constexpr (PAIRM) cluster_sync_all();  // both CTAs' barriers initialised and TMEM allocated before any cross-CTA traffic
-  else __syncthreads();
-  tc_fence_after();
-  // tile walk: CTA (pair) `walk_first` takes work units walk_first, walk_first + walk_step, ...; a unit is (row block, N tile),
-  // a row block being 128 rows (256 for a pair: rows [256 m + 128 rank, +128) belong to CTA `rank`)
-  const int walk_first = PAIRM ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int walk_step = PAIRM ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-  // warp-uniform by construction (shuffle from lane 0): lets the compiler keep the accumulator address in a uniform
-  // register instead of re-broadcasting it with an ELECT / R2UR loop in front of every tcgen05.mma
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);
-  pdl_trigger();  // the next kernel may start its own prologue on SMs this grid has left
-  pdl_wait();     // everything above overlapped the previous kernel's tail; its outputs are visible from here on
+  __syncthreads();
+  pdl_trigger();
+  pdl_wait();
 
-  long long cta_t0 = 0;
-  unsigned long long cta_g0 = 0;
-  if (p.trace && threadIdx.x == 0) {
-    cta_t0 = clock64();
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(cta_g0));
+  const int m_blk = blockIdx.x, n_blk = blockIdx.y;
+  const int num_kb = p.taps * p.kchunks;
+  if (warp == TC_CONSUMER_WARPS) {
+    // ===== TMA producer =====
+    if (lane == 0) {
+      for (int kb = 0; kb < num_kb; ++kb) {
+        const int s = kb % STAGES;
+        mbar_wait(&empty[s], ((kb / STAGES) & 1) ^ 1);
+        uint8_t* sa = smem + s * Ring::stage_bytes;
+        const int tap = kb / p.kchunks, kc = kb - tap * p.kchunks;
+        mbar_expect_tx(&full[s], Ring::stage_bytes);
+        tma_load_a_tile<TC_BK>(sa, &tmA, &full[s], p, m_blk, kb);
+        tma_load_2d(sa + TC_A_BYTES, &tmB, &full[s], tap * p.Cin + kc * TC_BK, n_blk * BN);
+      }
+    }
+    return;
   }
-  const int total_tiles = (PAIRM ? (p.m_tiles + 1) / 2 : p.m_tiles) * p.n_tiles;
-  const uint32_t a_bytes = (patch_mode || SCALE) ? 0u : (uint32_t)TC_BM * BK * 2;  // A bytes inside a ring stage
-  const uint32_t b_bytes = (uint32_t)p.b_rows * BK * 2;
-  const int nstages = p.nstages;
-  const int planes = p.kchunks * (BK / 8);  // 16-byte channel chunks per pixel in the patch (zero beyond Cin/8)
-
-  // The three single-issuer roles run with their whole warp CONVERGED and elect one lane per issue (the CUTLASS idiom):
-  // operands stay in uniform registers.  Under `if (lane == 0)` the compiler had to assume divergence, moved every
-  // descriptor / coordinate through R2UR and wrapped each UTCHMMA / UTMALDG in an ELECT loop: ~100 dependent instructions
-  // (~570 cycles, measured with the in-kernel trace and ncu's source view) per k-block whatever the MMA shape.
-  const bool trace_on = p.trace != nullptr && (int)blockIdx.x == p.trace_cta;
-  // loop-invariant kernel parameters of the issuer loops, pinned in registers (the compiler otherwise re-reads them from
-  // the constant bank inside the loops: each LDC sits on the single-warp critical path)
-  const int num_kb = pin(p.taps * p.kchunks);
-  const uint32_t stage_stride = pin((uint32_t)p.stage_stride);
-  const uint32_t smem_base = smem_u32(smem);
-  const uint32_t full0 = smem_u32(full), empty0 = smem_u32(empty);
-  if (warp == 8 && !patch_mode && !SCALE) {
-    // ===== A-operand TMA producer =====
-    uint32_t stage = 0, phase = 0, sa = smem_base;
-    int tr = 0;
-    const int kchunks = pin(p.kchunks);
-    TileWalk tw_(walk_first, walk_step, p.n_tiles);
-    // K rotation (opt-in, MTB_TC_ROT=1): CTA i starts every tile's K loop at k-block (i mod num_kb) and wraps, so that the
-    // CTAs of a wave do not read the SAME weight k-block at the same time.  Hypothesis was L2 same-line serialisation on
-    // the long-K / one-N-tile projection GEMMs; measured: no change (2.354 vs 2.357 ms per 18 launches), so it is off.
-    const int rot_kb = p.rot ? (int)(blockIdx.x % (unsigned)num_kb) : 0;
-    if (p.mode == 0) {
-      for (int t = walk_first; t < total_tiles; t += walk_step, tw_.next()) {
-        const int row0 = (PAIRM ? 2 * tw_.m_blk + (int)rank : tw_.m_blk) * TC_BM;
-        int kc = rot_kb;
-#pragma unroll 1
-        for (int i = 0; i < kchunks; ++i) {
-          mbar_wait_a(empty0 + stage * 8, phase ^ 1);
-          if (elect_one()) {
-            if constexpr (PAIRM) {  // both CTAs' A tiles complete on the LEADER's barrier
-              if (leader) mbar_expect_tx_a(full0 + stage * 8, 2u * a_bytes);
-              tma_load_2d_2sm(sa, &tmA, full0 + stage * 8, kc * BK, row0);
-            } else {
-              mbar_expect_tx_a(full0 + stage * 8, a_bytes);
-              tma_load_2d_a(sa, &tmA, full0 + stage * 8, kc * BK, row0);
-            }
-            if (trace_on && tr < 256) p.trace[tr++] = clock64();
-          }
-          __syncwarp();
-          if (++kc == kchunks) kc = 0;
-          sa += stage_stride;
-          if (++stage == (uint32_t)nstages) { stage = 0; phase ^= 1; sa = smem_base; }
-        }
-      }
-    } else {
-      const int R = pin(p.R), S = pin(p.S), dil = pin(p.dil);
-      const int tap0 = rot_kb / kchunks, kc0 = rot_kb - tap0 * kchunks, r0 = tap0 / S, s0 = tap0 - r0 * S;
-      for (int t = walk_first; t < total_tiles; t += walk_step, tw_.next()) {
-        const int m_blk = tw_.m_blk;
-        const int tw = m_blk % p.tiles_w;
-        const int th = (m_blk / p.tiles_w) % p.tiles_h;
-        const int b = m_blk / (p.tiles_w * p.tiles_h);
-        const int ih0 = th * TC_TILE_H * p.stride - p.pad_t;
-        const int iw0 = tw * TC_TILE_W * p.stride - p.pad_l;
-        int r = r0, s_ = s0, kc = kc0;
-#pragma unroll 1
-        for (int i = 0; i < num_kb; ++i) {
-          mbar_wait_a(empty0 + stage * 8, phase ^ 1);
-          if (elect_one()) {
-            mbar_expect_tx_a(full0 + stage * 8, a_bytes);
-            tma_load_4d_a(sa, &tmA, full0 + stage * 8, kc * BK, iw0 + s_ * dil, ih0 + r * dil, b);
-            if (trace_on && tr < 256) p.trace[tr++] = clock64();
-          }
-          __syncwarp();
-          if (++kc == kchunks) {
-            kc = 0;
-            if (++s_ == S) { s_ = 0; if (++r == R) r = 0; }
-          }
-          sa += stage_stride;
-          if (++stage == (uint32_t)nstages) { stage = 0; phase ^= 1; sa = smem_base; }
-        }
-      }
-    }
-  } else if (warp == 9) {
-    // ===== B-operand (weights) TMA producer =====
-    if (p.b_resident) {
-      // the whole weight panel stays in the ring: slot kb <- k-block kb, loaded once
-      if (lane == 0) {
-        int kb = 0;
-        for (int tap = 0; tap < p.taps; ++tap)
-          for (int kc = 0; kc < p.kchunks; ++kc, ++kb) {
-            mbar_expect_tx(&full[kb], b_bytes);
-            tma_load_2d(smem + kb * p.stage_stride, &tmB, &full[kb], tap * p.Cin + kc * BK, 0);
-          }
-      }
-    } else {
-      uint32_t stage = 0, phase = 0, sb = smem_base + a_bytes;
-      const int taps = pin(p.taps), kchunks = pin(p.kchunks), Cin = pin(p.Cin), bn = pin(p.bn);
-      // same K rotation as the A producer (mode 2 keeps the natural order: its MMA loop derives the patch offset from it)
-      const int rot_kb = (p.rot && !patch_mode) ? (int)(blockIdx.x % (unsigned)num_kb) : 0;
-      const int tap0 = rot_kb / kchunks, kc0 = rot_kb - tap0 * kchunks;
-      TileWalk tw_(walk_first, walk_step, p.n_tiles);
-      for (int t = walk_first; t < total_tiles; t += walk_step, tw_.next()) {
-        // PAIRM: this CTA stages rows [n0 + rank * n_mma / 2, + n_mma / 2) of the weight tile (n_mma = the MMA's N)
-        const int nrow = PAIRM ? tw_.n_blk * bn + (int)rank * ((((min(bn, p.Cout - tw_.n_blk * bn)) + 15) & ~15) >> 1) : tw_.n_blk * bn;
-        int tap = tap0, kc = kc0;
-#pragma unroll 1
-        for (int i = 0; i < num_kb; ++i) {
-          mbar_wait_a(empty0 + stage * 8, phase ^ 1);
-          if (elect_one()) {
-            if constexpr (PAIRM) {
-              if (leader) mbar_expect_tx_a(full0 + stage * 8, 2u * b_bytes);
-              tma_load_2d_2sm(sb, &tmB, full0 + stage * 8, tap * Cin + kc * BK, nrow);
-            } else {
-              mbar_expect_tx_a(full0 + stage * 8, b_bytes);
-              tma_load_2d_a(sb, &tmB, full0 + stage * 8, tap * Cin + kc * BK, nrow);
-            }
-          }
-          __syncwarp();
-          if (++kc == kchunks) { kc = 0; if (++tap == taps) tap = 0; }
-          sb += stage_stride;
-          if (++stage == (uint32_t)nstages) { stage = 0; phase ^= 1; sb = smem_base + a_bytes; }
-        }
-      }
-    }
-  } else if (warp == 10 && leader) {
-    // ===== MMA issuer (whole warp walks the pipeline, one elected lane issues; PAIRM: the leader CTA only) =====
-    int tr = 0;
-    uint32_t acc = 0, acc_phase = 0, pb = 0, pb_phase = 0;
-    // constant high words of the operand descriptors: SBO | version 1 | layout type
-    constexpr uint32_t hi_sw = (uint32_t)((8 * BK * 2) >> 4) | (1u << 14) | ((BK == 64 ? 2u : 4u) << 29);
-    constexpr uint32_t hi_patch = (uint32_t)((TC_PATCH_W * 16) >> 4) | (1u << 14);
-    constexpr uint32_t lbo_patch = (uint32_t)(TC_PLANE_BYTES >> 4) << 16;
-    constexpr uint32_t plane16 = TC_PLANE_BYTES >> 4;
-    const uint32_t stride16 = stage_stride >> 4;
-    const uint32_t base16 = smem_base >> 4;   // shared-window offsets stay below 2^18: the 14-bit address field never wraps
-    const uint32_t b_off16 = a_bytes >> 4;
-    const uint32_t fullw0 = p.a_scale ? smem_u32(scaled) : full0;
-    const uint32_t tmem_full0 = smem_u32(tmem_full), tmem_empty0 = smem_u32(tmem_empty);
-    const uint32_t patch_full0 = smem_u32(patch_full), patch_empty0 = smem_u32(patch_empty);
-    const int bn = pin(p.bn), Cout = pin(p.Cout);
-    TileWalk tw_(walk_first, walk_step, p.n_tiles);
-    if constexpr (SCALE) {
-      // ---- SCALE: B streams through the ring, A sits in one of three slots written by the loader warps ----
-      uint32_t stage = 0, phase = 0, b16 = base16, as = 0, a_phase = 0;
-      const uint32_t aslot16 = base16 + ((uint32_t)p.patch_off >> 4);
-      const uint32_t a_full0 = smem_u32(scaled), a_empty0 = patch_empty0;
-      for (int t = walk_first; t < total_tiles; t += walk_step, tw_.next()) {
-        const int n_valid = min(bn, Cout - tw_.n_blk * bn);
-        const uint32_t idesc = umma_idesc_bf16((n_valid + 15) & ~15);
-        mbar_wait_a(tmem_empty0 + acc * 8, acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * TC_MAX_BN;
-#pragma unroll 1
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait_a(full0 + stage * 8, phase);
-          mbar_wait_a(a_full0 + as * 8, a_phase);
-          tc_fence_after();
-          if (elect_one()) {
-            const uint32_t a16 = aslot16 + as * (uint32_t)(TC_A_BYTES >> 4);
+  // ===== consumers: warpgroup wg computes tile rows [64 wg, +64) =====
+  const int wg = warp >> 2;
+  float acc[BN / 2];
 #pragma unroll
-            for (int k = 0; k < 4; ++k)
-              umma_bf16(d_tmem, make_desc(a16 + 2 * k, hi_sw), make_desc(b16 + 2 * k, hi_sw), idesc, (uint32_t)(kb | k));
-            umma_commit_a(empty0 + stage * 8);
-            umma_commit_a(a_empty0 + as * 8);
-            if (kb == num_kb - 1) umma_commit_a(tmem_full0 + acc * 8);
-          }
-          __syncwarp();
-          b16 += stride16;
-          if (++stage == (uint32_t)nstages) { stage = 0; phase ^= 1; b16 = base16; }
-          if (++as == 3u) { as = 0; a_phase ^= 1; }
-        }
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    } else if (!patch_mode) {
-      // ---- modes 0 / 1: both operands stream through the ring; the k-block loop does not depend on the tap ----
-      uint32_t stage = 0, phase = 0, a16 = base16;
-      for (int t = walk_first; t < total_tiles; t += walk_step, tw_.next()) {
-        const int n_valid = min(bn, Cout - tw_.n_blk * bn);
-        const uint32_t idesc = PAIRM ? umma_idesc_bf16_m256((n_valid + 15) & ~15) : umma_idesc_bf16((n_valid + 15) & ~15);
-        if constexpr (PAIRM) mbar_wait_cl(tmem_empty0 + acc * 8, acc_phase ^ 1);  // collects the peer's epilogue warps too
-        else mbar_wait_a(tmem_empty0 + acc * 8, acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * TC_MAX_BN;
-#pragma unroll 1
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait_a(fullw0 + stage * 8, phase);
-          tc_fence_after();
-          if (elect_one()) {
-            if (trace_on && tr < 256) p.trace[256 + tr++] = clock64();
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  int prev = -1;
+  for (int kb = 0; kb < num_kb; ++kb) {
+    const int s = kb % STAGES;
+    mbar_wait(&full[s], (kb / STAGES) & 1);
+    const uint32_t a = smem_u32(smem + s * Ring::stage_bytes) + wg * 64 * 128;
+    const uint32_t b = smem_u32(smem + s * Ring::stage_bytes + TC_A_BYTES);
+    wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < BK / 16; ++k) {
-              if constexpr (PAIRM)
-                umma_bf16_2sm(d_tmem, make_desc(a16 + 2 * k, hi_sw), make_desc(a16 + b_off16 + 2 * k, hi_sw), idesc, (uint32_t)(kb | k));
-              else
-                umma_bf16(d_tmem, make_desc(a16 + 2 * k, hi_sw), make_desc(a16 + b_off16 + 2 * k, hi_sw), idesc, (uint32_t)(kb | k));
-            }
-            if constexpr (PAIRM) umma_commit_2sm(empty0 + stage * 8);  // both CTAs may refill this slot
-            else umma_commit_a(empty0 + stage * 8);  // frees the ring slot once these MMAs have read it
-            if (kb == num_kb - 1) {
-              if (trace_on && tr < 256) p.trace[256 + tr++] = -clock64();  // (negative) all MMAs of the tile issued
-              if constexpr (PAIRM) umma_commit_2sm(tmem_full0 + acc * 8);  // both CTAs' epilogues may read their accumulators
-              else umma_commit_a(tmem_full0 + acc * 8);  // accumulator complete -> epilogue
-            }
-          }
-          __syncwarp();
-          a16 += stride16;
-          if (++stage == (uint32_t)nstages) { stage = 0; phase ^= 1; a16 = base16; }
-        }
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    } else {
-      // ---- mode 2: A = the resident (tile + halo) patch.  Tap (r,s): the same patch, start shifted by r rows and s pixels;
-      //      8-row groups = patch rows (SBO), the two 16-byte K chunks of one MMA are one plane apart (LBO) ----
-      const bool b_res = p.b_resident != 0;
-      const int kchunks = pin(p.kchunks);
-      const uint32_t patch_off16 = (uint32_t)p.patch_off >> 4, patch_bytes16 = (uint32_t)p.patch_bytes >> 4;
-      uint32_t stage = 0, phase = 0, b16 = base16;
-      for (int t = walk_first; t < total_tiles; t += walk_step, tw_.next()) {
-        const int n_valid = min(bn, Cout - tw_.n_blk * bn);
-        const uint32_t idesc = umma_idesc_bf16((n_valid + 15) & ~15);
-        mbar_wait_a(tmem_empty0 + acc * 8, acc_phase ^ 1);
-        mbar_wait_a(patch_full0 + pb * 8, pb_phase);
-        if (b_res && t == walk_first)
-          for (int kb = 0; kb < num_kb; ++kb) mbar_wait_a(full0 + kb * 8, 0);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * TC_MAX_BN;
-        const uint32_t patch16 = base16 + patch_off16 + pb * patch_bytes16;
-        if (b_res) {
-          // weights resident (slot kb <-> k-block kb): nothing to wait for inside the tile, one elected lane issues it all
-          if (elect_one()) {
-            if (trace_on && tr < 256) p.trace[256 + tr++] = clock64();
-            uint32_t bk16 = base16, first = 0;
-#pragma unroll
-            for (int tap = 0; tap < 9; ++tap) {
-              uint32_t a_lo = patch16 + (uint32_t)((tap / 3) * TC_PATCH_W + (tap % 3));
-#pragma unroll 1
-              for (int kc = 0; kc < kchunks; ++kc) {
-#pragma unroll
-                for (int k = 0; k < BK / 16; ++k)
-                  umma_bf16(d_tmem, make_desc((a_lo + (uint32_t)(2 * k) * plane16) | lbo_patch, hi_patch), make_desc(bk16 + 2 * k, hi_sw),
-                            idesc, first | (uint32_t)k);
-                first = 1;
-                a_lo += (BK / 8) * plane16;
-                bk16 += stride16;
-              }
-            }
-            if (trace_on && tr < 256) p.trace[256 + tr++] = -clock64();
-            umma_commit_a(patch_empty0 + pb * 8);  // the patch may be overwritten once this tile's MMAs have read it
-            umma_commit_a(tmem_full0 + acc * 8);    // accumulator complete -> epilogue
-          }
-          __syncwarp();
-        } else {
-          uint32_t first = 0;
-#pragma unroll 1
-          for (int tap = 0; tap < 9; ++tap) {
-            uint32_t a_lo = patch16 + (uint32_t)((tap / 3) * TC_PATCH_W + (tap % 3));
-#pragma unroll 1
-            for (int kc = 0; kc < kchunks; ++kc) {
-              mbar_wait_a(full0 + stage * 8, phase);
-              tc_fence_after();
-              if (elect_one()) {
-                if (trace_on && tr < 256) p.trace[256 + tr++] = clock64();
-#pragma unroll
-                for (int k = 0; k < BK / 16; ++k)
-                  umma_bf16(d_tmem, make_desc((a_lo + (uint32_t)(2 * k) * plane16) | lbo_patch, hi_patch), make_desc(b16 + 2 * k, hi_sw),
-                            idesc, first | (uint32_t)k);
-                umma_commit_a(empty0 + stage * 8);
-              }
-              __syncwarp();
-              first = 1;
-              a_lo += (BK / 8) * plane16;
-              b16 += stride16;
-              if (++stage == (uint32_t)nstages) { stage = 0; phase ^= 1; b16 = base16; }
-            }
-          }
-          if (elect_one()) {
-            if (trace_on && tr < 256) p.trace[256 + tr++] = -clock64();
-            umma_commit_a(patch_empty0 + pb * 8);
-            umma_commit_a(tmem_full0 + acc * 8);
-          }
-          __syncwarp();
-        }
-        if (++pb == (uint32_t)p.npatch) { pb = 0; pb_phase ^= 1; }
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  }
-  if constexpr (SCALE) {
-    if ((warp >= 4 && warp < 8) || warp >= 11) {
-      // ===== A loaders + squeeze-excitation scalers (the reference's `scale * x` ahead of the projection conv,
-      // backbones/efficientnet.py:110-173; fp32 product rounded once to bf16 = bit-identical to se_scale_kernel).
-      // 256 threads: thread st owns the LOGICAL 16-byte chunk j = st & 7 (channels 8j .. 8j+7 of the k-block) of tile rows
-      // (st >> 3) + 32 i, i = 0..3 - all with the same row & 7, i.e. the same physical chunk position j ^ (row & 7) under the
-      // 128B swizzle.  A quarter-warp reads one 128-byte row segment from global memory and writes one 128-byte shared-memory
-      // row: coalesced and bank-conflict free.  Three k-blocks of loads are in flight per thread (12 x 16 B). =====
-      const int st = (warp < 8 ? warp - 4 : warp - 7) * 32 + lane;
-      const int j = st & 7, rb = st >> 3;
-      const uint32_t chunk_off = (uint32_t)p.patch_off + (uint32_t)(rb * 128 + ((j ^ (rb & 7)) << 4));
-      const int kchunks = pin(p.kchunks), Cin = pin(p.Cin), n_tiles = pin(p.n_tiles);
-      const __nv_bfloat16* __restrict__ A = (const __nv_bfloat16*)p.res_in;
-      const uint32_t a_full0 = smem_u32(scaled), a_empty0 = smem_u32(patch_empty);
-      uint4 av[3][4];
-      // load cursor (runs three k-blocks ahead of the store cursor)
-      int lt = walk_first, lkc = 0;
-      auto issue = [&](uint4 (&dst)[4]) {
-        const int m0 = (lt / n_tiles) * TC_BM + rb;
-        const int k = lkc * 64 + j * 8;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int m = m0 + 32 * i;
-          dst[i] = make_uint4(0u, 0u, 0u, 0u);  // M tail / K tail: zeros, as the TMA fill of the unscaled path
-          if (lt < total_tiles && m < p.M && k < Cin) dst[i] = __ldg(reinterpret_cast<const uint4*>(A + (size_t)m * Cin + k));
-        }
-        if (++lkc == kchunks) { lkc = 0; lt += walk_step; }
-      };
-#pragma unroll
-      for (int d = 0; d < 3; ++d) issue(av[d]);
-      uint32_t as = 0, a_phase = 0;
-      int t = walk_first, kc = 0;
-      const float* srow[4] = {p.a_scale, p.a_scale, p.a_scale, p.a_scale};
-      bool rok[4] = {false, false, false, false};
-      while (t < total_tiles) {
-#pragma unroll
-        for (int d = 0; d < 3; ++d) {
-          if (t < total_tiles) {
-            if (kc == 0) {
-              const int m0 = (t / n_tiles) * TC_BM + rb;
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const int m = m0 + 32 * i;
-                rok[i] = m < p.M;
-                srow[i] = p.a_scale + (size_t)(rok[i] ? m / p.a_scale_P : 0) * Cin + j * 8;
-              }
-            }
-            const bool kok = kc * 64 + j * 8 < Cin;
-            f32x2 sc[4][4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              float4 s0 = make_float4(0.f, 0.f, 0.f, 0.f), s1 = s0;
-              if (kok && rok[i]) {
-                s0 = __ldg(reinterpret_cast<const float4*>(srow[i] + kc * 64));
-                s1 = __ldg(reinterpret_cast<const float4*>(srow[i] + kc * 64 + 4));
-              }
-              sc[i][0] = f2_pack(s0.x, s0.y); sc[i][1] = f2_pack(s0.z, s0.w);
-              sc[i][2] = f2_pack(s1.x, s1.y); sc[i][3] = f2_pack(s1.z, s1.w);
-            }
-            mbar_wait_a(a_empty0 + as * 8, a_phase ^ 1);
-            uint8_t* sa = smem + chunk_off + as * TC_A_BYTES;
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const unsigned wd[4] = {av[d][i].x, av[d][i].y, av[d][i].z, av[d][i].w};
-              unsigned od[4];
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                float lo, hi;
-                f2_unpack(f2_mul(f2_pack(__uint_as_float(wd[e] << 16), __uint_as_float(wd[e] & 0xffff0000u)), sc[i][e]), lo, hi);
-                __nv_bfloat162 pk = __floats2bfloat162_rn(lo, hi);
-                od[e] = *reinterpret_cast<unsigned*>(&pk);
-              }
-              *reinterpret_cast<uint4*>(sa + i * 32 * 128) = make_uint4(od[0], od[1], od[2], od[3]);
-            }
-            fence_proxy_async();  // generic-proxy writes -> visible to the tensor core (async proxy)
-            __syncwarp();
-            if (lane == 0) mbar_arrive_a(a_full0 + as * 8);
-            if (++as == 3u) { as = 0; a_phase ^= 1; }
-            issue(av[d]);  // refill this register set: three k-blocks ahead
-            if (++kc == kchunks) { kc = 0; t += walk_step; }
-          }
-        }
-      }
-    }
-  }
-  if ((warp == 8 || warp == 11 || (warp == 9 && p.b_resident)) && patch_mode) {
-    // ===== mode 2: stage the (tile + halo) input patch, chunk-planar [plane][patch row][patch col][16 B], with cp.async
-    // (all of a thread's 16-byte copies in flight at once; out-of-image halo pixels and channels >= Cin zero-filled) =====
-    const int nload = p.b_resident ? 96 : 64;
-    const int lt = (warp == 8 ? 0 : warp == 11 ? 32 : 64) + lane;
-    const __nv_bfloat16* __restrict__ in = (const __nv_bfloat16*)p.res_in;
-    const int real_planes = p.Cin >> 3;
-    const int items = TC_PATCH_H * TC_PATCH_W * planes;
-    // two tiles of copies in flight per loader warp: tile t+1 is issued before tile t is waited for and handed over
-    int pb = 0, pb_sig = 0, pending = 0, ltr = 0;
-    uint32_t pb_phase = 0;
-    for (int t = walk_first; t < total_tiles; t += walk_step) {
-      const int m_blk = t / p.n_tiles;
-      const int tw = m_blk % p.tiles_w;
-      const int th = (m_blk / p.tiles_w) % p.tiles_h;
-      const int b = m_blk / (p.tiles_w * p.tiles_h);
-      const int ih0 = th * TC_PT_H - p.pad_t, iw0 = tw * TC_PT_W - p.pad_l;
-      uint32_t slot_free = 1;
-      if (pending) {  // warp-uniform poll (lane 0 decides)
-        slot_free = lane == 0 ? (uint32_t)mbar_try_wait(&patch_empty[pb], pb_phase ^ 1) : 0u;
-        slot_free = __shfl_sync(0xffffffffu, slot_free, 0);
-      }
-      if (!slot_free) {
-        // the next buffer is still being read: hand the tile in flight over first instead of holding it back
-        asm volatile("cp.async.wait_group 0;" ::: "memory");
-        if (!(p.debug & 256)) fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&patch_full[pb_sig]);
-        if (++pb_sig == p.npatch) pb_sig = 0;
-        pending = 0;
-      }
-      mbar_wait_a(smem_u32(&patch_empty[pb]), pb_phase ^ 1);
-      if (p.trace && (int)blockIdx.x == p.trace_cta && warp == 8 && lane == 0 && ltr < 256) p.trace[ltr++] = clock64();  // patch slot free
-      uint8_t* patch = smem + p.patch_off + pb * p.patch_bytes;
-      for (int i = lt; i < items && !(p.debug & 64); i += nload) {
-        const int j = i % planes, pix = i / planes;
-        const int ph = pix / TC_PATCH_W, pw = pix - ph * TC_PATCH_W;
-        const int ih = ih0 + ph, iw = iw0 + pw;
-        const bool ok = j < real_planes && ih >= 0 && ih < p.Hin && iw >= 0 && iw < p.Win && !(p.debug & 8);
-        const __nv_bfloat16* src = ok ? in + ((size_t)(b * p.Hin + ih) * p.Win + iw) * p.Cin + j * 8 : in;
-        cp_async_16(patch + j * TC_PLANE_BYTES + pix * 16, src, ok ? 16u : 0u);
-      }
-      asm volatile("cp.async.commit_group;" ::: "memory");
-      if (++pb == p.npatch) { pb = 0; pb_phase ^= 1; }
-      if (++pending == 2) {
-        asm volatile("cp.async.wait_group 1;" ::: "memory");  // the older of the two tiles has landed
-        if (!(p.debug & 256)) fence_proxy_async();  // generic-proxy writes -> visible to the tensor core (async proxy)
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&patch_full[pb_sig]);
-        if (p.trace && (int)blockIdx.x == p.trace_cta && warp == 8 && lane == 0 && ltr < 256) p.trace[ltr++] = clock64();  // patch staged
-        if (++pb_sig == p.npatch) pb_sig = 0;
-        --pending;
-      }
-    }
-    if (pending) {
-      asm volatile("cp.async.wait_group 0;" ::: "memory");
-      if (!(p.debug & 256)) fence_proxy_async();
+    for (int k = 0; k < TC_BK / 16; ++k) wgmma_bf16<BN>(acc, gmma_desc<128>(a + 32 * k), gmma_desc<128>(b + 32 * k), (uint32_t)(kb | k));
+    wgmma_commit();
+    wgmma_wait<1>();  // the previous k-block's MMAs are done: its stage goes back to the producer
+    if (prev >= 0) {
       __syncwarp();
-      if (lane == 0) mbar_arrive(&patch_full[pb_sig]);
+      if (lane == 0) mbar_arrive(&empty[prev]);
     }
+    prev = s;
   }
-  if (warp < (SCALE ? 4 : TCV_EPI_WARPS)) {
-    // ===== epilogue =====
-    constexpr int ch_step = SCALE ? 1 : 2;  // SCALE: one warp group walks every 64-column chunk of its rows
-    const int q = warp & 3, par = SCALE ? 0 : warp >> 2;
-    const int row = q * 32 + lane;
-    // long-K GEMMs (epi_single) run an epilogue once per >= 8 k-blocks: one staging slab per warp is enough there, and the
-    // other 32 KB buy one more operand stage in flight (those GEMMs stream A from HBM and are bound by bytes in flight)
-    uint8_t* slabs = p.epi_single ? smem + TCV_EPI_OFF + 8 * TCV_SLAB_BYTES + warp * TCV_SLAB_BYTES
-                                  : smem + TCV_EPI_OFF + warp * 2 * TCV_SLAB_BYTES;
-    float* bias_s = (float*)(smem + TCV_BIAS_OFF + warp * 256);
-    int acc = 0, etr = 0, tile_i = 0;
-    uint32_t acc_phase = 0, slab_count = 0;
-    const __nv_bfloat16* __restrict__ res = (const __nv_bfloat16*)p.res;
-    const int rows_per_q = 32 >> p.tile_w_log2;  // tile rows covered by one warp's 32 lanes (spatial modes)
-    const bool one_chunk = !SCALE && !PAIRM && p.n_tiles == 1 && p.Cout <= 64;
-    for (int t = walk_first; t < total_tiles; t += walk_step) {
-      if (one_chunk && (par ^ (tile_i & 1)) != 0) {
-        // one-chunk tiles belong to ONE warp group (even tiles: warps 0-3 / accumulator 0, odd tiles: warps 4-7 / accumulator
-        // 1); the other group must not even wait for the tile's tmem_full: nothing holds the MMA warp back from completing that
-        // barrier's NEXT phase before a lagging non-owner has looked at this one (parity waits cannot tell phase k from k + 2)
-        ++tile_i;
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-        continue;
-      }
-      const int m_unit = t / p.n_tiles, n_blk = t - m_unit * p.n_tiles;
-      const int m_blk = PAIRM ? 2 * m_unit + (int)rank : m_unit;  // this CTA's 128-row block
-      const int n0 = n_blk * p.bn;
-      const int n_valid = min(p.bn, p.Cout - n0);
-      bool valid;
-      size_t off;
-      int tw = 0, th = 0, b = 0;
-      if (p.mode == 0) {
-        int m = m_blk * TC_BM + row;
-        valid = m < p.M;
-        off = (size_t)m * p.Cout;
-      } else {
-        tw = m_blk % p.tiles_w;
-        th = (m_blk / p.tiles_w) % p.tiles_h;
-        b = m_blk / (p.tiles_w * p.tiles_h);
-        int oh = th * p.tile_h + (row >> p.tile_w_log2), ow = tw * p.tile_w + (row & (p.tile_w - 1));
-        valid = oh < p.Hout && ow < p.Wout;
-        off = ((size_t)(b * p.Hout + oh) * p.Wout + ow) * p.Cout;
-      }
-      const int nchunks = (n_valid + 63) >> 6;
-      const int ch_first = SCALE ? 0 : par ^ (nchunks == 1 ? (tile_i & 1) : 0);
-      // residual of this warp's FIRST half-chunk of the tile: issued BEFORE the accumulator wait, so its HBM round trip
-      // overlaps the tile's MMAs instead of starting when they end (the 32->32 stage-1 conv has one half-chunk per tile:
-      // its whole epilogue latency was this load)
-      uint4 rv_pre[4];
+  wgmma_wait<0>();
+  wgmma_fence_regs<BN / 2>(acc);
+
+  // ===== epilogue: thread rows r0 = 64 wg + 16 (warp & 3) + lane / 4 and r0 + 8, columns 8 j + 2 (lane % 4) + {0, 1} =====
+  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int c0 = n_blk * BN + 2 * (lane & 3);
+  const __nv_bfloat16* __restrict__ res = (const __nv_bfloat16*)p.res;
+  __nv_bfloat16* __restrict__ out = (__nv_bfloat16*)p.out;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    size_t off;
+    if (!tile_row_offset(p.mode, m_blk, r0 + 8 * h, p.M, p.Cout, p.tiles_w, p.tiles_h, p.Hout, p.Wout, off)) continue;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int c = c0 + 8 * j;
+      if (c >= p.Cout) break;  // Cout % 8 == 0: column c + 1 is valid with c
+      const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + c));
+      float o0 = acc[4 * j + 2 * h] + bv.x, o1 = acc[4 * j + 2 * h + 1] + bv.y;
       if constexpr (RES != 0) {
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          rv_pre[g] = make_uint4(0u, 0u, 0u, 0u);
-          if (ch_first < nchunks && valid && ch_first * 64 + g * 8 < n_valid && !(p.debug & 4))
-            rv_pre[g] = *reinterpret_cast<const uint4*>(res + off + n0 + ch_first * 64 + g * 8);
+        const float2 rv = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(res + off + c));
+        if constexpr (RES == 2) {
+          o0 = tc_act<ACT>(o0 + rv.x);
+          o1 = tc_act<ACT>(o1 + rv.y);
+        } else {
+          o0 = tc_act<ACT>(o0) + rv.x;
+          o1 = tc_act<ACT>(o1) + rv.y;
         }
+      } else {
+        o0 = tc_act<ACT>(o0);
+        o1 = tc_act<ACT>(o1);
       }
-      mbar_wait_a(smem_u32(&tmem_full[acc]), acc_phase);
-      tc_fence_after();
-      if (p.trace && (int)blockIdx.x == p.trace_cta && threadIdx.x == 0 && etr < 256) p.trace[512 + etr++] = clock64();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)acc * TC_MAX_BN;
-      bool released = false;
-      // two warp groups (par 0 / 1) alternate the 64-column chunks; one-chunk tiles alternate between the groups tile by tile
-      for (int ch = ch_first; ch < nchunks && !(p.debug & 128); ch += ch_step) {
-        const int c0 = ch * 64;
-        const int ncols = min(64, n_valid - c0);  // multiple of 8
-        // bias of the chunk -> this warp's staging (64 floats), broadcast-read below
-        __syncwarp();
-        if (lane < 16) {
-          float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (lane * 4 < ncols) bv = *reinterpret_cast<const float4*>(p.bias + n0 + c0 + lane * 4);
-          if constexpr (ACT == ACT_SILU && RES != 2) {  // staged HALVED: SiLU(v + b) = h + h tanh(h), h = 0.5 v + 0.5 b (one FMA)
-            bv.x *= 0.5f; bv.y *= 0.5f; bv.z *= 0.5f; bv.w *= 0.5f;
-          }
-          *reinterpret_cast<float4*>(bias_s + lane * 4) = bv;
-        }
-        uint8_t* slab = slabs + (p.epi_single ? 0u : (slab_count & 1)) * TCV_SLAB_BYTES;
-        if (lane == 0) {  // the store that last read this slab (2 chunks ago; the previous one with a single slab) is done with it
-          if (p.epi_single) tma_store_wait_read<0>();
-          else tma_store_wait_read<1>();
-        }
-        __syncwarp();
-        // two halves of 32 columns (keeps the live register set under the 128-register budget of a 416-thread CTA)
-#pragma unroll
-        for (int hf = 0; hf < 2; ++hf) {
-          const int cb = hf * 32;
-          // residual for this thread's row: issue the loads before waiting on TMEM
-          uint4 rv[4];
-          if constexpr (RES != 0) {
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              rv[g] = make_uint4(0u, 0u, 0u, 0u);
-              if (hf == 0 && ch == ch_first) rv[g] = rv_pre[g];
-              else if (valid && cb + g * 8 < ncols && !(p.debug & 4)) rv[g] = *reinterpret_cast<const uint4*>(res + off + n0 + c0 + cb + g * 8);
-            }
-          }
-          uint32_t v[32];
-          if (cb < ncols) tmem_ld16_issue(taddr + c0 + cb, v);
-          if (cb + 16 < ncols) tmem_ld16_issue(taddr + c0 + cb + 16, v + 16);
-          tmem_ld_wait();
-          if (hf == 1 && ch + ch_step >= nchunks) {  // last TMEM read of this warp in the tile
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-              if constexpr (PAIRM) mbar_arrive_leader(smem_u32(&tmem_empty[acc]), leader);
-              else mbar_arrive(&tmem_empty[acc]);
-            }
-            released = true;
-          }
-#pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            uint4 ov = make_uint4(0u, 0u, 0u, 0u);
-            if (cb + g * 8 < ncols && !(p.debug & 2)) {
-              const float4 b0 = *reinterpret_cast<const float4*>(bias_s + cb + g * 8);
-              const float4 b1 = *reinterpret_cast<const float4*>(bias_s + cb + g * 8 + 4);
-              float o[8];
-              if constexpr (ACT == ACT_SILU && RES != 2) {
-                // packed pairs (FFMA2): h = 0.5 v + 0.5 b, out = h + h tanh(h) [+ residual] - the arithmetic of tc_act<ACT_SILU>
-                // on (v + b), bit for bit (scaling by 0.5 is exact), in 2.5 instead of 4.5 instructions per element
-                const f32x2 hb[4] = {f2_pack(b0.x, b0.y), f2_pack(b0.z, b0.w), f2_pack(b1.x, b1.y), f2_pack(b1.z, b1.w)};
-                const f32x2 half2 = f2_pack(0.5f, 0.5f);
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                  const f32x2 h = f2_fma(f2_pack(__uint_as_float(v[g * 8 + 2 * i]), __uint_as_float(v[g * 8 + 2 * i + 1])), half2, hb[i]);
-                  float h0, h1;
-                  f2_unpack(h, h0, h1);
-                  f32x2 y = f2_fma(h, f2_pack(tanh_approx(h0), tanh_approx(h1)), h);
-                  if constexpr (RES == 1) {
-                    const unsigned wdi = i == 0 ? rv[g].x : i == 1 ? rv[g].y : i == 2 ? rv[g].z : rv[g].w;
-                    y = f2_add(y, f2_pack(__uint_as_float(wdi << 16), __uint_as_float(wdi & 0xffff0000u)));
-                  }
-                  f2_unpack(y, o[2 * i], o[2 * i + 1]);
-                }
-              } else {
-              o[0] = __uint_as_float(v[g * 8 + 0]) + b0.x; o[1] = __uint_as_float(v[g * 8 + 1]) + b0.y;
-              o[2] = __uint_as_float(v[g * 8 + 2]) + b0.z; o[3] = __uint_as_float(v[g * 8 + 3]) + b0.w;
-              o[4] = __uint_as_float(v[g * 8 + 4]) + b1.x; o[5] = __uint_as_float(v[g * 8 + 5]) + b1.y;
-              o[6] = __uint_as_float(v[g * 8 + 6]) + b1.z; o[7] = __uint_as_float(v[g * 8 + 7]) + b1.w;
-              if constexpr (RES != 0) {
-                const unsigned wd[4] = {rv[g].x, rv[g].y, rv[g].z, rv[g].w};
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                  const float r0 = __uint_as_float(wd[i] << 16), r1 = __uint_as_float(wd[i] & 0xffff0000u);
-                  o[2 * i] = RES == 2 ? tc_act<ACT>(o[2 * i] + r0) : tc_act<ACT>(o[2 * i]) + r0;
-                  o[2 * i + 1] = RES == 2 ? tc_act<ACT>(o[2 * i + 1] + r1) : tc_act<ACT>(o[2 * i + 1]) + r1;
-                }
-              } else {
-#pragma unroll
-                for (int i = 0; i < 8; ++i) o[i] = tc_act<ACT>(o[i]);
-              }
-              }
-              __nv_bfloat162* o2 = reinterpret_cast<__nv_bfloat162*>(&ov);
-#pragma unroll
-              for (int i = 0; i < 4; ++i) o2[i] = __floats2bfloat162_rn(o[2 * i], o[2 * i + 1]);
-            }
-            // 128B swizzle: 16-byte chunk j of slab row r lives at chunk position j ^ (r & 7)
-            const int j = hf * 4 + g;
-            *reinterpret_cast<uint4*>(slab + lane * 128 + ((j ^ (lane & 7)) << 4)) = ov;
-          }
-        }
-        if (!(p.debug & 256)) fence_proxy_async();  // generic-proxy smem writes -> visible to the TMA (async proxy)
-        __syncwarp();
-        if (lane == 0 && !(p.debug & 1)) {
-          if (p.mode == 0) tma_store_2d(&tmO, slab, n0 + c0, m_blk * TC_BM + q * 32);
-          else tma_store_4d(&tmO, slab, n0 + c0, tw * p.tile_w, th * p.tile_h + q * rows_per_q, b);
-          tma_store_commit();
-        }
-        ++slab_count;
-      }
-      if (!released && !one_chunk) {  // no chunk for this warp in the tile (narrow last tile): still
-        tc_fence_before();                                   // hand the accumulator back (one-chunk kernels: owner group only)
-        __syncwarp();
-        if (lane == 0) {
-          if constexpr (PAIRM) mbar_arrive_leader(smem_u32(&tmem_empty[acc]), leader);
-          else mbar_arrive(&tmem_empty[acc]);
-        }
-      }
-      if (p.trace && (int)blockIdx.x == p.trace_cta && threadIdx.x == 0 && etr < 256) p.trace[512 + etr++] = clock64();
-      ++tile_i;
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+      *reinterpret_cast<__nv_bfloat162*>(out + off + c) = __floats2bfloat162_rn(o0, o1);
     }
-    if (lane == 0) tma_store_wait_all();  // global writes complete before the CTA exits
-  }
-  tc_fence_before();
-  if constexpr (PAIRM) cluster_sync_all();  // neither CTA leaves while the pair's MMAs / remote arrivals may still touch it
-  else __syncthreads();
-  if (p.trace && threadIdx.x == 0) {  // per-CTA totals: cycles and nanoseconds from start to drained pipeline
-    unsigned long long g1;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g1));
-    p.trace[768 + 2 * blockIdx.x] = clock64() - cta_t0;
-    p.trace[768 + 2 * blockIdx.x + 1] = (long long)(g1 - cta_g0);
-  }
-  if (warp == 10) {
-    tc_fence_after();
-    if constexpr (PAIRM) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
-    else tmem_dealloc(tmem_base, 512);
   }
 }
 
-// in-place squeeze-excitation scaling  x[b,p,c] *= s[b,c]  ahead of a tcgen05 projection GEMM
+// in-place squeeze-excitation scaling  x[b,p,c] *= s[b,c]  ahead of a tensor-core projection GEMM
 __global__ void __launch_bounds__(256) se_scale_kernel(__nv_bfloat16* __restrict__ x, const float* __restrict__ s, int P, int C,
                                                        size_t total8) {
   pdl_trigger();
@@ -1226,65 +352,18 @@ struct TcWeights {
   int Cout = 0, Cin = 0, taps = 1, S = 1;
   // head
   int n_real = 0;
-  // per-shape launch state (A tensor map depends on the activation pointer and batch)
-  mutable CUtensorMap mapA, mapB, mapO;
+  mutable CUtensorMap mapA, mapB;
   mutable const void* cached_in = nullptr;
-  mutable const void* cached_out = nullptr;
-  mutable int cached_B = -1, cached_bn = 0;
-  // conv path: tensor maps per (input, output, batch, N tile) - a crop-chunked forward launches the same op on several
-  // buffer slices per step, and re-encoding three maps per launch would sit on the host's launch path
+  mutable int cached_B = -1;
+  // conv path: tensor maps per (input, batch, N tile) - re-encoding them per launch would sit on the host's launch path
   struct MapSet {
-    CUtensorMap a, b, o;
+    CUtensorMap a, b;
     const void* in = nullptr;
-    const void* out = nullptr;
-    int B = -1, bn = 0, pair = 0;
+    int B = -1, bn = 0;
   };
   mutable std::vector<MapSet> map_sets;
   mutable size_t map_rr = 0;
 };
-
-// MTB_FUSE_SE=1: the projection GEMM applies the squeeze-excitation scale itself (SCALE variant of tc_conv_kernel) instead of
-// an in-place se_scale_kernel pass ahead of it.  OFF by default - built three ways and measured each time (V2-L, 256 crops;
-// profiles/r2_fused_se_*):
-//   round 1: TMA -> 4 scaler warps rewrite the A tile in shared memory -> MMA: step 23.96 vs 22.65 ms;
-//   round 2: the same with 8 scaler warps, scale values prefetched, FMUL2: projections 5.40 vs 3.06 ms, i.e. again what the
-//            separate pass costs (2.45 ms); with the scalers reduced to wait + arrive still 1.65 vs 1.08 ms on the 2304->384
-//            GEMMs: the extra barrier hop on a 3-stage 48 KB/stage ring that is bound by bytes in flight;
-//   round 2: A loaded by 8 loader warps straight from global memory (registers three k-blocks ahead), scaled, stored swizzled
-//            (the version below): projections 6.04 ms; ncu: 22.6 M warp instructions per launch against 4.0 M (250 per thread
-//            and k-block against 384 cycles of MMA per k-block) - issue-bound.
-// What would change the picture is a cheaper multiply (bf16 x bf16 HMUL2 with a bf16 scale: 4 instructions per 16-byte chunk
-// instead of ~24, at the price of a second rounding) - not taken: it would move the mode further from the reference arithmetic.
-inline bool tc_fuse_se() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("MTB_FUSE_SE");
-    v = (e && e[0] == '1') ? 1 : 0;
-  }
-  return v == 1;
-}
-// the scaler warps of tc_conv_kernel handle flat 1x1 GEMMs with 128-byte (BK = 64) A rows and no activation (projections)
-inline bool tc_can_fuse_se(int R, int stride, int cin, int act = ACT_NONE) {
-  return tc_fuse_se() && R == 1 && stride == 1 && cin > 32 && cin % 8 == 0 && act == ACT_NONE;
-}
-
-inline bool tc_pair_enabled() {  // MTB_TC_PAIR=0: flat GEMMs on single CTAs (A/B runs)
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("MTB_TC_PAIR");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
-}
-
-inline bool tc_patch_disabled() {  // MTB_DISABLE_PATCH=1: 3x3 convs fall back to the per-tap TMA mode (A/B testing)
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("MTB_DISABLE_PATCH");
-    v = (e && e[0] == '1') ? 1 : 0;
-  }
-  return v == 1;
-}
 
 inline bool tc_disabled() {
   static int v = -1;
@@ -1331,193 +410,65 @@ inline const char* tc_prepare_weights(TcWeights& w, const float* wk, const float
   return nullptr;
 }
 
-// N-tile stride (multiple of 64).  Per-tile time model (cycles): the single-thread TMA / MMA issuers cost ~kb_floor per
-// k-block whatever its size (measured with the in-kernel clock64 trace), an MMA k-block takes (BK/16) * N/2, and the
-// epilogue (overlapped with the next tile's main loop) ~epi_chunk per pair of 64-column chunks.
-inline int tc_pick_bn(int cout, int m_tiles, int num_kb, int bk) {
-  const double kb_floor = 300.0, epi_chunk = 900.0;
-  int best = 64;
-  double best_cost = 1e30;
-  for (int bn = 256; bn >= 64; bn -= 64) {
-    int nt = (cout + bn - 1) / bn;
-    long tiles = (long)m_tiles * nt;
-    long waves = (tiles + 147) / 148;
-    int last = cout - (nt - 1) * bn;                          // width of the ragged last tile
-    double avg_n = ((double)(nt - 1) * bn + ((last + 15) & ~15)) / nt;
-    double mma_kb = (bk / 16) * avg_n / 2.0;
-    double mainloop = num_kb * (mma_kb > kb_floor ? mma_kb : kb_floor);
-    double epi = ((bn / 64 + 1) / 2) * epi_chunk;
-    double cost = (double)waves * ((mainloop > epi ? mainloop : epi) + 400.0);
-    if (cost < best_cost - 1e-9) {
-      best_cost = cost;
-      best = bn;
-    }
-  }
-  return best;
-}
+// N-tile width: the narrowest wgmma N in {32, 64, 128} that covers Cout, else 128 (Cout > 128 runs several N tiles)
+inline int tc_pick_bn(int cout) { return cout <= 32 ? 32 : cout <= 64 ? 64 : 128; }
 
-template <int ACT, int RES, int BK, bool PATCH, bool SCALE = false, bool PAIRM = false>
-inline const char* tc_conv_launch_k(int grid, const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& o, const TcConvParams& q,
-                                    cudaStream_t st) {
+template <int ACT, int RES, int BN>
+inline const char* tc_conv_launch_k(dim3 grid, const CUtensorMap& a, const CUtensorMap& b, const TcConvParams& q, cudaStream_t st) {
   static bool attr_set = false;
   if (!attr_set) {
-    if (cudaFuncSetAttribute(tc_conv_kernel<ACT, RES, BK, PATCH, SCALE, PAIRM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             TCV_SMEM_BYTES) != cudaSuccess)
+    if (cudaFuncSetAttribute(tc_conv_kernel<ACT, RES, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcRing<BN>::smem_bytes) !=
+        cudaSuccess)
       return "cannot raise dynamic shared memory for tc_conv_kernel";
     attr_set = true;
   }
-  cudaError_t e;
-  if constexpr (PAIRM) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(TC_THREADS);
-    cfg.dynamicSmemBytes = TCV_SMEM_BYTES;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    e = cudaLaunchKernelEx(&cfg, tc_conv_kernel<ACT, RES, BK, PATCH, SCALE, PAIRM>, a, b, o, q);
-  } else {
-    launch_k(tc_conv_kernel<ACT, RES, BK, PATCH, SCALE, PAIRM>, dim3(grid), dim3(TC_THREADS), TCV_SMEM_BYTES, st, a, b, o, q);
-    e = cudaGetLastError();
-  }
+  launch_k(tc_conv_kernel<ACT, RES, BN>, grid, dim3(TC_THREADS), TcRing<BN>::smem_bytes, st, a, b, q);
+  cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 template <int ACT, int RES>
-inline const char* tc_conv_launch_t(int grid, const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& o, const TcConvParams& q,
-                                    cudaStream_t st) {
-  if constexpr (ACT == ACT_NONE) {
-    if (q.a_scale != nullptr) return tc_conv_launch_k<ACT, RES, 64, false, true>(grid, a, b, o, q, st);
+inline const char* tc_conv_launch_t(int bn, dim3 grid, const CUtensorMap& a, const CUtensorMap& b, const TcConvParams& q, cudaStream_t st) {
+  switch (bn) {
+    case 32: return tc_conv_launch_k<ACT, RES, 32>(grid, a, b, q, st);
+    case 64: return tc_conv_launch_k<ACT, RES, 64>(grid, a, b, q, st);
+    default: return tc_conv_launch_k<ACT, RES, 128>(grid, a, b, q, st);
   }
-  if (q.pair) return tc_conv_launch_k<ACT, RES, 64, false, false, true>(grid, a, b, o, q, st);
-  if (q.mode == 2)
-    return q.bk == 32 ? tc_conv_launch_k<ACT, RES, 32, true>(grid, a, b, o, q, st) : tc_conv_launch_k<ACT, RES, 64, true>(grid, a, b, o, q, st);
-  return q.bk == 32 ? tc_conv_launch_k<ACT, RES, 32, false>(grid, a, b, o, q, st) : tc_conv_launch_k<ACT, RES, 64, false>(grid, a, b, o, q, st);
 }
-
 template <int ACT>
-inline const char* tc_conv_dispatch_res(int res_mode, int grid, const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& o,
-                                        const TcConvParams& q, cudaStream_t st) {
+inline const char* tc_conv_dispatch_res(int res_mode, int bn, dim3 grid, const CUtensorMap& a, const CUtensorMap& b, const TcConvParams& q,
+                                        cudaStream_t st) {
   switch (res_mode) {
-    case 0: return tc_conv_launch_t<ACT, 0>(grid, a, b, o, q, st);
-    case 1: return tc_conv_launch_t<ACT, 1>(grid, a, b, o, q, st);
-    default: return tc_conv_launch_t<ACT, 2>(grid, a, b, o, q, st);
-  }
-}
-
-inline const char* tc_conv_dispatch(int act, int res_mode, int grid, const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& o,
-                                    const TcConvParams& q, cudaStream_t st) {
-  switch (act) {
-    case ACT_NONE: return tc_conv_dispatch_res<ACT_NONE>(res_mode, grid, a, b, o, q, st);
-    case ACT_SILU: return tc_conv_dispatch_res<ACT_SILU>(res_mode, grid, a, b, o, q, st);
-    case ACT_RELU: return tc_conv_dispatch_res<ACT_RELU>(res_mode, grid, a, b, o, q, st);
-    case ACT_HSWISH: return tc_conv_dispatch_res<ACT_HSWISH>(res_mode, grid, a, b, o, q, st);
-    default: return "unsupported activation in the tensor-core epilogue";
+    case 0: return tc_conv_launch_t<ACT, 0>(bn, grid, a, b, q, st);
+    case 1: return tc_conv_launch_t<ACT, 1>(bn, grid, a, b, q, st);
+    default: return tc_conv_launch_t<ACT, 2>(bn, grid, a, b, q, st);
   }
 }
 
 inline const char* tc_conv_launch(const TcWeights& w, const ConvParams& p, bool res_first, cudaStream_t st) {
   TcConvParams q;
-  // Squeeze-excitation scale fused into the A tiles in shared memory (scaler warps 11-14; opt-in, see tc_fuse_se()).
-  q.a_scale = tc_can_fuse_se(p.R, p.stride, p.Cin, p.act) ? p.a_scale : nullptr;
-  q.a_scale_P = p.Hin * p.Win;
-  q.res = p.res; q.bias = w.d_bias;
-  const int bk0 = p.Cin <= 32 ? 32 : 64;  // 64B-swizzled half-width stages only when they do not add k-blocks
-  const int planes0 = ((p.Cin + bk0 - 1) / bk0) * (bk0 / 8);
+  q.res = p.res; q.bias = w.d_bias; q.out = p.out;
   q.mode = (p.R == 1 && p.stride == 1) ? 0 : 1;
-  if (p.R == 3 && p.S == 3 && p.stride == 1 && p.dil == 1 && planes0 <= TC_PATCH_MAX_PLANES && !tc_patch_disabled()) q.mode = 2;
-  q.tile_w = q.mode == 2 ? TC_PT_W : TC_TILE_W;
-  q.tile_h = q.mode == 2 ? TC_PT_H : TC_TILE_H;
-  q.tile_w_log2 = q.mode == 2 ? 3 : 4;
   q.Hin = p.Hin; q.Win = p.Win;
-  q.res_in = p.in;
-  {
-    static int dbg = -1;
-    if (dbg < 0) { const char* e = getenv("MTB_TC_DEBUG"); dbg = e ? atoi(e) : 0; }
-    q.debug = dbg;
-  }
   q.Cout = p.Cout; q.Cin = p.Cin;
-  q.taps = w.taps; q.R = p.R; q.S = w.S; q.stride = p.stride; q.dil = p.dil;
-  q.bk = bk0;  // every k-block costs ~0.3-0.5k cycles of single-thread TMA/MMA issue: never trade padding for more k-blocks
-  q.kchunks = (p.Cin + q.bk - 1) / q.bk;
+  q.taps = w.taps; q.S = w.S; q.stride = p.stride; q.dil = p.dil;
+  q.kchunks = (p.Cin + TC_BK - 1) / TC_BK;
   q.Hout = p.Hout; q.Wout = p.Wout; q.pad_t = p.pad_t; q.pad_l = p.pad_l;
-  q.tiles_w = (p.Wout + q.tile_w - 1) / q.tile_w;
-  q.tiles_h = (p.Hout + q.tile_h - 1) / q.tile_h;
+  q.tiles_w = (p.Wout + TC_TILE_W - 1) / TC_TILE_W;
+  q.tiles_h = (p.Hout + TC_TILE_H - 1) / TC_TILE_H;
   q.M = p.B * p.Hout * p.Wout;
-  q.m_tiles = q.mode == 0 ? (q.M + TC_BM - 1) / TC_BM : p.B * q.tiles_w * q.tiles_h;
-  const int bn = tc_pick_bn(p.Cout, q.m_tiles, q.taps * q.kchunks, q.bk);
-  q.bn = bn;
-  // CTA pairs for the flat GEMMs that re-read a wide weight tile per k-block (MBConv expand / projection, last conv, ResNet 1x1)
-  // Measured (V2-L, 256 crops, profiles/r2_tc_pair_vs_single.txt): projections with K >= 1344 gain 4-17 %, the 640 -> 3840
-  // expand 7 %; the short-K expand GEMMs (K <= 384) are bound by their SiLU epilogue, not by operand traffic, and lose 1-6 %.
-  q.pair = (tc_pair_enabled() && q.mode == 0 && q.a_scale == nullptr && q.bk == 64 && p.Cout > 64 && q.taps * q.kchunks >= 8 &&
-            (long)((q.m_tiles + 1) / 2) * ((p.Cout + bn - 1) / bn) >= 74) ? 1 : 0;  // at least one unit per pair of SMs
-  {
-    const int a_bytes = q.mode == 2 ? 0 : TC_BM * q.bk * 2;
-    // weight box: no zero-fill rows when a single N tile covers Cout (a 256-row box for Cout = 32 cost 8x the shared-memory
-    // fill and kept the weights from staying resident)
-    q.b_rows = (p.Cout + bn - 1) / bn == 1 ? (p.Cout + 15) / 16 * 16 : bn;
-    if (q.pair) q.b_rows /= 2;  // each CTA of a pair stages half of the tile's weight rows
-    q.stage_stride = (a_bytes + q.b_rows * q.bk * 2 + 1023) / 1024 * 1024;
-    q.patch_bytes = q.mode == 2 ? (planes0 * TC_PLANE_BYTES + 1023) / 1024 * 1024 : 0;
-    const int num_kb = q.taps * q.kchunks;
-    // four patch buffers when the weights still fit next to them (two loads in flight + one consumed + one ready)
-    q.npatch = 2;
-    if (q.mode == 2 && (p.Cout + bn - 1) / bn == 1 && num_kb <= TCV_MAX_STAGES &&
-        num_kb * q.stage_stride + 4 * q.patch_bytes <= TCV_RING_BYTES)
-      q.npatch = 4;
-    q.patch_off = TCV_RING_BYTES - q.npatch * q.patch_bytes;
-    int ring = q.mode == 2 ? q.patch_off : TCV_RING_BYTES;
-    q.epi_single = 0;
-    {
-      static int es_env = -1;  // MTB_TC_EPI_SINGLE=0 keeps the double-buffered epilogue slabs everywhere (A/B runs)
-      if (es_env < 0) { const char* e = getenv("MTB_TC_EPI_SINGLE"); es_env = (e && e[0] == '0') ? 0 : 1; }
-      const int ring_ext = TCV_RING_BYTES + 8 * TCV_SLAB_BYTES;
-      if (es_env && q.mode == 0 && num_kb >= 8 && ring_ext / q.stage_stride > ring / q.stage_stride &&
-          ring / q.stage_stride < TCV_MAX_STAGES) {
-        q.epi_single = 1;
-        ring = ring_ext;
-      }
-    }
-    q.nstages = ring / q.stage_stride;
-    if (q.nstages > TCV_MAX_STAGES) q.nstages = TCV_MAX_STAGES;
-    if (q.nstages < 2) return "operand ring too small for this tile";
-    q.b_resident = (q.mode == 2 && (p.Cout + bn - 1) / bn == 1 && num_kb <= q.nstages) ? 1 : 0;
-    if (q.b_resident) q.nstages = num_kb;
-    if (q.a_scale != nullptr) {
-      // SCALE: ring stages hold the weights only; three A slots (written by the loader warps) behind them; the four
-      // epilogue warps use one slab each, so the ring region is the extended 176 KB one
-      q.epi_single = 1;
-      q.stage_stride = (q.b_rows * q.bk * 2 + 1023) / 1024 * 1024;
-      q.nstages = (TCV_RING_BYTES + 8 * TCV_SLAB_BYTES - 3 * TC_A_BYTES) / q.stage_stride;
-      if (q.nstages > TCV_MAX_STAGES) q.nstages = TCV_MAX_STAGES;
-      if (q.nstages < 2) return "operand ring too small for this tile";
-      q.patch_off = q.nstages * q.stage_stride;
-    }
-  }
-  q.n_tiles = (p.Cout + bn - 1) / bn;
-  {
-    static int rot_env = -1;  // MTB_TC_ROT=1 enables the K rotation (measured: no effect on the projection GEMMs, so off)
-    if (rot_env < 0) { const char* e = getenv("MTB_TC_ROT"); rot_env = (e && e[0] == '1') ? 1 : 0; }
-    q.rot = (rot_env && q.mode != 2 && q.a_scale == nullptr) ? 1 : 0;
-  }
+  const int m_tiles = q.mode == 0 ? (q.M + TC_BM - 1) / TC_BM : p.B * q.tiles_w * q.tiles_h;
+  const int bn = tc_pick_bn(p.Cout);
   const TcWeights::MapSet* ms = nullptr;
   for (const TcWeights::MapSet& c : w.map_sets)
-    if (c.in == p.in && c.out == p.out && c.B == p.B && c.bn == bn && c.pair == q.pair) { ms = &c; break; }
+    if (c.in == p.in && c.B == p.B && c.bn == bn) { ms = &c; break; }
   if (!ms) {
     TcWeights::MapSet c;
-    const char* e = q.mode == 0 ? make_tmap_2d(&c.a, p.in, (uint64_t)q.M, (uint64_t)p.Cin, TC_BM, (uint32_t)q.bk)
-                                : make_tmap_nhwc(&c.a, p.in, p.B, p.Hin, p.Win, p.Cin, (uint32_t)p.stride, (uint32_t)q.bk);
+    const char* e = q.mode == 0 ? make_tmap_2d(&c.a, p.in, (uint64_t)q.M, (uint64_t)p.Cin, TC_BM)
+                                : make_tmap_nhwc(&c.a, p.in, p.B, p.Hin, p.Win, p.Cin, (uint32_t)p.stride);
     if (e) return e;
-    e = make_tmap_2d(&c.b, w.d_w, (uint64_t)p.Cout, (uint64_t)w.taps * p.Cin, (uint32_t)q.b_rows, (uint32_t)q.bk);
+    e = make_tmap_2d(&c.b, w.d_w, (uint64_t)p.Cout, (uint64_t)w.taps * p.Cin, (uint32_t)bn);
     if (e) return e;
-    // output boxes are per epilogue warp: 32 tile rows x 64 channels
-    e = q.mode == 0 ? make_tmap_2d(&c.o, p.out, (uint64_t)q.M, (uint64_t)p.Cout, 32)
-                    : make_tmap_nhwc(&c.o, p.out, p.B, p.Hout, p.Wout, p.Cout, 1, TC_BK, (uint32_t)q.tile_w, (uint32_t)(32 / q.tile_w));
-    if (e) return e;
-    c.in = p.in; c.out = p.out; c.B = p.B; c.bn = bn; c.pair = q.pair;
+    c.in = p.in; c.B = p.B; c.bn = bn;
     if (w.map_sets.size() < 16) {
       w.map_sets.push_back(c);
       ms = &w.map_sets.back();
@@ -1527,64 +478,15 @@ inline const char* tc_conv_launch(const TcWeights& w, const ConvParams& p, bool 
       ++w.map_rr;
     }
   }
-  const int total = (q.pair ? (q.m_tiles + 1) / 2 : q.m_tiles) * q.n_tiles;
-  int grid = total < 148 ? total : 148;
-  if (q.pair) grid = total < 74 ? 2 * total : 148;  // whole pairs
-  { static int g_env = -1; if (g_env < 0) { const char* e = getenv("MTB_TC_GRID"); g_env = e ? atoi(e) : 0; } if (g_env > 0 && g_env < grid) grid = g_env; }
+  const dim3 grid(m_tiles, (p.Cout + bn - 1) / bn);
   const int res_mode = p.res ? (res_first ? 2 : 1) : 0;
-  q.trace = nullptr;
-  q.trace_cta = 0;
-  { const char* e = getenv("MTB_TC_TRACE_CTA"); if (e) q.trace_cta = atoi(e); }
-  static const char* trace_env = getenv("MTB_TC_TRACE");  // "<Cin>x<Cout>": trace the first launch of that shape
-  static long long* trace_buf = nullptr;
-  static bool traced = false;
-  bool dump = false;
-  if (trace_env && !traced) {
-    int ci = 0, co = 0;
-    if (sscanf(trace_env, "%dx%d", &ci, &co) == 2 && ci == p.Cin && co == p.Cout) {
-      if (!trace_buf) cudaMalloc(&trace_buf, 1088 * sizeof(long long));
-      cudaMemsetAsync(trace_buf, 0, 1088 * sizeof(long long), st);
-      q.trace = trace_buf;
-      dump = traced = true;
-    }
+  switch (p.act) {
+    case ACT_NONE: return tc_conv_dispatch_res<ACT_NONE>(res_mode, bn, grid, ms->a, ms->b, q, st);
+    case ACT_SILU: return tc_conv_dispatch_res<ACT_SILU>(res_mode, bn, grid, ms->a, ms->b, q, st);
+    case ACT_RELU: return tc_conv_dispatch_res<ACT_RELU>(res_mode, bn, grid, ms->a, ms->b, q, st);
+    case ACT_HSWISH: return tc_conv_dispatch_res<ACT_HSWISH>(res_mode, bn, grid, ms->a, ms->b, q, st);
+    default: return "unsupported activation in the tensor-core epilogue";
   }
-  const char* err = tc_conv_dispatch(p.act, res_mode, grid, ms->a, ms->b, ms->o, q, st);
-  if (dump && !err) {
-    std::vector<long long> hbuf(1088);
-    cudaStreamSynchronize(st);
-    cudaMemcpy(hbuf.data(), trace_buf, 1088 * sizeof(long long), cudaMemcpyDeviceToHost);
-    {
-      long long cmin = 1LL << 60, cmax = 0, nmin = 1LL << 60, nmax = 0;
-      double csum = 0, nsum = 0;
-      for (int i = 0; i < grid; ++i) {
-        long long c = hbuf[768 + 2 * i], n = hbuf[768 + 2 * i + 1];
-        cmin = c < cmin ? c : cmin; cmax = c > cmax ? c : cmax; nmin = n < nmin ? n : nmin; nmax = n > nmax ? n : nmax;
-        csum += (double)c; nsum += (double)n;
-      }
-      if (q.debug & 32) {
-        fprintf(stderr, "  per-CTA cycles:");
-        for (int i = 0; i < grid; ++i) fprintf(stderr, " %lld", hbuf[768 + 2 * i] / 1000);
-        fprintf(stderr, "\n");
-      }
-      fprintf(stderr, "  per-CTA totals: cycles min %lld mean %.0f max %lld | ns min %lld mean %.0f max %lld | CTA0 %lld cyc %lld ns\n", cmin,
-              csum / grid, cmax, nmin, nsum / grid, nmax, hbuf[768], hbuf[769]);
-    }
-    long long t0 = hbuf[0] ? hbuf[0] : hbuf[256];
-    if (t0 < 0) t0 = -t0;
-    fprintf(stderr, "MTB_TC_TRACE Cin=%d Cout=%d mode=%d bk=%d bn=%d kb/tile=%d tiles=%d grid=%d\n", p.Cin, p.Cout, q.mode, q.bk, q.bn,
-            q.taps * q.kchunks, total, grid);
-    const char* names[3] = {"producer(TMA issued)", "mma(full wait done)", "epilogue(tmem_full done / tile end)"};
-    for (int r = 0; r < 3; ++r) {
-      fprintf(stderr, "  %s:", names[r]);
-      for (int i = 0; i < ((q.debug & 32) ? 256 : 70) && hbuf[r * 256 + i]; ++i) {
-        long long v = hbuf[r * 256 + i];
-        if (v < 0) fprintf(stderr, " [%lld]", -v - t0);
-        else fprintf(stderr, " %lld", v - t0);
-      }
-      fprintf(stderr, "\n");
-    }
-  }
-  return err;
 }
 
 inline const char* tc_se_scale_launch(void* x, const float* s, int B, int P, int C, cudaStream_t st) {
@@ -1597,8 +499,9 @@ inline const char* tc_se_scale_launch(void* x, const float* s, int B, int P, int
 // ----------------------------------------------------------------------------------------- fused head kernel
 // MetrabsHeads.forward (models/metrabs.py:75-85) with ptu.soft_argmax (ptu.py:47-75) fused behind the 1x1 conv:
 //   D[n, pixel] = sum_c W[n, c] * F[pixel, c]        A = head weights [N_out][C] (M = channels, 128 per tile)
-//                                                     B = features     [B*P][C]  (N = pixels, <= 256 per MMA)
-// Epilogue thread <-> one channel n = J + d*J + j (or n = j < J for the 2D head): it adds the bias and keeps the
+//                                                     B = features     [B*P][C]  (N = pixels, <= 256 per tile)
+// Each consumer warpgroup computes 64 channels x 256 pixels in registers and parks them in its half of a shared-memory
+// staging tile; then one thread per channel n = J + d*J + j (or n = j < J for the 2D head) adds the bias and keeps the
 // online-softmax state (max, sum e, sum e*x, sum e*y) of ITS pixels in registers, across the pixel tiles of a crop;
 // one float4 per (crop, channel) goes to a scratch, and head_finalize_kernel merges the D depth slices of every
 // joint (sum e*z = d * sum e), applies linspace(0,1,n) and heatmap_to_image / heatmap_to_metric.
@@ -1606,185 +509,172 @@ struct TcHeadParams {
   float4* states;     // [B][n_out] (m, s, sx, sy)
   const float* bias;  // [n_out]
   int B, P, W, n_out, C;
-  int bnp;            // pixels per MMA (N)
+  int bnp;            // pixels per tile (N)
   int cpt;            // crops per tile when P <= 256, else 0
   int npt;            // pixel tiles per crop when P > 256, else 1
-  int n_groups;       // crop groups
   int m_tiles;        // ceil(n_out / 128)
   int kblocks;        // ceil(C / 64)
-  uint32_t idesc;
 };
+constexpr int TCH_STAGES = 2;
+constexpr int TCH_STAGE_BYTES = TC_A_BYTES + 256 * TC_BK * 2;      // 48 KB
+constexpr int TCH_STG_OFF = TCH_STAGES * TCH_STAGE_BYTES;           // staging: [128 channels][256 pixels] fp32 = 128 KB
+constexpr int TCH_BAR_OFF = TCH_STG_OFF + 128 * 256 * 4;
+constexpr int TCH_SMEM_BYTES = TCH_BAR_OFF + 64 + 1024 /*align slack*/;
 
-__global__ void __launch_bounds__(256, 1)
+// staging element (row, col): 16-byte chunks of a row XOR-rotated by row & 7 (the row owners read along their rows)
+__device__ __forceinline__ uint32_t tch_stg(int row, int col) {
+  return (uint32_t)(row * 256 + ((((col >> 2) ^ (row & 7))) << 2) + (col & 3)) * 4u;
+}
+
+__global__ void __launch_bounds__(TC_THREADS, 1)
 tc_head_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmF, const TcHeadParams p) {
   extern __shared__ uint8_t tc_smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)tc_smem_raw + 1023) & ~(uintptr_t)1023);
-  uint64_t* bars = (uint64_t*)(smem + TC_STAGES * TC_STAGE_BYTES);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + TC_STAGES;
-  uint64_t* tmem_full = bars + 2 * TC_STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_slot = (uint32_t*)(tmem_empty + 2);
+  uint64_t* full = (uint64_t*)(smem + TCH_BAR_OFF);
+  uint64_t* empty = full + TCH_STAGES;
+  float* stg = (float*)(smem + TCH_STG_OFF);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == TC_CONSUMER_WARPS * 32) {
     tma_prefetch_desc(&tmW);
     tma_prefetch_desc(&tmF);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < TC_STAGES; ++i) {
+    for (int i = 0; i < TCH_STAGES; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 4);
+      mbar_init(&empty[i], TC_CONSUMER_WARPS);
     }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_trigger();
   pdl_wait();
 
-  const int items = p.n_groups * p.m_tiles;
-  const uint32_t stage_tx = TC_A_BYTES + (uint32_t)p.bnp * TC_BK * 2;
-
-  if (warp == 0) {
+  const int g = blockIdx.x / p.m_tiles, m_blk = blockIdx.x - g * p.m_tiles;
+  const int n_kb = p.npt * p.kblocks;
+  if (warp == TC_CONSUMER_WARPS) {
     if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int it = blockIdx.x; it < items; it += gridDim.x) {
-        const int g = it / p.m_tiles, m_blk = it - g * p.m_tiles;
-        for (int pt = 0; pt < p.npt; ++pt) {
-          const int row0 = p.cpt > 0 ? g * p.bnp : g * p.P + pt * p.bnp;
-          for (int kb = 0; kb < p.kblocks; ++kb) {
-            mbar_wait(&empty[stage], phase ^ 1);
-            uint8_t* sa = smem + stage * TC_STAGE_BYTES;
-            mbar_expect_tx(&full[stage], stage_tx);
-            tma_load_2d(sa, &tmW, &full[stage], kb * TC_BK, m_blk * TC_BM);
-            tma_load_2d(sa + TC_A_BYTES, &tmF, &full[stage], kb * TC_BK, row0);
-            if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
-          }
-        }
+      const uint32_t stage_tx = TC_A_BYTES + (uint32_t)p.bnp * TC_BK * 2;
+      for (int i = 0; i < n_kb; ++i) {
+        const int s = i % TCH_STAGES, pt = i / p.kblocks, kb = i - pt * p.kblocks;
+        mbar_wait(&empty[s], ((i / TCH_STAGES) & 1) ^ 1);
+        uint8_t* sa = smem + s * TCH_STAGE_BYTES;
+        const int row0 = p.cpt > 0 ? g * p.bnp : g * p.P + pt * p.bnp;
+        mbar_expect_tx(&full[s], stage_tx);
+        tma_load_2d(sa, &tmW, &full[s], kb * TC_BK, m_blk * TC_BM);
+        tma_load_2d(sa + TC_A_BYTES, &tmF, &full[s], kb * TC_BK, row0);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int it = blockIdx.x; it < items; it += gridDim.x) {
-        for (int pt = 0; pt < p.npt; ++pt) {
-          mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-          tc_fence_after();
-          const uint32_t d_tmem = tmem_base + (uint32_t)acc * TC_MAX_BN;
-          for (int kb = 0; kb < p.kblocks; ++kb) {
-            mbar_wait(&full[stage], phase);
-            tc_fence_after();
-            const uint32_t sa = smem_u32(smem + stage * TC_STAGE_BYTES);
-            const uint32_t sb = sa + TC_A_BYTES;
+    return;
+  }
+  const int wg = warp >> 2, tid = threadIdx.x & 127;
+  // row owners: threads 0-63 of each warpgroup, one channel each
+  const int row = wg * 64 + tid;
+  const int n = m_blk * TC_BM + row;
+  const bool owner = tid < 64;
+  const bool nvalid = owner && n < p.n_out;
+  const float bias_n = nvalid ? p.bias[n] : 0.f;
+  constexpr float L2E = 1.4426950408889634f;
+  int crop = p.cpt > 0 ? g * p.cpt : g;
+  int pix = 0, x = 0, y = 0;
+  float m = -INFINITY, mL = -INFINITY, s_ = 0.f, sx = 0.f, sy = 0.f;
+  int i = 0;
+  for (int pt = 0; pt < p.npt; ++pt) {
+    float acc[128];
 #pragma unroll
-            for (int k = 0; k < TC_BK / 16; ++k)
-              umma_bf16(d_tmem, umma_smem_desc(sa + k * 32), umma_smem_desc(sb + k * 32), p.idesc, (kb | k) != 0);
-            umma_commit(&empty[stage]);
-            if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
-          }
-          umma_commit(&tmem_full[acc]);
-          if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-        }
+    for (int k = 0; k < 128; ++k) acc[k] = 0.f;
+    int prev = -1;
+    for (int kb = 0; kb < p.kblocks; ++kb, ++i) {
+      const int s = i % TCH_STAGES;
+      mbar_wait(&full[s], (i / TCH_STAGES) & 1);
+      const uint32_t a = smem_u32(smem + s * TCH_STAGE_BYTES) + wg * 64 * 128;
+      const uint32_t b = smem_u32(smem + s * TCH_STAGE_BYTES + TC_A_BYTES);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < TC_BK / 16; ++k) wgmma_bf16<256>(acc, gmma_desc<128>(a + 32 * k), gmma_desc<128>(b + 32 * k), (uint32_t)(kb | k));
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[prev]);
+      }
+      prev = s;
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs<128>(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[prev]);
+    // fragment -> staging (this warpgroup's 64 rows)
+    {
+      const int fr = wg * 64 + (warp & 3) * 16 + (lane >> 2), fc = 2 * (lane & 3);
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        *reinterpret_cast<float2*>((uint8_t*)stg + tch_stg(fr, fc + 8 * j)) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>((uint8_t*)stg + tch_stg(fr + 8, fc + 8 * j)) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
       }
     }
-  } else if (warp >= 4) {
-    const int q = warp - 4;
-    const int row = q * 32 + lane;
-    constexpr float L2E = 1.4426950408889634f;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int it = blockIdx.x; it < items; it += gridDim.x) {
-      const int g = it / p.m_tiles, m_blk = it - g * p.m_tiles;
-      const int n = m_blk * TC_BM + row;
-      const bool nvalid = n < p.n_out;
-      const float bias_n = nvalid ? p.bias[n] : 0.f;
-      int crop = p.cpt > 0 ? g * p.cpt : g;
-      int pix = 0, x = 0, y = 0;
-      float m = -INFINITY, mL = -INFINITY, s = 0.f, sx = 0.f, sy = 0.f;
-      for (int pt = 0; pt < p.npt; ++pt) {
-        mbar_wait(&tmem_full[acc], acc_phase);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)acc * TC_MAX_BN;
-        for (int c0 = 0; c0 < p.bnp; c0 += 16) {
-          float v[16];
-          tmem_ld16(taddr + c0, v);
-          if (pix + 16 <= p.P) {
-            // whole chunk inside one crop: one rescale, then 16 exps
-            float vm = v[0];
+    wg_sync(wg);
+    if (owner) {
+      for (int c0 = 0; c0 < p.bnp; c0 += 16) {
+        float v[16];
 #pragma unroll
-            for (int i = 1; i < 16; ++i) vm = fmaxf(vm, v[i]);
-            vm += bias_n;
-            if (vm > m) {
-              const float mL_new = vm * L2E;
-              float f = ex2_fast(mL - mL_new);  // same rounded offsets as the elements use
-              s *= f; sx *= f; sy *= f;
-              m = vm;
+        for (int q = 0; q < 4; ++q) {
+          const float4 f = *reinterpret_cast<const float4*>((const uint8_t*)stg + tch_stg(row, c0 + 4 * q));
+          v[4 * q] = f.x; v[4 * q + 1] = f.y; v[4 * q + 2] = f.z; v[4 * q + 3] = f.w;
+        }
+        if (pix + 16 <= p.P) {
+          // whole chunk inside one crop: one rescale, then 16 exps
+          float vm = v[0];
+#pragma unroll
+          for (int q = 1; q < 16; ++q) vm = fmaxf(vm, v[q]);
+          vm += bias_n;
+          if (vm > m) {
+            const float mL_new = vm * L2E;
+            float f = ex2_fast(mL - mL_new);  // same rounded offsets as the elements use
+            s_ *= f; sx *= f; sy *= f;
+            m = vm;
+            mL = mL_new;
+          }
+          const float cL = fmaf(bias_n, L2E, -mL);
+#pragma unroll
+          for (int q = 0; q < 16; ++q) {
+            float e = ex2_fast(fmaf(v[q], L2E, cL));
+            s_ += e;
+            sx = fmaf(e, (float)x, sx);
+            sy = fmaf(e, (float)y, sy);
+            if (++x == p.W) { x = 0; ++y; }
+          }
+          pix += 16;
+          if (pix == p.P) {
+            if (nvalid && crop < p.B) p.states[(size_t)crop * p.n_out + n] = make_float4(m, s_, sx, sy);
+            ++crop; pix = 0; x = 0; y = 0;
+            m = -INFINITY; mL = -INFINITY; s_ = 0.f; sx = 0.f; sy = 0.f;
+          }
+        } else {
+          // chunk straddles a crop boundary (P % 16 != 0): element-wise
+#pragma unroll
+          for (int q = 0; q < 16; ++q) {
+            float vv = v[q] + bias_n;
+            if (vv > m) {
+              const float mL_new = vv * L2E;
+              float f = ex2_fast(mL - mL_new);
+              s_ *= f; sx *= f; sy *= f;
+              m = vv;
               mL = mL_new;
             }
-            const float cL = fmaf(bias_n, L2E, -mL);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              float e = ex2_fast(fmaf(v[i], L2E, cL));
-              s += e;
-              sx = fmaf(e, (float)x, sx);
-              sy = fmaf(e, (float)y, sy);
-              if (++x == p.W) { x = 0; ++y; }
-            }
-            pix += 16;
-            if (pix == p.P) {
-              if (nvalid && crop < p.B) p.states[(size_t)crop * p.n_out + n] = make_float4(m, s, sx, sy);
+            float e = ex2_fast(fmaf(vv, L2E, -mL));
+            s_ += e;
+            sx = fmaf(e, (float)x, sx);
+            sy = fmaf(e, (float)y, sy);
+            if (++x == p.W) { x = 0; ++y; }
+            if (++pix == p.P) {
+              if (nvalid && crop < p.B) p.states[(size_t)crop * p.n_out + n] = make_float4(m, s_, sx, sy);
               ++crop; pix = 0; x = 0; y = 0;
-              m = -INFINITY; mL = -INFINITY; s = 0.f; sx = 0.f; sy = 0.f;
-            }
-          } else {
-            // chunk straddles a crop boundary (P % 16 != 0): element-wise
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              float vv = v[i] + bias_n;
-              if (vv > m) {
-                const float mL_new = vv * L2E;
-                float f = ex2_fast(mL - mL_new);
-                s *= f; sx *= f; sy *= f;
-                m = vv;
-                mL = mL_new;
-              }
-              float e = ex2_fast(fmaf(vv, L2E, -mL));
-              s += e;
-              sx = fmaf(e, (float)x, sx);
-              sy = fmaf(e, (float)y, sy);
-              if (++x == p.W) { x = 0; ++y; }
-              if (++pix == p.P) {
-                if (nvalid && crop < p.B) p.states[(size_t)crop * p.n_out + n] = make_float4(m, s, sx, sy);
-                ++crop; pix = 0; x = 0; y = 0;
-                m = -INFINITY; mL = -INFINITY; s = 0.f; sx = 0.f; sy = 0.f;
-              }
+              m = -INFINITY; mL = -INFINITY; s_ = 0.f; sx = 0.f; sy = 0.f;
             }
           }
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+    wg_sync(wg);  // the staging tile is rewritten by the next pixel tile
   }
 }
 
@@ -1839,7 +729,7 @@ inline const char* tc_prepare_head(TcWeights& w, const float* wt, const float* b
   if (cudaMalloc((void**)&w.d_bias, (size_t)n_out * 4) != cudaSuccess) return "cudaMalloc failed";
   allocs.push_back(w.d_bias);
   if (cudaMemcpy(w.d_bias, bias, (size_t)n_out * 4, cudaMemcpyHostToDevice) != cudaSuccess) return "cudaMemcpy failed";
-  if (cudaFuncSetAttribute(tc_head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES) != cudaSuccess)
+  if (cudaFuncSetAttribute(tc_head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TCH_SMEM_BYTES) != cudaSuccess)
     return "cannot raise dynamic shared memory for tc_head_kernel";
   const char* e = make_tmap_2d(&w.mapA, w.d_w, (uint64_t)n_out, (uint64_t)C, TC_BM);
   if (e) return e;
@@ -1850,7 +740,6 @@ inline const char* tc_prepare_head(TcWeights& w, const float* wt, const float* b
   return nullptr;
 }
 
-// pixels-per-MMA plan; returns false when the feature map shape is not supported by the fused kernel
 inline bool tc_head_plan(int P, int* bnp, int* cpt, int* npt) {
   if (P <= 256) {
     for (int c = 256 / P; c >= 1; --c)
@@ -1872,18 +761,16 @@ inline const char* tc_head_launch(const TcWeights& w, const void* features, int 
   q.bias = w.d_bias;
   q.B = B; q.P = H * W; q.W = W; q.n_out = w.n_real; q.C = w.Cin;
   if (!tc_head_plan(q.P, &q.bnp, &q.cpt, &q.npt)) return "unsupported feature map shape for the fused head";
-  q.n_groups = q.cpt > 0 ? (B + q.cpt - 1) / q.cpt : B;
+  const int n_groups = q.cpt > 0 ? (B + q.cpt - 1) / q.cpt : B;
   q.m_tiles = (q.n_out + TC_BM - 1) / TC_BM;
   q.kblocks = (q.C + TC_BK - 1) / TC_BK;
-  q.idesc = umma_idesc_bf16(q.bnp);
   if (w.cached_in != features || w.cached_B != B) {
     const char* e = make_tmap_2d(&w.mapB, features, (uint64_t)B * q.P, (uint64_t)q.C, (uint32_t)q.bnp);
     if (e) return e;
     w.cached_in = features;
     w.cached_B = B;
   }
-  const int items = q.n_groups * q.m_tiles;
-  launch_k(tc_head_kernel, dim3(items < 148 ? items : 148), dim3(256), TC_SMEM_BYTES, st, w.mapA, w.mapB, q);
+  launch_k(tc_head_kernel, dim3(n_groups * q.m_tiles), dim3(TC_THREADS), TCH_SMEM_BYTES, st, w.mapA, w.mapB, q);
   launch_k(head_finalize_kernel, dim3(B), dim3(128), 0, st, q.states, c2d, c3d, J, D, H, W, sc);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);

@@ -1,45 +1,42 @@
-// 3xTF32 tensor-core path (sm_100a): the PARITY mode on tcgen05.  fp32 NHWC activations and fp32 weights are staged by
-// TMA exactly as they sit in HBM; "splitter" warps rewrite every landed operand tile in shared memory as
+// 3xTF32 tensor-core path (sm_90a): the PARITY mode on wgmma.  fp32 NHWC activations and fp32 weights are staged by TMA
+// exactly as they sit in HBM; each consumer warpgroup rewrites ITS 64 rows of every landed A tile in shared memory as
 //     x_hi = tf32(x)  (round to nearest, low 13 mantissa bits zero)      x_lo = x - x_hi  (exact in fp32)
-// and the MMA warp issues, per K step of 8, three tcgen05.mma kind::tf32 products:
+// (the weights arrive split: hi and lo planes prepared on the host) and issues, per K step of 8, three wgmma kind tf32
+// products:
 //     P += A_hi * B_hi          S += A_lo * B_hi          S += A_hi * B_lo
-// into TWO kinds of TMEM accumulators.  Why two (measured, round 2): the tensor core's fp32 accumulate TRUNCATES (round
-// toward zero, as on every generation since Volta), so a long accumulation chain carries a bias that grows linearly with
-// K - one accumulator for everything gave 2e-6 ... 2e-5 per conv (K = 288 ... 3840) and 1.6e-3 on EfficientNetV2-S features,
-// above the 1e-3 bar.  The cure is the one of Ootomo & Yokota (2022, "Recovering single precision accuracy from Tensor
-// Cores"): accumulate OUTSIDE the tensor core.  The main term runs in short chains of `chain` k-blocks (default 2 = 8 MMAs)
-// into a partial buffer P that the accumulator warps drain (tcgen05.ld) and add to fp32 REGISTER accumulators with
-// round-to-nearest FADDs; the correction terms are 2^-11 of the main term, so their truncation error is negligible and
-// they keep one TMEM accumulator S for the whole tile.
+// into TWO kinds of register accumulators.  Why two: the tensor core's fp32 accumulate TRUNCATES (round toward zero), so a
+// long accumulation chain carries a bias that grows linearly with K - one accumulator for everything lands above the 1e-3
+// bar on EfficientNetV2-S features.  The cure is the one of Ootomo & Yokota (2022, "Recovering single precision accuracy
+// from Tensor Cores"): accumulate OUTSIDE the tensor core.  The main term runs in short chains of T32_CHAIN k-blocks into a
+// partial accumulator P that is added to the fp32 accumulator with round-to-nearest FADDs; the correction terms are 2^-11 of
+// the main term, so their truncation error is negligible and they keep one accumulator S for the whole tile.
 //
 //   mode 0   1x1 stride-1 conv == GEMM  D[pixels, Cout] = A[pixels, Cin] * W[Cout, Cin]^T (2D TMA); the squeeze-excitation
-//            scale of an MBConv projection (backbones/efficientnet.py:110-173, `scale * x`) is applied by the splitter
-//            warps to the A tile before the split: the separate scaling pass of the bf16 mode does not exist here
+//            scale of an MBConv projection (backbones/efficientnet.py:110-173, `scale * x`) is applied to the A tile before
+//            the split: the separate scaling pass of the bf16 mode does not exist here
 //   mode 1   RxS conv (stride 1/2, dilation) as implicit GEMM: per tap the A tile is a shifted [8 x 16] pixel box of the
 //            NHWC input fetched by a 4D TMA; out-of-bounds = the reference's explicit zero padding (efficientnet.py:1127-1161)
-//   epilogue registers (+ S from TMEM) -> + folded-BN bias, exact activation (expf SiLU), + residual, fp32 NHWC store.
+//   epilogue registers -> + folded-BN bias, exact activation, + residual, fp32 NHWC store.
 //
-// Tiles: M = 128 pixels x N <= 128 channels (register accumulators: 64 fp32 per accumulator thread).  TMEM columns:
-// [0,128) S0, [128,256) S1 (double-buffered across tiles), [256,384) P0, [384,512) P1 (ring of partial buffers).
-// Shared-memory stage: [A raw/hi 128 rows | B raw/hi b_rows rows | A lo | B lo], rows of 128 bytes (32 fp32, 128B
-// swizzle).  The lo tiles mirror the raw tiles byte for byte, so the splitters never need to undo the TMA swizzle.
+// Tiles: M = 128 pixels x N = BN <= 64 channels.  Shared-memory stage: [A raw/hi 128 rows | B hi BN rows | A lo | B lo],
+// rows of 128 bytes (32 fp32, 128B swizzle).  The lo tile mirrors the raw tile byte for byte, so the split never needs to
+// undo the TMA swizzle.
 #pragma once
 #include "tc_gemm.cuh"
 
 namespace mtb {
 
-constexpr int T32_SPLIT_WARPS = 5;
-constexpr int T32_THREADS = (11 + T32_SPLIT_WARPS) * 32;  // warps 0-7 accumulate + epilogue, 8 A producer, 9 B producer, 10 MMA, 11.. splitters
-constexpr int T32_MAX_STAGES = 8;
-constexpr int T32_RING_BYTES = 192 * 1024;                  // three 64 KB stages at N = 128
-constexpr int T32_STG_OFF = T32_RING_BYTES;                 // epilogue staging: 8 warps x [32 rows x 128 B] (register row-domain ->
-constexpr int T32_STG_BYTES = 8 * 4096;                     // coalesced column-domain stores)
-constexpr int T32_BAR_OFF = T32_STG_OFF + T32_STG_BYTES;
-constexpr int T32_SMEM_BYTES = T32_BAR_OFF + 512 + 1024 /*align slack*/;
-constexpr int T32_BN = 128;                                 // accumulator columns per buffer
-constexpr int T32_ACC_SHARE = 64;                           // A-tile rows [0, 64) of every stage are split by the 8 accumulator warps,
-                                                            // rows [64, 128) by the dedicated splitter warps
-constexpr uint32_t T32_S_COL = 0, T32_P_COL = 2 * T32_BN;   // TMEM column bases of the S and P buffer pairs
+constexpr int T32_RB = 128;       // bytes per operand row (32 fp32)
+constexpr int T32_BK = T32_RB / 4;
+constexpr int T32_CHAIN = 2;      // k-blocks (8 MMAs of the main term) per partial chain
+
+template <int BN>
+struct T32Ring {
+  static constexpr int lo_off = (TC_BM + BN) * T32_RB;
+  static constexpr int stage_bytes = 2 * lo_off;
+  static constexpr int stages = 4;
+  static constexpr int smem_bytes = stages * stage_bytes + 1024 /*align slack*/ + 256 /*barriers*/;
+};
 
 struct Tc32Params {
   const float* res;
@@ -51,33 +48,10 @@ struct Tc32Params {
   int Hin, Win;
   int M;                 // mode 0: rows
   int Cout, Cin;
-  int bn, b_rows;        // N-tile stride (<= 128); rows of the weight TMA box
-  int n_tiles, m_tiles, kchunks, taps;
-  int nstages, stage_stride, lo_off;
-  int chain;             // k-blocks per partial accumulation chain (drained into registers after each)
-  int epi_col;           // epilogue in the column domain (Cout > 64); row-domain stores are cheaper when a pixel's channels fit 256 B
-  int debug;             // MTB_T32_DEBUG bits (perf experiments only, results are wrong): 1 splitters skip their work, 2 accumulator
-                         // warps skip the TMEM drains, 4 skip the epilogue math + stores
-  int Hout, Wout, tiles_w, tiles_h, pad_t, pad_l, R, S, stride, dil;
+  int kchunks, taps;
+  int Hout, Wout, tiles_w, tiles_h, pad_t, pad_l, S, stride, dil;
 };
 
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// kind::tf32 instruction descriptor: D fp32, A/B tf32, both K-major, M = 128, N = n
-__host__ __device__ inline uint32_t umma_idesc_tf32(int n) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
-// variant for the MTB_T32_DEBUG=8 experiment: the raw tile stays in place (the tensor core is assumed to ignore the low 13
-// mantissa bits = truncation) and only lo = x - trunc(x) is written
-__device__ __forceinline__ float split_tf32_lo_trunc(float x) { return x - __uint_as_float(__float_as_uint(x) & 0xffffe000u); }
 // hi = x rounded to tf32 (nearest, ties away: integer add on the bit pattern, carries into the exponent correctly),
 // lo = x - hi (exact: hi and x agree in sign/exponent up to one binade, the difference has <= 13 significant bits)
 __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
@@ -93,18 +67,6 @@ __device__ __forceinline__ float4 lds128(uint32_t addr) {
 }
 __device__ __forceinline__ void sts128(uint32_t addr, const float4& v) {
   asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
-}
-// acc[0..63] += 64 TMEM columns of this warp's 32 lanes (columns >= n_ld were not written by the MMA and are skipped)
-__device__ __forceinline__ void t32_drain(uint32_t taddr, int n_ld, float* acc) {
-#pragma unroll
-  for (int g = 0; g < 4; ++g) {
-    if (g * 16 < n_ld) {  // warp-uniform
-      float v[16];
-      tmem_ld16(taddr + g * 16, v);
-#pragma unroll
-      for (int i = 0; i < 16; ++i) acc[g * 16 + i] += v[i];
-    }
-  }
 }
 // SiLU for the parity epilogue: x * 1/(1 + 2^(-x log2 e)) on the MUFU units (ex2.approx, rcp.approx: ~2 ulp each); the
 // CUDA-core fp32 mode's expf + IEEE division costs ~3x the instructions and sat on the accumulator warps' critical path
@@ -169,395 +131,119 @@ __device__ __forceinline__ void t32_split_a(uint32_t base, uint32_t lo_off, int 
   }
 }
 
-// The accumulator warps' side job: while they wait (for a partial chain, for the correction accumulator) or between the
-// store groups of their epilogue they split THEIR share of whatever operand stage has landed next - the dedicated splitter
-// warps alone made the split the bottleneck (MTB_T32_DEBUG=1: 31 vs 48-54 ms of kernel time per 128 crops without / with it).
-// Stages are helped strictly in order, each exactly once; nothing here blocks.
-template <int RB>
-struct T32Helper {
-  uint32_t stage = 0, phase = 0;
-  int tile, kb = 0;
-  __device__ __forceinline__ bool help(const Tc32Params& p, uint32_t smem_base, uint32_t full0, uint64_t* split, int total_tiles, int num_kb,
-                                       int tid256, int lane) {
-    if (tile >= total_tiles) return false;
-    uint32_t ok = lane == 0 ? (uint32_t)mbar_try_wait_a(full0 + stage * 8, phase) : 0u;
-    ok = __shfl_sync(0xffffffffu, ok, 0);
-    if (!ok) return false;
-    constexpr int CPR = RB / 16, BK = RB / 4;
-    const int kc = kb % p.kchunks;
-    const uint32_t base = smem_base + stage * (uint32_t)p.stage_stride;
-    if (!(p.debug & 1))
-      t32_split_a<RB>(base, (uint32_t)p.lo_off, tid256, T32_ACC_SHARE * CPR, 256, p.a_scale, (tile / p.n_tiles) * TC_BM, p.M, p.a_scale_P,
-                      p.Cin, kc * BK);
-    fence_proxy_async();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&split[stage]);
-    if (++kb == num_kb) { kb = 0; tile += gridDim.x; }
-    if (++stage == (uint32_t)p.nstages) { stage = 0; phase ^= 1; }
-    return true;
-  }
-};
-
-template <int ACT, int RES, int RB>  // RB: bytes per operand row of a stage: 128 (32 fp32, 128B swizzle) or 64 (16 fp32, 64B swizzle)
-__global__ void __launch_bounds__(T32_THREADS, 1)
+template <int ACT, int RES, int BN>
+__global__ void __launch_bounds__(TC_THREADS, 1)
 tc32_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const Tc32Params p) {
-  constexpr int BK = RB / 4;       // fp32 elements per row
-  constexpr int KSTEPS = RB / 32;  // K steps (K = 8 tf32 = 32 bytes) per stage
+  using Ring = T32Ring<BN>;
+  constexpr int STAGES = Ring::stages;
+  constexpr int NR = BN / 2;  // accumulator registers per thread
   extern __shared__ uint8_t tc_smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)tc_smem_raw + 1023) & ~(uintptr_t)1023);
-  uint64_t* bars = (uint64_t*)(smem + T32_BAR_OFF);
-  uint64_t* full = bars;                          // [8]  TMA landed (A + B producers)
-  uint64_t* split = bars + T32_MAX_STAGES;        // [8]  hi/lo tiles written (splitter warps)
-  uint64_t* empty = bars + 2 * T32_MAX_STAGES;    // [8]  tcgen05.commit
-  uint64_t* p_full = bars + 3 * T32_MAX_STAGES;   // [2]  partial chain complete
-  uint64_t* p_empty = p_full + 2;                 // [2]  drained by the 8 accumulator warps
-  uint64_t* s_full = p_empty + 2;                 // [2]  correction-term accumulator of a tile complete
-  uint64_t* s_empty = s_full + 2;                 // [2]
-  uint32_t* tmem_slot = (uint32_t*)(s_empty + 2);
+  uint64_t* full = (uint64_t*)(smem + STAGES * Ring::stage_bytes);
+  uint64_t* empty = full + STAGES;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 8 && lane == 0) {
+  if (threadIdx.x == TC_CONSUMER_WARPS * 32) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-  }
-  if (warp == 9 && lane == 0) {
-    for (int i = 0; i < T32_MAX_STAGES; ++i) {
-      mbar_init(&full[i], 2);
-      mbar_init(&split[i], T32_SPLIT_WARPS + TCV_EPI_WARPS);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&p_full[i], 1);
-      mbar_init(&p_empty[i], TCV_EPI_WARPS);
-      mbar_init(&s_full[i], 1);
-      mbar_init(&s_empty[i], TCV_EPI_WARPS);
+    for (int i = 0; i < STAGES; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], TC_CONSUMER_WARPS);
     }
     fence_barrier_init();
   }
-  if (warp == 10) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);
   pdl_trigger();
   pdl_wait();
 
-  const int total_tiles = p.m_tiles * p.n_tiles;
-  const uint32_t a_bytes = (uint32_t)TC_BM * RB;
-  const uint32_t b_bytes = (uint32_t)p.b_rows * RB;
-  const int nstages = p.nstages;
-  const int num_kb = pin(p.taps * p.kchunks);
-  const int chain = pin(p.chain);
-  const uint32_t stage_stride = pin((uint32_t)p.stage_stride);
-  const uint32_t smem_base = smem_u32(smem);
-  const uint32_t full0 = smem_u32(full), empty0 = smem_u32(empty), split0 = smem_u32(split);
-
-  if (warp == 8) {
-    // ===== A-operand TMA producer =====
-    uint32_t stage = 0, phase = 0, sa = smem_base;
-    const int kchunks = pin(p.kchunks);
-    TileWalk tw_(blockIdx.x, gridDim.x, p.n_tiles);
-    if (p.mode == 0) {
-      for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, tw_.next()) {
-        const int row0 = tw_.m_blk * TC_BM;
-#pragma unroll 1
-        for (int kc = 0; kc < kchunks; ++kc) {
-          mbar_wait_a(empty0 + stage * 8, phase ^ 1);
-          if (elect_one()) {
-            mbar_expect_tx_a(full0 + stage * 8, a_bytes);
-            tma_load_2d_a(sa, &tmA, full0 + stage * 8, kc * BK, row0);
-          }
-          __syncwarp();
-          sa += stage_stride;
-          if (++stage == (uint32_t)nstages) { stage = 0; phase ^= 1; sa = smem_base; }
-        }
+  const int m_blk = blockIdx.x, n_blk = blockIdx.y;
+  const int num_kb = p.taps * p.kchunks;
+  if (warp == TC_CONSUMER_WARPS) {
+    // ===== TMA producer: A raw, weights hi plane (rows [0, Cout)) and lo plane (rows [Cout, 2 Cout)) =====
+    if (lane == 0) {
+      for (int kb = 0; kb < num_kb; ++kb) {
+        const int s = kb % STAGES;
+        mbar_wait(&empty[s], ((kb / STAGES) & 1) ^ 1);
+        uint8_t* sa = smem + s * Ring::stage_bytes;
+        const int tap = kb / p.kchunks, kc = kb - tap * p.kchunks;
+        mbar_expect_tx(&full[s], (TC_BM + 2 * BN) * T32_RB);
+        tma_load_a_tile<T32_BK>(sa, &tmA, &full[s], p, m_blk, kb);
+        tma_load_2d(sa + TC_BM * T32_RB, &tmB, &full[s], tap * p.Cin + kc * T32_BK, n_blk * BN);
+        tma_load_2d(sa + Ring::lo_off + TC_BM * T32_RB, &tmB, &full[s], tap * p.Cin + kc * T32_BK, p.Cout + n_blk * BN);
       }
+    }
+    return;
+  }
+  // ===== consumers: warpgroup wg splits and multiplies tile rows [64 wg, +64) =====
+  const int wg = warp >> 2, tid = threadIdx.x & 127;
+  constexpr int CPR = T32_RB / 16;  // 16-byte chunks per row
+  float acc[NR], pacc[NR], sacc[NR];
+#pragma unroll
+  for (int i = 0; i < NR; ++i) acc[i] = pacc[i] = sacc[i] = 0.f;
+  int pos = 0;
+  for (int kb = 0; kb < num_kb; ++kb) {
+    const int s = kb % STAGES;
+    mbar_wait(&full[s], (kb / STAGES) & 1);
+    const uint32_t base = smem_u32(smem + s * Ring::stage_bytes);
+    const int kc = kb % p.kchunks;
+    t32_split_a<T32_RB>(base, (uint32_t)Ring::lo_off, wg * 64 * CPR + tid, (wg + 1) * 64 * CPR, 128, p.a_scale, m_blk * TC_BM, p.M,
+                        p.a_scale_P, p.Cin, kc * T32_BK);
+    fence_proxy_async();  // generic-proxy writes -> visible to the tensor core (async proxy)
+    wg_sync(wg);
+    const uint32_t a_hi = base + wg * 64 * T32_RB, b_hi = base + TC_BM * T32_RB;
+    const uint32_t a_lo = a_hi + Ring::lo_off, b_lo = b_hi + Ring::lo_off;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < T32_RB / 32; ++k) {
+      wgmma_tf32<BN>(sacc, gmma_desc<T32_RB>(a_lo + 32 * k), gmma_desc<T32_RB>(b_hi + 32 * k), (uint32_t)(kb | k));
+      wgmma_tf32<BN>(sacc, gmma_desc<T32_RB>(a_hi + 32 * k), gmma_desc<T32_RB>(b_lo + 32 * k), 1u);
+      wgmma_tf32<BN>(pacc, gmma_desc<T32_RB>(a_hi + 32 * k), gmma_desc<T32_RB>(b_hi + 32 * k), (uint32_t)(pos | k));
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs<NR>(pacc);
+    wgmma_fence_regs<NR>(sacc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[s]);
+    if (pos == T32_CHAIN - 1 || kb == num_kb - 1) {
+#pragma unroll
+      for (int i = 0; i < NR; ++i) acc[i] += pacc[i];
+      pos = 0;
     } else {
-      const int S = pin(p.S), dil = pin(p.dil);
-      for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, tw_.next()) {
-        const int m_blk = tw_.m_blk;
-        const int tw = m_blk % p.tiles_w;
-        const int th = (m_blk / p.tiles_w) % p.tiles_h;
-        const int b = m_blk / (p.tiles_w * p.tiles_h);
-        const int ih0 = th * TC_TILE_H * p.stride - p.pad_t;
-        const int iw0 = tw * TC_TILE_W * p.stride - p.pad_l;
-        int r = 0, s_ = 0, kc = 0;
-#pragma unroll 1
-        for (int i = 0; i < num_kb; ++i) {
-          mbar_wait_a(empty0 + stage * 8, phase ^ 1);
-          if (elect_one()) {
-            mbar_expect_tx_a(full0 + stage * 8, a_bytes);
-            tma_load_4d_a(sa, &tmA, full0 + stage * 8, kc * BK, iw0 + s_ * dil, ih0 + r * dil, b);
-          }
-          __syncwarp();
-          if (++kc == kchunks) {
-            kc = 0;
-            if (++s_ == S) { s_ = 0; ++r; }
-          }
-          sa += stage_stride;
-          if (++stage == (uint32_t)nstages) { stage = 0; phase ^= 1; sa = smem_base; }
-        }
-      }
-    }
-  } else if (warp == 9) {
-    // ===== B-operand (weights) TMA producer =====
-    uint32_t stage = 0, phase = 0, sb = smem_base + a_bytes;
-    const int taps = pin(p.taps), kchunks = pin(p.kchunks), Cin = pin(p.Cin), bn = pin(p.bn), Cout_rows = pin(p.Cout);
-    const uint32_t lo_off_u = pin((uint32_t)p.lo_off);
-    TileWalk tw_(blockIdx.x, gridDim.x, p.n_tiles);
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, tw_.next()) {
-      const int nrow = tw_.n_blk * bn;
-      int tap = 0, kc = 0;
-#pragma unroll 1
-      for (int i = 0; i < num_kb; ++i) {
-        mbar_wait_a(empty0 + stage * 8, phase ^ 1);
-        if (elect_one()) {
-          // weights are split on the host: plane 0 = hi (tf32-rounded), plane 1 = lo, stacked as [2 * Cout][K]
-          mbar_expect_tx_a(full0 + stage * 8, 2 * b_bytes);
-          tma_load_2d_a(sb, &tmB, full0 + stage * 8, tap * Cin + kc * BK, nrow);
-          tma_load_2d_a(sb + lo_off_u, &tmB, full0 + stage * 8, tap * Cin + kc * BK, Cout_rows + nrow);
-        }
-        __syncwarp();
-        if (++kc == kchunks) { kc = 0; if (++tap == taps) tap = 0; }
-        sb += stage_stride;
-        if (++stage == (uint32_t)nstages) { stage = 0; phase ^= 1; sb = smem_base + a_bytes; }
-      }
-    }
-  } else if (warp == 10) {
-    // ===== MMA issuer: main term into the partial buffer P (short chain), correction terms into S (whole tile) =====
-    constexpr uint32_t hi_sw = (uint32_t)((8 * RB) >> 4) | (1u << 14) | ((RB == 128 ? 2u : 4u) << 29);
-    const uint32_t stride16 = stage_stride >> 4;
-    const uint32_t base16 = smem_base >> 4;
-    const uint32_t b_off16 = a_bytes >> 4;
-    const uint32_t lo16 = (uint32_t)p.lo_off >> 4;
-    const uint32_t p_full0 = smem_u32(p_full), p_empty0 = smem_u32(p_empty), s_full0 = smem_u32(s_full), s_empty0 = smem_u32(s_empty);
-    const int bn = pin(p.bn), Cout = pin(p.Cout);
-    TileWalk tw_(blockIdx.x, gridDim.x, p.n_tiles);
-    uint32_t stage = 0, phase = 0, a16 = base16;
-    uint32_t sbuf = 0, s_phase = 0, pbuf = 0, p_phase = 0;
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, tw_.next()) {
-      const int n_valid = min(bn, Cout - tw_.n_blk * bn);
-      const uint32_t idesc = umma_idesc_tf32((n_valid + 15) & ~15);
-      mbar_wait_a(s_empty0 + sbuf * 8, s_phase ^ 1);
-      const uint32_t s_tmem = tmem_base + T32_S_COL + sbuf * T32_BN;
-      int pos = 0;
-#pragma unroll 1
-      for (int kb = 0; kb < num_kb; ++kb) {
-        if (pos == 0) mbar_wait_a(p_empty0 + pbuf * 8, p_phase ^ 1);
-        mbar_wait_a(split0 + stage * 8, phase);
-        tc_fence_after();
-        const bool last_in_chain = pos == chain - 1 || kb == num_kb - 1;
-        if (elect_one()) {
-          const uint32_t p_tmem = tmem_base + T32_P_COL + pbuf * T32_BN;
-#pragma unroll
-          for (int k = 0; k < KSTEPS; ++k) {
-            const uint64_t a_hi = make_desc(a16 + 2 * k, hi_sw), b_hi = make_desc(a16 + b_off16 + 2 * k, hi_sw);
-            const uint64_t a_lo = make_desc(a16 + lo16 + 2 * k, hi_sw), b_lo = make_desc(a16 + lo16 + b_off16 + 2 * k, hi_sw);
-            umma_tf32(s_tmem, a_lo, b_hi, idesc, (uint32_t)(kb | k));
-            umma_tf32(s_tmem, a_hi, b_lo, idesc, 1u);
-            umma_tf32(p_tmem, a_hi, b_hi, idesc, (uint32_t)(pos | k));
-          }
-          umma_commit_a(empty0 + stage * 8);
-          if (last_in_chain) umma_commit_a(p_full0 + pbuf * 8);
-          if (kb == num_kb - 1) umma_commit_a(s_full0 + sbuf * 8);
-        }
-        __syncwarp();
-        if (last_in_chain) {
-          pos = 0;
-          if (++pbuf == 2) { pbuf = 0; p_phase ^= 1; }
-        } else {
-          ++pos;
-        }
-        a16 += stride16;
-        if (++stage == (uint32_t)nstages) { stage = 0; phase ^= 1; a16 = base16; }
-      }
-      if (++sbuf == 2) { sbuf = 0; s_phase ^= 1; }
-    }
-  } else if (warp >= 11) {
-    // ===== dedicated splitters: rows [T32_ACC_SHARE, 128) of the A tile of every stage (the accumulator warps take the rest;
-    // the weight tile arrives already split into hi / lo planes) =====
-    constexpr int NT = T32_SPLIT_WARPS * 32;
-    constexpr int CPR = RB / 16;
-    const int st = (warp - 11) * 32 + lane;
-    const uint32_t lo_off = (uint32_t)p.lo_off;
-    const int kchunks = pin(p.kchunks);
-    uint32_t stage = 0, phase = 0;
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-      const int m_row0 = (t / p.n_tiles) * TC_BM;
-      int kc = 0;
-#pragma unroll 1
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait_a(full0 + stage * 8, phase);
-        const uint32_t base = smem_base + stage * stage_stride;
-        if (!(p.debug & 1))
-          t32_split_a<RB>(base, lo_off, T32_ACC_SHARE * CPR + st, TC_BM * CPR, NT, p.a_scale, m_row0, p.M, p.a_scale_P, p.Cin, kc * BK);
-        fence_proxy_async();  // generic-proxy writes -> visible to the tensor core (async proxy)
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&split[stage]);
-        if (++kc == kchunks) kc = 0;
-        if (++stage == (uint32_t)nstages) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else {
-    // ===== accumulator + epilogue warps 0-7: warp w owns tile rows [32(w&3), +32) and columns [64(w>>2), +64) of the tile.
-    // Every partial chain is drained from TMEM and added to the register accumulators with round-to-nearest FADDs. =====
-    const int q = warp & 3, half = warp >> 2;
-    const int row = q * 32 + lane;
-    uint32_t sbuf = 0, s_phase = 0, pbuf = 0, p_phase = 0;
-    const float* __restrict__ res = p.res;
-    float* __restrict__ out = p.out;
-    const uint32_t lane_base = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(half * 64);
-    const int n_chains = (num_kb + chain - 1) / chain;
-    T32Helper<RB> helper;
-    helper.tile = blockIdx.x;
-    const int tid256 = warp * 32 + lane;
-    auto help = [&]() { return helper.help(p, smem_base, full0, split, total_tiles, num_kb, tid256, lane); };
-    auto wait_helping = [&](uint32_t bar, uint32_t parity) {  // warp-uniform poll (lane 0 decides); split work fills the wait
-      for (;;) {
-        uint32_t ok = lane == 0 ? (uint32_t)mbar_try_wait_a(bar, parity) : 0u;
-        ok = __shfl_sync(0xffffffffu, ok, 0);
-        if (ok) break;
-        help();
-      }
-    };
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-      const int m_blk = t / p.n_tiles, n_blk = t - m_blk * p.n_tiles;
-      const int n0 = n_blk * p.bn + half * 64;                       // first channel of this warp's columns
-      const int n_tile = min(p.bn, p.Cout - n_blk * p.bn);           // valid channels of the tile
-      const int ncols = max(0, min(64, n_tile - half * 64));         // valid columns of this warp (multiple of 4)
-      const int n_ld = min(64, max(0, ((n_tile + 15) & ~15) - half * 64));  // columns of this warp the MMA wrote
-      // tile geometry (the rows of this warp are resolved in the epilogue's column domain)
-      int tw = 0, th = 0, tb = 0;
-      if (p.mode != 0) {
-        tw = m_blk % p.tiles_w;
-        th = (m_blk / p.tiles_w) % p.tiles_h;
-        tb = m_blk / (p.tiles_w * p.tiles_h);
-      }
-      float acc[64];
-#pragma unroll
-      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-      for (int c = 0; c < n_chains; ++c) {
-        wait_helping(smem_u32(&p_full[pbuf]), p_phase);
-        tc_fence_after();
-        const uint32_t taddr = lane_base + T32_P_COL + pbuf * T32_BN;
-        if (!(p.debug & 2)) t32_drain(taddr, n_ld, acc);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&p_empty[pbuf]);
-        if (++pbuf == 2) { pbuf = 0; p_phase ^= 1; }
-      }
-      wait_helping(smem_u32(&s_full[sbuf]), s_phase);
-      tc_fence_after();
-      {
-        const uint32_t taddr = lane_base + T32_S_COL + sbuf * T32_BN;
-        t32_drain(taddr, n_ld, acc);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&s_empty[sbuf]);
-      if (++sbuf == 2) { sbuf = 0; s_phase ^= 1; }
-      // epilogue.  The accumulators sit in the ROW domain (thread = one pixel, 64 channels): storing from there writes 32
-      // scattered 16-byte pieces per instruction (measured: the epilogue cost 7-10 ms of 45 per 128 crops).  Each warp therefore
-      // transposes 32 columns at a time through its private swizzled staging tile and runs bias + activation + residual + store
-      // in the COLUMN domain: 4 rows x 128 contiguous bytes per load / store instruction.
-      if (!p.epi_col) {
-        // narrow outputs (Cout <= 64: a pixel's channels are <= 256 contiguous bytes and neighbouring pixels are adjacent):
-        // store straight from the row domain - the transposition costs more than the scattered 16-byte pieces here
-        // (measured: 32->32 3x3 @128^2 3.34 vs 4.14 ms, 256->64 1x1 @64^2 1.78 vs 2.63 ms per 128 crops)
-        bool valid;
-        size_t off;
-        if (p.mode == 0) {
-          const int m = m_blk * TC_BM + row;
-          valid = m < p.M;
-          off = (size_t)m * p.Cout;
-        } else {
-          const int oh = th * TC_TILE_H + (row >> 4), ow = tw * TC_TILE_W + (row & 15);
-          valid = oh < p.Hout && ow < p.Wout;
-          off = ((size_t)(tb * p.Hout + oh) * p.Wout + ow) * p.Cout;
-        }
-        const bool do_store = valid && !(p.debug & 4);
-#pragma unroll
-        for (int g = 0; g < 16; ++g) {
-          if (do_store && g * 4 < ncols) {
-            const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.bias + n0 + g * 4));
-            float o[4] = {acc[g * 4 + 0] + b4.x, acc[g * 4 + 1] + b4.y, acc[g * 4 + 2] + b4.z, acc[g * 4 + 3] + b4.w};
-            if constexpr (RES != 0) {
-              const float4 rv = *reinterpret_cast<const float4*>(res + off + n0 + g * 4);
-              if constexpr (RES == 2) {
-                o[0] = t32_act<ACT>(o[0] + rv.x); o[1] = t32_act<ACT>(o[1] + rv.y);
-                o[2] = t32_act<ACT>(o[2] + rv.z); o[3] = t32_act<ACT>(o[3] + rv.w);
-              } else {
-                o[0] = t32_act<ACT>(o[0]) + rv.x; o[1] = t32_act<ACT>(o[1]) + rv.y;
-                o[2] = t32_act<ACT>(o[2]) + rv.z; o[3] = t32_act<ACT>(o[3]) + rv.w;
-              }
-            } else {
-#pragma unroll
-              for (int i = 0; i < 4; ++i) o[i] = t32_act<ACT>(o[i]);
-            }
-            *reinterpret_cast<float4*>(out + off + n0 + g * 4) = make_float4(o[0], o[1], o[2], o[3]);
-          }
-          if ((g & 3) == 3) help();  // all lanes, whatever `do_store`: keeps the operand pipeline fed during the epilogue
-        }
-      } else {
-        const uint32_t stg = smem_base + T32_STG_OFF + warp * 4096;
-        const int cj = lane & 7, rsub = lane >> 3;
-#pragma unroll
-        for (int rd = 0; rd < 2; ++rd) {
-          if (rd * 32 < ncols) {  // warp-uniform
-#pragma unroll
-            for (int g = 0; g < 8; ++g)
-              sts128(stg + lane * 128 + ((g ^ (lane & 7)) << 4),
-                     make_float4(acc[rd * 32 + g * 4 + 0], acc[rd * 32 + g * 4 + 1], acc[rd * 32 + g * 4 + 2], acc[rd * 32 + g * 4 + 3]));
-            __syncwarp();
-            const int col = rd * 32 + cj * 4;
-            const bool cok = col < ncols && !(p.debug & 4);
-            const float4 b4 = cok ? __ldg(reinterpret_cast<const float4*>(p.bias + n0 + col)) : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-            for (int it = 0; it < 8; ++it) {
-              const int rr = rsub + it * 4;  // row of this warp's 32
-              const float4 v = lds128(stg + rr * 128 + ((cj ^ (rr & 7)) << 4));
-              bool rvalid;
-              size_t off;
-              if (p.mode == 0) {
-                const int m = m_blk * TC_BM + q * 32 + rr;
-                rvalid = m < p.M;
-                off = (size_t)m * p.Cout;
-              } else {
-                const int trow = q * 32 + rr;
-                const int oh = th * TC_TILE_H + (trow >> 4), ow = tw * TC_TILE_W + (trow & 15);
-                rvalid = oh < p.Hout && ow < p.Wout;
-                off = ((size_t)(tb * p.Hout + oh) * p.Wout + ow) * p.Cout;
-              }
-              if (rvalid && cok) {
-                float o[4] = {v.x + b4.x, v.y + b4.y, v.z + b4.z, v.w + b4.w};
-                if constexpr (RES != 0) {
-                  const float4 rv = *reinterpret_cast<const float4*>(res + off + n0 + col);
-                  if constexpr (RES == 2) {
-                    o[0] = t32_act<ACT>(o[0] + rv.x); o[1] = t32_act<ACT>(o[1] + rv.y);
-                    o[2] = t32_act<ACT>(o[2] + rv.z); o[3] = t32_act<ACT>(o[3] + rv.w);
-                  } else {
-                    o[0] = t32_act<ACT>(o[0]) + rv.x; o[1] = t32_act<ACT>(o[1]) + rv.y;
-                    o[2] = t32_act<ACT>(o[2]) + rv.z; o[3] = t32_act<ACT>(o[3]) + rv.w;
-                  }
-                } else {
-#pragma unroll
-                  for (int i = 0; i < 4; ++i) o[i] = t32_act<ACT>(o[i]);
-                }
-                *reinterpret_cast<float4*>(out + off + n0 + col) = make_float4(o[0], o[1], o[2], o[3]);
-              }
-            }
-            __syncwarp();  // the staging tile is rewritten by the next round
-          }
-          help();  // all lanes: keeps the operand pipeline fed during the epilogue
-        }
-      }
+      ++pos;
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 10) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+#pragma unroll
+  for (int i = 0; i < NR; ++i) acc[i] += sacc[i];
+
+  // ===== epilogue: thread rows r0 = 64 wg + 16 (warp & 3) + lane / 4 and r0 + 8, columns 8 j + 2 (lane % 4) + {0, 1} =====
+  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int c0 = n_blk * BN + 2 * (lane & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    size_t off;
+    if (!tile_row_offset(p.mode, m_blk, r0 + 8 * h, p.M, p.Cout, p.tiles_w, p.tiles_h, p.Hout, p.Wout, off)) continue;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int c = c0 + 8 * j;
+      if (c >= p.Cout) break;  // Cout % 4 == 0: column c + 1 is valid with c
+      const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + c));
+      float o0 = acc[4 * j + 2 * h] + bv.x, o1 = acc[4 * j + 2 * h + 1] + bv.y;
+      if constexpr (RES != 0) {
+        const float2 rv = *reinterpret_cast<const float2*>(p.res + off + c);
+        if constexpr (RES == 2) {
+          o0 = t32_act<ACT>(o0 + rv.x);
+          o1 = t32_act<ACT>(o1 + rv.y);
+        } else {
+          o0 = t32_act<ACT>(o0) + rv.x;
+          o1 = t32_act<ACT>(o1) + rv.y;
+        }
+      } else {
+        o0 = t32_act<ACT>(o0);
+        o1 = t32_act<ACT>(o1);
+      }
+      *reinterpret_cast<float2*>(p.out + off + c) = make_float2(o0, o1);
+    }
   }
 }
 
@@ -639,48 +325,27 @@ inline bool tc32_eligible(bool is_conv, bool depthwise, bool small_io, int k, in
   return (stride == 1 || stride == 2) && (k == 1 || k == 3);
 }
 
-// N-tile stride (<= 128: the register accumulators hold 64 columns per accumulator thread).  Per k-block: three products x
-// 4 K steps x N/2 cycles of MMA against ~350 cycles of fixed issue cost and the L2 -> SM operand fill at ~40 B/clk.
-inline int tc32_pick_bn(int cout, int m_tiles, int num_kb) {
-  int best = 64;
-  double best_cost = 1e30;
-  for (int bn = 128; bn >= 32; bn -= 32) {
-    const int nt = (cout + bn - 1) / bn;
-    const long tiles = (long)m_tiles * nt;
-    const long waves = (tiles + 147) / 148;
-    const int last = cout - (nt - 1) * bn;
-    const double avg_n = ((double)(nt - 1) * bn + ((last + 15) & ~15)) / nt;
-    const double mma_kb = 3.0 * 4.0 * (avg_n < 32 ? 32 : avg_n) / 2.0;
-    const double fill_kb = (128.0 + (nt == 1 ? ((cout + 15) & ~15) : bn)) * 128.0 / 40.0;
-    double per_kb = mma_kb;
-    if (fill_kb > per_kb) per_kb = fill_kb;
-    if (per_kb < 350.0) per_kb = 350.0;
-    const double cost = (double)waves * (num_kb * per_kb + 800.0);
-    if (cost < best_cost - 1e-9) { best_cost = cost; best = bn; }
-  }
-  return best;
-}
-
-template <int ACT, int RES, int RB>
-inline const char* tc32_launch_k(int grid, const CUtensorMap& a, const CUtensorMap& b, const Tc32Params& q, cudaStream_t st) {
+template <int ACT, int RES, int BN>
+inline const char* tc32_launch_k(dim3 grid, const CUtensorMap& a, const CUtensorMap& b, const Tc32Params& q, cudaStream_t st) {
   static bool attr_set = false;
   if (!attr_set) {
-    if (cudaFuncSetAttribute(tc32_conv_kernel<ACT, RES, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, T32_SMEM_BYTES) != cudaSuccess)
+    if (cudaFuncSetAttribute(tc32_conv_kernel<ACT, RES, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, T32Ring<BN>::smem_bytes) !=
+        cudaSuccess)
       return "cannot raise dynamic shared memory for tc32_conv_kernel";
     attr_set = true;
   }
-  launch_k(tc32_conv_kernel<ACT, RES, RB>, dim3(grid), dim3(T32_THREADS), T32_SMEM_BYTES, st, a, b, q);
+  launch_k(tc32_conv_kernel<ACT, RES, BN>, grid, dim3(TC_THREADS), T32Ring<BN>::smem_bytes, st, a, b, q);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 template <int ACT>
-inline const char* tc32_dispatch_res(int res_mode, int rb, int grid, const CUtensorMap& a, const CUtensorMap& b, const Tc32Params& q,
+inline const char* tc32_dispatch_res(int res_mode, int bn, dim3 grid, const CUtensorMap& a, const CUtensorMap& b, const Tc32Params& q,
                                      cudaStream_t st) {
-  if (rb == 128) {
+  if (bn == 32) {
     switch (res_mode) {
-      case 0: return tc32_launch_k<ACT, 0, 128>(grid, a, b, q, st);
-      case 1: return tc32_launch_k<ACT, 1, 128>(grid, a, b, q, st);
-      default: return tc32_launch_k<ACT, 2, 128>(grid, a, b, q, st);
+      case 0: return tc32_launch_k<ACT, 0, 32>(grid, a, b, q, st);
+      case 1: return tc32_launch_k<ACT, 1, 32>(grid, a, b, q, st);
+      default: return tc32_launch_k<ACT, 2, 32>(grid, a, b, q, st);
     }
   }
   switch (res_mode) {
@@ -699,54 +364,25 @@ inline const char* tc32_conv_launch(const Tc32Weights& w, const ConvParams& p, b
   q.a_scale_P = p.Hin * p.Win;
   q.Hin = p.Hin; q.Win = p.Win;
   q.Cout = p.Cout; q.Cin = p.Cin;
-  q.taps = w.taps; q.R = p.R; q.S = w.S; q.stride = p.stride; q.dil = p.dil;
+  q.taps = w.taps; q.S = w.S; q.stride = p.stride; q.dil = p.dil;
   q.Hout = p.Hout; q.Wout = p.Wout; q.pad_t = p.pad_t; q.pad_l = p.pad_l;
   q.tiles_w = (p.Wout + TC_TILE_W - 1) / TC_TILE_W;
   q.tiles_h = (p.Hout + TC_TILE_H - 1) / TC_TILE_H;
   q.M = p.B * p.Hout * p.Wout;
-  q.m_tiles = q.mode == 0 ? (q.M + TC_BM - 1) / TC_BM : p.B * q.tiles_w * q.tiles_h;
-  // 128-byte rows (K = 32 per stage, three 64 KB stages at N = 128).  64-byte rows (six 32 KB stages) were measured SLOWER
-  // (64.6 vs 55.8 ms of tc32 time per 128 crops): the per-k-block costs of the issuing warps double; MTB_T32_RB=64 selects them
-  int rb = 128;
-  int bn = tc32_pick_bn(p.Cout, q.m_tiles, q.taps * ((p.Cin + 31) / 32));
-  {
-    static int rb_env = -1;
-    if (rb_env < 0) { const char* e = getenv("MTB_T32_RB"); rb_env = e ? atoi(e) : 0; }
-    if (rb_env == 64 || rb_env == 128) rb = rb_env;
-  }
-  q.chain = rb == 128 ? 2 : 4;  // 8 main-term MMAs per partial chain either way
-  {
-    static int bn_env = -1, chain_env = -1;  // A/B switches: MTB_T32_BN = 32..128, MTB_T32_CHAIN = k-blocks per partial chain
-    if (bn_env < 0) { const char* e = getenv("MTB_T32_BN"); bn_env = e ? atoi(e) : 0; }
-    if (chain_env < 0) { const char* e = getenv("MTB_T32_CHAIN"); chain_env = e ? atoi(e) : 0; }
-    if (bn_env >= 32 && bn_env <= 128 && bn_env % 32 == 0) bn = bn_env;
-    if (chain_env >= 1) q.chain = chain_env;
-    static int dbg_env = -1;
-    if (dbg_env < 0) { const char* e = getenv("MTB_T32_DEBUG"); dbg_env = e ? atoi(e) : 0; }
-    q.debug = dbg_env;
-  }
-  q.epi_col = p.Cout > 64 ? 1 : 0;
-  const int bk = rb / 4;
-  q.bn = bn;
-  q.n_tiles = (p.Cout + bn - 1) / bn;
-  q.kchunks = (p.Cin + bk - 1) / bk;
-  q.b_rows = q.n_tiles == 1 ? (p.Cout + 15) / 16 * 16 : bn;
-  q.lo_off = (TC_BM + q.b_rows) * rb;
-  q.stage_stride = (2 * q.lo_off + 1023) / 1024 * 1024;
-  q.nstages = T32_RING_BYTES / q.stage_stride;
-  if (q.nstages > T32_MAX_STAGES) q.nstages = T32_MAX_STAGES;
-  if (q.nstages < 2) return "operand ring too small for this tile";
+  q.kchunks = (p.Cin + T32_BK - 1) / T32_BK;
+  const int m_tiles = q.mode == 0 ? (q.M + TC_BM - 1) / TC_BM : p.B * q.tiles_w * q.tiles_h;
+  const int bn = p.Cout <= 32 ? 32 : 64;
   const Tc32Weights::MapSet* ms = nullptr;
   for (const Tc32Weights::MapSet& c : w.map_sets)
-    if (c.in == p.in && c.B == p.B && c.bn == bn && c.rb == rb) { ms = &c; break; }
+    if (c.in == p.in && c.B == p.B && c.bn == bn) { ms = &c; break; }
   if (!ms) {
     Tc32Weights::MapSet c;
-    const char* e = q.mode == 0 ? make_tmap_2d_f32(&c.a, p.in, (uint64_t)q.M, (uint64_t)p.Cin, TC_BM, (uint32_t)bk)
-                                : make_tmap_nhwc_f32(&c.a, p.in, p.B, p.Hin, p.Win, p.Cin, (uint32_t)p.stride, (uint32_t)bk);
+    const char* e = q.mode == 0 ? make_tmap_2d_f32(&c.a, p.in, (uint64_t)q.M, (uint64_t)p.Cin, TC_BM, (uint32_t)T32_BK)
+                                : make_tmap_nhwc_f32(&c.a, p.in, p.B, p.Hin, p.Win, p.Cin, (uint32_t)p.stride, (uint32_t)T32_BK);
     if (e) return e;
-    e = make_tmap_2d_f32(&c.b, w.d_w, (uint64_t)2 * p.Cout, (uint64_t)w.taps * p.Cin, (uint32_t)q.b_rows, (uint32_t)bk);
+    e = make_tmap_2d_f32(&c.b, w.d_w, (uint64_t)2 * p.Cout, (uint64_t)w.taps * p.Cin, (uint32_t)bn, (uint32_t)T32_BK);
     if (e) return e;
-    c.in = p.in; c.B = p.B; c.bn = bn; c.rb = rb;
+    c.in = p.in; c.B = p.B; c.bn = bn;
     if (w.map_sets.size() < 16) {
       w.map_sets.push_back(c);
       ms = &w.map_sets.back();
@@ -756,14 +392,13 @@ inline const char* tc32_conv_launch(const Tc32Weights& w, const ConvParams& p, b
       ++w.map_rr;
     }
   }
-  const int total = q.m_tiles * q.n_tiles;
-  const int grid = total < 148 ? total : 148;
+  const dim3 grid(m_tiles, (p.Cout + bn - 1) / bn);
   const int res_mode = p.res ? (res_first ? 2 : 1) : 0;
   switch (p.act) {
-    case ACT_NONE: return tc32_dispatch_res<ACT_NONE>(res_mode, rb, grid, ms->a, ms->b, q, st);
-    case ACT_SILU: return tc32_dispatch_res<ACT_SILU>(res_mode, rb, grid, ms->a, ms->b, q, st);
-    case ACT_RELU: return tc32_dispatch_res<ACT_RELU>(res_mode, rb, grid, ms->a, ms->b, q, st);
-    case ACT_HSWISH: return tc32_dispatch_res<ACT_HSWISH>(res_mode, rb, grid, ms->a, ms->b, q, st);
+    case ACT_NONE: return tc32_dispatch_res<ACT_NONE>(res_mode, bn, grid, ms->a, ms->b, q, st);
+    case ACT_SILU: return tc32_dispatch_res<ACT_SILU>(res_mode, bn, grid, ms->a, ms->b, q, st);
+    case ACT_RELU: return tc32_dispatch_res<ACT_RELU>(res_mode, bn, grid, ms->a, ms->b, q, st);
+    case ACT_HSWISH: return tc32_dispatch_res<ACT_HSWISH>(res_mode, bn, grid, ms->a, ms->b, q, st);
     default: return "unsupported activation in the 3xTF32 epilogue";
   }
 }

@@ -1,7 +1,7 @@
 """Config c5 (head-only isolation, BASELINE.md section 2): roofline sweep of
   (1) the standalone soft-argmax over materialised logits (reference layout [B,D,J,H,W], ptu.soft_argmax) - HBM-bound,
       algorithmic bytes = B*J*D*H*W*sizeof(elt) + 12*B*J  (SURVEY.md 8d);
-  (2) the fused head (1x1-conv GEMM on tcgen05 + soft-argmax epilogue, logits never stored), readings 5a (8x8, D=8) and
+  (2) the fused head (1x1-conv GEMM on wgmma + soft-argmax epilogue, logits never stored), readings 5a (8x8, D=8) and
       5b (32x32, D=32) of the inconsistent BASELINE.json c5 line: FLOPs 2*B*H*W*C*N, bytes 2*B*H*W*C + 2*C*N + 20*B*J.
 Prints one JSON line per point; peaks from MEASURED_PEAKS.json."""
 import json

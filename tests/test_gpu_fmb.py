@@ -2,7 +2,7 @@
 launch, the expanded tile never leaves the SM) against
 
 * plain ``torch.nn.functional.conv2d`` arithmetic (oracle/port_ops.py restates the two reference layers,
-  /root/reference/metrabs_pytorch/backbones/efficientnet.py:176-234) on the same bf16-rounded input and weights, with the
+  metrabs_pytorch/backbones/efficientnet.py:176-234 of the reference) on the same bf16-rounded input and weights, with the
   expanded activation rounded to bf16 between the two convs (what the unfused path stores): bar = one bf16 ulp of the
   output plus the propagated ulp flips of the intermediate (1e-2 on ||.||inf/||ref||inf; a descriptor / layout / pipeline
   bug gives O(1) errors);
@@ -35,7 +35,7 @@ def _block_reference(sd, spec, names, i, x):
 
 @pytest.mark.parametrize('name,side,batch', [('efficientnetv2-s', 256, 3), ('efficientnetv2-l', 256, 2), ('efficientnetv2-l', 384, 1),
                                              ('efficientnetv2-m', 192, 2), ('efficientnetv2-tiny', 64, 5),  # tiny: Cin 16, one 64-wide chunk
-                                             ('efficientnetv2-l', 32, 3)])  # 8x8 / 4x4 maps, 3 crops: an ODD number of tiles (a CTA pair runs a dummy tile)
+                                             ('efficientnetv2-l', 32, 3)])  # 8x8 / 4x4 maps, 3 crops: tiles mostly outside the map
 def test_fused_block_vs_conv2d_and_unfused(H, name, side, batch):
     pcfg = port.PathConfig(proc_side=side)
     spec = port.effnet_spec(name)
@@ -68,7 +68,7 @@ def test_fused_block_vs_conv2d_and_unfused(H, name, side, batch):
 
 @pytest.mark.parametrize('batch', [64, 256])
 def test_fused_block_at_bench_batch(H, batch):
-    """multi-wave persistent tile walk (8192 / 2048 tiles over 148 CTAs) on the two EfficientNetV2-L@256 block shapes"""
+    """many waves of tiles (8192 / 2048 tiles) on the two EfficientNetV2-L@256 block shapes"""
     name, side = 'efficientnetv2-l', 256
     pcfg = port.PathConfig(proc_side=side)
     spec = port.effnet_spec(name)

@@ -166,7 +166,7 @@ def test_tiny_model_golden(H, golden_dir, fname):
     ('efficientnetv2-l', 384, 24, 1, 'effnetv2l_s384_j24.npz'),
 ])
 def test_full_models_parity_modes(H, golden_dir, name, side, j, batch, fname, precision):
-    """The two modes that must meet BASELINE.json's 1e-3 bar - 'fp32' (CUDA-core FMA) and 'tf32x3' (tcgen05 kind::tf32, three
+    """The two modes that must meet BASELINE.json's 1e-3 bar - 'fp32' (CUDA-core FMA) and 'tf32x3' (wgmma tf32, three
     split products, fp32 accumulate) - against the oracle port on the same weights/inputs AND against the goldens the
     unmodified reference produced (/root/reference/metrabs_pytorch/models/metrabs.py:47-64), the latter at the golden's
     own batch size (reconstruct_ref_fullpersp normalises with batch-global RMS, ptu3d.py:71-74)."""

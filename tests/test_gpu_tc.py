@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 tensor-core kernels (MTB_PRECISION_BF16_TC) against the CUDA-core kernels on IDENTICAL bf16 inputs
+"""GPU: the wgmma tensor-core kernels (MTB_PRECISION_BF16_TC) against the CUDA-core kernels on IDENTICAL bf16 inputs
 and bf16-rounded weights (MTB_PRECISION_BF16_SIMT; those kernels are themselves pinned to the oracle in fp32 mode by
 test_gpu_parity.py), and the fused head against the oracle on bf16-rounded operands.
 

@@ -1,7 +1,7 @@
 """GPU: every conv/GEMM kernel shape of the tensor-core modes against plain ``torch.nn.functional.conv2d`` arithmetic on
 identical operands (oracle/port_ops.py restates one reference layer at a time) - NOT against other kernels of this repo.
 
-* 'tf32x3' (tc32_conv_kernel: tcgen05 kind::tf32, hi/lo split operands, three products, fp32 accumulate): vs fp64 conv2d,
+* 'tf32x3' (tc32_conv_kernel: wgmma tf32, hi/lo split operands, three products, fp32 accumulate): vs fp64 conv2d,
   bar 5e-5 on ||.||inf/||ref||inf (fp32-chain quality; the 1e-3 joint bar of BASELINE.json is checked end to end in
   test_gpu_parity.py::test_full_models_parity_modes).
 * 'bf16' (tc_conv_kernel: kind::f16 bf16 operands, fp32 accumulate, bf16 store): vs conv2d on the same bf16-rounded input

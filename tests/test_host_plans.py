@@ -34,56 +34,3 @@ def test_depthwise_tma_plan_covers_the_map_within_the_shared_memory_budget():
     assert _plan(12, 12)[1:3] == (12, 1)
     g, bh, nrb, _ = _plan(24, 24)
     assert g == 1 and nrb * bh >= 24 and nrb <= 8
-
-
-def _fmb_plan(cin, cexp, cout, pair):
-    v = [C.c_int() for _ in range(4)]
-    assert _lib.lib().mtb_debug_fmb_plan(cin, cexp, cout, int(pair), *[C.byref(x) for x in v]) == 0
-    return tuple(x.value for x in v)  # nstages, npatch, stage_bytes, smem_bytes
-
-
-@pytest.mark.skipif(not os.path.exists(_lib.LIB_PATH), reason='libmetrabs_b200.so not built')
-def test_fused_mbconv_plan_fits_shared_memory_for_every_effnetv2_block_shape():
-    """fmb_kernel (csrc/tc_fmb.cuh): ring + patches + GEMM-2 operand + slabs + bias + barriers within the 227 KB opt-in limit,
-    at least 3 ring stages and 2 patch slots, for the stride-1 FusedMBConv shapes of EfficientNetV2-S/M/L/XL (Cin = Cout, x4)."""
-    for cin in (16, 32, 48, 64, 80, 96):
-        for pair in (False, True):
-            ns, npatch, sb, smem = _fmb_plan(cin, 4 * cin, cin, pair)
-            if pair and (4 * cin) % 128 != 0:
-                assert ns == 0          # pairs need whole 128-channel chunks (equal half blocks = one TMA box)
-                continue
-            assert ns >= 3 and npatch >= 2 and smem <= 227 * 1024, (cin, pair, ns, npatch, smem)
-            assert sb >= 128 * cin * 2 // (2 if pair else 1) and sb % 1024 == 0
-            if pair:
-                assert ns >= _fmb_plan(cin, 4 * cin, cin, False)[0]   # half-size stages: never a shallower ring
-    assert _fmb_plan(24, 96, 24, False) == (0, 0, 0, 0)   # Cin not a multiple of 16: stays two tc_conv_kernel launches
-    assert _fmb_plan(64, 256, 96, False) == (0, 0, 0, 0)  # not identity-shaped
-
-
-@pytest.mark.skipif(not os.path.exists(_lib.LIB_PATH), reason='libmetrabs_b200.so not built')
-@pytest.mark.parametrize('cin,cexp,pair', [(16, 64, False), (48, 192, False), (64, 256, True), (96, 384, True), (80, 320, False)])
-def test_fused_mbconv_weight_images_follow_the_documented_layout(cin, cexp, pair):
-    """The stage images the weight producers copy verbatim into shared memory: canonical K-major core-matrix layout
-    [K/8 planes][rows][8]; per (chunk, tap) for the 3x3 weights, per chunk for the 1x1 weights; pair: [half] outermost."""
-    import numpy as np
-    rng = np.random.default_rng(cin)
-    cout = cin
-    w1 = rng.integers(0, 65536, size=(cexp, 9 * cin), dtype=np.uint16)
-    w2 = rng.integers(0, 65536, size=(cout, cexp), dtype=np.uint16)
-    i1, i2 = np.zeros(w1.size, np.uint16), np.zeros(w2.size, np.uint16)
-    rc = _lib.lib().mtb_debug_fmb_pack(w1.ctypes.data, w2.ctypes.data, cin, cexp, cout, int(pair), i1.ctypes.data, i2.ctypes.data)
-    assert rc == 0
-    halves = 2 if pair else 1
-    e1, e2 = [], []
-    for c0 in range(0, cexp, 128):
-        wc = min(128, cexp - c0)
-        for tap in range(9):
-            blk = w1[c0:c0 + wc, tap * cin:(tap + 1) * cin]                       # [rows][cin]
-            for hf in range(halves):
-                rows = blk[hf * wc // halves:(hf + 1) * wc // halves]
-                e1.append(rows.reshape(-1, cin // 8, 8).transpose(1, 0, 2).ravel())  # [plane][row][8]
-        blk2 = w2[:, c0:c0 + wc]                                                   # [cout][wc]
-        for hf in range(halves):
-            rows = blk2[hf * cout // halves:(hf + 1) * cout // halves]
-            e2.append(rows.reshape(-1, wc // 8, 8).transpose(1, 0, 2).ravel())
-    assert np.array_equal(i1, np.concatenate(e1)) and np.array_equal(i2, np.concatenate(e2))
