@@ -5,42 +5,11 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include <cstdlib>
 #include <utility>
 
 namespace mtb {
 
 enum Act : int { ACT_NONE = 0, ACT_SILU = 1, ACT_RELU = 2, ACT_HSWISH = 3, ACT_SIGMOID = 4, ACT_HSIGMOID = 5 };
-
-// Programmatic dependent launch (PDL): every kernel is launched with cudaLaunchAttributeProgrammaticStreamSerialization.
-// pdl_trigger() lets the NEXT kernel in the stream start launching once all CTAs of this grid have started (its prologue
-// then overlaps this grid's tail); pdl_wait() blocks until the PREVIOUS grid has completed and its writes are visible - it
-// must precede the first global-memory access of a kernel.
-__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-
-// Dependents that launch early hold SM slots while spinning in griddepcontrol.wait, so PDL is OFF unless MTB_ENABLE_PDL=1;
-// without the launch attribute griddepcontrol.* are no-ops.
-inline bool pdl_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("MTB_ENABLE_PDL");
-    v = (e && e[0] == '1') ? 1 : 0;
-  }
-  return v == 1;
-}
-
-// Scoped PDL for a chain of tiny dependent launches (the squeeze-excitation FCs): their launch latency, not their work, is
-// what the step pays for, and a small early-launched grid does not hold the SM slots a tensor-core CTA would.
-inline int& pdl_force_depth() {
-  static thread_local int d = 0;
-  return d;
-}
-struct PdlScope {
-  bool on;
-  explicit PdlScope(bool enable) : on(enable) { if (on) ++pdl_force_depth(); }
-  ~PdlScope() { if (on) --pdl_force_depth(); }
-};
 
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
@@ -49,11 +18,6 @@ inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, siz
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = (pdl_enabled() || pdl_force_depth() > 0) ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kernel, KArgs(std::forward<Args>(args))...);
 }
 

@@ -29,8 +29,6 @@ struct ConvParams {
 template <int BM, int BN, int TM, int TN, typename TIn, typename TOut>
 __global__ void __launch_bounds__((BM / TM) * (BN / TN))
 conv_igemm_kernel(ConvParams p) {
-  pdl_trigger();
-  pdl_wait();
   constexpr int BK = 16;
   constexpr int NT = (BM / TM) * (BN / TN);
   constexpr int A_LD = (BM * BK / 4) / NT;  // float4 loads of A per thread per tile
@@ -224,8 +222,6 @@ conv_igemm_kernel(ConvParams p) {
 // ----------------------------------------------------------------------------------------------------------
 template <typename T>
 __global__ void __launch_bounds__(256) dwconv_kernel(ConvParams p) {
-  pdl_trigger();
-  pdl_wait();
   const T* __restrict__ in = reinterpret_cast<const T*>(p.in);
   T* __restrict__ out = reinterpret_cast<T*>(p.out);
   const int C4 = p.Cout >> 2;
@@ -289,8 +285,6 @@ __device__ __forceinline__ float fast_act(float x) {  // compile-time activation
 
 template <int STRIDE, int ACT, int OW = 4>
 __global__ void __launch_bounds__(256, OW == 2 ? 3 : 2) dwconv3x3_pool_bf16_kernel(ConvParams p, float* __restrict__ pooled) {
-  pdl_trigger();
-  pdl_wait();
   // OW outputs per thread along W
   constexpr int NCOL = (OW - 1) * STRIDE + 3;    // input columns feeding them
   const __nv_bfloat16* __restrict__ in = reinterpret_cast<const __nv_bfloat16*>(p.in);
@@ -402,8 +396,6 @@ __global__ void __launch_bounds__(256, OW == 2 ? 3 : 2) dwconv3x3_pool_bf16_kern
 // per thread, exact activation (expf SiLU), the same block-reduced partial pooling slices.  grid (ceil(C/128), slices, B).
 template <int STRIDE, int ACT, int OW = 4>
 __global__ void __launch_bounds__(256, 3) dwconv3x3_pool_f32_kernel(ConvParams p, float* __restrict__ pooled) {
-  pdl_trigger();
-  pdl_wait();
   constexpr int NCOL = (OW - 1) * STRIDE + 3;
   const float* __restrict__ in = reinterpret_cast<const float*>(p.in);
   float* __restrict__ out = reinterpret_cast<float*>(p.out);
@@ -496,8 +488,6 @@ struct StemParams {
 
 template <typename TOut>
 __global__ void __launch_bounds__(256) stem_conv_kernel(StemParams p) {
-  pdl_trigger();
-  pdl_wait();
   extern __shared__ float sw[];  // weights [R*S*Cin][Cout] + bias [Cout]
   const int K = p.R * p.S * p.Cin;
   for (int i = threadIdx.x; i < K * p.Cout; i += blockDim.x) sw[i] = p.w[i];
@@ -545,8 +535,6 @@ __global__ void __launch_bounds__(256) stem_conv_kernel(StemParams p) {
 // ----------------------------------------------------------------------------------------------------------
 template <typename TOut, int CPT>
 __global__ void __launch_bounds__(128) stem_conv_wide_kernel(StemParams p) {
-  pdl_trigger();
-  pdl_wait();
   extern __shared__ float sw[];  // weights [R*S*Cin][Cout] + bias [Cout]
   const int K = p.R * p.S * p.Cin;
   for (int i = threadIdx.x; i < K * p.Cout; i += blockDim.x) sw[i] = p.w[i];
@@ -605,8 +593,6 @@ __global__ void __launch_bounds__(128) stem_conv_wide_kernel(StemParams p) {
 // ----------------------------------------------------------------------------------------------------------
 template <typename TOut, int CPT>
 __global__ void __launch_bounds__(128) stem3x3s2_kernel(StemParams p) {
-  pdl_trigger();
-  pdl_wait();
   extern __shared__ float sw[];  // weights [27][Cout] + bias [Cout]
   for (int i = threadIdx.x; i < 27 * CPT; i += blockDim.x) sw[i] = p.w[i];
   float* sb = sw + 27 * CPT;
@@ -668,8 +654,6 @@ __global__ void __launch_bounds__(128) stem3x3s2_kernel(StemParams p) {
 // ----------------------------------------------------------------------------------------------------------
 template <typename T>
 __global__ void __launch_bounds__(256) pool_mean_kernel(const T* __restrict__ in, float* __restrict__ out, int P, int C) {
-  pdl_trigger();
-  pdl_wait();
   __shared__ float4 red[8][32];
   const int c = (blockIdx.x * 32 + threadIdx.x) * 4;
   const int b = blockIdx.y;
@@ -699,8 +683,6 @@ __global__ void __launch_bounds__(256) pool_mean_kernel(const T* __restrict__ in
 // activation: hidden[b][c] = act(sum_z partial[z][b][c] + bias[c]).  Fixed summation order (deterministic).
 __global__ void __launch_bounds__(256) se_reduce_kernel(const float* __restrict__ partial, const float* __restrict__ bias,
                                                         float* __restrict__ out, int n, int C, int ksplit, int act) {
-  pdl_trigger();
-  pdl_wait();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   float v = 0.f;
@@ -712,8 +694,6 @@ __global__ void __launch_bounds__(256) se_reduce_kernel(const float* __restrict_
 // pools VALID, so an out-of-bounds tap contributes the value 0 to the max.
 template <typename T>
 __global__ void __launch_bounds__(256) maxpool_kernel(ConvParams p) {
-  pdl_trigger();
-  pdl_wait();
   const T* __restrict__ in = reinterpret_cast<const T*>(p.in);
   T* __restrict__ out = reinterpret_cast<T*>(p.out);
   const int C4 = p.Cout >> 2;

@@ -109,8 +109,6 @@ template <typename T, int VEC, bool POW2>
 __global__ void __launch_bounds__(256) softargmax_bdjhw_kernel(const T* __restrict__ logits, float* __restrict__ out,
                                                                int J, int D, int H, int W, int two_d, int hw_shift,
                                                                int w_shift) {
-  pdl_trigger();
-  pdl_wait();
   constexpr int UNROLL = 4;
   const int row = blockIdx.x;  // b*J + j
   const int b = row / J, j = row - b * J;
@@ -242,8 +240,6 @@ template <typename T>
 __global__ void __launch_bounds__(512) softargmax_bhwn_kernel(const T* __restrict__ logits, float* __restrict__ out2d,
                                                               float* __restrict__ out3d, int J, int D, int H, int W,
                                                               int ld, DecodeScale sc) {
-  pdl_trigger();
-  pdl_wait();
   extern __shared__ float sm[];  // [N][4] per-channel (m, s, sx, sy) + [PY][128][4] merge scratch
   const int N = J * (1 + D);
   const int P = H * W;
@@ -351,8 +347,6 @@ __device__ __forceinline__ void inv3x3(const float* k, float* inv) {
 }
 
 __global__ void __launch_bounds__(128) recon_pass1_kernel(ReconParams p) {
-  pdl_trigger();
-  pdl_wait();
   const int b = blockIdx.x;
   __shared__ float kinv[9];
   __shared__ double red[4][2];
@@ -388,8 +382,6 @@ __global__ void __launch_bounds__(128) recon_pass1_kernel(ReconParams p) {
 }
 
 __global__ void __launch_bounds__(128) recon_pass2_kernel(ReconParams p) {
-  pdl_trigger();
-  pdl_wait();
   const int b = blockIdx.x;
   __shared__ double red[4][9 + 3];
   __shared__ double tot[2];

@@ -22,7 +22,7 @@ constexpr int DWT_MAX_STAGE = 52 * 1024;
 constexpr int DWT_MAX_G = 8;
 
 struct DwTmaParams {
-  void* out;           // bf16 or fp32 NHWC
+  void* out;           // bf16 NHWC
   const float* w;      // [9][C] fp32 (BN folded)
   const float* bias;   // [C]
   float* pooled;       // [n_rb][B][C] partial means (nullptr: no squeeze-excitation behind this op)
@@ -33,7 +33,6 @@ struct DwTmaParams {
   int strips_w, bands, nstrips;  // per item: column strips, row runs per crop, G * bands * strips_w
   int stage_bytes;
   float inv_hw;
-  int rev;             // walk the items last-to-first (see dw_tma_launch)
 };
 
 struct DwTmaPlan {
@@ -69,17 +68,17 @@ inline DwTmaPlan dw_tma_plan(int H, int W) {
   return best;
 }
 
-// rank-4 NHWC tensor [B][H][W][C] (bf16: es = 2, fp32: es = 4); box = 128 bytes of channels (64 bf16 / 32 fp32) x (W+2) x
-// (BH+2) x G, no swizzle (quarter-warps read whole 128-byte pixel rows: conflict-free as is)
+// rank-4 bf16 NHWC tensor [B][H][W][C]; box = 64 channels (128 bytes) x (W+2) x (BH+2) x G, no swizzle (quarter-warps read
+// whole 128-byte pixel rows: conflict-free as is)
 inline const char* make_tmap_dw(CUtensorMap* m, const void* ptr, uint64_t B, uint64_t H, uint64_t W, uint64_t C, uint32_t pw,
-                                uint32_t ph, uint32_t g, uint32_t es = 2) {
+                                uint32_t ph, uint32_t g) {
   tmap_encode_fn enc = get_tmap_encode();
   if (!enc) return "cuTensorMapEncodeTiled unavailable";
   cuuint64_t dims[4] = {C, W, H, B};
-  cuuint64_t strides[3] = {C * es, W * C * es, H * W * C * es};
-  cuuint32_t box[4] = {128 / es, pw, ph, g};
+  cuuint64_t strides[3] = {C * 2, W * C * 2, H * W * C * 2};
+  cuuint32_t box[4] = {DWT_CG, pw, ph, g};
   cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(m, es == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<void*>(ptr), dims, strides, box, estr,
+  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? nullptr : "cuTensorMapEncodeTiled(dw) failed";
@@ -100,16 +99,12 @@ __device__ __forceinline__ f32x2 f2_act(f32x2 x) {
   }
 }
 
-// T = __nv_bfloat16: 64 channels per item, 8 per thread (4 fp32 pairs), tanh.approx SiLU (the throughput mode);
-// T = float (the 3xTF32 parity mode): 32 channels per item, 4 per thread (2 pairs), EXACT activation, fp32 in and out.
-// Either way a pixel is 128 bytes of shared memory, so the tiling plan, the strips and the stages are the same.
-template <int ACT, typename T = __nv_bfloat16>
+// 64 channels per item, 8 per thread (4 fp32 pairs), tanh.approx SiLU
+template <int ACT>
 __global__ void __launch_bounds__(DWT_THREADS, 2)
 dw3x3s1_tma_kernel(const __grid_constant__ CUtensorMap tmIn, const DwTmaParams p) {
-  constexpr bool F32 = sizeof(T) == 4;
-  constexpr int NV = F32 ? 2 : 4;          // fp32 pairs per thread
+  constexpr int NV = 4;                    // fp32 pairs per thread
   constexpr int CPT = 2 * NV;              // channels per thread
-  constexpr int CG = F32 ? 32 : DWT_CG;    // channels per item
   extern __shared__ uint8_t dwt_smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)dwt_smem_raw + 127) & ~(uintptr_t)127);
   __shared__ uint64_t full[DWT_STAGES];
@@ -125,22 +120,22 @@ dw3x3s1_tma_kernel(const __grid_constant__ CUtensorMap tmIn, const DwTmaParams p
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_trigger();
-  pdl_wait();
 
   const int PW = p.W + 2, PHB = p.BH + 2;
   const uint32_t stage_tx = (uint32_t)(128 * PW * PHB * p.G);
   const int strips_per_crop = p.bands * p.strips_w;
-  constexpr int GSTEP = DWT_THREADS / CG;
-  const int own_ch = tid & (CG - 1), own_g0 = tid / CG;  // blocksum owner: channel own_ch, crops own_g0, own_g0 + GSTEP, ...
+  constexpr int GSTEP = DWT_THREADS / DWT_CG;
+  const int own_ch = tid & (DWT_CG - 1), own_g0 = tid / DWT_CG;  // blocksum owner: channel own_ch, crops own_g0, own_g0 + GSTEP, ...
 
+  // Items are walked last-to-first: the expand GEMM before this op wrote its output first-crop-to-last, so the END of the
+  // tensor is what the L2 still holds, and the BEGINNING of this op's output stays in L2 for the projection GEMM that follows.
   auto issue = [&](int it_, int stage) {
-    const int it = p.rev ? p.items - 1 - it_ : it_;
+    const int it = p.items - 1 - it_;
     const int cg = it % p.n_cg;
     const int t2 = it / p.n_cg;
     const int rb = t2 % p.n_rb, bg = t2 / p.n_rb;
     mbar_expect_tx(&full[stage], stage_tx);
-    tma_load_4d(smem + (size_t)stage * p.stage_bytes, &tmIn, &full[stage], cg * CG, -p.pad_l, rb * p.BH - p.pad_t, bg * p.G);
+    tma_load_4d(smem + (size_t)stage * p.stage_bytes, &tmIn, &full[stage], cg * DWT_CG, -p.pad_l, rb * p.BH - p.pad_t, bg * p.G);
   };
 
   if (tid == 0 && (int)blockIdx.x < p.items) issue(blockIdx.x, 0);
@@ -148,11 +143,11 @@ dw3x3s1_tma_kernel(const __grid_constant__ CUtensorMap tmIn, const DwTmaParams p
   for (int it_ = blockIdx.x; it_ < p.items; it_ += gridDim.x, ++li) {
     const int stage = li & 1;
     if (tid == 0 && it_ + (int)gridDim.x < p.items) issue(it_ + gridDim.x, stage ^ 1);
-    const int it = p.rev ? p.items - 1 - it_ : it_;
+    const int it = p.items - 1 - it_;
     const int cg = it % p.n_cg;
     const int t2 = it / p.n_cg;
     const int rb = t2 % p.n_rb, bg = t2 / p.n_rb;
-    const int c = cg * CG + j * CPT;
+    const int c = cg * DWT_CG + j * CPT;
     const bool c_ok = c < p.C;
     const int b0 = bg * p.G, row0 = rb * p.BH;
     const int rows_item = min(p.BH, p.H - row0);  // output rows of this item
@@ -195,7 +190,7 @@ dw3x3s1_tma_kernel(const __grid_constant__ CUtensorMap tmIn, const DwTmaParams p
         const int rows_run = min(DWT_RUN, rows_item - orow0);   // >= 1 by construction of `bands`
         if (b < p.B && rows_run > 0) {
           const uint8_t* prow = patch + (size_t)((g * PHB + orow0) * PW + ow0) * 128;
-          T* obase = reinterpret_cast<T*>(p.out) + ((size_t)(b * p.H + row0 + orow0) * p.W + ow0) * p.C + c;
+          __nv_bfloat16* obase = reinterpret_cast<__nv_bfloat16*>(p.out) + ((size_t)(b * p.H + row0 + orow0) * p.W + ow0) * p.C + c;
           f32x2 acc[3][DWT_OW][NV];
 #pragma unroll
           for (int pr = 0; pr < DWT_RUN + 2; ++pr) {
@@ -207,13 +202,8 @@ dw3x3s1_tma_kernel(const __grid_constant__ CUtensorMap tmIn, const DwTmaParams p
                 const uint4 raw = *reinterpret_cast<const uint4*>(prow + (size_t)(pr * PW + x) * 128);
                 const unsigned wd[4] = {raw.x, raw.y, raw.z, raw.w};
                 f32x2 v[NV];
-                if constexpr (F32) {
-                  v[0] = f2_pack(__uint_as_float(wd[0]), __uint_as_float(wd[1]));
-                  v[1] = f2_pack(__uint_as_float(wd[2]), __uint_as_float(wd[3]));
-                } else {
 #pragma unroll
-                  for (int k = 0; k < NV; ++k) v[k] = f2_pack(__uint_as_float(wd[k] << 16), __uint_as_float(wd[k] & 0xffff0000u));
-                }
+                for (int k = 0; k < NV; ++k) v[k] = f2_pack(__uint_as_float(wd[k] << 16), __uint_as_float(wd[k] & 0xffff0000u));
 #pragma unroll
                 for (int r = 0; r < 3; ++r) {
                   const int o = pr - r;  // compile-time
@@ -232,34 +222,21 @@ dw3x3s1_tma_kernel(const __grid_constant__ CUtensorMap tmIn, const DwTmaParams p
               // output row pr - 2 is complete
               if (pr >= 2 && pr - 2 < rows_run) {
                 const int o = pr - 2, slot = o % 3;
-                T* orow = obase + (size_t)o * p.W * p.C;
+                __nv_bfloat16* orow = obase + (size_t)o * p.W * p.C;
 #pragma unroll
                 for (int i = 0; i < DWT_OW; ++i) {
                   if (ow0 + i < p.W) {
-                    if constexpr (F32) {
-                      float a[4];
+                    uint4 ov;
+                    __nv_bfloat162* o2 = reinterpret_cast<__nv_bfloat162*>(&ov);
 #pragma unroll
-                      for (int k = 0; k < NV; ++k) {
-                        float x0, x1;
-                        f2_unpack(acc[slot][i][k], x0, x1);
-                        a[2 * k] = act_t<ACT>(x0);      // exact activation: this is the parity mode
-                        a[2 * k + 1] = act_t<ACT>(x1);
-                        psum[k] = f2_add(psum[k], f2_pack(a[2 * k], a[2 * k + 1]));
-                      }
-                      *reinterpret_cast<float4*>(orow + (size_t)i * p.C) = make_float4(a[0], a[1], a[2], a[3]);
-                    } else {
-                      uint4 ov;
-                      __nv_bfloat162* o2 = reinterpret_cast<__nv_bfloat162*>(&ov);
-#pragma unroll
-                      for (int k = 0; k < NV; ++k) {
-                        const f32x2 a = f2_act<ACT>(acc[slot][i][k]);
-                        float a0, a1;
-                        f2_unpack(a, a0, a1);
-                        o2[k] = __floats2bfloat162_rn(a0, a1);
-                        psum[k] = f2_add(psum[k], a);
-                      }
-                      *reinterpret_cast<uint4*>(orow + (size_t)i * p.C) = ov;
+                    for (int k = 0; k < NV; ++k) {
+                      const f32x2 a = f2_act<ACT>(acc[slot][i][k]);
+                      float a0, a1;
+                      f2_unpack(a, a0, a1);
+                      o2[k] = __floats2bfloat162_rn(a0, a1);
+                      psum[k] = f2_add(psum[k], a);
                     }
+                    *reinterpret_cast<uint4*>(orow + (size_t)i * p.C) = ov;
                   }
                 }
               }
@@ -270,7 +247,7 @@ dw3x3s1_tma_kernel(const __grid_constant__ CUtensorMap tmIn, const DwTmaParams p
       if (p.pooled) {
         // fixed-order reduction of this pass: strip slots -> (crop, channel) owner threads
         *reinterpret_cast<float4*>(&red[sidx][j * CPT]) = make_float4(psum[0].x, psum[0].y, psum[1].x, psum[1].y);
-        if constexpr (!F32) *reinterpret_cast<float4*>(&red[sidx][j * CPT + 4]) = make_float4(psum[2].x, psum[2].y, psum[3].x, psum[3].y);
+        *reinterpret_cast<float4*>(&red[sidx][j * CPT + 4]) = make_float4(psum[2].x, psum[2].y, psum[3].x, psum[3].y);
         __syncthreads();
         for (int g = own_g0; g < p.G; g += GSTEP) {
           // strip slots of crop g in this pass: [g * strips_per_crop, (g + 1) * strips_per_crop) - s0, clipped
@@ -284,7 +261,7 @@ dw3x3s1_tma_kernel(const __grid_constant__ CUtensorMap tmIn, const DwTmaParams p
       }
     }
     if (p.pooled) {
-      const int ch = cg * CG + own_ch;
+      const int ch = cg * DWT_CG + own_ch;
       if (ch < p.C) {
         for (int g = own_g0; g < p.G; g += GSTEP) {
           if (b0 + g < p.B) p.pooled[((size_t)rb * p.B + b0 + g) * p.C + ch] = blocksum[g][own_ch] * p.inv_hw;
@@ -302,14 +279,12 @@ struct DwTmaCache {
 };
 
 inline const char* dw_tma_launch(DwTmaCache& cache, const DwTmaPlan& plan, const void* in, void* out, const float* w, const float* bias,
-                                 float* pooled, int B, int H, int W, int C, int pad_t, int pad_l, int act, cudaStream_t st,
-                                 bool f32 = false) {
+                                 float* pooled, int B, int H, int W, int C, int pad_t, int pad_l, int act, cudaStream_t st) {
   DwTmaParams p;
   p.out = out; p.w = w; p.bias = bias; p.pooled = pooled;
   p.B = B; p.H = H; p.W = W; p.C = C; p.pad_t = pad_t; p.pad_l = pad_l;
   p.G = plan.G; p.BH = plan.BH; p.n_rb = plan.n_rb;
-  const int cg_ch = f32 ? 32 : DWT_CG;
-  p.n_cg = (C + cg_ch - 1) / cg_ch;
+  p.n_cg = (C + DWT_CG - 1) / DWT_CG;
   const int n_bg = (B + plan.G - 1) / plan.G;
   p.items = n_bg * p.n_rb * p.n_cg;
   p.strips_w = (W + DWT_OW - 1) / DWT_OW;
@@ -317,17 +292,9 @@ inline const char* dw_tma_launch(DwTmaCache& cache, const DwTmaPlan& plan, const
   p.nstrips = plan.G * p.bands * p.strips_w;
   p.stage_bytes = 128 * (W + 2) * (plan.BH + 2) * plan.G;
   p.inv_hw = 1.0f / (float)(H * W);
-  {
-    // Serpentine traversal (MTB_DW_REV=0 disables; measured 22.47 vs 22.58 ms per step): the expand GEMM before this op wrote its output
-    // first-crop-to-last, so the END of the tensor is what the L2 still holds; walking the items last-to-first reads that
-    // part from L2, and leaves the BEGINNING of this op's output in L2 for the projection GEMM that follows.
-    static int rev_env = -1;
-    if (rev_env < 0) { const char* e = getenv("MTB_DW_REV"); rev_env = (e && e[0] == '0') ? 0 : 1; }
-    p.rev = rev_env;
-  }
   if (cache.in != in || cache.B != B) {
     const char* e = make_tmap_dw(&cache.map, in, (uint64_t)B, (uint64_t)H, (uint64_t)W, (uint64_t)C, (uint32_t)(W + 2),
-                                 (uint32_t)(plan.BH + 2), (uint32_t)plan.G, f32 ? 4u : 2u);
+                                 (uint32_t)(plan.BH + 2), (uint32_t)plan.G);
     if (e) return e;
     cache.in = in;
     cache.B = B;
@@ -335,20 +302,16 @@ inline const char* dw_tma_launch(DwTmaCache& cache, const DwTmaPlan& plan, const
   // + one pixel row of slack: the last strip of a ragged row may read (never use) a few pixels past the patch
   const size_t smem = (size_t)DWT_STAGES * p.stage_bytes + 128 + 8 * 128;
   const int grid = std::min(p.items, 2 * num_sms());
-#define MTB_DWT_LAUNCH_T(A, T)                                                                                             \
+#define MTB_DWT_LAUNCH(A)                                                                                                  \
   {                                                                                                                        \
     static bool attr_set = false;                                                                                          \
     if (!attr_set) {                                                                                                       \
-      if (cudaFuncSetAttribute(dw3x3s1_tma_kernel<A, T>, cudaFuncAttributeMaxDynamicSharedMemorySize,                       \
+      if (cudaFuncSetAttribute(dw3x3s1_tma_kernel<A>, cudaFuncAttributeMaxDynamicSharedMemorySize,                          \
                                DWT_STAGES * DWT_MAX_STAGE + 128 + 8 * 128) != cudaSuccess)                                 \
         return "cannot raise dynamic shared memory for dw3x3s1_tma_kernel";                                                \
       attr_set = true;                                                                                                     \
     }                                                                                                                      \
-    launch_k(dw3x3s1_tma_kernel<A, T>, dim3(grid), dim3(DWT_THREADS), smem, st, cache.map, p);                              \
-  }
-#define MTB_DWT_LAUNCH(A)                                                                                                  \
-  {                                                                                                                        \
-    if (f32) MTB_DWT_LAUNCH_T(A, float) else MTB_DWT_LAUNCH_T(A, __nv_bfloat16)                                             \
+    launch_k(dw3x3s1_tma_kernel<A>, dim3(grid), dim3(DWT_THREADS), smem, st, cache.map, p);                                 \
   }
   switch (act) {
     case ACT_SILU: MTB_DWT_LAUNCH(ACT_SILU); break;

@@ -8,6 +8,7 @@
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
 #include <map>
 #include <string>
@@ -29,6 +30,8 @@ namespace {
 std::string g_error;
 
 enum OpType { OP_STEM = 0, OP_CONV = 1, OP_DW = 2, OP_POOL = 3, OP_MAXPOOL = 4 };
+// depthwise kernels: TMA-staged (dw_tma.cuh), bf16 / fp32 strip (SE pooling fused), generic (dwconv_kernel)
+enum DwKernel { DW_GENERIC = 0, DW_TMA = 1, DW_STRIP_BF16 = 2, DW_STRIP_F32 = 3 };
 // kernel classes for the CUDA-event profiler (mtb_profile_begin / mtb_profile_end)
 enum KClass { KC_STEM = 0, KC_IGEMM_SIMT = 1, KC_DWCONV = 2, KC_POOL = 3, KC_SE_FC = 4, KC_TC_GEMM = 5, KC_FMB = 6,
               KC_HEAD_FUSED = 7, KC_HEAD_CONV_SIMT = 8, KC_SOFTARGMAX = 9, KC_RECON = 10, KC_OTHER = 11, KC_SE_SCALE = 12, KC_TC32 = 13,
@@ -58,7 +61,10 @@ struct Op {
   bool depthwise = false;
   bool small_io = false;  // squeeze-excitation FCs on [B,1,1,C] fp32 tensors
   float pre_scale[3] = {2.f, 2.f, 2.f}, pre_shift[3] = {-1.f, -1.f, -1.f};  // stem input affine (PreprocLayer: x*2-1)
-  bool fused_pool = false;  // bf16 modes: this depthwise op also produces the SE pooled means (next op is skipped)
+  bool fused_pool = false;  // this depthwise op also produces the SE pooled means (next op is skipped)
+  DwKernel dw_kernel = DW_GENERIC;  // depthwise: the kernel that runs it (set by mtb_finalize_weights)
+  DwTmaPlan dw_plan;                // DW_TMA: its tiling plan
+  int pool_slices = 1;              // DW_TMA / DW_STRIP_*: partial pooling slices it leaves (= its gridDim.y / dw_plan.n_rb)
   bool res_first = false;  // residual added BEFORE the activation (ResNet); EfficientNet adds it after
   int pool_src = -1;       // fc1: index of the OP_POOL op that produces its input (fused pooling leaves partial slices)
   int ksplit = 1;          // split-K (squeeze-excitation fc1): raw sums, bias/act deferred to the consumer
@@ -104,7 +110,7 @@ struct mtb_handle {
     bool used = false;         // `done` has been recorded at least once
   };
   HostSlot slots[2];
-  // MTB_GRAPH=1: captured forwards keyed by (buffers, batch, stream)
+  // mtb_forward's captured forwards keyed by (buffers, batch, stream)
   struct GraphEntry {
     const void *crops = nullptr, *k = nullptr, *out = nullptr, *ws = nullptr;
     int batch = 0;
@@ -117,7 +123,7 @@ struct mtb_handle {
   void* pipe_ws = nullptr;
   size_t pipe_ws_bytes = 0;
   cudaStream_t copy_stream = nullptr;
-  cudaStream_t graph_stream = nullptr;  // MTB_GRAPH=1 with the legacy default stream: captured forwards run here
+  cudaStream_t graph_stream = nullptr;  // mtb_forward on the legacy default stream: captured forwards run here
   cudaEvent_t graph_in = nullptr, graph_out = nullptr;
   // profiler
   unsigned prof_mask = 0;
@@ -203,13 +209,12 @@ struct Planner {
     // the small buffer (capacity >= cexp floats per crop)
     f1.ksplit = std::max(1, std::min({32, cexp / 64, cexp / csq}));
     h->ops.push_back(f1);
-    const int f1_index = (int)h->ops.size() - 1;
     Op f2;
     f2.type = OP_CONV; f2.name = name + ".fc2"; f2.wkey = fc2 + ".weight"; f2.biaskey = fc2 + ".bias";
     f2.Cin = csq; f2.Cout = cexp; f2.act = act2; f2.small_io = true; f2.pad_ok = true;
     f2.in_buf = BUF_SMALL0 + 1; f2.out_buf = BUF_SMALL0 + 2;
     f2.flops = 2.0 * cexp * csq_real;
-    (void)f1_index;  // (fc2 summing the slices on its A load was measured slower than the tiny reduce kernel)
+    // (fc2 summing fc1's split-K slices on its A load was measured slower than the tiny reduce kernel)
     h->ops.push_back(f2);
     max_small = std::max(max_small, cexp);
   }
@@ -314,8 +319,7 @@ void plan_effnet(mtb_handle* h) {
   {
     char key[64];
     snprintf(key, sizeof(key), "%s.%d", pre.c_str(), c.n_stages + 1);
-    Op& last = P.conv(key, c.last_channel, 1, 1, 0, 0, ACT_SILU, P.cur, BUF_FEATURES);  // :319-324
-    (void)last;
+    P.conv(key, c.last_channel, 1, 1, 0, 0, ACT_SILU, P.cur, BUF_FEATURES);  // :319-324
   }
   h->feat_side = P.H;
   h->feat_c = P.C;
@@ -587,11 +591,11 @@ int prepare_op_weights(mtb_handle* h, Op& op) {
   if (rc) return rc;
   rc = upload(h, bias.data(), bias.size() * 4, (void**)&op.d_bias);
   if (rc) return rc;
-  if (h->cfg.precision == MTB_PRECISION_BF16_TC && tc_like && !tc_disabled()) {
+  if (h->cfg.precision == MTB_PRECISION_BF16_TC && tc_like) {
     const char* e = tc_prepare_weights(op.tc, wk.data(), bias.data(), K, op.Cout, op.R, op.S, op.Cin, h->dev_allocs);
     if (e) return fail(h, MTB_ERR_CUDA, "tensor-core weight prep for '%s': %s", op.name.c_str(), e);
   }
-  if (h->cfg.precision == MTB_PRECISION_TF32X3 && !tc_disabled() &&
+  if (h->cfg.precision == MTB_PRECISION_TF32X3 &&
       tc32_eligible(op.type == OP_CONV, op.depthwise, op.small_io, op.R, op.stride, op.Cin, op.Cout)) {
     const char* e = tc32_prepare_weights(op.tc32, wk.data(), bias.data(), K, op.Cout, op.R, op.S, op.Cin, h->dev_allocs);
     if (e) return fail(h, MTB_ERR_CUDA, "3xTF32 weight prep for '%s': %s", op.name.c_str(), e);
@@ -602,7 +606,6 @@ int prepare_op_weights(mtb_handle* h, Op& op) {
 // --------------------------------------------------------------------------------------------- workspace
 struct Workspace {
   char* base;
-  int b0 = 0;  // first crop the ops address (0: every op runs on the whole batch; kept for batch-slice experiments)
   size_t big_stride, small_stride;
   size_t off_small, off_features, off_logits, off_c2d, off_c3d, off_n2d, off_partial, total;
 };
@@ -632,13 +635,6 @@ void* buf_ptr(const Workspace& w, int id, void* features) {
   if (id < 0) return nullptr;
   if (id < kNumBig) return w.base + w.big_stride * id;
   return w.base + w.off_small + w.small_stride * (id - BUF_SMALL0);
-}
-
-// activation tensor [B,hh,ww,cc] in buffer `id`, from crop w.b0 on (small [B,C] buffers are never sliced)
-void* act_ptr(const mtb_handle* h, const Workspace& w, int id, void* features, int hh, int ww, int cc) {
-  char* base = (char*)buf_ptr(w, id, features);
-  if (!base || id >= kNumBig) return base;
-  return base + (size_t)w.b0 * hh * ww * cc * elem_size(h);
 }
 
 // ---------------------------------------------------------------------------------------------- profiler
@@ -677,45 +673,32 @@ bool dw_strip_eligible(const Op& op) {
          (op.act == ACT_SILU || op.act == ACT_RELU || op.act == ACT_HSWISH);
 }
 
-// number of partial pooling slices the fused depthwise kernel writes (= its gridDim.y)
 constexpr int kDwOW = 4;  // outputs per thread along W in dwconv3x3_pool_bf16_kernel (measured: 4 -> 3.65 ms, 2 -> 4.25 ms per 128 crops)
-// stride-1 3x3 depthwise ops run the TMA-staged kernel (dw_tma.cuh); MTB_DW_TMA=0 falls back to the strip kernel (A/B runs)
-// MTB_DW_F32_TMA=1: the 3xTF32 mode runs the fp32 variant of the TMA-staged depthwise kernel instead of the fp32 strip kernel.
-// OFF: measured 11.08 vs 9.92 ms per 256 crops (V2-L; joints 6.9e-6 vs 7.4e-6 from the oracle) - with 32 channels per item and the
-// exact expf / divide SiLU of the parity mode the kernel is more issue-bound than the strip kernel is latency-bound.
-bool dw_f32_tma_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("MTB_DW_F32_TMA");
-    v = (e && e[0] == '1') ? 1 : 0;
+
+// Picks the kernel of a depthwise op and the number of partial pooling slices it writes (fc1 sums that many).  bf16
+// tensor-core mode: stride-1 ops run the TMA-staged kernel when a plan fits, the rest the bf16 strip kernel.  3xTF32 mode:
+// the fp32 strip kernel (exact activation).  Other modes and shapes: the generic kernel, which does not pool.
+void choose_dw_kernel(const mtb_handle* h, Op& op) {
+  op.dw_kernel = DW_GENERIC;
+  if (!dw_strip_eligible(op)) return;
+  if (h->cfg.precision == MTB_PRECISION_BF16_TC) {
+    if (op.stride == 1 && op.Hin == op.Hout && op.Win == op.Wout) {
+      const DwTmaPlan pl = dw_tma_plan(op.Hout, op.Wout);
+      if (pl.ok && pl.n_rb <= kPoolSlices) {
+        op.dw_kernel = DW_TMA;
+        op.dw_plan = pl;
+        op.pool_slices = pl.n_rb;
+        return;
+      }
+    }
+    op.dw_kernel = DW_STRIP_BF16;
+  } else if (h->cfg.precision == MTB_PRECISION_TF32X3) {
+    op.dw_kernel = DW_STRIP_F32;
+  } else {
+    return;
   }
-  return v == 1;
-}
-bool dw_tma_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("MTB_DW_TMA");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
-}
-// tma_ok: the handle runs a mode the TMA-staged kernel covers (bf16 tensor-core mode; 3xTF32 mode: its fp32 variant, C % 4 == 0)
-DwTmaPlan dw_tma_plan_for(const Op& op, bool tma_ok = true) {
-  DwTmaPlan none;
-  if (!tma_ok) return none;
-  if (!dw_tma_enabled() || !dw_strip_eligible(op) || op.stride != 1 || op.Hin != op.Hout || op.Win != op.Wout) return none;
-  DwTmaPlan pl = dw_tma_plan(op.Hout, op.Wout);
-  if (!pl.ok || pl.n_rb > kPoolSlices) return none;
-  return pl;
-}
-bool dw_tma_mode(const mtb_handle* h, const Op& op) {
-  return h->cfg.precision == MTB_PRECISION_BF16_TC || (h->cfg.precision == MTB_PRECISION_TF32X3 && op.Cout % 4 == 0 && dw_f32_tma_enabled());
-}
-int dw_pool_slices(const Op& dw, bool tma_ok = true) {
-  const DwTmaPlan pl = dw_tma_plan_for(dw, tma_ok);
-  if (pl.ok) return pl.n_rb;
-  const int strips = dw.Hout * ((dw.Wout + kDwOW - 1) / kDwOW);
-  return std::min((strips + 7) / 8, kPoolSlices);
+  const int strips = op.Hout * ((op.Wout + kDwOW - 1) / kDwOW);
+  op.pool_slices = std::min((strips + 7) / 8, kPoolSlices);
 }
 
 int op_class(const Op& op) {
@@ -727,7 +710,7 @@ int op_class(const Op& op) {
     default: break;
   }
   if (op.small_io) return KC_SE_FC;
-  if (op.fmb.ready && fmb_enabled()) return KC_FMB;
+  if (op.fmb.ready) return KC_FMB;
   if (op.tc.ready) return KC_TC_GEMM;  // one class per kernel: every tensor-core conv/GEMM launch is tc_conv_kernel
   if (op.tc32.ready) return KC_TC32;
   return KC_IGEMM_SIMT;
@@ -744,8 +727,7 @@ double op_bytes(const mtb_handle* h, const Op& op, int B) {
   double out = (double)B * op.Hout * op.Wout * op.Cout * es;
   if (op.type == OP_POOL) out = (double)B * op.Cout * 4.0;
   double res = op.res_buf != BUF_NONE ? out : 0.0;
-  double w = (op.type == OP_POOL || op.type == OP_MAXPOOL) ? 0.0 : (double)op.R * op.S * (op.depthwise ? 1 : op.Cin) * op.Cout * (op.tc.ready ? 2.0 : 4.0);
-  return in + out + res + w;
+  return in + out + res + op_weight_bytes(op);
 }
 
 // ---------------------------------------------------------------------------------------------- executor
@@ -758,25 +740,14 @@ bool stem_fast_enabled() {  // MTB_STEM_FAST=0: the generic stem kernel (A/B run
   return v == 1;
 }
 
-bool pdl_se_enabled() {  // MTB_PDL_SE=1: programmatic dependent launch for the squeeze-excitation chain only
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("MTB_PDL_SE");
-    v = (e && e[0] == '1') ? 1 : 0;
-  }
-  return v == 1;
-}
-
 template <typename T>
 int run_op_t(mtb_handle* h, const Op& op, const float* crops, int B, const Workspace& ws, void* features,
              cudaStream_t st) {
-  PdlScope pdl_scope(pdl_se_enabled() && op.small_io);
   if (op.type == OP_CONV && op.tc.ready && op.scale_buf != BUF_NONE) {
     // squeeze-excitation scale applied in place ahead of the bf16 tensor-core conv
-    void* x = act_ptr(h, ws, op.in_buf, features, op.Hin, op.Win, op.Cin);
+    void* x = buf_ptr(ws, op.in_buf, features);
     const double bytes = 2.0 * B * op.Hin * op.Win * op.Cin * elem_size(h);
     ProfScope ps(h, KC_SE_SCALE, 0.0, bytes, st, false);
-    PdlScope pdl_scale(pdl_se_enabled());
     const char* e = tc_se_scale_launch(x, (const float*)buf_ptr(ws, op.scale_buf, features), B, op.Hin * op.Win, op.Cin, st);
     if (e) return fail(h, MTB_ERR_CUDA, "se scale %s: %s", op.name.c_str(), e);
     h->launches++;
@@ -785,8 +756,8 @@ int run_op_t(mtb_handle* h, const Op& op, const float* crops, int B, const Works
   switch (op.type) {
     case OP_STEM: {
       StemParams p;
-      p.in = crops + (size_t)ws.b0 * op.Cin * op.Hin * op.Win;
-      p.out = act_ptr(h, ws, op.out_buf, features, op.Hout, op.Wout, op.Cout); p.w = op.d_w; p.bias = op.d_bias;
+      p.in = crops;
+      p.out = buf_ptr(ws, op.out_buf, features); p.w = op.d_w; p.bias = op.d_bias;
       for (int i = 0; i < 3; ++i) { p.pre_scale[i] = op.pre_scale[i]; p.pre_shift[i] = op.pre_shift[i]; }
       p.pre_scale[3] = 1.f; p.pre_shift[3] = 0.f;
       p.B = B; p.Hin = op.Hin; p.Win = op.Win; p.Cin = op.Cin; p.Hout = op.Hout; p.Wout = op.Wout; p.Cout = op.Cout;
@@ -807,26 +778,22 @@ int run_op_t(mtb_handle* h, const Op& op, const float* crops, int B, const Works
     case OP_DW:
     case OP_MAXPOOL: {
       ConvParams p;
-      p.in = act_ptr(h, ws, op.in_buf, features, op.Hin, op.Win, op.Cin);
-      p.out = act_ptr(h, ws, op.out_buf, features, op.Hout, op.Wout, op.Cout);
-      p.res = act_ptr(h, ws, op.res_buf, features, op.Hout, op.Wout, op.Cout);
+      p.in = buf_ptr(ws, op.in_buf, features);
+      p.out = buf_ptr(ws, op.out_buf, features);
+      p.res = buf_ptr(ws, op.res_buf, features);
       p.a_scale = (const float*)buf_ptr(ws, op.scale_buf, features);
       p.w = op.d_w; p.bias = op.d_bias;
       p.B = B; p.Hin = op.Hin; p.Win = op.Win; p.Cin = op.Cin; p.Hout = op.Hout; p.Wout = op.Wout; p.Cout = op.Cout;
       p.R = op.R; p.S = op.S; p.stride = op.stride; p.dil = op.dil; p.pad_t = op.pad_t; p.pad_l = op.pad_l; p.act = op.act;
       p.res_first = op.res_first ? 1 : 0;
       if (op.type == OP_DW) {
-        if (h->cfg.precision == MTB_PRECISION_BF16_TC && dw_strip_eligible(op)) {
-          float* pooled = op.fused_pool ? (float*)buf_ptr(ws, BUF_SMALL0, features) : nullptr;
-          const DwTmaPlan tma_plan = dw_tma_plan_for(op);
-          if (tma_plan.ok) {
-            const char* e = dw_tma_launch(op.dw_cache, tma_plan, p.in, p.out, op.d_w, op.d_bias, pooled, B, op.Hout, op.Wout, op.Cout,
-                                          op.pad_t, op.pad_l, op.act, st);
-            if (e) return fail(h, MTB_ERR_CUDA, "depthwise (TMA) launch %s: %s", op.name.c_str(), e);
-            h->launches++;
-            break;
-          }
-          dim3 grid((op.Cout / 8 + 31) / 32, dw_pool_slices(op), B), block(32, 8);
+        float* pooled = op.fused_pool ? (float*)buf_ptr(ws, BUF_SMALL0, features) : nullptr;
+        if (op.dw_kernel == DW_TMA) {
+          const char* e = dw_tma_launch(op.dw_cache, op.dw_plan, p.in, p.out, op.d_w, op.d_bias, pooled, B, op.Hout, op.Wout, op.Cout,
+                                        op.pad_t, op.pad_l, op.act, st);
+          if (e) return fail(h, MTB_ERR_CUDA, "depthwise (TMA) launch %s: %s", op.name.c_str(), e);
+        } else if (op.dw_kernel == DW_STRIP_BF16) {
+          dim3 grid((op.Cout / 8 + 31) / 32, op.pool_slices, B), block(32, 8);
           if (op.act == ACT_SILU) {
             if (op.stride == 1) launch_k(dwconv3x3_pool_bf16_kernel<1, ACT_SILU, kDwOW>, dim3(grid), dim3(block), 0, st, p, pooled);
             else launch_k(dwconv3x3_pool_bf16_kernel<2, ACT_SILU, kDwOW>, dim3(grid), dim3(block), 0, st, p, pooled);
@@ -837,18 +804,9 @@ int run_op_t(mtb_handle* h, const Op& op, const float* crops, int B, const Works
             if (op.stride == 1) launch_k(dwconv3x3_pool_bf16_kernel<1, ACT_HSWISH, kDwOW>, dim3(grid), dim3(block), 0, st, p, pooled);
             else launch_k(dwconv3x3_pool_bf16_kernel<2, ACT_HSWISH, kDwOW>, dim3(grid), dim3(block), 0, st, p, pooled);
           }
-        } else if (h->cfg.precision == MTB_PRECISION_TF32X3 && dw_strip_eligible(op) && op.Cout % 4 == 0) {
-          float* pooled = op.fused_pool ? (float*)buf_ptr(ws, BUF_SMALL0, features) : nullptr;
-          const DwTmaPlan tma_plan = dw_tma_plan_for(op, dw_tma_mode(h, op));
-          if (tma_plan.ok) {  // the TMA-staged kernel, fp32 variant (exact activation)
-            const char* e = dw_tma_launch(op.dw_cache, tma_plan, p.in, p.out, op.d_w, op.d_bias, pooled, B, op.Hout, op.Wout, op.Cout,
-                                          op.pad_t, op.pad_l, op.act, st, true);
-            if (e) return fail(h, MTB_ERR_CUDA, "depthwise (TMA, fp32) launch %s: %s", op.name.c_str(), e);
-            h->launches++;
-            break;
-          }
+        } else if (op.dw_kernel == DW_STRIP_F32) {
           // fp32 strip kernel: 4 channels x 4 pixels per thread, SE squeeze fused (partial slices summed by fc1)
-          dim3 grid((op.Cout / 4 + 31) / 32, dw_pool_slices(op, false), B), block(32, 8);
+          dim3 grid((op.Cout / 4 + 31) / 32, op.pool_slices, B), block(32, 8);
 #define MTB_DWF32(ST, AC) launch_k(dwconv3x3_pool_f32_kernel<ST, AC, kDwOW>, dim3(grid), dim3(block), 0, st, p, pooled)
           if (op.act == ACT_SILU) { if (op.stride == 1) MTB_DWF32(1, ACT_SILU); else MTB_DWF32(2, ACT_SILU); }
           else if (op.act == ACT_RELU) { if (op.stride == 1) MTB_DWF32(1, ACT_RELU); else MTB_DWF32(2, ACT_RELU); }
@@ -863,7 +821,7 @@ int run_op_t(mtb_handle* h, const Op& op, const float* crops, int B, const Works
         launch_k(maxpool_kernel<T>, dim3(grid_for(total, 256)), dim3(256), 0, st, p);
       } else if (op.small_io) {
         if (op.pool_src > 0 && h->ops[op.pool_src].fused_pool) {  // input = partial pooling slices of the depthwise kernel
-          p.a_splits = dw_pool_slices(h->ops[op.pool_src - 1], dw_tma_mode(h, h->ops[op.pool_src - 1]));
+          p.a_splits = h->ops[op.pool_src - 1].pool_slices;
           p.a_split_stride = (size_t)B * op.Cin;
         }
         float* final_out = (float*)p.out;
@@ -895,7 +853,7 @@ int run_op_t(mtb_handle* h, const Op& op, const float* crops, int B, const Works
     }
     case OP_POOL: {
       dim3 grid((op.Cin + 127) / 128, B), block(32, 8);
-      launch_k(pool_mean_kernel<T>, dim3(grid), dim3(block), 0, st, (const T*)act_ptr(h, ws, op.in_buf, features, op.Hin, op.Win, op.Cin),
+      launch_k(pool_mean_kernel<T>, dim3(grid), dim3(block), 0, st, (const T*)buf_ptr(ws, op.in_buf, features),
                                                    (float*)buf_ptr(ws, op.out_buf, features), op.Hin * op.Win, op.Cin);
       h->launches++;
       break;
@@ -916,8 +874,8 @@ int run_op(mtb_handle* h, const Op& op, const float* crops, int B, const Workspa
 // makes smaller launches, and these kernels are latency / issue bound at small batches rather than bandwidth bound.
 // one fmb_kernel launch for the FusedMBConv block (a = 3x3 expand, b = 1x1 projection [+ residual = a's input])
 int run_fused_block(mtb_handle* h, const Op& a, const Op& b, int B, const Workspace& ws, void* features, cudaStream_t st) {
-  const void* in = act_ptr(h, ws, a.in_buf, features, a.Hin, a.Win, a.Cin);
-  void* out = act_ptr(h, ws, b.out_buf, features, b.Hout, b.Wout, b.Cout);
+  const void* in = buf_ptr(ws, a.in_buf, features);
+  void* out = buf_ptr(ws, b.out_buf, features);
   const double bytes = 2.0 * B * a.Hin * a.Win * (a.Cin + b.Cout) + 2.0 * (9.0 * a.Cin * a.Cout + (double)b.Cin * b.Cout);
   ProfScope prof(h, KC_FMB, (a.flops + b.flops) * B, bytes, st);
   const char* e = fmb_launch(a.fmb, in, out, B, a.Hin, a.Win, a.pad_t, a.pad_l, b.res_buf != BUF_NONE, st);
@@ -932,7 +890,7 @@ int run_ops_range(mtb_handle* h, size_t first, size_t last, const float* crops, 
   for (size_t k = first; k < last; ++k) {
     h->prof_cur_op = (int)k;
     int rc;
-    if (h->ops[k].fmb.ready && fmb_enabled() && k + 1 < last) {
+    if (h->ops[k].fmb.ready && k + 1 < last) {
       rc = run_fused_block(h, h->ops[k], h->ops[k + 1], B, ws, features, st);
       ++k;
     } else {
@@ -1050,23 +1008,17 @@ int recon_impl(mtb_handle* h, const float* c2d, const float* c3d, const float* K
 }
 
 __global__ void to_float_kernel(const __nv_bfloat16* in, float* out, size_t n) {
-  pdl_trigger();
-  pdl_wait();
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
     out[i] = __bfloat162float(in[i]);
 }
 
 __global__ void from_float_kernel(const float* in, __nv_bfloat16* out, size_t n) {
-  pdl_trigger();
-  pdl_wait();
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
     out[i] = __float2bfloat16_rn(in[i]);
 }
 
 // [b,J,2] + [b,J,3] -> [b,J,5] (what travels in the all-gather) and back
 __global__ void pack_decoded_kernel(const float* __restrict__ c2d, const float* __restrict__ c3d, float* __restrict__ packed, int n) {
-  pdl_trigger();
-  pdl_wait();
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     packed[(size_t)i * 5 + 0] = c2d[(size_t)i * 2 + 0];
     packed[(size_t)i * 5 + 1] = c2d[(size_t)i * 2 + 1];
@@ -1076,8 +1028,6 @@ __global__ void pack_decoded_kernel(const float* __restrict__ c2d, const float* 
   }
 }
 __global__ void unpack_decoded_kernel(const float* __restrict__ packed, float* __restrict__ c2d, float* __restrict__ c3d, int n) {
-  pdl_trigger();
-  pdl_wait();
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     c2d[(size_t)i * 2 + 0] = packed[(size_t)i * 5 + 0];
     c2d[(size_t)i * 2 + 1] = packed[(size_t)i * 5 + 1];
@@ -1142,17 +1092,10 @@ int mtb_create(const mtb_config* cfg, mtb_handle** out) {
 
 int mtb_destroy(mtb_handle* h) {
   if (!h) return MTB_OK;
-  const bool trace = getenv("MTB_TRACE_DESTROY") != nullptr;
-  if (trace) fprintf(stderr, "mtb_destroy: handle %p device %d allocs %zu events %zu stage %p\n", (void*)h, h->cfg.device,
-                     h->dev_allocs.size(), h->prof_events.size(), h->stage);
   {
     DeviceGuard g(h->cfg.device);
     for (void* p : h->dev_allocs) cudaFree(p);
-    if (trace) fprintf(stderr, "mtb_destroy: weights freed\n");
-    if (h->stage) {
-      cudaError_t e = cudaFree(h->stage);
-      if (trace) fprintf(stderr, "mtb_destroy: stage freed (%s)\n", cudaGetErrorString(e));
-    }
+    if (h->stage) cudaFree(h->stage);
     for (auto& sl : h->slots) {
       if (sl.buf) cudaFree(sl.buf);
       if (sl.h2d_done) cudaEventDestroy(sl.h2d_done);
@@ -1167,14 +1110,11 @@ int mtb_destroy(mtb_handle* h) {
     if (h->graph_out) cudaEventDestroy(h->graph_out);
     cudaGetLastError();
     for (size_t i = 0; i < h->prof_events.size(); ++i) {
-      cudaError_t e = cudaEventDestroy(h->prof_events[i]);
-      if (trace && (i < 2 || e != cudaSuccess)) fprintf(stderr, "mtb_destroy: event %zu destroyed (%s)\n", i, cudaGetErrorString(e));
-      if (e != cudaSuccess) {  // e.g. cudaErrorContextIsDestroyed during process teardown: the driver owns them now
+      if (cudaEventDestroy(h->prof_events[i]) != cudaSuccess) {  // e.g. cudaErrorContextIsDestroyed during process teardown: the driver owns them now
         cudaGetLastError();
         break;
       }
     }
-    if (trace) fprintf(stderr, "mtb_destroy: events destroyed\n");
     if (h->nccl_comm && h->nccl_lib) {
       typedef int (*destroy_t)(void*);
       destroy_t f = (destroy_t)dlsym(h->nccl_lib, "ncclCommDestroy");
@@ -1182,7 +1122,6 @@ int mtb_destroy(mtb_handle* h) {
     }
   }
   delete h;
-  if (trace) fprintf(stderr, "mtb_destroy: done\n");
   return MTB_OK;
 }
 
@@ -1230,12 +1169,12 @@ int mtb_finalize_weights(mtb_handle* h) {
   h->graphs.clear();
   for (void* p : h->dev_allocs) cudaFree(p);
   h->dev_allocs.clear();
-  for (auto& op : h->ops) op.fused_pool = false;
-  for (size_t i = 0; i + 1 < h->ops.size(); ++i) {
-    const bool fuse = (h->cfg.precision == MTB_PRECISION_BF16_TC || h->cfg.precision == MTB_PRECISION_TF32X3) &&
-                      dw_strip_eligible(h->ops[i]) && h->ops[i + 1].type == OP_POOL;
-    if (fuse) h->ops[i].fused_pool = h->ops[i + 1].fused_pool = true;
+  for (auto& op : h->ops) {
+    op.fused_pool = false;
+    choose_dw_kernel(h, op);
   }
+  for (size_t i = 0; i + 1 < h->ops.size(); ++i)  // the strip and TMA-staged depthwise kernels also pool for the SE block behind them
+    if (h->ops[i].dw_kernel != DW_GENERIC && h->ops[i + 1].type == OP_POOL) h->ops[i].fused_pool = h->ops[i + 1].fused_pool = true;
   for (auto& op : h->ops) {
     int rc = prepare_op_weights(h, op);
     if (rc) return rc;
@@ -1420,8 +1359,8 @@ static int forward_body(mtb_handle* h, const float* crops, const float* intrinsi
 // mtb_forward captures its own launches into a CUDA graph the second time it sees the same (buffers, batch, stream) and
 // replays that graph from then on: the ~465 launches of a step cost less as one graph launch than as stream submissions
 // (measured, round 2: 12.28 k vs 11.83 k crops/s end to end through mtb_forward_host_submit/_wait, EfficientNetV2-L@256, 256
-// crops).  MTB_GRAPH=0 disables it.  A profiling window bypasses it (events cannot be timed inside a graph), a caller that
-// is itself capturing the stream just records our launches, any capture failure falls back to plain launches for that key.
+// crops).  A profiling window bypasses it (events cannot be timed inside a graph), a caller that is itself capturing the
+// stream just records our launches, any capture failure falls back to plain launches for that key.
 static void drop_graphs_on(mtb_handle* h, const void* ws) {
   for (size_t i = 0; i < h->graphs.size();) {
     if (ws == nullptr || h->graphs[i].ws == ws) {
@@ -1433,15 +1372,6 @@ static void drop_graphs_on(mtb_handle* h, const void* ws) {
   }
 }
 
-static bool graph_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("MTB_GRAPH");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
-}
-
 int mtb_forward(mtb_handle* h, const float* crops, const float* intrinsics, int batch, float* coords3d_abs,
                 void* workspace, size_t workspace_bytes, void* stream) {
   int rc = check_common(h, batch, workspace_bytes, workspace);
@@ -1450,7 +1380,7 @@ int mtb_forward(mtb_handle* h, const float* crops, const float* intrinsics, int 
   if (h->ops.empty()) return fail(h, MTB_ERR_UNSUPPORTED, "this handle has no backbone (head-only)");
   DeviceGuard g(h->cfg.device);
   cudaStream_t st = (cudaStream_t)stream;
-  if (graph_enabled() && h->prof_mask == 0) {
+  if (h->prof_mask == 0) {
     cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
     cudaStreamIsCapturing(st, &cs);
     if (cs == cudaStreamCaptureStatusNone) {  // (a caller capturing this stream itself just records our launches)
@@ -1962,7 +1892,7 @@ int mtb_debug_run_op(mtb_handle* h, int op_index, const float* in, const float* 
 }
 
 int mtb_op_is_fused_block(const mtb_handle* h, int op_index) {
-  return (h && op_index >= 0 && op_index + 1 < (int)h->ops.size() && h->ops[op_index].fmb.ready && fmb_enabled()) ? 1 : 0;
+  return (h && op_index >= 0 && op_index + 1 < (int)h->ops.size() && h->ops[op_index].fmb.ready) ? 1 : 0;
 }
 
 int mtb_debug_run_fused_block(mtb_handle* h, int op_index, const float* in, int batch, float* out, size_t out_floats, void* workspace,

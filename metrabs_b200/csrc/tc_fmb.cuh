@@ -53,8 +53,6 @@ fmb_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_trigger();
-  pdl_wait();
 
   const int m_blk = blockIdx.x;
   const int num_kb = g.taps * g.kchunks;
@@ -191,15 +189,6 @@ struct FmbWeights {
   mutable const void* cached_in = nullptr;
   mutable int cached_B = -1;
 };
-
-inline bool fmb_enabled() {  // MTB_FMB=0: FusedMBConv blocks run as two tc_conv_kernel launches (A/B runs)
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("MTB_FMB");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
-}
 
 // shapes the fused kernel covers: 3x3 stride-1 expand (SiLU) + 1x1 projection, Cin = Cout (identity-shaped block)
 inline bool fmb_shape_ok(int cin, int cexp, int cout) {

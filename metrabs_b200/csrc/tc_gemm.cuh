@@ -196,8 +196,6 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_trigger();
-  pdl_wait();
 
   const int m_blk = blockIdx.x, n_blk = blockIdx.y;
   const int num_kb = p.taps * p.kchunks;
@@ -277,8 +275,6 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 // in-place squeeze-excitation scaling  x[b,p,c] *= s[b,c]  ahead of a tensor-core projection GEMM
 __global__ void __launch_bounds__(256) se_scale_kernel(__nv_bfloat16* __restrict__ x, const float* __restrict__ s, int P, int C,
                                                        size_t total8) {
-  pdl_trigger();
-  pdl_wait();
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total8; i += (size_t)gridDim.x * blockDim.x) {
     size_t e = i * 8;
     int c = (int)(e % C);
@@ -364,15 +360,6 @@ struct TcWeights {
   mutable std::vector<MapSet> map_sets;
   mutable size_t map_rr = 0;
 };
-
-inline bool tc_disabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("MTB_DISABLE_TC");
-    v = (e && e[0] == '1') ? 1 : 0;
-  }
-  return v == 1;
-}
 
 inline bool tc_eligible(bool is_conv, bool depthwise, bool small_io, int k, int stride, int cin, int cout) {
   if (!is_conv || depthwise || small_io) return false;
@@ -545,8 +532,6 @@ tc_head_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_trigger();
-  pdl_wait();
 
   const int g = blockIdx.x / p.m_tiles, m_blk = blockIdx.x - g * p.m_tiles;
   const int n_kb = p.npt * p.kblocks;
@@ -682,8 +667,6 @@ tc_head_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
 __global__ void __launch_bounds__(128) head_finalize_kernel(const float4* __restrict__ states, float* __restrict__ out2d,
                                                             float* __restrict__ out3d, int J, int D, int H, int W,
                                                             DecodeScale sc) {
-  pdl_trigger();
-  pdl_wait();
   const int b = blockIdx.x;
   const int n_out = J * (1 + D);
   for (int j = threadIdx.x; j < J; j += blockDim.x) {
@@ -720,7 +703,7 @@ __global__ void __launch_bounds__(128) head_finalize_kernel(const float4* __rest
 
 // w: fp32 [n_out][C] (torch conv weight [N,C,1,1]); returns nullptr on success.  Not eligible -> ready stays false.
 inline const char* tc_prepare_head(TcWeights& w, const float* wt, const float* bias, int C, int n_out, std::vector<void*>& allocs) {
-  if (tc_disabled() || C % 8 != 0) return nullptr;
+  if (C % 8 != 0) return nullptr;
   std::vector<__nv_bfloat16> t((size_t)n_out * C);
   for (size_t i = 0; i < t.size(); ++i) t[i] = host_bf16(wt[i]);
   if (cudaMalloc((void**)&w.d_w, t.size() * 2) != cudaSuccess) return "cudaMalloc failed";

@@ -153,8 +153,6 @@ tc32_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_trigger();
-  pdl_wait();
 
   const int m_blk = blockIdx.x, n_blk = blockIdx.y;
   const int num_kb = p.taps * p.kchunks;

@@ -90,8 +90,8 @@ def test_fused_block_at_bench_batch(H, batch):
 
 
 def test_whole_backbone_with_and_without_fusion(H, monkeypatch):
-    """EfficientNetV2-S features through the fused blocks vs the same engine with MTB_FMB=0 semantics (unfused op chain
-    via debug_run_op is covered above); here: the full forward stays finite and close to the bf16 CUDA-core chain."""
+    """EfficientNetV2-S features through the fused blocks (the unfused op chain via debug_run_op is covered above);
+    here: the full forward stays finite and close to the bf16 CUDA-core chain."""
     name, side, batch = 'efficientnetv2-s', 256, 4
     pcfg = port.PathConfig(proc_side=side)
     sd = port.make_effnet_state_dict(port.effnet_spec(name), pcfg, 8, seed=0)
