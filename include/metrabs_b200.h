@@ -115,6 +115,25 @@ const char* mtb_version(void);
 int mtb_load_weight(mtb_handle* h, const char* name, const void* data, int dtype, const int64_t* shape, int ndim);
 int mtb_finalize_weights(mtb_handle* h);
 
+/* Latent-point models (Metrabs.__init__ with affine_weights, models/metrabs.py:23-45 and :53-62; the recombination itself
+ * is metrabs_tf/models/metrabs.py:80-81).  `weights` is a HOST fp32 array [n_latents][n_out] (the autoencoder's w2; it is
+ * copied).  From then on the forward reconstructs head points [0, n_latents) and maps them to n_out joints per crop:
+ * joints[b,J',c] = sum_l abs[b,l,c] * w2[l,J'].  transform_coords: n_latents = cfg.n_joints; predict_all_and_latents:
+ * cfg.n_joints = n_latents + J, and mtb_finalize_weights keeps only the head channels of the first n_latents points (the
+ * checkpoint still holds the full [(n_latents+J)(1+D),C,1,1] weight).  mtb_head_decode, mtb_reconstruct_absolute and the
+ * all-gather of mtb_forward_sharded then work on n_latents points; mtb_forward* write n_out joints per crop.  Must be called
+ * before mtb_finalize_weights; a second call replaces the first.  MTB_ERR_INVALID_ARG for n_latents outside
+ * [1, cfg.n_joints], n_out outside [1, 4096], a null pointer, a non-finite weight, a finalized or a head-only handle. */
+int mtb_set_latent_recombination(mtb_handle* h, const float* weights, int n_latents, int n_out);
+/* Joints per crop that mtb_forward / mtb_forward_host* / mtb_forward_sharded write: n_out after
+ * mtb_set_latent_recombination, cfg.n_joints otherwise (0 for a null handle). */
+int mtb_output_joints(const mtb_handle* h);
+/* tfu3d.linear_combine_points (metrabs_tf/tfu3d.py:48-49), handle-free: points [batch,n_in,3] and weights [n_in,n_out]
+ * (device, fp32) -> out [batch,n_out,3] = einsum('bjc,jJ->bJc').  fp32 FMA over the n_in points in ascending order, the
+ * kernel the forward of a latent-point model runs.  n_in <= 4096, n_out <= 4096. */
+int mtb_linear_combine_points(const float* points, int batch, int n_in, const float* weights, int n_out, float* out,
+                              void* stream);
+
 size_t mtb_workspace_bytes(const mtb_handle* h, int batch);
 /* Elements per crop of the feature map [H*W*C] and its spatial side, after finalize. */
 int mtb_feature_shape(const mtb_handle* h, int* hw_side, int* channels);
@@ -143,7 +162,8 @@ int mtb_reconstruct_absolute(mtb_handle* h, const float* coords2d, const float* 
                              const float* intrinsics, int batch, float* coords3d_abs, void* scratch,
                              void* stream);
 
-/* Metrabs.forward (models/metrabs.py:47-64): crops [B,3,S,S] fp32 + intrinsics [B,3,3] fp32 -> [B,J,3] fp32. */
+/* Metrabs.forward (models/metrabs.py:47-64): crops [B,3,S,S] fp32 + intrinsics [B,3,3] fp32 -> [B,J,3] fp32
+ * (J = mtb_output_joints(h)). */
 int mtb_forward(mtb_handle* h, const float* crops, const float* intrinsics, int batch, float* coords3d_abs,
                 void* workspace, size_t workspace_bytes, void* stream);
 

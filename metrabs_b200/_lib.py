@@ -71,6 +71,9 @@ _SIGNATURES = {
     'mtb_version': (C.c_char_p, []),
     'mtb_load_weight': (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int, C.POINTER(C.c_int64), C.c_int]),
     'mtb_finalize_weights': (C.c_int, [C.c_void_p]),
+    'mtb_set_latent_recombination': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
+    'mtb_output_joints': (C.c_int, [C.c_void_p]),
+    'mtb_linear_combine_points': (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     'mtb_workspace_bytes': (C.c_size_t, [C.c_void_p, C.c_int]),
     'mtb_feature_shape': (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     'mtb_backbone_forward': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t,

@@ -470,4 +470,29 @@ __global__ void __launch_bounds__(128) recon_pass2_kernel(ReconParams p) {
   }
 }
 
+// tfu3d.linear_combine_points (metrabs_tf/tfu3d.py:48-49): out[b,J',c] = sum_l pts[b,l,c] * w[l,J'].  Grid (B, ceil(n_out/128)),
+// 128 threads; the CTA stages its crop's [L,3] points in shared memory (dynamic, L*3 floats), each thread owns one output point
+// and accumulates in fp32 with l ascending, reading w[l*n_out + j] coalesced across the warp.
+__global__ void __launch_bounds__(128) combine_points_kernel(const float* __restrict__ pts, const float* __restrict__ w,
+                                                             float* __restrict__ out, int L, int n_out) {
+  extern __shared__ float sp[];
+  const int b = blockIdx.x;
+  const float* src = pts + (size_t)b * L * 3;
+  for (int i = threadIdx.x; i < L * 3; i += blockDim.x) sp[i] = src[i];
+  __syncthreads();
+  const int j = blockIdx.y * blockDim.x + threadIdx.x;
+  if (j >= n_out) return;
+  float x = 0.f, y = 0.f, z = 0.f;
+  for (int l = 0; l < L; ++l) {
+    const float wl = __ldg(w + (size_t)l * n_out + j);
+    x = fmaf(sp[l * 3 + 0], wl, x);
+    y = fmaf(sp[l * 3 + 1], wl, y);
+    z = fmaf(sp[l * 3 + 2], wl, z);
+  }
+  float* o = out + ((size_t)b * n_out + j) * 3;
+  o[0] = x;
+  o[1] = y;
+  o[2] = z;
+}
+
 }  // namespace mtb

@@ -35,11 +35,13 @@ enum DwKernel { DW_GENERIC = 0, DW_TMA = 1, DW_STRIP_BF16 = 2, DW_STRIP_F32 = 3 
 // kernel classes for the CUDA-event profiler (mtb_profile_begin / mtb_profile_end)
 enum KClass { KC_STEM = 0, KC_IGEMM_SIMT = 1, KC_DWCONV = 2, KC_POOL = 3, KC_SE_FC = 4, KC_TC_GEMM = 5, KC_FMB = 6,
               KC_HEAD_FUSED = 7, KC_HEAD_CONV_SIMT = 8, KC_SOFTARGMAX = 9, KC_RECON = 10, KC_OTHER = 11, KC_SE_SCALE = 12, KC_TC32 = 13,
-              KC_COUNT = 14 };
+              KC_COMBINE = 14, KC_COUNT = 15 };
 const char* kKClassNames[KC_COUNT] = {"stem_conv_kernel", "conv_igemm_kernel", "dwconv_kernel", "pool_mean_kernel",
                                       "se_fc(conv_igemm_kernel)", "tc_conv_kernel", "fmb_kernel",
                                       "tc_head_softargmax_kernel", "head_conv(conv_igemm_kernel)",
-                                      "softargmax_bhwn_kernel", "recon_pass1+2_kernel", "other", "se_scale_kernel", "tc32_conv_kernel"};
+                                      "softargmax_bhwn_kernel", "recon_pass1+2_kernel", "other", "se_scale_kernel", "tc32_conv_kernel",
+                                      "combine_points_kernel"};
+constexpr int kMaxCombinePoints = 4096;  // n_in and n_out of combine_points_kernel (its shared memory holds n_in * 3 floats)
 enum { BUF_FEATURES = -2, BUF_NONE = -1, BUF_SMALL0 = 4 };  // 0..3 big activation buffers, 4..6 small [B,C]
 constexpr int kNumBig = 4, kNumSmall = 3;
 constexpr int kPoolSlices = 8;  // the fused depthwise+pool kernel leaves up to 8 partial slices [slice][B][C]
@@ -89,6 +91,11 @@ struct mtb_handle {
   std::map<std::string, HostTensor> raw;
   std::vector<Op> ops;
   Op head;
+  // latent-point model (mtb_set_latent_recombination): the forward reconstructs head points [0, n_latents) and maps them to
+  // n_out joints with recomb [n_latents][n_out]; n_latents == 0 for a plain model
+  int n_latents = 0, n_out = 0;
+  std::vector<float> recomb;
+  float* d_recomb = nullptr;  // device copy in the weight arena (uploaded by mtb_finalize_weights)
   bool finalized = false;
   mutable std::string err;
   std::vector<void*> dev_allocs;
@@ -163,6 +170,15 @@ int fail(const mtb_handle* h, int code, const char* fmt, ...) {
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 inline bool is_bf16(const mtb_handle* h) { return h->cfg.precision == MTB_PRECISION_BF16_TC || h->cfg.precision == MTB_PRECISION_BF16_SIMT; }
 inline size_t elem_size(const mtb_handle* h) { return is_bf16(h) ? 2 : 4; }
+// points the head decodes and the reconstruction solves for: the latents of a latent-point model, cfg.n_joints otherwise
+inline int head_points(const mtb_handle* h) { return h->n_latents > 0 ? h->n_latents : h->cfg.n_joints; }
+inline int output_joints(const mtb_handle* h) { return h->n_latents > 0 ? h->n_out : h->cfg.n_joints; }
+// head channel count (1 + D per point) padded to a multiple of 4 with zero weights (J=122: 1098 -> 1100), and its FLOPs
+inline void size_head(mtb_handle* h) {
+  Op& hd = h->head;
+  hd.Cout = (head_points(h) * (1 + h->cfg.depth) + 3) / 4 * 4;
+  hd.flops = 2.0 * hd.Hout * hd.Wout * hd.Cin * hd.Cout;
+}
 
 // ------------------------------------------------------------------------------------------- plan building
 struct Planner {
@@ -519,9 +535,8 @@ int plan(mtb_handle* h) {
   hd.biaskey = hd.name + ".bias";
   hd.Hin = hd.Win = hd.Hout = hd.Wout = h->feat_side;
   hd.Cin = h->feat_c;
-  hd.Cout = (c.n_joints * (1 + c.depth) + 3) / 4 * 4;  // channels padded to a multiple of 4 with zero weights (J=122: 1098 -> 1100)
   hd.act = ACT_NONE;
-  hd.flops = 2.0 * hd.Hout * hd.Wout * hd.Cin * hd.Cout;
+  size_head(h);
   return MTB_OK;
 }
 
@@ -607,7 +622,7 @@ int prepare_op_weights(mtb_handle* h, Op& op) {
 struct Workspace {
   char* base;
   size_t big_stride, small_stride;
-  size_t off_small, off_features, off_logits, off_c2d, off_c3d, off_n2d, off_partial, total;
+  size_t off_small, off_features, off_logits, off_c2d, off_c3d, off_n2d, off_partial, off_latents, total;
 };
 
 Workspace layout(const mtb_handle* h, int B, void* base) {
@@ -620,12 +635,15 @@ Workspace layout(const mtb_handle* h, int B, void* base) {
   w.off_small = o; o += w.small_stride * kNumSmall;
   const size_t P = (size_t)h->feat_side * h->feat_side;
   w.off_features = o; o += align_up(P * h->feat_c * B * es, 1024);
-  const int N = (h->cfg.n_joints * (1 + h->cfg.depth) + 3) / 4 * 4;
+  const size_t J = (size_t)head_points(h);
+  const int N = (int)((J * (1 + h->cfg.depth) + 3) / 4 * 4);
   w.off_logits = o; o += align_up(std::max<size_t>(P, 4) * N * B * 4, 1024);  // also the fused head's state scratch
-  w.off_c2d = o; o += align_up((size_t)B * h->cfg.n_joints * 2 * 4, 1024);
-  w.off_c3d = o; o += align_up((size_t)B * h->cfg.n_joints * 3 * 4, 1024);
-  w.off_n2d = o; o += align_up((size_t)B * h->cfg.n_joints * 2 * 4, 1024);
+  w.off_c2d = o; o += align_up((size_t)B * J * 2 * 4, 1024);
+  w.off_c3d = o; o += align_up((size_t)B * J * 3 * 4, 1024);
+  w.off_n2d = o; o += align_up((size_t)B * J * 2 * 4, 1024);
   w.off_partial = o; o += align_up((size_t)B * 2 * 8, 1024);
+  w.off_latents = o;  // latent-point model: absolute latents [B,L,3] between the reconstruction and the recombination
+  if (h->n_latents > 0) o += align_up((size_t)B * J * 3 * 4, 1024);
   w.total = o;
   return w;
 }
@@ -952,11 +970,12 @@ int head_decode_impl(mtb_handle* h, const void* features, int B, float* c2d, flo
   const Op& op = h->head;
   const double P = (double)h->feat_side * h->feat_side;
   const double feat_bytes = (double)B * P * op.Cin * elem_size(h);
-  const double out_bytes = (double)B * c.n_joints * 5 * 4;
+  const int J = head_points(h);
+  const double out_bytes = (double)B * J * 5 * 4;
   if (op.tc.ready) {
     // fused: 1x1-conv GEMM on the tensor cores with the soft-argmax reduction in the epilogue; logits never reach HBM
     ProfScope prof(h, KC_HEAD_FUSED, op.flops * B, feat_bytes + (double)op.Cin * op.Cout * 2 + out_bytes, st);
-    const char* e = tc_head_launch(op.tc, features, B, h->feat_side, h->feat_side, c.n_joints, c.depth, make_scale(c),
+    const char* e = tc_head_launch(op.tc, features, B, h->feat_side, h->feat_side, J, c.depth, make_scale(c),
                                    c2d, c3d, ws.base + ws.off_logits, st);
     if (e) return fail(h, MTB_ERR_CUDA, "fused head: %s", e);
     h->launches += 2;
@@ -981,7 +1000,7 @@ int head_decode_impl(mtb_handle* h, const void* features, int B, float* c2d, flo
   }
   if (e != cudaSuccess) return fail(h, MTB_ERR_CUDA, "head conv: %s", cudaGetErrorString(e));
   ProfScope prof(h, KC_SOFTARGMAX, 0.0, logit_bytes + out_bytes, st);
-  int rc = launch_softargmax_bhwn<float>(p.out, c2d, c3d, B, c.n_joints, c.depth, op.Hin, op.Win, op.Cout, make_scale(c), st);
+  int rc = launch_softargmax_bhwn<float>(p.out, c2d, c3d, B, J, c.depth, op.Hin, op.Win, op.Cout, make_scale(c), st);
   if (rc) return fail(h, MTB_ERR_CUDA, "softargmax: %s", cudaGetErrorString((cudaError_t)rc));
   h->launches += 2;
   return MTB_OK;
@@ -992,19 +1011,45 @@ int recon_impl(mtb_handle* h, const float* c2d, const float* c3d, const float* K
   const mtb_config& c = h->cfg;
   ReconParams p;
   p.c2d = c2d; p.c3d = c3d; p.K = K; p.out = out; p.partial = partial; p.n2d = n2d;
-  p.B = B; p.J = c.n_joints;
+  p.B = B; p.J = head_points(h);
   float offset = c.centered_stride ? 0.f : -(float)c.stride_train / 2.f;  // is_within_fov (ptu3d.py:113-121)
   p.fov_lower = (float)c.stride_train * 0.75f + offset;
   p.fov_upper = (float)c.proc_side - (float)c.stride_train * 0.75f + offset;
   p.use_mix = c.mix_3d_inside_fov >= 0.f;
   p.mix = c.mix_3d_inside_fov;
-  ProfScope prof(h, KC_RECON, 0.0, (double)B * c.n_joints * 8 * 4 + (double)B * 36, st);
+  ProfScope prof(h, KC_RECON, 0.0, (double)B * p.J * 8 * 4 + (double)B * 36, st);
   launch_k(recon_pass1_kernel, dim3(B), dim3(128), 0, st, p);
   launch_k(recon_pass2_kernel, dim3(B), dim3(128), 0, st, p);
   h->launches += 2;
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(h, MTB_ERR_CUDA, "reconstruct: %s", cudaGetErrorString(e));
   return MTB_OK;
+}
+
+// points [B,L,3] @ w [L,n_out] -> out [B,n_out,3] (combine_points_kernel; the forward and mtb_linear_combine_points)
+int launch_combine(const float* pts, int B, int L, const float* w, int n_out, float* out, cudaStream_t st) {
+  launch_k(combine_points_kernel, dim3(B, (n_out + 127) / 128), dim3(128), (size_t)L * 3 * sizeof(float), st, pts, w, out, L,
+           n_out);
+  return (int)cudaGetLastError();
+}
+
+// the recombination of a latent-point model: absolute latents [B,L,3] -> joints [B,n_out,3]
+int combine_impl(mtb_handle* h, const float* latents, int B, float* out, cudaStream_t st) {
+  const double L = h->n_latents, n = h->n_out;
+  ProfScope prof(h, KC_COMBINE, 2.0 * B * L * n * 3, (double)B * (L + n) * 3 * 4 + L * n * 4, st);
+  int e = launch_combine(latents, B, h->n_latents, h->d_recomb, h->n_out, out, st);
+  h->launches += 1;
+  if (e) return fail(h, MTB_ERR_CUDA, "combine points: %s", cudaGetErrorString((cudaError_t)e));
+  return MTB_OK;
+}
+
+// reconstruction into the caller's output, or (latent-point model) into `latents` and then recombined into the output
+int recon_and_combine(mtb_handle* h, const float* c2d, const float* c3d, const float* K, int B, float* out, float* n2d,
+                      double* partial, float* latents, cudaStream_t st) {
+  if (h->n_latents == 0) return recon_impl(h, c2d, c3d, K, B, out, n2d, partial, st);
+  int rc = recon_impl(h, c2d, c3d, K, B, latents, n2d, partial, st);
+  if (rc) return rc;
+  return combine_impl(h, latents, B, out, st);
 }
 
 __global__ void to_float_kernel(const __nv_bfloat16* in, float* out, size_t n) {
@@ -1197,11 +1242,35 @@ int mtb_finalize_weights(mtb_handle* h) {
     Op& hd = h->head;
     const HostTensor* w = find(h, hd.wkey);
     if (!w) return fail(h, MTB_ERR_MISSING_WEIGHT, "missing weight '%s'", hd.wkey.c_str());
-    const int n_real = h->cfg.n_joints * (1 + h->cfg.depth);
-    if (w->shape.size() != 4 || w->shape[0] != n_real || w->shape[1] != hd.Cin)
-      return fail(h, MTB_ERR_INVALID_ARG, "'%s' must be [%d,%d,1,1]", hd.wkey.c_str(), n_real, hd.Cin);
+    const int n_raw = h->cfg.n_joints, D = h->cfg.depth;
+    if (w->shape.size() != 4 || w->shape[0] != n_raw * (1 + D) || w->shape[1] != hd.Cin)
+      return fail(h, MTB_ERR_INVALID_ARG, "'%s' must be [%d,%d,1,1]", hd.wkey.c_str(), n_raw * (1 + D), hd.Cin);
     const HostTensor* hb = find(h, hd.biaskey);
-    if (!hb || (int)hb->data.size() != n_real) return fail(h, MTB_ERR_MISSING_WEIGHT, "missing weight '%s'", hd.biaskey.c_str());
+    if (!hb || (int)hb->data.size() != n_raw * (1 + D))
+      return fail(h, MTB_ERR_MISSING_WEIGHT, "missing weight '%s'", hd.biaskey.c_str());
+    const int P = head_points(h);
+    if (P < n_raw) {
+      // predict_all_and_latents: the forward reconstructs only points [0, P) (models/metrabs.py:53-55), so keep just their
+      // channels - 2D row j and 3D row n_raw + d*n_raw + j - repacked as a P-point head (channel P + d*P + j).  Every
+      // channel is an independent dot product, so this is the reference computation minus the discarded points.
+      HostTensor ws, bs;
+      ws.shape = {(int64_t)P * (1 + D), hd.Cin, 1, 1};
+      bs.shape = {(int64_t)P * (1 + D)};
+      ws.data.resize((size_t)P * (1 + D) * hd.Cin);
+      bs.data.resize((size_t)P * (1 + D));
+      for (int d = -1; d < D; ++d)
+        for (int j = 0; j < P; ++j) {
+          const size_t src = d < 0 ? (size_t)j : (size_t)n_raw + (size_t)d * n_raw + j;
+          const size_t dst = d < 0 ? (size_t)j : (size_t)P + (size_t)d * P + j;
+          std::copy_n(w->data.begin() + src * hd.Cin, hd.Cin, ws.data.begin() + dst * hd.Cin);
+          bs.data[dst] = hb->data[src];
+        }
+      h->raw[hd.wkey] = std::move(ws);
+      h->raw[hd.biaskey] = std::move(bs);
+      w = find(h, hd.wkey);
+      hb = find(h, hd.biaskey);
+    }
+    const int n_real = P * (1 + D);
     if (n_real != hd.Cout) {  // zero-pad the output channels
       HostTensor wp = *w, bp = *hb;
       wp.data.resize((size_t)hd.Cout * hd.Cin, 0.f);
@@ -1228,8 +1297,45 @@ int mtb_finalize_weights(mtb_handle* h) {
       }
     }
   }
+  h->d_recomb = nullptr;
+  if (h->n_latents > 0) {
+    int rc = upload(h, h->recomb.data(), h->recomb.size() * sizeof(float), (void**)&h->d_recomb);
+    if (rc) return rc;
+  }
   h->raw.clear();
   h->finalized = true;
+  return MTB_OK;
+}
+
+int mtb_set_latent_recombination(mtb_handle* h, const float* weights, int n_latents, int n_out) {
+  if (!h) return fail(nullptr, MTB_ERR_INVALID_ARG, "null handle");
+  if (!weights) return fail(h, MTB_ERR_INVALID_ARG, "null recombination weights");
+  if (h->finalized)
+    return fail(h, MTB_ERR_INVALID_ARG, "the latent recombination must be set before mtb_finalize_weights (load the weights again first)");
+  if (h->cfg.arch == MTB_ARCH_HEAD_ONLY) return fail(h, MTB_ERR_INVALID_ARG, "a head-only handle has no forward to recombine");
+  if (n_latents < 1 || n_latents > h->cfg.n_joints)
+    return fail(h, MTB_ERR_INVALID_ARG, "n_latents must be in [1, %d] (the head's points), got %d", h->cfg.n_joints, n_latents);
+  if (n_out < 1 || n_out > kMaxCombinePoints)
+    return fail(h, MTB_ERR_INVALID_ARG, "n_out must be in [1, %d], got %d", kMaxCombinePoints, n_out);
+  const size_t n = (size_t)n_latents * n_out;
+  for (size_t i = 0; i < n; ++i)
+    if (!std::isfinite(weights[i])) return fail(h, MTB_ERR_INVALID_ARG, "recombination weight %zu is not finite", i);
+  h->recomb.assign(weights, weights + n);
+  h->n_latents = n_latents;
+  h->n_out = n_out;
+  size_head(h);
+  return MTB_OK;
+}
+
+int mtb_output_joints(const mtb_handle* h) { return h ? output_joints(h) : 0; }
+
+int mtb_linear_combine_points(const float* points, int batch, int n_in, const float* weights, int n_out, float* out, void* stream) {
+  if (!points || !weights || !out) return fail(nullptr, MTB_ERR_INVALID_ARG, "null argument");
+  if (batch <= 0 || n_in < 1 || n_in > kMaxCombinePoints || n_out < 1 || n_out > kMaxCombinePoints)
+    return fail(nullptr, MTB_ERR_INVALID_ARG, "invalid sizes (batch=%d n_in=%d n_out=%d; n_in and n_out must be in [1, %d])", batch,
+                n_in, n_out, kMaxCombinePoints);
+  int e = launch_combine(points, batch, n_in, weights, n_out, out, (cudaStream_t)stream);
+  if (e) return fail(nullptr, MTB_ERR_CUDA, "combine points launch: %s", cudaGetErrorString((cudaError_t)e));
   return MTB_OK;
 }
 
@@ -1332,7 +1438,7 @@ int mtb_reconstruct_absolute(mtb_handle* h, const float* coords2d, const float* 
   if (!h) return fail(nullptr, MTB_ERR_INVALID_ARG, "null handle");
   if (!coords2d || !coords3d_rel || !intrinsics || !coords3d_abs || !scratch || batch <= 0)
     return fail(h, MTB_ERR_INVALID_ARG, "null/invalid argument");
-  if (h->cfg.n_joints > 4096) return fail(h, MTB_ERR_UNSUPPORTED, "more than 4096 joints");
+  if (head_points(h) > 4096) return fail(h, MTB_ERR_UNSUPPORTED, "more than 4096 joints");
   DeviceGuard g(h->cfg.device);
   h->launches = 0;
   double* partial = (double*)scratch;
@@ -1352,8 +1458,8 @@ static int forward_body(mtb_handle* h, const float* crops, const float* intrinsi
   float* c3d = (float*)(ws.base + ws.off_c3d);
   rc = head_decode_impl(h, features, batch, c2d, c3d, ws, st);
   if (rc) return rc;
-  return recon_impl(h, c2d, c3d, intrinsics, batch, coords3d_abs, (float*)(ws.base + ws.off_n2d),
-                    (double*)(ws.base + ws.off_partial), st);
+  return recon_and_combine(h, c2d, c3d, intrinsics, batch, coords3d_abs, (float*)(ws.base + ws.off_n2d),
+                           (double*)(ws.base + ws.off_partial), (float*)(ws.base + ws.off_latents), st);
 }
 
 // mtb_forward captures its own launches into a CUDA graph the second time it sees the same (buffers, batch, stream) and
@@ -1454,7 +1560,7 @@ int mtb_forward_host(mtb_handle* h, const float* host_crops, const float* host_i
   cudaStream_t st = (cudaStream_t)stream;
   const size_t S = h->cfg.proc_side;
   const size_t crops_b = align_up((size_t)batch * 3 * S * S * 4, 1024), k_b = align_up((size_t)batch * 9 * 4, 1024),
-               out_b = align_up((size_t)batch * h->cfg.n_joints * 3 * 4, 1024);
+               out_b = align_up((size_t)batch * output_joints(h) * 3 * 4, 1024);
   const size_t ws_b = layout(h, batch, nullptr).total;
   const size_t need = crops_b + k_b + out_b + ws_b;
   if (need > h->stage_bytes) {  // grows only when a larger batch than ever before arrives
@@ -1476,7 +1582,7 @@ int mtb_forward_host(mtb_handle* h, const float* host_crops, const float* host_i
   CUDA_TRY(h, cudaMemcpyAsync(d_k, host_intrinsics, (size_t)batch * 9 * 4, cudaMemcpyHostToDevice, st));
   int rc = mtb_forward(h, d_crops, d_k, batch, d_out, d_ws, ws_b, stream);
   if (rc) return rc;
-  CUDA_TRY(h, cudaMemcpyAsync(host_coords3d_abs, d_out, (size_t)batch * h->cfg.n_joints * 3 * 4, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(h, cudaMemcpyAsync(host_coords3d_abs, d_out, (size_t)batch * output_joints(h) * 3 * 4, cudaMemcpyDeviceToHost, st));
   CUDA_TRY(h, cudaStreamSynchronize(st));
   return MTB_OK;
 }
@@ -1491,7 +1597,7 @@ int mtb_forward_host_submit(mtb_handle* h, const float* host_crops, const float*
   cudaStream_t st = (cudaStream_t)stream;
   const size_t S = h->cfg.proc_side;
   const size_t crops_b = align_up((size_t)batch * 3 * S * S * 4, 1024), k_b = align_up((size_t)batch * 9 * 4, 1024),
-               out_b = align_up((size_t)batch * h->cfg.n_joints * 3 * 4, 1024);
+               out_b = align_up((size_t)batch * output_joints(h) * 3 * 4, 1024);
   const size_t ws_b = layout(h, batch, nullptr).total;
   mtb_handle::HostSlot& sl = h->slots[slot];
   if (!h->copy_stream) CUDA_TRY(h, cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking));
@@ -1528,7 +1634,7 @@ int mtb_forward_host_submit(mtb_handle* h, const float* host_crops, const float*
   CUDA_TRY(h, cudaStreamWaitEvent(st, sl.h2d_done, 0));
   int rc = mtb_forward(h, d_crops, d_k, batch, d_out, h->pipe_ws, h->pipe_ws_bytes, stream);
   if (rc) return rc;
-  CUDA_TRY(h, cudaMemcpyAsync(host_coords3d_abs, d_out, (size_t)batch * h->cfg.n_joints * 3 * 4, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(h, cudaMemcpyAsync(host_coords3d_abs, d_out, (size_t)batch * output_joints(h) * 3 * 4, cudaMemcpyDeviceToHost, st));
   CUDA_TRY(h, cudaEventRecord(sl.done, st));
   sl.used = true;
   return MTB_OK;
@@ -1692,9 +1798,9 @@ int mtb_filter_poses(const mtb_filter_args* a, void* stream) {
 // batch-global RMS scalars (ptu3d.py:71-74), so only a full-batch solve reproduces the unsharded result exactly.
 size_t mtb_sharded_scratch_bytes(const mtb_handle* h, int batch_local) {
   if (!h || batch_local <= 0 || h->nccl_world <= 0) return 0;
-  const size_t J = (size_t)h->cfg.n_joints, bl = (size_t)batch_local, bt = bl * (size_t)h->nccl_world;
+  const size_t J = (size_t)head_points(h), bl = (size_t)batch_local, bt = bl * (size_t)h->nccl_world;
   return align_up(bl * J * 5 * 4, 256) + align_up(bt * J * 5 * 4, 256) + align_up(bt * J * 2 * 4, 256) + align_up(bt * J * 3 * 4, 256) +
-         align_up(bt * J * 2 * 4, 256) + align_up(bt * 2 * 8, 256);
+         align_up(bt * J * 2 * 4, 256) + align_up(bt * 2 * 8, 256) + (h->n_latents > 0 ? align_up(bt * J * 3 * 4, 256) : 0);
 }
 
 int mtb_forward_sharded(mtb_handle* h, const float* crops_local, int batch_local, const float* intrinsics_all, float* coords3d_abs_all,
@@ -1706,14 +1812,15 @@ int mtb_forward_sharded(mtb_handle* h, const float* crops_local, int batch_local
   if (h->ops.empty()) return fail(h, MTB_ERR_UNSUPPORTED, "this handle has no backbone (head-only)");
   DeviceGuard g(h->cfg.device);
   cudaStream_t st = (cudaStream_t)stream;
-  const size_t J = (size_t)h->cfg.n_joints, bl = (size_t)batch_local, bt = bl * (size_t)h->nccl_world;
+  const size_t J = (size_t)head_points(h), bl = (size_t)batch_local, bt = bl * (size_t)h->nccl_world;
   char* sp = (char*)scratch;
   float* packed_local = (float*)sp; sp += align_up(bl * J * 5 * 4, 256);
   float* packed_all = (float*)sp;   sp += align_up(bt * J * 5 * 4, 256);
   float* c2d_all = (float*)sp;      sp += align_up(bt * J * 2 * 4, 256);
   float* c3d_all = (float*)sp;      sp += align_up(bt * J * 3 * 4, 256);
   float* n2d = (float*)sp;          sp += align_up(bt * J * 2 * 4, 256);
-  double* partial = (double*)sp;
+  double* partial = (double*)sp;    sp += align_up(bt * 2 * 8, 256);
+  float* latents = (float*)sp;      // [bt,L,3], latent-point models only
   h->launches = 0;
   Workspace ws = layout(h, batch_local, workspace);
   void* features = ws.base + ws.off_features;
@@ -1731,8 +1838,8 @@ int mtb_forward_sharded(mtb_handle* h, const float* crops_local, int batch_local
   launch_k(unpack_decoded_kernel, dim3(grid_for(bt * J, 256)), dim3(256), 0, st, (const float*)packed_all, c2d_all, c3d_all, (int)(bt * J));
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(h, MTB_ERR_CUDA, "pack/unpack launch: %s", cudaGetErrorString(e));
-  rc = recon_impl(h, c2d_all, c3d_all, intrinsics_all, (int)bt, coords3d_abs_all, n2d, partial, st);
-  h->launches = before + 3 + 2;  // pack, all-gather, unpack, reconstruction passes
+  rc = recon_and_combine(h, c2d_all, c3d_all, intrinsics_all, (int)bt, coords3d_abs_all, n2d, partial, latents, st);
+  h->launches = before + 3 + 2 + (h->n_latents > 0 ? 1 : 0);  // pack, all-gather, unpack, reconstruction passes, recombination
   return rc;
 }
 

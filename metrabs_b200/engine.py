@@ -69,6 +69,7 @@ class Engine:
         check(lib().mtb_feature_shape(self._h, C.byref(hw), C.byref(ch)), self._h)
         self.feature_side, self.feature_channels = hw.value, ch.value
         self.n_joints, self.depth = mtb_config.n_joints, mtb_config.depth
+        self._recombination = None  # (host fp32 [L, n_out] weights, device copy) of a latent-point model
         self.feature_dtype = (torch.float32 if mtb_config.precision in (_lib.PRECISION_FP32, _lib.PRECISION_TF32X3)
                               else torch.bfloat16)
 
@@ -85,6 +86,33 @@ class Engine:
             pass
 
     # ---- weights ------------------------------------------------------------------------------------
+    def set_latent_recombination(self, weights):
+        """Makes this a latent-point model (transform_coords / predict_all_and_latents): the forward reconstructs head
+        points [0, L) and maps them to n_out joints, ``joints = einsum('blc,lJ->bJc', latents, weights)`` with
+        ``weights`` [L, n_out].  Takes effect at the next load_state_dict (mtb_set_latent_recombination precedes every
+        mtb_finalize_weights)."""
+        w = torch.as_tensor(weights, dtype=torch.float32).detach().to('cpu').contiguous()
+        if w.ndim != 2:
+            raise ValueError(f'recombination weights must be [n_latents, n_out], got shape {tuple(w.shape)}')
+        self._recombination = (w, w.to(self.device))
+
+    @property
+    def n_points(self):
+        """Points the head decodes and the reconstruction solves for (the latents of a latent-point model)."""
+        return self.n_joints if self._recombination is None else self._recombination[0].shape[0]
+
+    @property
+    def n_out(self):
+        """Joints per crop of forward / forward_host* / forward_sharded (mtb_output_joints)."""
+        return int(lib().mtb_output_joints(self._h))
+
+    def combine_latents(self, points):
+        """Absolute latents [B, L, 3] -> joints [B, n_out, 3] on the device (the forward's recombination); the identity
+        for a model without one."""
+        if self._recombination is None:
+            return points
+        return linear_combine_points(points, self._recombination[1])
+
     def load_state_dict(self, state_dict):
         """One mtb_load_weight per entry (reference key schema), then fold/repack/upload."""
         for name, t in state_dict.items():
@@ -94,6 +122,9 @@ class Engine:
             shape = (C.c_int64 * max(t.ndim, 1))(*t.shape)
             check(lib().mtb_load_weight(self._h, name.encode(), C.c_void_p(t.data_ptr()), _DTYPES[t.dtype], shape,
                                         t.ndim), self._h)
+        if self._recombination is not None:
+            w = self._recombination[0]
+            check(lib().mtb_set_latent_recombination(self._h, C.c_void_p(w.data_ptr()), w.shape[0], w.shape[1]), self._h)
         check(lib().mtb_finalize_weights(self._h), self._h)
 
     # ---- buffers --------------------------------------------------------------------------------------
@@ -128,8 +159,8 @@ class Engine:
         b = features_nhwc.shape[0]
         f = self._check_in(features_nhwc, (b, self.feature_side, self.feature_side, self.feature_channels),
                            self.feature_dtype)
-        c2d = torch.empty(b, self.n_joints, 2, dtype=torch.float32, device=self.device)
-        c3d = torch.empty(b, self.n_joints, 3, dtype=torch.float32, device=self.device)
+        c2d = torch.empty(b, self.n_points, 2, dtype=torch.float32, device=self.device)
+        c3d = torch.empty(b, self.n_points, 3, dtype=torch.float32, device=self.device)
         ws = self.workspace(b)
         check(lib().mtb_head_decode(self._h, f.data_ptr(), b, c2d.data_ptr(), c3d.data_ptr(), ws.data_ptr(),
                                     ws.numel(), _stream_ptr(self.device)), self._h)
@@ -137,10 +168,10 @@ class Engine:
 
     def reconstruct_absolute(self, coords2d, coords3d_rel, intrinsics):
         b = coords2d.shape[0]
-        c2d = self._check_in(coords2d, (b, self.n_joints, 2))
-        c3d = self._check_in(coords3d_rel, (b, self.n_joints, 3))
+        c2d = self._check_in(coords2d, (b, self.n_points, 2))
+        c3d = self._check_in(coords3d_rel, (b, self.n_points, 3))
         k = self._check_in(intrinsics, (b, 3, 3))
-        out = torch.empty(b, self.n_joints, 3, dtype=torch.float32, device=self.device)
+        out = torch.empty(b, self.n_points, 3, dtype=torch.float32, device=self.device)
         need = lib().mtb_reconstruct_scratch_bytes(b)
         if self._scratch is None or self._scratch.numel() < need:
             self._scratch = torch.empty(need, dtype=torch.uint8, device=self.device)
@@ -153,7 +184,7 @@ class Engine:
         crops = self._check_in(crops, (b, 3, s, s))
         k = self._check_in(intrinsics, (b, 3, 3))
         if out is None:
-            out = torch.empty(b, self.n_joints, 3, dtype=torch.float32, device=self.device)
+            out = torch.empty(b, self.n_out, 3, dtype=torch.float32, device=self.device)
         ws = self.workspace(b)
         check(lib().mtb_forward(self._h, crops.data_ptr(), k.data_ptr(), b, out.data_ptr(), ws.data_ptr(), ws.numel(),
                                 _stream_ptr(self.device)), self._h)
@@ -184,7 +215,7 @@ class Engine:
         crops_host = crops_host.contiguous().float()
         intrinsics_host = intrinsics_host.contiguous().float()
         if out_host is None:
-            out_host = torch.empty(b, self.n_joints, 3, dtype=torch.float32).pin_memory()
+            out_host = torch.empty(b, self.n_out, 3, dtype=torch.float32).pin_memory()
         check(lib().mtb_forward_host(self._h, crops_host.data_ptr(), intrinsics_host.data_ptr(), b,
                                      out_host.data_ptr(), _stream_ptr(self.device)), self._h)
         return out_host
@@ -222,7 +253,7 @@ class Engine:
         crops_local = self._check_in(crops_local, (b, 3, s, s))
         k = self._check_in(intrinsics_all, (self.world_size * b, 3, 3))
         if out is None:
-            out = torch.empty(self.world_size * b, self.n_joints, 3, dtype=torch.float32, device=self.device)
+            out = torch.empty(self.world_size * b, self.n_out, 3, dtype=torch.float32, device=self.device)
         need = lib().mtb_sharded_scratch_bytes(self._h, b)
         if getattr(self, '_sh_scratch', None) is None or self._sh_scratch.numel() < need:
             self._sh_scratch = torch.empty(need, dtype=torch.uint8, device=self.device)
@@ -328,6 +359,27 @@ class Engine:
     @property
     def backbone_flops_per_crop(self):
         return float(lib().mtb_backbone_flops_per_crop(self._h))
+
+
+def linear_combine_points(points, weights):
+    """tfu3d.linear_combine_points on the device (mtb_linear_combine_points): points [B, n_in, 3] and weights
+    [n_in, n_out], CUDA tensors on one device -> [B, n_out, 3] = einsum('bjc,jJ->bJc') in fp32."""
+    if not points.is_cuda or not weights.is_cuda:
+        raise _lib.MetrabsB200Error('linear_combine_points needs CUDA tensors (no CPU fallback)')
+    if points.device != weights.device:
+        raise ValueError(f'points on {points.device}, weights on {weights.device}')
+    if points.ndim != 3 or points.shape[-1] != 3 or weights.ndim != 2 or weights.shape[0] != points.shape[1]:
+        raise ValueError(f'expected points [B, n, 3] and weights [n, n_out], got {tuple(points.shape)} and '
+                         f'{tuple(weights.shape)}')
+    points = points.float().contiguous()
+    weights = weights.float().contiguous()
+    out = torch.empty(points.shape[0], weights.shape[1], 3, dtype=torch.float32, device=points.device)
+    if points.shape[0] == 0:
+        return out
+    with torch.cuda.device(points.device):
+        check(lib().mtb_linear_combine_points(points.data_ptr(), points.shape[0], points.shape[1], weights.data_ptr(),
+                                              weights.shape[1], out.data_ptr(), _stream_ptr(points.device)))
+    return out
 
 
 def soft_argmax_device(logits, layout, n_joints, depth, height, width):

@@ -5,7 +5,8 @@ decode, so rank r processes the contiguous chunk ``shard_range(B, world, r)`` wi
 exchange is ONE all-gather per forward.  Because ``reconstruct_ref_fullpersp`` normalises with batch-global RMS
 scalars (ptu3d.py:71-74), the gathered tensor is ``[coords2d | coords3d_rel]`` (5 floats per joint) and every rank
 runs the (tiny) absolute reconstruction on the full batch: the sharded result is then identical to the unsharded
-reference, not merely within tolerance.  Chunk order = rank order, so the gather is a plain concatenation."""
+reference, not merely within tolerance.  Chunk order = rank order, so the gather is a plain concatenation.  A
+latent-point model gathers and reconstructs its latents and maps them to joints after the reconstruction."""
 import torch
 
 
@@ -45,7 +46,8 @@ class ShardedMetrabs:
     """Runs ``model`` (metrabs_b200.models.metrabs.Metrabs) data-parallel: every rank passes the FULL flat crop batch
     (or just its own chunk with ``presharded=True``) and gets the full [B,J,3] result.  ``engine`` (optional) replaces
     ``model.engine(device)``: any object with ``n_joints``, ``backbone``, ``head_decode``, ``allgather``,
-    ``reconstruct_absolute`` (and optionally ``forward_sharded``) - the CPU tests drive the host logic through it."""
+    ``reconstruct_absolute`` (and optionally ``forward_sharded``, and ``n_points`` / ``combine_latents`` for a
+    latent-point model) - the CPU tests drive the host logic through it."""
 
     def __init__(self, model, rank, world_size, engine=None):
         self.model, self.rank, self.world, self._engine = model, rank, world_size, engine
@@ -65,11 +67,14 @@ class ShardedMetrabs:
         if local.shape[0] == 0:
             # fewer crops than ranks (e.g. 3 person-crops on 8 GPUs): this rank has nothing to compute but must still
             # take part in the collective
-            packed_local = torch.zeros((0, eng.n_joints, 5), dtype=torch.float32, device=crops.device)
+            packed_local = torch.zeros((0, getattr(eng, 'n_points', eng.n_joints), 5), dtype=torch.float32,
+                                       device=crops.device)
         else:
             feats = eng.backbone(local)
             c2d, c3d = eng.head_decode(feats)
             packed_local = pack_decoded(c2d, c3d)
         packed = gather_decoded(packed_local, n_total, self.world, lambda t: eng.allgather(t).clone())
         g2d, g3d = unpack_decoded(packed)
-        return eng.reconstruct_absolute(g2d, g3d, intrinsics)
+        out = eng.reconstruct_absolute(g2d, g3d, intrinsics)
+        combine = getattr(eng, 'combine_latents', None)
+        return combine(out) if combine is not None else out

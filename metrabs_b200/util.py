@@ -20,6 +20,7 @@ class Config:
     affine_weights: Optional[str] = None
     transform_coords: bool = False
     predict_all_and_latents: bool = False
+    regularize_to_manifold: bool = False
     # build-specific: arithmetic of the conv kernels ('fp32' parity mode or 'bf16' tensor-core throughput mode)
     precision: str = 'fp32'
 
