@@ -57,7 +57,14 @@ typedef enum { MTB_PRECISION_FP32 = 0, MTB_PRECISION_BF16_TC = 1,
                /* the 1e-3 parity mode ON TENSOR CORES: fp32 storage, every conv/GEMM as three wgmma tf32
                 * products of hi/lo-split operands (a_hi*b_hi + a_lo*b_hi + a_hi*b_lo) with fp32 accumulation in registers;
                 * conv outputs agree with the fp32 FMA chain to ~1e-6 */
-               MTB_PRECISION_TF32X3 = 3 } mtb_precision;
+               MTB_PRECISION_TF32X3 = 3,
+               /* the reference's deployment arithmetic (fp16 autocast, multiperson_model.py:240-242) on tensor cores: fp16
+                * activations in HBM, fp16-rounded GEMM weights, wgmma .f32.f16.f16 with fp32 accumulation in registers;
+                * outputs round to nearest even and overflow to inf (no saturation), as under autocast */
+               MTB_PRECISION_F16_TC = 4,
+               /* verification mode: same fp16 storage and fp16-rounded weights as F16_TC, but every conv on CUDA cores
+                * (fp32 FMA) - what BF16_SIMT is for BF16_TC */
+               MTB_PRECISION_F16_SIMT = 5 } mtb_precision;
 
 /* Layout of a logits tensor handed to the standalone soft-argmax. */
 typedef enum {
@@ -139,7 +146,7 @@ size_t mtb_workspace_bytes(const mtb_handle* h, int batch);
 int mtb_feature_shape(const mtb_handle* h, int* hw_side, int* channels);
 
 /* self.backbone(image) (models/metrabs.py:50): crops fp32 NCHW [B,3,S,S] in [0,1] -> features NHWC
- * [B,S/s,S/s,C] (fp32, or bf16 in BF16_TC mode). */
+ * [B,S/s,S/s,C]: fp32 in FP32 / TF32X3 mode, bf16 in BF16_TC / BF16_SIMT, fp16 in F16_TC / F16_SIMT. */
 int mtb_backbone_forward(mtb_handle* h, const float* crops, int batch, void* features, void* workspace,
                          size_t workspace_bytes, void* stream);
 
@@ -296,12 +303,12 @@ int mtb_op_output_shape(const mtb_handle* h, int op, int* height, int* width, in
 int mtb_op_input_shape(const mtb_handle* h, int op, int* height, int* width, int* channels, int* has_residual,
                        int* has_scale);
 /* Runs ONE backbone op in isolation on caller-provided fp32 NHWC device tensors (converted to the handle's
- * storage type): in [B,Hin,Win,Cin] (the stem takes NCHW crops), optional residual [B,Hout,Wout,Cout] and
+ * storage type - fp32, or bf16 / fp16 rounded to nearest even): in [B,Hin,Win,Cin] (the stem takes NCHW crops), optional residual [B,Hout,Wout,Cout] and
  * squeeze-excitation scale [B,Cin]; out receives [B,Hout,Wout,Cout] as fp32.  Lets tests compare the tensor-core
  * kernels with the CUDA-core kernels on identical inputs. */
 int mtb_debug_run_op(mtb_handle* h, int op_index, const float* in, const float* res, const float* scale, int batch,
                      float* out, size_t out_floats, void* workspace, size_t workspace_bytes, void* stream);
-/* FusedMBConv block fusion (bf16 tensor-core mode): 1 when backbone op `op_index` (a 3x3 stride-1 expand conv) and the op
+/* FusedMBConv block fusion (BF16_TC and F16_TC modes): 1 when backbone op `op_index` (a 3x3 stride-1 expand conv) and the op
  * after it (the 1x1 projection, + residual) run as ONE fmb_kernel launch (reference block:
  * metrabs_pytorch/backbones/efficientnet.py:176-234).  mtb_debug_run_fused_block runs that pair in isolation on a
  * caller-provided fp32 NHWC device tensor `in` [B,H,W,Cin] (also the residual when the block has one); `out` receives the
@@ -318,7 +325,7 @@ int mtb_profile_end(mtb_handle* h, double* ms, double* flops, double* bytes, int
 /* Per-op view of the last profiling window: device ms per backbone op, its algorithmic FLOPs and bytes per crop and
  * its kernel class; arrays hold mtb_num_ops() entries. */
 int mtb_profile_op_times(const mtb_handle* h, double* ms, double* flops_per_crop, double* bytes_per_crop, int* cls, int n);
-/* Weight bytes the op reads once per launch (bf16 on the tensor-core path, fp32 otherwise); `bytes_per_crop` above counts
+/* Weight bytes the op reads once per launch (bf16 / fp16 on the tensor-core path, fp32 otherwise); `bytes_per_crop` above counts
  * activations (input + output + residual) only, so a launch on B crops moves B * bytes_per_crop + weight bytes. */
 double mtb_op_weight_bytes(const mtb_handle* h, int op);
 int mtb_num_kernel_classes(void);

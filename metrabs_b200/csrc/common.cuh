@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
 #include <utility>
 
 namespace mtb {
@@ -72,7 +73,7 @@ __device__ __forceinline__ void act_dispatch(int act, F&& f) {
   }
 }
 
-// ---- 4-wide vector load/store for fp32 and bf16 activation storage -------------------------------------
+// ---- 4-wide vector load/store for fp32, bf16 and fp16 activation storage -------------------------------------
 template <typename T>
 __device__ __forceinline__ float4 load4(const T* p);
 template <>
@@ -87,11 +88,26 @@ __device__ __forceinline__ float4 load4<__nv_bfloat16>(const __nv_bfloat16* p) {
   float2 fa = __bfloat1622float2(a), fb = __bfloat1622float2(b);
   return make_float4(fa.x, fa.y, fb.x, fb.y);
 }
+template <>
+__device__ __forceinline__ float4 load4<__half>(const __half* p) {
+  uint2 u = *reinterpret_cast<const uint2*>(p);
+  float2 fa = __half22float2(*reinterpret_cast<__half2*>(&u.x)), fb = __half22float2(*reinterpret_cast<__half2*>(&u.y));
+  return make_float4(fa.x, fa.y, fb.x, fb.y);
+}
 template <typename T>
 __device__ __forceinline__ void store4(T* p, float4 v);
 template <>
 __device__ __forceinline__ void store4<float>(float* p, float4 v) {
   *reinterpret_cast<float4*>(p) = v;
+}
+template <>
+__device__ __forceinline__ void store4<__half>(__half* p, float4 v) {
+  __half2 a = __floats2half2_rn(v.x, v.y);
+  __half2 b = __floats2half2_rn(v.z, v.w);
+  uint2 u;
+  u.x = *reinterpret_cast<uint32_t*>(&a);
+  u.y = *reinterpret_cast<uint32_t*>(&b);
+  *reinterpret_cast<uint2*>(p) = u;
 }
 template <>
 __device__ __forceinline__ void store4<__nv_bfloat16>(__nv_bfloat16* p, float4 v) {
@@ -116,6 +132,38 @@ template <>
 __device__ __forceinline__ void store1<float>(float* p, float v) { *p = v; }
 template <>
 __device__ __forceinline__ void store1<__nv_bfloat16>(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
+template <>
+__device__ __forceinline__ void store1<__half>(__half* p, float v) { *p = __float2half_rn(v); }
+
+// ---- 16-bit activation storage (bf16 or fp16): packed pairs, rounded to nearest even (fp16 overflow gives inf) -----------
+template <typename T>
+struct Pair16;
+template <>
+struct Pair16<__nv_bfloat16> {
+  typedef __nv_bfloat162 type;
+  static __device__ __forceinline__ type pack(float a, float b) { return __floats2bfloat162_rn(a, b); }
+  static __device__ __forceinline__ float2 unpack(type v) { return __bfloat1622float2(v); }
+};
+template <>
+struct Pair16<__half> {
+  typedef __half2 type;
+  static __device__ __forceinline__ type pack(float a, float b) { return __floats2half2_rn(a, b); }
+  static __device__ __forceinline__ float2 unpack(type v) { return __half22float2(v); }
+};
+template <typename T>
+constexpr bool is_f16 = std::is_same<T, __half>::value;
+
+// SiLU of the fp16 kernels: x * rcp(1 + 2^(-x log2 e)) with ex2.approx and rcp.approx, ~2 fp32 ulps of error.  Cost: two MUFU
+// ops and three FP32 ops per element, against one MUFU op and two FP32 ops for the bf16 kernels' h + h * tanh.approx(h)
+// (h = x / 2), whose ~2^-11 relative error is below a bf16 ulp but a whole fp16 ulp (and far more relative to the small
+// outputs of negative x).  The .ftz forms skip the denormal fix-ups __expf / __fdividef add: a flushed 2^(-x log2 e) (x > 87)
+// gives x, a flushed reciprocal (x < -87) gives -0, both what the exact value rounds to in fp16.
+__device__ __forceinline__ float silu_f16out(float x) {
+  float e, r;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(x * -1.4426950408889634f));
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + e));
+  return x * r;
+}
 
 // fp32 pairs: kernels written against two-wide arithmetic (f2_fma / f2_mul / f2_add).  Each half is the scalar IEEE
 // fma / mul / add with round-to-nearest (__fmaf_rn etc. are never contracted or reassociated), so a kernel using them is

@@ -257,7 +257,7 @@ __global__ void __launch_bounds__(256) dwconv_kernel(ConvParams p) {
 }
 
 // ----------------------------------------------------------------------------------------------------------
-// depthwise 3x3 (+ stride 2) + bias + activation + squeeze-excitation pooling, bf16 NHWC, 8 channels x 4 output
+// depthwise 3x3 (+ stride 2) + bias + activation + squeeze-excitation pooling, bf16 or fp16 NHWC, 8 channels x 4 output
 // pixels per thread: every input column vector is loaded once per row and reused by the outputs it feeds
 // (18 / 27 16-byte loads per 4 outputs instead of 36), and the per-channel sums of the SE squeeze are reduced in the
 // block and stored (already divided by Hout*Wout) as partial slice pooled[blockIdx.y][b][c]; the consumer (fc1) sums the
@@ -269,9 +269,12 @@ __device__ __forceinline__ float fast_tanh(float x) {
   asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-template <int ACT>
-__device__ __forceinline__ float fast_act(float x) {  // compile-time activation; SiLU with one MUFU op (bf16 outputs)
-  if constexpr (ACT == ACT_SILU) {
+// compile-time activation; SiLU with one MUFU op for bf16 outputs, silu_f16out (two) for fp16 outputs
+template <int ACT, typename T = __nv_bfloat16>
+__device__ __forceinline__ float fast_act(float x) {
+  if constexpr (ACT == ACT_SILU && is_f16<T>) {
+    return silu_f16out(x);
+  } else if constexpr (ACT == ACT_SILU) {
     float h = 0.5f * x;
     return fmaf(h, fast_tanh(h), h);
   } else if constexpr (ACT == ACT_RELU) {
@@ -283,12 +286,23 @@ __device__ __forceinline__ float fast_act(float x) {  // compile-time activation
   }
 }
 
-template <int STRIDE, int ACT, int OW = 4>
-__global__ void __launch_bounds__(256, OW == 2 ? 3 : 2) dwconv3x3_pool_bf16_kernel(ConvParams p, float* __restrict__ pooled) {
-  // OW outputs per thread along W
+// one packed word of two 16-bit elements -> fp32 pair.  bf16 widens with a 16-bit shift / mask (one ALU op per element);
+// fp16 needs a real conversion (HADD2.F32 / F2F per pair).
+template <typename T>
+__device__ __forceinline__ f32x2 unpack2_16b(unsigned w) {
+  if constexpr (is_f16<T>) {
+    return __half22float2(*reinterpret_cast<const __half2*>(&w));
+  } else {
+    return f2_pack(__uint_as_float(w << 16), __uint_as_float(w & 0xffff0000u));
+  }
+}
+
+template <typename T, int STRIDE, int ACT, int OW = 4>
+__global__ void __launch_bounds__(256, OW == 2 ? 3 : 2) dwconv3x3_pool_16b_kernel(ConvParams p, float* __restrict__ pooled) {
+  // OW outputs per thread along W; T: element type (__nv_bfloat16 or __half)
   constexpr int NCOL = (OW - 1) * STRIDE + 3;    // input columns feeding them
-  const __nv_bfloat16* __restrict__ in = reinterpret_cast<const __nv_bfloat16*>(p.in);
-  __nv_bfloat16* __restrict__ out = reinterpret_cast<__nv_bfloat16*>(p.out);
+  const T* __restrict__ in = reinterpret_cast<const T*>(p.in);
+  T* __restrict__ out = reinterpret_cast<T*>(p.out);
   const int C = p.Cout;
   const int cv = blockIdx.x * 32 + threadIdx.x;  // channel vector (8 channels)
   const int c = cv * 8;
@@ -336,14 +350,10 @@ __global__ void __launch_bounds__(256, OW == 2 ? 3 : 2) dwconv3x3_pool_bf16_kern
       }
 #pragma unroll
       for (int x = 0; x < NCOL; ++x) {
-        // bf16 -> fp32 is a 16-bit shift / mask of the packed words: one ALU op per element
         const unsigned wd[4] = {raw[x].x, raw[x].y, raw[x].z, raw[x].w};
         float v[8];
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          v[2 * k] = __uint_as_float(wd[k] << 16);
-          v[2 * k + 1] = __uint_as_float(wd[k] & 0xffff0000u);
-        }
+        for (int k = 0; k < 4; ++k) f2_unpack(unpack2_16b<T>(wd[k]), v[2 * k], v[2 * k + 1]);
 #pragma unroll
         for (int i = 0; i < OW; ++i) {
           const int s_ = x - i * STRIDE;  // compile-time after unrolling
@@ -354,16 +364,16 @@ __global__ void __launch_bounds__(256, OW == 2 ? 3 : 2) dwconv3x3_pool_bf16_kern
         }
       }
     }
-    __nv_bfloat16* orow = out + ((size_t)(b * p.Hout + oh) * p.Wout + ow0) * C + c;
+    T* orow = out + ((size_t)(b * p.Hout + oh) * p.Wout + ow0) * C + c;
 #pragma unroll
     for (int i = 0; i < OW; ++i) {
       if (ow0 + i >= p.Wout) continue;
       uint4 ov;
-      __nv_bfloat162* o2 = reinterpret_cast<__nv_bfloat162*>(&ov);
+      typename Pair16<T>::type* o2 = reinterpret_cast<typename Pair16<T>::type*>(&ov);
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
-        float a0 = fast_act<ACT>(acc[i][2 * k]), a1 = fast_act<ACT>(acc[i][2 * k + 1]);
-        o2[k] = __floats2bfloat162_rn(a0, a1);
+        float a0 = fast_act<ACT, T>(acc[i][2 * k]), a1 = fast_act<ACT, T>(acc[i][2 * k + 1]);
+        o2[k] = Pair16<T>::pack(a0, a1);
         psum[2 * k] += a0;
         psum[2 * k + 1] += a1;
       }

@@ -1,7 +1,7 @@
-// Depthwise 3x3 stride-1 conv + bias + activation + squeeze-excitation pooling for bf16 NHWC tensors (the MBConv middle
+// Depthwise 3x3 stride-1 conv + bias + activation + squeeze-excitation pooling for bf16 or fp16 NHWC tensors (the MBConv middle
 // op, backbones/efficientnet.py:110-173), staged through shared memory by TMA.
 //
-// Why: the strip kernel (dwconv3x3_pool_bf16_kernel) ran at ~2 TB/s whatever the batch (so not HBM-bound): every thread
+// Why: the strip kernel (dwconv3x3_pool_16b_kernel) ran at ~2 TB/s whatever the batch (so not HBM-bound): every thread
 // lived for ONE strip - one global-load round trip, then compute, then a block reduction - and nothing overlapped the
 // load latency.  Here a persistent CTA walks (crop group, 64-channel group, row band) items; the (rows+2) x (W+2) x 64ch
 // input patch of the NEXT item is in flight (one 4D TMA box, out-of-image halo = TMA zero fill = the reference's explicit
@@ -22,7 +22,7 @@ constexpr int DWT_MAX_STAGE = 52 * 1024;
 constexpr int DWT_MAX_G = 8;
 
 struct DwTmaParams {
-  void* out;           // bf16 NHWC
+  void* out;           // bf16 / fp16 NHWC
   const float* w;      // [9][C] fp32 (BN folded)
   const float* bias;   // [C]
   float* pooled;       // [n_rb][B][C] partial means (nullptr: no squeeze-excitation behind this op)
@@ -68,8 +68,9 @@ inline DwTmaPlan dw_tma_plan(int H, int W) {
   return best;
 }
 
-// rank-4 bf16 NHWC tensor [B][H][W][C]; box = 64 channels (128 bytes) x (W+2) x (BH+2) x G, no swizzle (quarter-warps read
+// rank-4 16-bit NHWC tensor [B][H][W][C]; box = 64 channels (128 bytes) x (W+2) x (BH+2) x G, no swizzle (quarter-warps read
 // whole 128-byte pixel rows: conflict-free as is)
+template <typename T>
 inline const char* make_tmap_dw(CUtensorMap* m, const void* ptr, uint64_t B, uint64_t H, uint64_t W, uint64_t C, uint32_t pw,
                                 uint32_t ph, uint32_t g) {
   tmap_encode_fn enc = get_tmap_encode();
@@ -78,16 +79,21 @@ inline const char* make_tmap_dw(CUtensorMap* m, const void* ptr, uint64_t B, uin
   cuuint64_t strides[3] = {C * 2, W * C * 2, H * W * C * 2};
   cuuint32_t box[4] = {DWT_CG, pw, ph, g};
   cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, estr,
+  CUresult r = enc(m, tmap_dtype<T>(), 4, const_cast<void*>(ptr), dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? nullptr : "cuTensorMapEncodeTiled(dw) failed";
 }
 
-// activation of a pair; SiLU(x) = h + h * tanh(h), h = x / 2 (same arithmetic as fast_act<ACT_SILU>)
-template <int ACT>
+// activation of a pair; SiLU(x) = h + h * tanh(h), h = x / 2 for bf16 outputs, silu_f16out for fp16 ones (same arithmetic as
+// fast_act<ACT_SILU, T>)
+template <int ACT, typename T>
 __device__ __forceinline__ f32x2 f2_act(f32x2 x) {
-  if constexpr (ACT == ACT_SILU) {
+  if constexpr (ACT == ACT_SILU && is_f16<T>) {
+    float x0, x1;
+    f2_unpack(x, x0, x1);
+    return f2_pack(silu_f16out(x0), silu_f16out(x1));
+  } else if constexpr (ACT == ACT_SILU) {
     const f32x2 h = f2_mul(x, f2_pack(0.5f, 0.5f));
     float h0, h1;
     f2_unpack(h, h0, h1);
@@ -95,12 +101,12 @@ __device__ __forceinline__ f32x2 f2_act(f32x2 x) {
   } else {
     float x0, x1;
     f2_unpack(x, x0, x1);
-    return f2_pack(fast_act<ACT>(x0), fast_act<ACT>(x1));
+    return f2_pack(fast_act<ACT, T>(x0), fast_act<ACT, T>(x1));
   }
 }
 
-// 64 channels per item, 8 per thread (4 fp32 pairs), tanh.approx SiLU
-template <int ACT>
+// 64 channels per item, 8 per thread (4 fp32 pairs); T: element type (__nv_bfloat16 or __half)
+template <typename T, int ACT>
 __global__ void __launch_bounds__(DWT_THREADS, 2)
 dw3x3s1_tma_kernel(const __grid_constant__ CUtensorMap tmIn, const DwTmaParams p) {
   constexpr int NV = 4;                    // fp32 pairs per thread
@@ -190,7 +196,7 @@ dw3x3s1_tma_kernel(const __grid_constant__ CUtensorMap tmIn, const DwTmaParams p
         const int rows_run = min(DWT_RUN, rows_item - orow0);   // >= 1 by construction of `bands`
         if (b < p.B && rows_run > 0) {
           const uint8_t* prow = patch + (size_t)((g * PHB + orow0) * PW + ow0) * 128;
-          __nv_bfloat16* obase = reinterpret_cast<__nv_bfloat16*>(p.out) + ((size_t)(b * p.H + row0 + orow0) * p.W + ow0) * p.C + c;
+          T* obase = reinterpret_cast<T*>(p.out) + ((size_t)(b * p.H + row0 + orow0) * p.W + ow0) * p.C + c;
           f32x2 acc[3][DWT_OW][NV];
 #pragma unroll
           for (int pr = 0; pr < DWT_RUN + 2; ++pr) {
@@ -203,7 +209,7 @@ dw3x3s1_tma_kernel(const __grid_constant__ CUtensorMap tmIn, const DwTmaParams p
                 const unsigned wd[4] = {raw.x, raw.y, raw.z, raw.w};
                 f32x2 v[NV];
 #pragma unroll
-                for (int k = 0; k < NV; ++k) v[k] = f2_pack(__uint_as_float(wd[k] << 16), __uint_as_float(wd[k] & 0xffff0000u));
+                for (int k = 0; k < NV; ++k) v[k] = unpack2_16b<T>(wd[k]);
 #pragma unroll
                 for (int r = 0; r < 3; ++r) {
                   const int o = pr - r;  // compile-time
@@ -222,18 +228,18 @@ dw3x3s1_tma_kernel(const __grid_constant__ CUtensorMap tmIn, const DwTmaParams p
               // output row pr - 2 is complete
               if (pr >= 2 && pr - 2 < rows_run) {
                 const int o = pr - 2, slot = o % 3;
-                __nv_bfloat16* orow = obase + (size_t)o * p.W * p.C;
+                T* orow = obase + (size_t)o * p.W * p.C;
 #pragma unroll
                 for (int i = 0; i < DWT_OW; ++i) {
                   if (ow0 + i < p.W) {
                     uint4 ov;
-                    __nv_bfloat162* o2 = reinterpret_cast<__nv_bfloat162*>(&ov);
+                    typename Pair16<T>::type* o2 = reinterpret_cast<typename Pair16<T>::type*>(&ov);
 #pragma unroll
                     for (int k = 0; k < NV; ++k) {
-                      const f32x2 a = f2_act<ACT>(acc[slot][i][k]);
+                      const f32x2 a = f2_act<ACT, T>(acc[slot][i][k]);
                       float a0, a1;
                       f2_unpack(a, a0, a1);
-                      o2[k] = __floats2bfloat162_rn(a0, a1);
+                      o2[k] = Pair16<T>::pack(a0, a1);
                       psum[k] = f2_add(psum[k], a);
                     }
                     *reinterpret_cast<uint4*>(orow + (size_t)i * p.C) = ov;
@@ -278,6 +284,7 @@ struct DwTmaCache {
   int B = -1;
 };
 
+template <typename T>
 inline const char* dw_tma_launch(DwTmaCache& cache, const DwTmaPlan& plan, const void* in, void* out, const float* w, const float* bias,
                                  float* pooled, int B, int H, int W, int C, int pad_t, int pad_l, int act, cudaStream_t st) {
   DwTmaParams p;
@@ -293,7 +300,7 @@ inline const char* dw_tma_launch(DwTmaCache& cache, const DwTmaPlan& plan, const
   p.stage_bytes = 128 * (W + 2) * (plan.BH + 2) * plan.G;
   p.inv_hw = 1.0f / (float)(H * W);
   if (cache.in != in || cache.B != B) {
-    const char* e = make_tmap_dw(&cache.map, in, (uint64_t)B, (uint64_t)H, (uint64_t)W, (uint64_t)C, (uint32_t)(W + 2),
+    const char* e = make_tmap_dw<T>(&cache.map, in, (uint64_t)B, (uint64_t)H, (uint64_t)W, (uint64_t)C, (uint32_t)(W + 2),
                                  (uint32_t)(plan.BH + 2), (uint32_t)plan.G);
     if (e) return e;
     cache.in = in;
@@ -306,12 +313,12 @@ inline const char* dw_tma_launch(DwTmaCache& cache, const DwTmaPlan& plan, const
   {                                                                                                                        \
     static bool attr_set = false;                                                                                          \
     if (!attr_set) {                                                                                                       \
-      if (cudaFuncSetAttribute(dw3x3s1_tma_kernel<A>, cudaFuncAttributeMaxDynamicSharedMemorySize,                          \
+      if (cudaFuncSetAttribute(dw3x3s1_tma_kernel<T, A>, cudaFuncAttributeMaxDynamicSharedMemorySize,                          \
                                DWT_STAGES * DWT_MAX_STAGE + 128 + 8 * 128) != cudaSuccess)                                 \
         return "cannot raise dynamic shared memory for dw3x3s1_tma_kernel";                                                \
       attr_set = true;                                                                                                     \
     }                                                                                                                      \
-    launch_k(dw3x3s1_tma_kernel<A>, dim3(grid), dim3(DWT_THREADS), smem, st, cache.map, p);                                 \
+    launch_k(dw3x3s1_tma_kernel<T, A>, dim3(grid), dim3(DWT_THREADS), smem, st, cache.map, p);                                 \
   }
   switch (act) {
     case ACT_SILU: MTB_DWT_LAUNCH(ACT_SILU); break;

@@ -30,8 +30,8 @@ namespace {
 std::string g_error;
 
 enum OpType { OP_STEM = 0, OP_CONV = 1, OP_DW = 2, OP_POOL = 3, OP_MAXPOOL = 4 };
-// depthwise kernels: TMA-staged (dw_tma.cuh), bf16 / fp32 strip (SE pooling fused), generic (dwconv_kernel)
-enum DwKernel { DW_GENERIC = 0, DW_TMA = 1, DW_STRIP_BF16 = 2, DW_STRIP_F32 = 3 };
+// depthwise kernels: TMA-staged (dw_tma.cuh), 16-bit (bf16 / fp16) or fp32 strip (SE pooling fused), generic (dwconv_kernel)
+enum DwKernel { DW_GENERIC = 0, DW_TMA = 1, DW_STRIP_16B = 2, DW_STRIP_F32 = 3 };
 // kernel classes for the CUDA-event profiler (mtb_profile_begin / mtb_profile_end)
 enum KClass { KC_STEM = 0, KC_IGEMM_SIMT = 1, KC_DWCONV = 2, KC_POOL = 3, KC_SE_FC = 4, KC_TC_GEMM = 5, KC_FMB = 6,
               KC_HEAD_FUSED = 7, KC_HEAD_CONV_SIMT = 8, KC_SOFTARGMAX = 9, KC_RECON = 10, KC_OTHER = 11, KC_SE_SCALE = 12, KC_TC32 = 13,
@@ -76,9 +76,9 @@ struct Op {
   float bn_eps = 1e-3f;
   float* d_w = nullptr;     // fp32 [R*S*Cin][Cout]  (dw: [R*S][C])
   float* d_bias = nullptr;  // fp32 [Cout]
-  TcWeights tc;             // bf16 K-major copy + TMA descriptor state for the wgmma path
+  TcWeights tc;             // 16-bit (bf16 / fp16) K-major copy + TMA descriptor state for the wgmma path
   Tc32Weights tc32;         // fp32 K-major copy + TMA descriptor state for the 3xTF32 wgmma path (MTB_PRECISION_TF32X3)
-  FmbWeights fmb;           // bf16 mode: this 3x3 expand conv and the NEXT op (1x1 projection) run as one fmb_kernel launch
+  FmbWeights fmb;           // 16-bit tensor-core modes: this 3x3 expand conv and the NEXT op (1x1 projection) run as one fmb_kernel launch
   mutable DwTmaCache dw_cache;  // input tensor map of the TMA-staged depthwise kernel
   double flops = 0;         // 2*MACs per crop
   int stage = 0;            // EfficientNet stage (1-based; 0 = stem / last conv / other backbones)
@@ -168,8 +168,32 @@ int fail(const mtb_handle* h, int code, const char* fmt, ...) {
   } while (0)
 
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
-inline bool is_bf16(const mtb_handle* h) { return h->cfg.precision == MTB_PRECISION_BF16_TC || h->cfg.precision == MTB_PRECISION_BF16_SIMT; }
-inline size_t elem_size(const mtb_handle* h) { return is_bf16(h) ? 2 : 4; }
+// element type of the activations in HBM: bf16 (BF16_TC / BF16_SIMT), fp16 (F16_TC / F16_SIMT) or fp32 (FP32 / TF32X3)
+enum Storage { ST_F32 = 0, ST_BF16 = 1, ST_F16 = 2 };
+inline Storage storage(const mtb_handle* h) {
+  switch (h->cfg.precision) {
+    case MTB_PRECISION_BF16_TC:
+    case MTB_PRECISION_BF16_SIMT: return ST_BF16;
+    case MTB_PRECISION_F16_TC:
+    case MTB_PRECISION_F16_SIMT: return ST_F16;
+    default: return ST_F32;
+  }
+}
+inline bool is_16b(const mtb_handle* h) { return storage(h) != ST_F32; }
+inline size_t elem_size(const mtb_handle* h) { return is_16b(h) ? 2 : 4; }
+// the wgmma modes with 16-bit operands (bf16 or fp16): tc_conv_kernel, fmb_kernel, tc_head_kernel, the TMA depthwise kernel
+inline bool is_tc16(const mtb_handle* h) {
+  return h->cfg.precision == MTB_PRECISION_BF16_TC || h->cfg.precision == MTB_PRECISION_F16_TC;
+}
+// calls f((T*)nullptr) with T the storage element type of the handle's mode
+template <typename F>
+int with_storage(const mtb_handle* h, F&& f) {
+  switch (storage(h)) {
+    case ST_BF16: return f((__nv_bfloat16*)nullptr);
+    case ST_F16: return f((__half*)nullptr);
+    default: return f((float*)nullptr);
+  }
+}
 // points the head decodes and the reconstruction solves for: the latents of a latent-point model, cfg.n_joints otherwise
 inline int head_points(const mtb_handle* h) { return h->n_latents > 0 ? h->n_latents : h->cfg.n_joints; }
 inline int output_joints(const mtb_handle* h) { return h->n_latents > 0 ? h->n_out : h->cfg.n_joints; }
@@ -600,14 +624,17 @@ int prepare_op_weights(mtb_handle* h, Op& op) {
         }
   }
   const bool tc_like = tc_eligible(op.type == OP_CONV, op.depthwise, op.small_io, op.R, op.stride, op.Cin, op.Cout);
-  if (is_bf16(h) && tc_like)  // both bf16 modes see the same bf16-rounded GEMM weights
+  if (storage(h) == ST_BF16 && tc_like)  // both bf16 modes see the same bf16-rounded GEMM weights
     for (float& v : wk) v = __bfloat162float(host_bf16(v));
+  if (storage(h) == ST_F16 && tc_like)  // both fp16 modes see the same fp16-rounded GEMM weights
+    for (float& v : wk) v = __half2float(host_f16(v));
   int rc = upload(h, wk.data(), wk.size() * 4, (void**)&op.d_w);
   if (rc) return rc;
   rc = upload(h, bias.data(), bias.size() * 4, (void**)&op.d_bias);
   if (rc) return rc;
-  if (h->cfg.precision == MTB_PRECISION_BF16_TC && tc_like) {
-    const char* e = tc_prepare_weights(op.tc, wk.data(), bias.data(), K, op.Cout, op.R, op.S, op.Cin, h->dev_allocs);
+  if (is_tc16(h) && tc_like) {
+    const char* e = storage(h) == ST_F16 ? tc_prepare_weights<__half>(op.tc, wk.data(), bias.data(), K, op.Cout, op.R, op.S, op.Cin, h->dev_allocs)
+                                         : tc_prepare_weights<__nv_bfloat16>(op.tc, wk.data(), bias.data(), K, op.Cout, op.R, op.S, op.Cin, h->dev_allocs);
     if (e) return fail(h, MTB_ERR_CUDA, "tensor-core weight prep for '%s': %s", op.name.c_str(), e);
   }
   if (h->cfg.precision == MTB_PRECISION_TF32X3 &&
@@ -685,21 +712,21 @@ struct ProfScope {
   }
 };
 
-// shapes covered by the strip depthwise kernels (dwconv3x3_pool_bf16_kernel / dwconv3x3_pool_f32_kernel)
+// shapes covered by the strip depthwise kernels (dwconv3x3_pool_16b_kernel / dwconv3x3_pool_f32_kernel)
 bool dw_strip_eligible(const Op& op) {
   return op.type == OP_DW && op.R == 3 && op.S == 3 && op.dil == 1 && op.Cout % 8 == 0 && (op.stride == 1 || op.stride == 2) &&
          (op.act == ACT_SILU || op.act == ACT_RELU || op.act == ACT_HSWISH);
 }
 
-constexpr int kDwOW = 4;  // outputs per thread along W in dwconv3x3_pool_bf16_kernel (measured: 4 -> 3.65 ms, 2 -> 4.25 ms per 128 crops)
+constexpr int kDwOW = 4;  // outputs per thread along W in dwconv3x3_pool_16b_kernel (measured: 4 -> 3.65 ms, 2 -> 4.25 ms per 128 crops)
 
-// Picks the kernel of a depthwise op and the number of partial pooling slices it writes (fc1 sums that many).  bf16
-// tensor-core mode: stride-1 ops run the TMA-staged kernel when a plan fits, the rest the bf16 strip kernel.  3xTF32 mode:
+// Picks the kernel of a depthwise op and the number of partial pooling slices it writes (fc1 sums that many).  bf16 and fp16
+// tensor-core modes: stride-1 ops run the TMA-staged kernel when a plan fits, the rest the 16-bit strip kernel.  3xTF32 mode:
 // the fp32 strip kernel (exact activation).  Other modes and shapes: the generic kernel, which does not pool.
 void choose_dw_kernel(const mtb_handle* h, Op& op) {
   op.dw_kernel = DW_GENERIC;
   if (!dw_strip_eligible(op)) return;
-  if (h->cfg.precision == MTB_PRECISION_BF16_TC) {
+  if (is_tc16(h)) {
     if (op.stride == 1 && op.Hin == op.Hout && op.Win == op.Wout) {
       const DwTmaPlan pl = dw_tma_plan(op.Hout, op.Wout);
       if (pl.ok && pl.n_rb <= kPoolSlices) {
@@ -709,7 +736,7 @@ void choose_dw_kernel(const mtb_handle* h, Op& op) {
         return;
       }
     }
-    op.dw_kernel = DW_STRIP_BF16;
+    op.dw_kernel = DW_STRIP_16B;
   } else if (h->cfg.precision == MTB_PRECISION_TF32X3) {
     op.dw_kernel = DW_STRIP_F32;
   } else {
@@ -758,17 +785,21 @@ bool stem_fast_enabled() {  // MTB_STEM_FAST=0: the generic stem kernel (A/B run
   return v == 1;
 }
 
+// T: the storage element type (float, __nv_bfloat16 or __half); the tensor-core and TMA kernels only exist for the 16-bit types
 template <typename T>
 int run_op_t(mtb_handle* h, const Op& op, const float* crops, int B, const Workspace& ws, void* features,
              cudaStream_t st) {
-  if (op.type == OP_CONV && op.tc.ready && op.scale_buf != BUF_NONE) {
-    // squeeze-excitation scale applied in place ahead of the bf16 tensor-core conv
-    void* x = buf_ptr(ws, op.in_buf, features);
-    const double bytes = 2.0 * B * op.Hin * op.Win * op.Cin * elem_size(h);
-    ProfScope ps(h, KC_SE_SCALE, 0.0, bytes, st, false);
-    const char* e = tc_se_scale_launch(x, (const float*)buf_ptr(ws, op.scale_buf, features), B, op.Hin * op.Win, op.Cin, st);
-    if (e) return fail(h, MTB_ERR_CUDA, "se scale %s: %s", op.name.c_str(), e);
-    h->launches++;
+  constexpr bool k16 = sizeof(T) == 2;
+  if constexpr (k16) {
+    if (op.type == OP_CONV && op.tc.ready && op.scale_buf != BUF_NONE) {
+      // squeeze-excitation scale applied in place ahead of the 16-bit tensor-core conv
+      void* x = buf_ptr(ws, op.in_buf, features);
+      const double bytes = 2.0 * B * op.Hin * op.Win * op.Cin * elem_size(h);
+      ProfScope ps(h, KC_SE_SCALE, 0.0, bytes, st, false);
+      const char* e = tc_se_scale_launch<T>(x, (const float*)buf_ptr(ws, op.scale_buf, features), B, op.Hin * op.Win, op.Cin, st);
+      if (e) return fail(h, MTB_ERR_CUDA, "se scale %s: %s", op.name.c_str(), e);
+      h->launches++;
+    }
   }
   ProfScope prof(h, op_class(op), op.flops * B, op_bytes(h, op, B), st);
   switch (op.type) {
@@ -806,21 +837,20 @@ int run_op_t(mtb_handle* h, const Op& op, const float* crops, int B, const Works
       p.res_first = op.res_first ? 1 : 0;
       if (op.type == OP_DW) {
         float* pooled = op.fused_pool ? (float*)buf_ptr(ws, BUF_SMALL0, features) : nullptr;
-        if (op.dw_kernel == DW_TMA) {
-          const char* e = dw_tma_launch(op.dw_cache, op.dw_plan, p.in, p.out, op.d_w, op.d_bias, pooled, B, op.Hout, op.Wout, op.Cout,
-                                        op.pad_t, op.pad_l, op.act, st);
-          if (e) return fail(h, MTB_ERR_CUDA, "depthwise (TMA) launch %s: %s", op.name.c_str(), e);
-        } else if (op.dw_kernel == DW_STRIP_BF16) {
-          dim3 grid((op.Cout / 8 + 31) / 32, op.pool_slices, B), block(32, 8);
-          if (op.act == ACT_SILU) {
-            if (op.stride == 1) launch_k(dwconv3x3_pool_bf16_kernel<1, ACT_SILU, kDwOW>, dim3(grid), dim3(block), 0, st, p, pooled);
-            else launch_k(dwconv3x3_pool_bf16_kernel<2, ACT_SILU, kDwOW>, dim3(grid), dim3(block), 0, st, p, pooled);
-          } else if (op.act == ACT_RELU) {
-            if (op.stride == 1) launch_k(dwconv3x3_pool_bf16_kernel<1, ACT_RELU, kDwOW>, dim3(grid), dim3(block), 0, st, p, pooled);
-            else launch_k(dwconv3x3_pool_bf16_kernel<2, ACT_RELU, kDwOW>, dim3(grid), dim3(block), 0, st, p, pooled);
+        if (op.dw_kernel == DW_TMA || op.dw_kernel == DW_STRIP_16B) {
+          if constexpr (!k16) {
+            return fail(h, MTB_ERR_CUDA, "depthwise %s: 16-bit kernel chosen for fp32 storage", op.name.c_str());
+          } else if (op.dw_kernel == DW_TMA) {
+            const char* e = dw_tma_launch<T>(op.dw_cache, op.dw_plan, p.in, p.out, op.d_w, op.d_bias, pooled, B, op.Hout, op.Wout,
+                                             op.Cout, op.pad_t, op.pad_l, op.act, st);
+            if (e) return fail(h, MTB_ERR_CUDA, "depthwise (TMA) launch %s: %s", op.name.c_str(), e);
           } else {
-            if (op.stride == 1) launch_k(dwconv3x3_pool_bf16_kernel<1, ACT_HSWISH, kDwOW>, dim3(grid), dim3(block), 0, st, p, pooled);
-            else launch_k(dwconv3x3_pool_bf16_kernel<2, ACT_HSWISH, kDwOW>, dim3(grid), dim3(block), 0, st, p, pooled);
+            dim3 grid((op.Cout / 8 + 31) / 32, op.pool_slices, B), block(32, 8);
+#define MTB_DW16(ST, AC) launch_k(dwconv3x3_pool_16b_kernel<T, ST, AC, kDwOW>, dim3(grid), dim3(block), 0, st, p, pooled)
+            if (op.act == ACT_SILU) { if (op.stride == 1) MTB_DW16(1, ACT_SILU); else MTB_DW16(2, ACT_SILU); }
+            else if (op.act == ACT_RELU) { if (op.stride == 1) MTB_DW16(1, ACT_RELU); else MTB_DW16(2, ACT_RELU); }
+            else { if (op.stride == 1) MTB_DW16(1, ACT_HSWISH); else MTB_DW16(2, ACT_HSWISH); }
+#undef MTB_DW16
           }
         } else if (op.dw_kernel == DW_STRIP_F32) {
           // fp32 strip kernel: 4 channels x 4 pixels per thread, SE squeeze fused (partial slices summed by fc1)
@@ -857,8 +887,11 @@ int run_op_t(mtb_handle* h, const Op& op, const float* crops, int B, const Works
         }
         if (e != cudaSuccess) return fail(h, MTB_ERR_CUDA, "launch %s: %s", op.name.c_str(), cudaGetErrorString(e));
       } else if (op.tc.ready) {
-        const char* e = tc_conv_launch(op.tc, p, op.res_first, st);
-        if (e) return fail(h, MTB_ERR_CUDA, "tensor-core launch %s: %s", op.name.c_str(), e);
+        if constexpr (!k16) return fail(h, MTB_ERR_CUDA, "%s: tensor-core weights in an fp32 mode", op.name.c_str());
+        else {
+          const char* e = tc_conv_launch<T>(op.tc, p, op.res_first, st);
+          if (e) return fail(h, MTB_ERR_CUDA, "tensor-core launch %s: %s", op.name.c_str(), e);
+        }
       } else if (op.tc32.ready) {
         const char* e = tc32_conv_launch(op.tc32, p, op.res_first, st);  // SE scale (p.a_scale) applied by the splitter warps
         if (e) return fail(h, MTB_ERR_CUDA, "3xTF32 launch %s: %s", op.name.c_str(), e);
@@ -884,8 +917,7 @@ int run_op_t(mtb_handle* h, const Op& op, const float* crops, int B, const Works
 
 int run_op(mtb_handle* h, const Op& op, const float* crops, int B, const Workspace& ws, void* features, cudaStream_t st) {
   if (op.type == OP_POOL && op.fused_pool) return MTB_OK;  // produced by the preceding depthwise kernel
-  if (is_bf16(h)) return run_op_t<__nv_bfloat16>(h, op, crops, B, ws, features, st);
-  return run_op_t<float>(h, op, crops, B, ws, features, st);
+  return with_storage(h, [&](auto* tag) { return run_op_t<std::remove_pointer_t<decltype(tag)>>(h, op, crops, B, ws, features, st); });
 }
 
 // The executor runs every op on the whole batch: running a stage crop chunk by crop chunk (intermediates resident in L2)
@@ -896,7 +928,8 @@ int run_fused_block(mtb_handle* h, const Op& a, const Op& b, int B, const Worksp
   void* out = buf_ptr(ws, b.out_buf, features);
   const double bytes = 2.0 * B * a.Hin * a.Win * (a.Cin + b.Cout) + 2.0 * (9.0 * a.Cin * a.Cout + (double)b.Cin * b.Cout);
   ProfScope prof(h, KC_FMB, (a.flops + b.flops) * B, bytes, st);
-  const char* e = fmb_launch(a.fmb, in, out, B, a.Hin, a.Win, a.pad_t, a.pad_l, b.res_buf != BUF_NONE, st);
+  const char* e = storage(h) == ST_F16 ? fmb_launch<__half>(a.fmb, in, out, B, a.Hin, a.Win, a.pad_t, a.pad_l, b.res_buf != BUF_NONE, st)
+                                       : fmb_launch<__nv_bfloat16>(a.fmb, in, out, B, a.Hin, a.Win, a.pad_t, a.pad_l, b.res_buf != BUF_NONE, st);
   if (e) return fail(h, MTB_ERR_CUDA, "fused FusedMBConv launch %s: %s", a.name.c_str(), e);
   h->launches++;
   return MTB_OK;
@@ -975,8 +1008,10 @@ int head_decode_impl(mtb_handle* h, const void* features, int B, float* c2d, flo
   if (op.tc.ready) {
     // fused: 1x1-conv GEMM on the tensor cores with the soft-argmax reduction in the epilogue; logits never reach HBM
     ProfScope prof(h, KC_HEAD_FUSED, op.flops * B, feat_bytes + (double)op.Cin * op.Cout * 2 + out_bytes, st);
-    const char* e = tc_head_launch(op.tc, features, B, h->feat_side, h->feat_side, J, c.depth, make_scale(c),
-                                   c2d, c3d, ws.base + ws.off_logits, st);
+    const char* e = storage(h) == ST_F16 ? tc_head_launch<__half>(op.tc, features, B, h->feat_side, h->feat_side, J, c.depth,
+                                                                  make_scale(c), c2d, c3d, ws.base + ws.off_logits, st)
+                                         : tc_head_launch<__nv_bfloat16>(op.tc, features, B, h->feat_side, h->feat_side, J, c.depth,
+                                                                         make_scale(c), c2d, c3d, ws.base + ws.off_logits, st);
     if (e) return fail(h, MTB_ERR_CUDA, "fused head: %s", e);
     h->launches += 2;
     return MTB_OK;
@@ -995,8 +1030,9 @@ int head_decode_impl(mtb_handle* h, const void* features, int B, float* c2d, flo
     e = cudaSuccess;
   } else {
     ProfScope prof(h, KC_HEAD_CONV_SIMT, op.flops * B, feat_bytes + (double)op.Cin * op.Cout * 4 + logit_bytes, st);
-    e = is_bf16(h) ? launch_conv_igemm<__nv_bfloat16, float>(p, st)
-                                             : launch_conv_igemm<float, float>(p, st);
+    e = storage(h) == ST_BF16  ? launch_conv_igemm<__nv_bfloat16, float>(p, st)
+        : storage(h) == ST_F16 ? launch_conv_igemm<__half, float>(p, st)
+                               : launch_conv_igemm<float, float>(p, st);
   }
   if (e != cudaSuccess) return fail(h, MTB_ERR_CUDA, "head conv: %s", cudaGetErrorString(e));
   ProfScope prof(h, KC_SOFTARGMAX, 0.0, logit_bytes + out_bytes, st);
@@ -1052,14 +1088,34 @@ int recon_and_combine(mtb_handle* h, const float* c2d, const float* c3d, const f
   return combine_impl(h, latents, B, out, st);
 }
 
-__global__ void to_float_kernel(const __nv_bfloat16* in, float* out, size_t n) {
+// 16-bit (bf16 / fp16) <-> fp32 copies of the debug entry points; fp32 from_float rounds to nearest even
+template <typename T>
+__global__ void to_float_kernel(const T* in, float* out, size_t n) {
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-    out[i] = __bfloat162float(in[i]);
+    out[i] = load1<T>(in + i);
 }
 
-__global__ void from_float_kernel(const float* in, __nv_bfloat16* out, size_t n) {
+template <typename T>
+__global__ void from_float_kernel(const float* in, T* out, size_t n) {
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-    out[i] = __float2bfloat16_rn(in[i]);
+    store1<T>(out + i, in[i]);
+}
+
+// storage -> fp32 copy of n elements (a plain copy for fp32 storage)
+void copy_to_float(const mtb_handle* h, const void* src, float* out, size_t n, cudaStream_t st) {
+  switch (storage(h)) {
+    case ST_BF16: launch_k(to_float_kernel<__nv_bfloat16>, dim3(grid_for(n, 256)), dim3(256), 0, st, (const __nv_bfloat16*)src, out, n); break;
+    case ST_F16: launch_k(to_float_kernel<__half>, dim3(grid_for(n, 256)), dim3(256), 0, st, (const __half*)src, out, n); break;
+    default: cudaMemcpyAsync(out, src, n * 4, cudaMemcpyDeviceToDevice, st); break;
+  }
+}
+// fp32 -> storage copy of n elements
+void copy_from_float(const mtb_handle* h, const float* src, void* out, size_t n, cudaStream_t st) {
+  switch (storage(h)) {
+    case ST_BF16: launch_k(from_float_kernel<__nv_bfloat16>, dim3(grid_for(n, 256)), dim3(256), 0, st, src, (__nv_bfloat16*)out, n); break;
+    case ST_F16: launch_k(from_float_kernel<__half>, dim3(grid_for(n, 256)), dim3(256), 0, st, src, (__half*)out, n); break;
+    default: cudaMemcpyAsync(out, src, n * 4, cudaMemcpyDeviceToDevice, st); break;
+  }
 }
 
 // [b,J,2] + [b,J,3] -> [b,J,5] (what travels in the all-gather) and back
@@ -1114,7 +1170,7 @@ int mtb_create(const mtb_config* cfg, mtb_handle** out) {
                 cfg->depth, cfg->proc_side, cfg->stride_test);
   if (cfg->arch == MTB_ARCH_EFFNET && (cfg->n_stages <= 0 || cfg->n_stages > MTB_MAX_STAGES))
     return fail(nullptr, MTB_ERR_INVALID_ARG, "n_stages out of range");
-  if (cfg->precision < MTB_PRECISION_FP32 || cfg->precision > MTB_PRECISION_TF32X3)
+  if (cfg->precision < MTB_PRECISION_FP32 || cfg->precision > MTB_PRECISION_F16_SIMT)
     return fail(nullptr, MTB_ERR_INVALID_ARG, "unknown precision %d", cfg->precision);
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
@@ -1229,13 +1285,13 @@ int mtb_finalize_weights(mtb_handle* h) {
     Op& a = h->ops[i];
     const Op& b = h->ops[i + 1];
     a.fmb.ready = false;
-    if (h->cfg.precision != MTB_PRECISION_BF16_TC || !a.tc.ready || !b.tc.ready) continue;
+    if (!is_tc16(h) || !a.tc.ready || !b.tc.ready) continue;
     if (a.type != OP_CONV || b.type != OP_CONV || a.small_io || b.small_io) continue;
     if (a.R != 3 || a.S != 3 || a.stride != 1 || a.dil != 1 || a.act != ACT_SILU || a.res_buf != BUF_NONE || a.scale_buf != BUF_NONE) continue;
     if (b.R != 1 || b.stride != 1 || b.act != ACT_NONE || b.scale_buf != BUF_NONE || b.res_first || b.in_buf != a.out_buf) continue;
     if (b.res_buf != BUF_NONE && b.res_buf != a.in_buf) continue;
     if (a.Hin != a.Hout || a.Win != a.Wout || b.out_buf == a.in_buf) continue;
-    const char* e = fmb_prepare(a.fmb, a.tc, b.tc);
+    const char* e = storage(h) == ST_F16 ? fmb_prepare<__half>(a.fmb, a.tc, b.tc) : fmb_prepare<__nv_bfloat16>(a.fmb, a.tc, b.tc);
     if (e) return fail(h, MTB_ERR_CUDA, "fused FusedMBConv weight prep for '%s': %s", a.name.c_str(), e);
   }
   {
@@ -1283,7 +1339,7 @@ int mtb_finalize_weights(mtb_handle* h) {
     }
     int rc = prepare_op_weights(h, hd);
     if (rc) return rc;
-    if (h->cfg.precision == MTB_PRECISION_BF16_TC) {
+    if (is_tc16(h)) {
       int bnp, cpt, npt;
       if (tc_head_plan(h->feat_side * h->feat_side, &bnp, &cpt, &npt)) {
         // the ORIGINAL (unpadded) [n_real][C] weight: the fused kernel masks rows itself
@@ -1292,7 +1348,8 @@ int mtb_finalize_weights(mtb_handle* h) {
           b0[n] = find(h, hd.biaskey)->data[n];
           for (int cc = 0; cc < hd.Cin; ++cc) w0[(size_t)n * hd.Cin + cc] = w->data[(size_t)n * hd.Cin + cc];
         }
-        const char* e = tc_prepare_head(hd.tc, w0.data(), b0.data(), hd.Cin, n_real, h->dev_allocs);
+        const char* e = storage(h) == ST_F16 ? tc_prepare_head<__half>(hd.tc, w0.data(), b0.data(), hd.Cin, n_real, h->dev_allocs)
+                                             : tc_prepare_head<__nv_bfloat16>(hd.tc, w0.data(), b0.data(), hd.Cin, n_real, h->dev_allocs);
         if (e) return fail(h, MTB_ERR_CUDA, "tensor-core head weight prep: %s", e);
       }
     }
@@ -1876,11 +1933,9 @@ int mtb_debug_run_ops(mtb_handle* h, const float* crops, int batch, int n_ops, f
   size_t n = (size_t)batch * (small ? 1 : (size_t)o.Hout * o.Wout) * o.Cout;
   if (n > out_floats) return fail(h, MTB_ERR_INVALID_ARG, "debug output buffer too small (%zu > %zu)", n, out_floats);
   void* src = buf_ptr(ws, o.out_buf, features);
-  if (small || !is_bf16(h)) {
-    CUDA_TRY(h, cudaMemcpyAsync(out, src, n * 4, cudaMemcpyDeviceToDevice, st));
-  } else {
-    launch_k(to_float_kernel, dim3(grid_for(n, 256)), dim3(256), 0, st, (const __nv_bfloat16*)src, out, n);
-  }
+  if (small) CUDA_TRY(h, cudaMemcpyAsync(out, src, n * 4, cudaMemcpyDeviceToDevice, st));
+  else copy_to_float(h, src, out, n, st);
+  CUDA_TRY(h, cudaGetLastError());
   return MTB_OK;
 }
 
@@ -1969,8 +2024,8 @@ int mtb_debug_run_op(mtb_handle* h, int op_index, const float* in, const float* 
     return fail(h, MTB_ERR_INVALID_ARG, "op %d: residual/scale inputs do not match the op (see mtb_op_input_shape)", op_index);
   auto put = [&](const float* src, int buf, size_t n, bool as_f32) {
     void* dst = buf_ptr(ws, buf, nullptr);
-    if (as_f32 || !is_bf16(h)) cudaMemcpyAsync(dst, src, n * 4, cudaMemcpyDeviceToDevice, st);
-    else launch_k(from_float_kernel, dim3(grid_for(n, 256)), dim3(256), 0, st, src, (__nv_bfloat16*)dst, n);
+    if (as_f32) cudaMemcpyAsync(dst, src, n * 4, cudaMemcpyDeviceToDevice, st);
+    else copy_from_float(h, src, dst, n, st);
   };
   const float* crops = nullptr;
   if (o.type == OP_STEM) {
@@ -1993,8 +2048,9 @@ int mtb_debug_run_op(mtb_handle* h, int op_index, const float* in, const float* 
   rc = run_op(h, o, crops, batch, ws, nullptr, st);
   if (rc) return rc;
   void* src = buf_ptr(ws, o.out_buf, nullptr);
-  if (small || !is_bf16(h)) CUDA_TRY(h, cudaMemcpyAsync(out, src, n_out * 4, cudaMemcpyDeviceToDevice, st));
-  else launch_k(to_float_kernel, dim3(grid_for(n_out, 256)), dim3(256), 0, st, (const __nv_bfloat16*)src, out, n_out);
+  if (small) CUDA_TRY(h, cudaMemcpyAsync(out, src, n_out * 4, cudaMemcpyDeviceToDevice, st));
+  else copy_to_float(h, src, out, n_out, st);
+  CUDA_TRY(h, cudaGetLastError());
   return MTB_OK;
 }
 
@@ -2014,13 +2070,14 @@ int mtb_debug_run_fused_block(mtb_handle* h, int op_index, const float* in, int 
   Op a = h->ops[op_index], b = h->ops[op_index + 1];
   const size_t n_in = (size_t)batch * a.Hin * a.Win * a.Cin, n_out = (size_t)batch * b.Hout * b.Wout * b.Cout;
   if (n_out > out_floats) return fail(h, MTB_ERR_INVALID_ARG, "debug output buffer too small");
-  launch_k(from_float_kernel, dim3(grid_for(n_in, 256)), dim3(256), 0, st, in, (__nv_bfloat16*)buf_ptr(ws, 0, nullptr), n_in);
+  copy_from_float(h, in, buf_ptr(ws, 0, nullptr), n_in, st);
   a.in_buf = 0; a.out_buf = 1; b.in_buf = 1; b.out_buf = 2;
   if (b.res_buf != BUF_NONE) b.res_buf = 0;
   a.fmb.cached_in = nullptr;  // the copy must not reuse a tensor map encoded for other buffers
   rc = run_fused_block(h, a, b, batch, ws, nullptr, st);
   if (rc) return rc;
-  launch_k(to_float_kernel, dim3(grid_for(n_out, 256)), dim3(256), 0, st, (const __nv_bfloat16*)buf_ptr(ws, 2, nullptr), out, n_out);
+  copy_to_float(h, buf_ptr(ws, 2, nullptr), out, n_out, st);
+  CUDA_TRY(h, cudaGetLastError());
   return MTB_OK;
 }
 

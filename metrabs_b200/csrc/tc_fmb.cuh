@@ -1,17 +1,17 @@
 // Fused FusedMBConv block (backbones/efficientnet.py:176-234, expand_ratio != 1, stride 1):
 //
-//     y = x + BN2(conv1x1( SiLU(BN1(conv3x3(x))) ))            x: [B,H,W,Cin] bf16 NHWC, expanded width Cexp = 4*Cin
+//     y = x + BN2(conv1x1( SiLU(BN1(conv3x3(x))) ))            x: [B,H,W,Cin] bf16 or fp16 NHWC, expanded width Cexp = 4*Cin
 //
 // as ONE kernel: the 128-pixel x Cexp expanded tile never leaves the SM.  Per output tile (16 x 8 pixels, as mode 1 of
 // tc_conv_kernel) and per chunk of 128 expanded channels:
 //   GEMM-1  (3x3 expand, implicit GEMM)   acc1[128 x 128] = shifted input boxes (4D TMA per tap) x W1[chunk rows]^T
-//   epilogue-1  acc1 -> + folded-BN bias -> SiLU -> bf16 -> shared memory in the 128B-swizzled K-major operand layout:
+//   epilogue-1  acc1 -> + folded-BN bias -> SiLU -> bf16 / fp16 -> shared memory in the 128B-swizzled K-major operand layout:
 //           it IS the A operand of GEMM-2 (channels >= Cexp are written as zeros)
 //   GEMM-2  (1x1 projection)  acc2[128 x Cout] += A2 x W2[:, chunk]^T, the W2 slice travelling through the same TMA ring
-// and after the last chunk epilogue-2: acc2 -> + bias -> + residual x -> bf16 store.  Each consumer warpgroup owns 64 rows
+// and after the last chunk epilogue-2: acc2 -> + bias -> + residual x -> 16-bit store.  Each consumer warpgroup owns 64 rows
 // of the tile in both GEMMs, so the A2 hand-over needs only a warpgroup barrier.  The MMA sequence of every output element
 // (tap-major K of GEMM-1, chunk-major K of GEMM-2, K = 16 per wgmma) and every rounding are those of the two-launch path
-// (tc_conv_kernel twice), so the fused block reproduces it.
+// (tc_conv_kernel twice, with the same activation form per element type), so the fused block reproduces it.
 #pragma once
 #include "tc_gemm.cuh"
 
@@ -31,7 +31,7 @@ struct FmbParams {
   int Cexp, nch, has_res;
 };
 
-template <int BN2>
+template <typename T, int BN2>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 fmb_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW1, const __grid_constant__ CUtensorMap tmW2,
            const FmbParams p) {
@@ -101,7 +101,7 @@ fmb_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < TC_BK / 16; ++k)
-        wgmma_bf16<FMB_NC>(acc1, gmma_desc<128>(a + 32 * k), gmma_desc<128>(b + 32 * k), (uint32_t)(kb | k));
+        wgmma_16b<T, FMB_NC>(acc1, gmma_desc<128>(a + 32 * k), gmma_desc<128>(b + 32 * k), (uint32_t)(kb | k));
       wgmma_commit();
       wgmma_wait<1>();
       if (prev >= 0) {
@@ -114,7 +114,7 @@ fmb_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
     wgmma_fence_regs<FMB_NC / 2>(acc1);
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[prev]);
-    // ---- epilogue-1: + bias, SiLU, bf16 -> A2 (this warpgroup's rows; 16-byte chunk j of row r at j ^ (r & 7)) ----
+    // ---- epilogue-1: + bias, SiLU, 16-bit -> A2 (this warpgroup's rows; 16-byte chunk j of row r at j ^ (r & 7)) ----
 #pragma unroll
     for (int j = 0; j < FMB_NC / 8; ++j) {
       const int cc = 8 * j + 2 * (lane & 3);  // column within the chunk
@@ -125,11 +125,11 @@ fmb_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int r = r0 + 8 * h;
-        __nv_bfloat162 v = __floats2bfloat162_rn(0.f, 0.f);
+        typename Pair16<T>::type v = Pair16<T>::pack(0.f, 0.f);
         if (col < p.Cexp)
-          v = __floats2bfloat162_rn(tc_act<ACT_SILU>(acc1[4 * j + 2 * h] + bv.x), tc_act<ACT_SILU>(acc1[4 * j + 2 * h + 1] + bv.y));
+          v = Pair16<T>::pack(tc_act<ACT_SILU, T>(acc1[4 * j + 2 * h] + bv.x), tc_act<ACT_SILU, T>(acc1[4 * j + 2 * h + 1] + bv.y));
         const uint32_t off = sub + (uint32_t)r * 128 + ((((kc >> 3) ^ (uint32_t)(r & 7))) << 4) + (kc & 7) * 2;
-        *reinterpret_cast<__nv_bfloat162*>(smem + FMB_A2_OFF + off) = v;
+        *reinterpret_cast<typename Pair16<T>::type*>(smem + FMB_A2_OFF + off) = v;
       }
     }
     fence_proxy_async();  // generic-proxy writes -> visible to the tensor core (async proxy)
@@ -143,7 +143,7 @@ fmb_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
 #pragma unroll
       for (int k = 0; k < FMB_NC / 16; ++k) {
         const uint32_t sub = (uint32_t)(k >> 2), ko = (uint32_t)(k & 3) * 32;
-        wgmma_bf16<BN2>(acc2, gmma_desc<128>(a2 + sub * (TC_BM * 128) + wg * 64 * 128 + ko), gmma_desc<128>(b + sub * (BN2 * 128) + ko),
+        wgmma_16b<T, BN2>(acc2, gmma_desc<128>(a2 + sub * (TC_BM * 128) + wg * 64 * 128 + ko), gmma_desc<128>(b + sub * (BN2 * 128) + ko),
                         (uint32_t)(c | k));
       }
       wgmma_commit();
@@ -154,9 +154,10 @@ fmb_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
       ++it;
     }
   }
-  // ---- epilogue-2: + bias, + residual x, bf16 store ----
-  const __nv_bfloat16* __restrict__ res = (const __nv_bfloat16*)g.res;
-  __nv_bfloat16* __restrict__ out = (__nv_bfloat16*)g.out;
+  // ---- epilogue-2: + bias, + residual x, 16-bit store ----
+  typedef typename Pair16<T>::type T2;
+  const T* __restrict__ res = (const T*)g.res;
+  T* __restrict__ out = (T*)g.out;
   const int c0 = 2 * (lane & 3);
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
@@ -169,11 +170,11 @@ fmb_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
       const float2 bv = __ldg(reinterpret_cast<const float2*>(g.bias + cidx));
       float o0 = acc2[4 * j + 2 * h] + bv.x, o1 = acc2[4 * j + 2 * h + 1] + bv.y;
       if (p.has_res) {
-        const float2 rv = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(res + off + cidx));
+        const float2 rv = Pair16<T>::unpack(*reinterpret_cast<const T2*>(res + off + cidx));
         o0 += rv.x;
         o1 += rv.y;
       }
-      *reinterpret_cast<__nv_bfloat162*>(out + off + cidx) = __floats2bfloat162_rn(o0, o1);
+      *reinterpret_cast<T2*>(out + off + cidx) = Pair16<T>::pack(o0, o1);
     }
   }
 }
@@ -181,7 +182,7 @@ fmb_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
 // ------------------------------------------------------------------------------------------------ host side
 struct FmbWeights {
   bool ready = false;
-  const TcWeights* w1 = nullptr;  // the expand conv's bf16 K-major weights [Cexp][9*Cin] + bias
+  const TcWeights* w1 = nullptr;  // the expand conv's 16-bit K-major weights [Cexp][9*Cin] + bias
   const TcWeights* w2 = nullptr;  // the projection's [Cout][Cexp] + bias
   int Cin = 0, Cexp = 0, Cout = 0, bn2 = 0;
   CUtensorMap mapW1, mapW2;
@@ -195,15 +196,16 @@ inline bool fmb_shape_ok(int cin, int cexp, int cout) {
   return cin % 16 == 0 && cin >= 16 && cin <= 96 && cout == cin && cexp % 16 == 0 && cexp >= 32 && cexp <= 512;
 }
 
+template <typename T>
 inline const char* fmb_prepare(FmbWeights& f, const TcWeights& w1, const TcWeights& w2) {
   f.ready = false;
   if (!fmb_shape_ok(w1.Cin, w1.Cout, w2.Cout) || w2.Cin != w1.Cout || w1.taps != 9) return nullptr;
   f.w1 = &w1; f.w2 = &w2;
   f.Cin = w1.Cin; f.Cexp = w1.Cout; f.Cout = w2.Cout;
   f.bn2 = tc_pick_bn(f.Cout);
-  const char* e = make_tmap_2d(&f.mapW1, w1.d_w, (uint64_t)f.Cexp, (uint64_t)9 * f.Cin, FMB_NC);
+  const char* e = make_tmap_2d<T>(&f.mapW1, w1.d_w, (uint64_t)f.Cexp, (uint64_t)9 * f.Cin, FMB_NC);
   if (e) return e;
-  e = make_tmap_2d(&f.mapW2, w2.d_w, (uint64_t)f.Cout, (uint64_t)f.Cexp, (uint32_t)f.bn2);
+  e = make_tmap_2d<T>(&f.mapW2, w2.d_w, (uint64_t)f.Cout, (uint64_t)f.Cexp, (uint32_t)f.bn2);
   if (e) return e;
   f.cached_in = nullptr;
   f.cached_B = -1;
@@ -211,19 +213,20 @@ inline const char* fmb_prepare(FmbWeights& f, const TcWeights& w1, const TcWeigh
   return nullptr;
 }
 
-template <int BN2>
+template <typename T, int BN2>
 inline const char* fmb_launch_k(int grid, const FmbWeights& f, const FmbParams& q, cudaStream_t st) {
   static bool attr_set = false;
   if (!attr_set) {
-    if (cudaFuncSetAttribute(fmb_kernel<BN2>, cudaFuncAttributeMaxDynamicSharedMemorySize, FMB_SMEM_BYTES) != cudaSuccess)
+    if (cudaFuncSetAttribute(fmb_kernel<T, BN2>, cudaFuncAttributeMaxDynamicSharedMemorySize, FMB_SMEM_BYTES) != cudaSuccess)
       return "cannot raise dynamic shared memory for fmb_kernel";
     attr_set = true;
   }
-  launch_k(fmb_kernel<BN2>, dim3(grid), dim3(TC_THREADS), FMB_SMEM_BYTES, st, f.mapA, f.mapW1, f.mapW2, q);
+  launch_k(fmb_kernel<T, BN2>, dim3(grid), dim3(TC_THREADS), FMB_SMEM_BYTES, st, f.mapA, f.mapW1, f.mapW2, q);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 
+template <typename T>
 inline const char* fmb_launch(const FmbWeights& f, const void* in, void* out, int B, int H, int W, int pad_t, int pad_l, bool has_res,
                               cudaStream_t st) {
   if (!f.ready) return "fused FusedMBConv block not prepared";
@@ -243,16 +246,16 @@ inline const char* fmb_launch(const FmbWeights& f, const void* in, void* out, in
   q.nch = (f.Cexp + FMB_NC - 1) / FMB_NC;
   q.has_res = has_res ? 1 : 0;
   if (f.cached_in != in || f.cached_B != B) {
-    const char* e = make_tmap_nhwc(&f.mapA, in, B, H, W, f.Cin, 1);
+    const char* e = make_tmap_nhwc<T>(&f.mapA, in, B, H, W, f.Cin, 1);
     if (e) return e;
     f.cached_in = in;
     f.cached_B = B;
   }
   const int grid = B * g.tiles_w * g.tiles_h;
   switch (f.bn2) {
-    case 32: return fmb_launch_k<32>(grid, f, q, st);
-    case 64: return fmb_launch_k<64>(grid, f, q, st);
-    default: return fmb_launch_k<128>(grid, f, q, st);
+    case 32: return fmb_launch_k<T, 32>(grid, f, q, st);
+    case 64: return fmb_launch_k<T, 64>(grid, f, q, st);
+    default: return fmb_launch_k<T, 128>(grid, f, q, st);
   }
 }
 

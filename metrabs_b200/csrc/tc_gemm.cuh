@@ -1,11 +1,11 @@
-// Tensor-core path (sm_90a): bf16 operands staged by TMA into 128B-swizzled shared memory, fp32 accumulators in registers of
+// Tensor-core path (sm_90a): 16-bit operands (bf16, or fp16 in the fp16 mode) staged by TMA into 128B-swizzled shared memory, fp32 accumulators in registers of
 // two consumer warpgroups (wgmma.mma_async), an mbarrier ring between one TMA producer warp and the consumers.
 //
 //   tc_conv_kernel   1x1 conv == GEMM  D[pixels, Cout] = A[pixels, Cin] * W[Cout, Cin]^T          (mode 0, 2D TMA)
 //                    RxS conv (stride 1/2, dilation) as implicit GEMM: per tap (r,s) the A tile is a shifted [8 x 16] pixel box
 //                    of the NHWC input fetched by a 4D TMA (out-of-bounds = the reference's explicit zero padding,
 //                    backbones/efficientnet.py:1127-1161)                                             (mode 1)
-//                    epilogue: registers -> + folded-BN bias, activation, + residual, bf16 NHWC store.
+//                    epilogue: registers -> + folded-BN bias, activation, + residual, 16-bit NHWC store.
 //   tc_head_kernel   MetrabsHeads (models/metrabs.py:75-85): swapped operands, D[channel, pixel] = W[N, C] * F^T, so every
 //                    epilogue thread owns one (d,j) channel and reduces its pixels in registers: the J x D x H x W logits
 //                    never leave the SM.
@@ -130,11 +130,14 @@ __device__ __forceinline__ float tanh_approx(float x) {
   return y;
 }
 // Epilogue activation, COMPILE-TIME selected (a runtime switch inside the per-element code gets if-converted into all
-// branches: ncu showed ~110 executed instructions per output element).  SiLU(x) = h + h*tanh(h), h = x/2: one MUFU op,
-// error ~2^-11, below bf16 resolution.
-template <int ACT>
+// branches: ncu showed ~110 executed instructions per output element).  bf16 outputs: SiLU(x) = h + h*tanh(h), h = x/2: one
+// MUFU op, error ~2^-11, below bf16 resolution.  fp16 outputs (T = __half): silu_f16out, one more MUFU op per element,
+// because 2^-11 is a whole fp16 ulp.
+template <int ACT, typename T = __nv_bfloat16>
 __device__ __forceinline__ float tc_act(float x) {
-  if constexpr (ACT == ACT_SILU) {
+  if constexpr (ACT == ACT_SILU && is_f16<T>) {
+    return silu_f16out(x);
+  } else if constexpr (ACT == ACT_SILU) {
     float h = 0.5f * x;
     return fmaf(h, tanh_approx(h), h);
   } else if constexpr (ACT == ACT_RELU) {
@@ -174,8 +177,8 @@ __device__ __forceinline__ void tma_load_a_tile(void* dst, const CUtensorMap* ma
 }
 
 // ACT: epilogue activation; RES: 0 no residual, 1 residual added AFTER the activation (EfficientNet), 2 BEFORE (ResNet);
-// BN: output channels per tile (wgmma N).
-template <int ACT, int RES, int BN>
+// BN: output channels per tile (wgmma N); T: operand and activation element type (__nv_bfloat16 or __half).
+template <typename T, int ACT, int RES, int BN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcConvParams p) {
   using Ring = TcRing<BN>;
@@ -227,7 +230,7 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const uint32_t b = smem_u32(smem + s * Ring::stage_bytes + TC_A_BYTES);
     wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < TC_BK / 16; ++k) wgmma_bf16<BN>(acc, gmma_desc<128>(a + 32 * k), gmma_desc<128>(b + 32 * k), (uint32_t)(kb | k));
+    for (int k = 0; k < TC_BK / 16; ++k) wgmma_16b<T, BN>(acc, gmma_desc<128>(a + 32 * k), gmma_desc<128>(b + 32 * k), (uint32_t)(kb | k));
     wgmma_commit();
     wgmma_wait<1>();  // the previous k-block's MMAs are done: its stage goes back to the producer
     if (prev >= 0) {
@@ -242,8 +245,9 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   // ===== epilogue: thread rows r0 = 64 wg + 16 (warp & 3) + lane / 4 and r0 + 8, columns 8 j + 2 (lane % 4) + {0, 1} =====
   const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
   const int c0 = n_blk * BN + 2 * (lane & 3);
-  const __nv_bfloat16* __restrict__ res = (const __nv_bfloat16*)p.res;
-  __nv_bfloat16* __restrict__ out = (__nv_bfloat16*)p.out;
+  typedef typename Pair16<T>::type T2;
+  const T* __restrict__ res = (const T*)p.res;
+  T* __restrict__ out = (T*)p.out;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     size_t off;
@@ -255,39 +259,41 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + c));
       float o0 = acc[4 * j + 2 * h] + bv.x, o1 = acc[4 * j + 2 * h + 1] + bv.y;
       if constexpr (RES != 0) {
-        const float2 rv = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(res + off + c));
+        const float2 rv = Pair16<T>::unpack(*reinterpret_cast<const T2*>(res + off + c));
         if constexpr (RES == 2) {
-          o0 = tc_act<ACT>(o0 + rv.x);
-          o1 = tc_act<ACT>(o1 + rv.y);
+          o0 = tc_act<ACT, T>(o0 + rv.x);
+          o1 = tc_act<ACT, T>(o1 + rv.y);
         } else {
-          o0 = tc_act<ACT>(o0) + rv.x;
-          o1 = tc_act<ACT>(o1) + rv.y;
+          o0 = tc_act<ACT, T>(o0) + rv.x;
+          o1 = tc_act<ACT, T>(o1) + rv.y;
         }
       } else {
-        o0 = tc_act<ACT>(o0);
-        o1 = tc_act<ACT>(o1);
+        o0 = tc_act<ACT, T>(o0);
+        o1 = tc_act<ACT, T>(o1);
       }
-      *reinterpret_cast<__nv_bfloat162*>(out + off + c) = __floats2bfloat162_rn(o0, o1);
+      *reinterpret_cast<T2*>(out + off + c) = Pair16<T>::pack(o0, o1);
     }
   }
 }
 
-// in-place squeeze-excitation scaling  x[b,p,c] *= s[b,c]  ahead of a tensor-core projection GEMM
-__global__ void __launch_bounds__(256) se_scale_kernel(__nv_bfloat16* __restrict__ x, const float* __restrict__ s, int P, int C,
+// in-place squeeze-excitation scaling  x[b,p,c] *= s[b,c]  ahead of a tensor-core projection GEMM (T: bf16 or fp16)
+template <typename T>
+__global__ void __launch_bounds__(256) se_scale_kernel(T* __restrict__ x, const float* __restrict__ s, int P, int C,
                                                        size_t total8) {
+  typedef typename Pair16<T>::type T2;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total8; i += (size_t)gridDim.x * blockDim.x) {
     size_t e = i * 8;
     int c = (int)(e % C);
     int b = (int)(e / ((size_t)P * C));
     uint4 v = *reinterpret_cast<uint4*>(x + e);
-    __nv_bfloat162* v2 = reinterpret_cast<__nv_bfloat162*>(&v);
+    T2* v2 = reinterpret_cast<T2*>(&v);
     const float4 s0 = *reinterpret_cast<const float4*>(s + (size_t)b * C + c);
     const float4 s1 = *reinterpret_cast<const float4*>(s + (size_t)b * C + c + 4);
     const float sc[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      float2 f = __bfloat1622float2(v2[k]);
-      v2[k] = __floats2bfloat162_rn(f.x * sc[2 * k], f.y * sc[2 * k + 1]);
+      float2 f = Pair16<T>::unpack(v2[k]);
+      v2[k] = Pair16<T>::pack(f.x * sc[2 * k], f.y * sc[2 * k + 1]);
     }
     *reinterpret_cast<uint4*>(x + e) = v;
   }
@@ -309,7 +315,13 @@ inline tmap_encode_fn get_tmap_encode() {
   return fn;
 }
 
-// rank-2 bf16 tensor [rows][cols] (cols contiguous), box [box_rows][64], 128B swizzle, OOB -> 0
+template <typename T>
+constexpr CUtensorMapDataType tmap_dtype() {
+  return std::is_same<T, __half>::value ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+}
+
+// rank-2 16-bit tensor [rows][cols] (cols contiguous), box [box_rows][64], 128B swizzle, OOB -> 0
+template <typename T = __nv_bfloat16>
 inline const char* make_tmap_2d(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows,
                                 uint32_t box_cols = TC_BK) {
   tmap_encode_fn enc = get_tmap_encode();
@@ -318,14 +330,15 @@ inline const char* make_tmap_2d(CUtensorMap* m, const void* ptr, uint64_t rows, 
   cuuint64_t strides[1] = {cols * 2};
   cuuint32_t box[2] = {box_cols, box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+  CUresult r = enc(m, tmap_dtype<T>(), 2, const_cast<void*>(ptr), dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, box_cols == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? nullptr : "cuTensorMapEncodeTiled(2d) failed";
 }
-// rank-4 bf16 NHWC tensor [B][H][W][C]; box = 64 channels x (TILE_W x TILE_H) pixels sampled every `stride` pixels
+// rank-4 16-bit NHWC tensor [B][H][W][C]; box = 64 channels x (TILE_W x TILE_H) pixels sampled every `stride` pixels
 // (element strides: to load N elements along a dimension with traversal stride s, boxDim = N*s)
+template <typename T = __nv_bfloat16>
 inline const char* make_tmap_nhwc(CUtensorMap* m, const void* ptr, uint64_t B, uint64_t H, uint64_t W, uint64_t C, uint32_t stride,
                                   uint32_t box_c = TC_BK, uint32_t tile_w = TC_TILE_W, uint32_t tile_h = TC_TILE_H) {
   tmap_encode_fn enc = get_tmap_encode();
@@ -334,7 +347,7 @@ inline const char* make_tmap_nhwc(CUtensorMap* m, const void* ptr, uint64_t B, u
   cuuint64_t strides[3] = {C * 2, W * C * 2, H * W * C * 2};
   cuuint32_t box[4] = {box_c, tile_w * stride, tile_h * stride, 1};
   cuuint32_t estr[4] = {1, stride, stride, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, estr,
+  CUresult r = enc(m, tmap_dtype<T>(), 4, const_cast<void*>(ptr), dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, box_c == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -343,7 +356,7 @@ inline const char* make_tmap_nhwc(CUtensorMap* m, const void* ptr, uint64_t B, u
 
 struct TcWeights {
   bool ready = false;
-  __nv_bfloat16* d_w = nullptr;  // [Cout][taps*Cin] K-major
+  void* d_w = nullptr;           // [Cout][taps*Cin] K-major, bf16 or fp16 (the mode's storage type)
   float* d_bias = nullptr;       // [Cout]
   int Cout = 0, Cin = 0, taps = 1, S = 1;
   // head
@@ -378,13 +391,22 @@ inline __nv_bfloat16 host_bf16(float f) {
   return out;
 }
 
-// wk: fp32 [K = taps*Cin][Cout] (BN folded) -> bf16 [Cout][K]
+// fp16 twin of host_bf16: round to nearest even, overflow to inf
+inline __half host_f16(float f) { return __float2half_rn(f); }
+template <typename T>
+inline T host_16b(float f) {
+  if constexpr (std::is_same<T, __half>::value) return host_f16(f);
+  else return host_bf16(f);
+}
+
+// wk: fp32 [K = taps*Cin][Cout] (BN folded) -> T (bf16 or fp16) [Cout][K]
+template <typename T>
 inline const char* tc_prepare_weights(TcWeights& w, const float* wk, const float* bias, int K, int cout, int R, int S, int cin,
                                       std::vector<void*>& allocs) {
-  std::vector<__nv_bfloat16> t((size_t)K * cout);
+  std::vector<T> t((size_t)K * cout);
   for (int k = 0; k < K; ++k)
-    for (int n = 0; n < cout; ++n) t[(size_t)n * K + k] = host_bf16(wk[(size_t)k * cout + n]);
-  if (cudaMalloc((void**)&w.d_w, t.size() * 2) != cudaSuccess) return "cudaMalloc failed";
+    for (int n = 0; n < cout; ++n) t[(size_t)n * K + k] = host_16b<T>(wk[(size_t)k * cout + n]);
+  if (cudaMalloc(&w.d_w, t.size() * 2) != cudaSuccess) return "cudaMalloc failed";
   allocs.push_back(w.d_w);
   if (cudaMemcpy(w.d_w, t.data(), t.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess) return "cudaMemcpy failed";
   if (cudaMalloc((void**)&w.d_bias, (size_t)cout * 4) != cudaSuccess) return "cudaMalloc failed";
@@ -400,37 +422,39 @@ inline const char* tc_prepare_weights(TcWeights& w, const float* wk, const float
 // N-tile width: the narrowest wgmma N in {32, 64, 128} that covers Cout, else 128 (Cout > 128 runs several N tiles)
 inline int tc_pick_bn(int cout) { return cout <= 32 ? 32 : cout <= 64 ? 64 : 128; }
 
-template <int ACT, int RES, int BN>
+template <typename T, int ACT, int RES, int BN>
 inline const char* tc_conv_launch_k(dim3 grid, const CUtensorMap& a, const CUtensorMap& b, const TcConvParams& q, cudaStream_t st) {
   static bool attr_set = false;
   if (!attr_set) {
-    if (cudaFuncSetAttribute(tc_conv_kernel<ACT, RES, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcRing<BN>::smem_bytes) !=
+    if (cudaFuncSetAttribute(tc_conv_kernel<T, ACT, RES, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcRing<BN>::smem_bytes) !=
         cudaSuccess)
       return "cannot raise dynamic shared memory for tc_conv_kernel";
     attr_set = true;
   }
-  launch_k(tc_conv_kernel<ACT, RES, BN>, grid, dim3(TC_THREADS), TcRing<BN>::smem_bytes, st, a, b, q);
+  launch_k(tc_conv_kernel<T, ACT, RES, BN>, grid, dim3(TC_THREADS), TcRing<BN>::smem_bytes, st, a, b, q);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
-template <int ACT, int RES>
+template <typename T, int ACT, int RES>
 inline const char* tc_conv_launch_t(int bn, dim3 grid, const CUtensorMap& a, const CUtensorMap& b, const TcConvParams& q, cudaStream_t st) {
   switch (bn) {
-    case 32: return tc_conv_launch_k<ACT, RES, 32>(grid, a, b, q, st);
-    case 64: return tc_conv_launch_k<ACT, RES, 64>(grid, a, b, q, st);
-    default: return tc_conv_launch_k<ACT, RES, 128>(grid, a, b, q, st);
+    case 32: return tc_conv_launch_k<T, ACT, RES, 32>(grid, a, b, q, st);
+    case 64: return tc_conv_launch_k<T, ACT, RES, 64>(grid, a, b, q, st);
+    default: return tc_conv_launch_k<T, ACT, RES, 128>(grid, a, b, q, st);
   }
 }
-template <int ACT>
+template <typename T, int ACT>
 inline const char* tc_conv_dispatch_res(int res_mode, int bn, dim3 grid, const CUtensorMap& a, const CUtensorMap& b, const TcConvParams& q,
                                         cudaStream_t st) {
   switch (res_mode) {
-    case 0: return tc_conv_launch_t<ACT, 0>(bn, grid, a, b, q, st);
-    case 1: return tc_conv_launch_t<ACT, 1>(bn, grid, a, b, q, st);
-    default: return tc_conv_launch_t<ACT, 2>(bn, grid, a, b, q, st);
+    case 0: return tc_conv_launch_t<T, ACT, 0>(bn, grid, a, b, q, st);
+    case 1: return tc_conv_launch_t<T, ACT, 1>(bn, grid, a, b, q, st);
+    default: return tc_conv_launch_t<T, ACT, 2>(bn, grid, a, b, q, st);
   }
 }
 
+// T: the storage type the weights were prepared in (tc_prepare_weights<T>)
+template <typename T>
 inline const char* tc_conv_launch(const TcWeights& w, const ConvParams& p, bool res_first, cudaStream_t st) {
   TcConvParams q;
   q.res = p.res; q.bias = w.d_bias; q.out = p.out;
@@ -450,10 +474,10 @@ inline const char* tc_conv_launch(const TcWeights& w, const ConvParams& p, bool 
     if (c.in == p.in && c.B == p.B && c.bn == bn) { ms = &c; break; }
   if (!ms) {
     TcWeights::MapSet c;
-    const char* e = q.mode == 0 ? make_tmap_2d(&c.a, p.in, (uint64_t)q.M, (uint64_t)p.Cin, TC_BM)
-                                : make_tmap_nhwc(&c.a, p.in, p.B, p.Hin, p.Win, p.Cin, (uint32_t)p.stride);
+    const char* e = q.mode == 0 ? make_tmap_2d<T>(&c.a, p.in, (uint64_t)q.M, (uint64_t)p.Cin, TC_BM)
+                                : make_tmap_nhwc<T>(&c.a, p.in, p.B, p.Hin, p.Win, p.Cin, (uint32_t)p.stride);
     if (e) return e;
-    e = make_tmap_2d(&c.b, w.d_w, (uint64_t)p.Cout, (uint64_t)w.taps * p.Cin, (uint32_t)bn);
+    e = make_tmap_2d<T>(&c.b, w.d_w, (uint64_t)p.Cout, (uint64_t)w.taps * p.Cin, (uint32_t)bn);
     if (e) return e;
     c.in = p.in; c.B = p.B; c.bn = bn;
     if (w.map_sets.size() < 16) {
@@ -468,17 +492,18 @@ inline const char* tc_conv_launch(const TcWeights& w, const ConvParams& p, bool 
   const dim3 grid(m_tiles, (p.Cout + bn - 1) / bn);
   const int res_mode = p.res ? (res_first ? 2 : 1) : 0;
   switch (p.act) {
-    case ACT_NONE: return tc_conv_dispatch_res<ACT_NONE>(res_mode, bn, grid, ms->a, ms->b, q, st);
-    case ACT_SILU: return tc_conv_dispatch_res<ACT_SILU>(res_mode, bn, grid, ms->a, ms->b, q, st);
-    case ACT_RELU: return tc_conv_dispatch_res<ACT_RELU>(res_mode, bn, grid, ms->a, ms->b, q, st);
-    case ACT_HSWISH: return tc_conv_dispatch_res<ACT_HSWISH>(res_mode, bn, grid, ms->a, ms->b, q, st);
+    case ACT_NONE: return tc_conv_dispatch_res<T, ACT_NONE>(res_mode, bn, grid, ms->a, ms->b, q, st);
+    case ACT_SILU: return tc_conv_dispatch_res<T, ACT_SILU>(res_mode, bn, grid, ms->a, ms->b, q, st);
+    case ACT_RELU: return tc_conv_dispatch_res<T, ACT_RELU>(res_mode, bn, grid, ms->a, ms->b, q, st);
+    case ACT_HSWISH: return tc_conv_dispatch_res<T, ACT_HSWISH>(res_mode, bn, grid, ms->a, ms->b, q, st);
     default: return "unsupported activation in the tensor-core epilogue";
   }
 }
 
+template <typename T>
 inline const char* tc_se_scale_launch(void* x, const float* s, int B, int P, int C, cudaStream_t st) {
   size_t total8 = (size_t)B * P * C / 8;
-  launch_k(se_scale_kernel, dim3(grid_for(total8, 256)), dim3(256), 0, st, (__nv_bfloat16*)x, s, P, C, total8);
+  launch_k(se_scale_kernel<T>, dim3(grid_for(total8, 256)), dim3(256), 0, st, (T*)x, s, P, C, total8);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
@@ -513,6 +538,7 @@ __device__ __forceinline__ uint32_t tch_stg(int row, int col) {
   return (uint32_t)(row * 256 + ((((col >> 2) ^ (row & 7))) << 2) + (col & 3)) * 4u;
 }
 
+template <typename T>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_head_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmF, const TcHeadParams p) {
   extern __shared__ uint8_t tc_smem_raw[];
@@ -574,7 +600,7 @@ tc_head_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
       const uint32_t b = smem_u32(smem + s * TCH_STAGE_BYTES + TC_A_BYTES);
       wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < TC_BK / 16; ++k) wgmma_bf16<256>(acc, gmma_desc<128>(a + 32 * k), gmma_desc<128>(b + 32 * k), (uint32_t)(kb | k));
+      for (int k = 0; k < TC_BK / 16; ++k) wgmma_16b<T, 256>(acc, gmma_desc<128>(a + 32 * k), gmma_desc<128>(b + 32 * k), (uint32_t)(kb | k));
       wgmma_commit();
       wgmma_wait<1>();
       if (prev >= 0) {
@@ -701,20 +727,22 @@ __global__ void __launch_bounds__(128) head_finalize_kernel(const float4* __rest
   }
 }
 
-// w: fp32 [n_out][C] (torch conv weight [N,C,1,1]); returns nullptr on success.  Not eligible -> ready stays false.
+// w: fp32 [n_out][C] (torch conv weight [N,C,1,1]) -> T (bf16 or fp16); returns nullptr on success.  Not eligible -> ready
+// stays false.
+template <typename T>
 inline const char* tc_prepare_head(TcWeights& w, const float* wt, const float* bias, int C, int n_out, std::vector<void*>& allocs) {
   if (C % 8 != 0) return nullptr;
-  std::vector<__nv_bfloat16> t((size_t)n_out * C);
-  for (size_t i = 0; i < t.size(); ++i) t[i] = host_bf16(wt[i]);
-  if (cudaMalloc((void**)&w.d_w, t.size() * 2) != cudaSuccess) return "cudaMalloc failed";
+  std::vector<T> t((size_t)n_out * C);
+  for (size_t i = 0; i < t.size(); ++i) t[i] = host_16b<T>(wt[i]);
+  if (cudaMalloc(&w.d_w, t.size() * 2) != cudaSuccess) return "cudaMalloc failed";
   allocs.push_back(w.d_w);
   if (cudaMemcpy(w.d_w, t.data(), t.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess) return "cudaMemcpy failed";
   if (cudaMalloc((void**)&w.d_bias, (size_t)n_out * 4) != cudaSuccess) return "cudaMalloc failed";
   allocs.push_back(w.d_bias);
   if (cudaMemcpy(w.d_bias, bias, (size_t)n_out * 4, cudaMemcpyHostToDevice) != cudaSuccess) return "cudaMemcpy failed";
-  if (cudaFuncSetAttribute(tc_head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TCH_SMEM_BYTES) != cudaSuccess)
+  if (cudaFuncSetAttribute(tc_head_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, TCH_SMEM_BYTES) != cudaSuccess)
     return "cannot raise dynamic shared memory for tc_head_kernel";
-  const char* e = make_tmap_2d(&w.mapA, w.d_w, (uint64_t)n_out, (uint64_t)C, TC_BM);
+  const char* e = make_tmap_2d<T>(&w.mapA, w.d_w, (uint64_t)n_out, (uint64_t)C, TC_BM);
   if (e) return e;
   w.Cout = n_out; w.Cin = C; w.n_real = n_out;
   w.ready = true;
@@ -737,6 +765,7 @@ inline bool tc_head_plan(int P, int* bnp, int* cpt, int* npt) {
   return true;
 }
 
+template <typename T>
 inline const char* tc_head_launch(const TcWeights& w, const void* features, int B, int H, int W, int J, int D, DecodeScale sc,
                                   float* c2d, float* c3d, void* scratch, cudaStream_t st) {
   TcHeadParams q;
@@ -748,12 +777,12 @@ inline const char* tc_head_launch(const TcWeights& w, const void* features, int 
   q.m_tiles = (q.n_out + TC_BM - 1) / TC_BM;
   q.kblocks = (q.C + TC_BK - 1) / TC_BK;
   if (w.cached_in != features || w.cached_B != B) {
-    const char* e = make_tmap_2d(&w.mapB, features, (uint64_t)B * q.P, (uint64_t)q.C, (uint32_t)q.bnp);
+    const char* e = make_tmap_2d<T>(&w.mapB, features, (uint64_t)B * q.P, (uint64_t)q.C, (uint32_t)q.bnp);
     if (e) return e;
     w.cached_in = features;
     w.cached_B = B;
   }
-  launch_k(tc_head_kernel, dim3(n_groups * q.m_tiles), dim3(TC_THREADS), TCH_SMEM_BYTES, st, w.mapA, w.mapB, q);
+  launch_k(tc_head_kernel<T>, dim3(n_groups * q.m_tiles), dim3(TC_THREADS), TCH_SMEM_BYTES, st, w.mapA, w.mapB, q);
   launch_k(head_finalize_kernel, dim3(B), dim3(128), 0, st, q.states, c2d, c3d, J, D, H, W, sc);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);

@@ -3,7 +3,10 @@
 // (warp w of the warpgroup, lane l) holds, for j = 0 .. N/8 - 1, rows 16 w + l / 4 (d[4j], d[4j+1]) and 16 w + l / 4 + 8
 // (d[4j+2], d[4j+3]) at columns 8 j + 2 (l % 4) + {0, 1}.
 #pragma once
+#include <cuda_fp16.h>
 #include <stdint.h>
+
+#include <type_traits>
 
 namespace mtb {
 
@@ -103,12 +106,94 @@ __device__ __forceinline__ void wgmma_tf32_n64(float* d, uint64_t da, uint64_t d
       : "l"(da), "l"(db), "r"(accumulate));
 }
 
+// fp16 operands (.f32.f16.f16): the same shapes, fragment layout and descriptors as the bf16 forms above.  Operand lists of
+// 16 / 32 / 64 / 128 accumulators, written once:
+#define MTB_ACC8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+#define MTB_ACC16(i) MTB_ACC8(i), MTB_ACC8(i + 8)
+#define MTB_ACC32(i) MTB_ACC16(i), MTB_ACC16(i + 16)
+#define MTB_ACC64(i) MTB_ACC32(i), MTB_ACC32(i + 32)
+#define MTB_ACC128(i) MTB_ACC64(i), MTB_ACC64(i + 64)
+
+// D (+)= A * B^T, M = 64, N = 32, K = 16 (fp16); accumulate = 0 overwrites D
+__device__ __forceinline__ void wgmma_f16_n32(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+      "%16, %17, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : MTB_ACC16(0)
+      : "l"(da), "l"(db), "r"(accumulate));
+}
+
+// D (+)= A * B^T, M = 64, N = 64, K = 16 (fp16); accumulate = 0 overwrites D
+__device__ __forceinline__ void wgmma_f16_n64(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : MTB_ACC32(0)
+      : "l"(da), "l"(db), "r"(accumulate));
+}
+
+// D (+)= A * B^T, M = 64, N = 128, K = 16 (fp16); accumulate = 0 overwrites D
+__device__ __forceinline__ void wgmma_f16_n128(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : MTB_ACC64(0)
+      : "l"(da), "l"(db), "r"(accumulate));
+}
+
+// D (+)= A * B^T, M = 64, N = 256, K = 16 (fp16); accumulate = 0 overwrites D
+__device__ __forceinline__ void wgmma_f16_n256(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %130, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : MTB_ACC128(0)
+      : "l"(da), "l"(db), "r"(accumulate));
+}
+#undef MTB_ACC128
+#undef MTB_ACC64
+#undef MTB_ACC32
+#undef MTB_ACC16
+#undef MTB_ACC8
+
 template <int N>
 __device__ __forceinline__ void wgmma_bf16(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
   if constexpr (N == 32) wgmma_bf16_n32(d, da, db, accumulate);
   else if constexpr (N == 64) wgmma_bf16_n64(d, da, db, accumulate);
   else if constexpr (N == 128) wgmma_bf16_n128(d, da, db, accumulate);
   else wgmma_bf16_n256(d, da, db, accumulate);
+}
+template <int N>
+__device__ __forceinline__ void wgmma_f16(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+  if constexpr (N == 32) wgmma_f16_n32(d, da, db, accumulate);
+  else if constexpr (N == 64) wgmma_f16_n64(d, da, db, accumulate);
+  else if constexpr (N == 128) wgmma_f16_n128(d, da, db, accumulate);
+  else wgmma_f16_n256(d, da, db, accumulate);
+}
+// 16-bit operands of element type T (__nv_bfloat16 or __half)
+template <typename T, int N>
+__device__ __forceinline__ void wgmma_16b(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+  if constexpr (std::is_same<T, __half>::value) wgmma_f16<N>(d, da, db, accumulate);
+  else wgmma_bf16<N>(d, da, db, accumulate);
 }
 template <int N>
 __device__ __forceinline__ void wgmma_tf32(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {

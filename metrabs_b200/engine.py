@@ -23,7 +23,8 @@ def make_config(cfg, n_joints, stages=None, last_channel=0, arch=_lib.ARCH_EFFNE
     c.abi_version = _lib.MTB_ABI_VERSION
     c.arch = arch
     c.precision = {'fp32': _lib.PRECISION_FP32, 'bf16': _lib.PRECISION_BF16_TC,
-                   'bf16_simt': _lib.PRECISION_BF16_SIMT, 'tf32x3': _lib.PRECISION_TF32X3}[cfg.precision]
+                   'bf16_simt': _lib.PRECISION_BF16_SIMT, 'tf32x3': _lib.PRECISION_TF32X3,
+                   'fp16': _lib.PRECISION_F16_TC, 'fp16_simt': _lib.PRECISION_F16_SIMT}[cfg.precision]
     c.device = device
     c.proc_side = int(cfg.proc_side)
     c.stride_train = int(cfg.stride_train)
@@ -70,8 +71,9 @@ class Engine:
         self.feature_side, self.feature_channels = hw.value, ch.value
         self.n_joints, self.depth = mtb_config.n_joints, mtb_config.depth
         self._recombination = None  # (host fp32 [L, n_out] weights, device copy) of a latent-point model
-        self.feature_dtype = (torch.float32 if mtb_config.precision in (_lib.PRECISION_FP32, _lib.PRECISION_TF32X3)
-                              else torch.bfloat16)
+        self.feature_dtype = {_lib.PRECISION_FP32: torch.float32, _lib.PRECISION_TF32X3: torch.float32,
+                              _lib.PRECISION_BF16_TC: torch.bfloat16, _lib.PRECISION_BF16_SIMT: torch.bfloat16,
+                              _lib.PRECISION_F16_TC: torch.float16, _lib.PRECISION_F16_SIMT: torch.float16}[mtb_config.precision]
 
     def close(self):
         if getattr(self, '_h', None):

@@ -21,7 +21,9 @@ class Config:
     transform_coords: bool = False
     predict_all_and_latents: bool = False
     regularize_to_manifold: bool = False
-    # build-specific: arithmetic of the conv kernels ('fp32' parity mode or 'bf16' tensor-core throughput mode)
+    # build-specific: arithmetic of the conv kernels: 'fp32' and 'tf32x3' (parity modes), 'bf16' (tensor-core throughput
+    # mode), 'fp16' (tensor cores, the reference's fp16-autocast arithmetic); 'bf16_simt' / 'fp16_simt' are their CUDA-core
+    # verification twins
     precision: str = 'fp32'
 
 
