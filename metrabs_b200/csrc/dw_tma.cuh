@@ -133,8 +133,9 @@ dw3x3s1_tma_kernel(const __grid_constant__ CUtensorMap tmIn, const DwTmaParams p
   constexpr int GSTEP = DWT_THREADS / DWT_CG;
   const int own_ch = tid & (DWT_CG - 1), own_g0 = tid / DWT_CG;  // blocksum owner: channel own_ch, crops own_g0, own_g0 + GSTEP, ...
 
-  // Items are walked last-to-first: the expand GEMM before this op wrote its output first-crop-to-last, so the END of the
-  // tensor is what the L2 still holds, and the BEGINNING of this op's output stays in L2 for the projection GEMM that follows.
+  // Items are walked last-to-first: the expand GEMM before this op wrote its output first-crop-to-last, all channels of a
+  // pixel block together (tc_conv_kernel's tile order is N fastest), so the END of the whole tensor is what the L2 still
+  // holds, and the BEGINNING of this op's output stays in L2 for the projection GEMM that follows.
   auto issue = [&](int it_, int stage) {
     const int it = p.items - 1 - it_;
     const int cg = it % p.n_cg;

@@ -10,12 +10,13 @@
 //                    epilogue thread owns one (d,j) channel and reduces its pixels in registers: the J x D x H x W logits
 //                    never leave the SM.
 //
-// One CTA per output tile of 128 rows (64 per consumer warpgroup) x BN columns; the 1-2 CTAs an SM holds overlap one tile's
-// epilogue with another's main loop.  Descriptor encodings: the sm_90 GMMA shared-memory descriptor (PTX ISA, "Matrix
-// Descriptor Format" of wgmma).
+// tc_conv_kernel is persistent (one CTA per SM walking output tiles of 128 rows x BN columns, two consumer warpgroups
+// taking alternate tiles, so one tile's epilogue overlaps the next tile's main loop); tc_head_kernel runs one CTA per tile.
+// Descriptor encodings: the sm_90 GMMA shared-memory descriptor (PTX ISA, "Matrix Descriptor Format" of wgmma).
 #pragma once
 #include <cuda.h>
 
+#include <algorithm>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -81,6 +82,20 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, u
       "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map), "r"(smem_u32(src)), "r"(c0),
+               "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, const void* src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(map), "r"(smem_u32(src)),
+               "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the shared-memory source of every committed bulk store has been read (it may be overwritten)
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
@@ -103,13 +118,21 @@ constexpr int TC_A_BYTES = TC_BM * TC_BK * 2;       // 16 KB
 constexpr int TC_THREADS = 288;                     // warps 0-7: two consumer warpgroups; warp 8: TMA producer
 constexpr int TC_CONSUMER_WARPS = 8;
 constexpr int TC_TILE_W = 16, TC_TILE_H = 8;        // spatial M tile of mode 1 (16 x 8 = 128 output pixels)
+constexpr int TCP_THREADS = 384;                    // tc_conv_kernel: warpgroup 0 TMA producer, warpgroups 1, 2 consumers
 
-// ring depth per N tile: 96 KB of stages at BN = 128 (two CTAs per SM), four stages below
+// tc_conv_kernel's shared memory (one CTA per SM): the ring, shared by the CTA's whole tile sequence, then one output staging
+// tile per consumer warpgroup, [BN / SW slabs][128 rows][SW columns] 16-bit in the TMA's swizzled layout (SW = 64: 128-byte
+// rows, SWIZZLE_128B; SW = 32: 64-byte rows, SWIZZLE_64B).  BN = 128: 5 x 32 KB + 2 x 32 KB; BN = 64: 8 x 24 KB + 2 x 16 KB;
+// BN = 32: 8 x 20 KB + 2 x 8 KB.
 template <int BN>
 struct TcRing {
-  static constexpr int stages = BN >= 128 ? 3 : 4;
+  static constexpr int stages = BN >= 128 ? 5 : 8;
   static constexpr int stage_bytes = TC_A_BYTES + BN * TC_BK * 2;
-  static constexpr int smem_bytes = stages * stage_bytes + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int slab_cols = BN < 64 ? BN : 64;
+  static constexpr int out_bytes = TC_BM * BN * 2;
+  static constexpr int out_off = stages * stage_bytes;
+  static constexpr int bar_off = out_off + 2 * out_bytes;
+  static constexpr int smem_bytes = bar_off + 256 /*barriers*/ + 1024 /*align slack*/;
 };
 
 struct TcConvParams {
@@ -122,7 +145,17 @@ struct TcConvParams {
   int Cout, Cin;
   int kchunks, taps;
   int Hout, Wout, tiles_w, tiles_h, pad_t, pad_l, S, stride, dil;
+  int m_tiles, n_tiles;  // tc_conv_kernel's tile grid (tile t = m_blk * n_tiles + n_blk)
 };
+
+// warpgroup register budgets of tc_conv_kernel: 128 x 40 + 256 x 232 = 64512 of the SM's 65536 registers
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+// named barrier between the two consumer warpgroups (256 threads): one side arrives, the other waits
+__device__ __forceinline__ void named_bar_sync(int id) { asm volatile("bar.sync %0, 256;" ::"r"(id) : "memory"); }
+__device__ __forceinline__ void named_bar_arrive(int id) { asm volatile("bar.arrive %0, 256;" ::"r"(id) : "memory"); }
 
 __device__ __forceinline__ float tanh_approx(float x) {
   float y;
@@ -176,104 +209,163 @@ __device__ __forceinline__ void tma_load_a_tile(void* dst, const CUtensorMap* ma
   }
 }
 
-// ACT: epilogue activation; RES: 0 no residual, 1 residual added AFTER the activation (EfficientNet), 2 BEFORE (ResNet);
-// BN: output channels per tile (wgmma N); T: operand and activation element type (__nv_bfloat16 or __half).
+// Persistent conv / GEMM kernel.  ACT: epilogue activation; RES: 0 no residual, 1 residual added AFTER the activation
+// (EfficientNet), 2 BEFORE (ResNet); BN: output channels per tile (wgmma N); T: operand and activation element type
+// (__nv_bfloat16 or __half).
+//
+// CTA b walks tiles t = b, b + gridDim.x, ...; tile t is (m_blk, n_blk) = (t / n_tiles, t % n_tiles): N fastest, so the CTAs
+// running at the same time cover every N tile of a few M blocks and each A tile comes from HBM once, the re-reads from L2.
+// Warpgroup 0 (one thread) streams the k-blocks of the CTA's whole tile sequence through one ring; consumer warpgroups 1
+// and 2 take alternate tiles (ping-pong), each owning a whole 128-row tile (two m64nBNk16 wgmmas per K step).  A named
+// barrier orders their main loops: a consumer starts waiting on its tile's stages only after the other finished the previous
+// tile's, which keeps every mbarrier wait within one phase of the barrier, and lets one warpgroup's epilogue run under the
+// other's MMAs.  Every output element sees the wgmma sequence and the roundings of a one-CTA-per-tile kernel.
 template <typename T, int ACT, int RES, int BN>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcConvParams p) {
+__global__ void __launch_bounds__(TCP_THREADS, 1)
+tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
+               const TcConvParams p) {
   using Ring = TcRing<BN>;
   constexpr int STAGES = Ring::stages;
   extern __shared__ uint8_t tc_smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)tc_smem_raw + 1023) & ~(uintptr_t)1023);  // SWIZZLE_128B needs 1024 B alignment
-  uint64_t* full = (uint64_t*)(smem + STAGES * Ring::stage_bytes);
+  uint64_t* full = (uint64_t*)(smem + Ring::bar_off);
   uint64_t* empty = full + STAGES;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == TC_CONSUMER_WARPS * 32) {
+  const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    tma_prefetch_desc(&tmO);
     for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full[i], 1);                  // the producer's arrive.expect_tx
-      mbar_init(&empty[i], TC_CONSUMER_WARPS); // one arrive per consumer warp
+      mbar_init(&full[i], 1);  // the producer's arrive.expect_tx
+      mbar_init(&empty[i], 4); // one arrive per warp of the consuming warpgroup
     }
     fence_barrier_init();
   }
   __syncthreads();
 
-  const int m_blk = blockIdx.x, n_blk = blockIdx.y;
+  const int tiles = p.m_tiles * p.n_tiles;
   const int num_kb = p.taps * p.kchunks;
-  if (warp == TC_CONSUMER_WARPS) {
+  if (wg == 0) {
     // ===== TMA producer =====
-    if (lane == 0) {
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % STAGES;
-        mbar_wait(&empty[s], ((kb / STAGES) & 1) ^ 1);
-        uint8_t* sa = smem + s * Ring::stage_bytes;
-        const int tap = kb / p.kchunks, kc = kb - tap * p.kchunks;
-        mbar_expect_tx(&full[s], Ring::stage_bytes);
-        tma_load_a_tile<TC_BK>(sa, &tmA, &full[s], p, m_blk, kb);
-        tma_load_2d(sa + TC_A_BYTES, &tmB, &full[s], tap * p.Cin + kc * TC_BK, n_blk * BN);
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      int it = 0;
+      for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+        const int m_blk = t / p.n_tiles, n_blk = t - m_blk * p.n_tiles;
+        for (int kb = 0; kb < num_kb; ++kb, ++it) {
+          const int s = it % STAGES;
+          mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
+          uint8_t* sa = smem + s * Ring::stage_bytes;
+          const int tap = kb / p.kchunks, kc = kb - tap * p.kchunks;
+          mbar_expect_tx(&full[s], Ring::stage_bytes);
+          tma_load_a_tile<TC_BK>(sa, &tmA, &full[s], p, m_blk, kb);
+          tma_load_2d(sa + TC_A_BYTES, &tmB, &full[s], tap * p.Cin + kc * TC_BK, n_blk * BN);
+        }
       }
     }
     return;
   }
-  // ===== consumers: warpgroup wg computes tile rows [64 wg, +64) =====
-  const int wg = warp >> 2;
-  float acc[BN / 2];
-#pragma unroll
-  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-  int prev = -1;
-  for (int kb = 0; kb < num_kb; ++kb) {
-    const int s = kb % STAGES;
-    mbar_wait(&full[s], (kb / STAGES) & 1);
-    const uint32_t a = smem_u32(smem + s * Ring::stage_bytes) + wg * 64 * 128;
-    const uint32_t b = smem_u32(smem + s * Ring::stage_bytes + TC_A_BYTES);
-    wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < TC_BK / 16; ++k) wgmma_16b<T, BN>(acc, gmma_desc<128>(a + 32 * k), gmma_desc<128>(b + 32 * k), (uint32_t)(kb | k));
-    wgmma_commit();
-    wgmma_wait<1>();  // the previous k-block's MMAs are done: its stage goes back to the producer
-    if (prev >= 0) {
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty[prev]);
-    }
-    prev = s;
-  }
-  wgmma_wait<0>();
-  wgmma_fence_regs<BN / 2>(acc);
-
-  // ===== epilogue: thread rows r0 = 64 wg + 16 (warp & 3) + lane / 4 and r0 + 8, columns 8 j + 2 (lane % 4) + {0, 1} =====
-  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-  const int c0 = n_blk * BN + 2 * (lane & 3);
+  // ===== consumers: warpgroup 1 + c computes the CTA's tiles c, c + 2, ... (rows [0, 64) in acc, [64, 128) in acc + BN/2) =====
+  setmaxnreg_inc<232>();
+  const int c = wg - 1;
+  constexpr int SW = Ring::slab_cols, RB = SW * 2;  // staging slab: columns, bytes per row
   typedef typename Pair16<T>::type T2;
   const T* __restrict__ res = (const T*)p.res;
-  T* __restrict__ out = (T*)p.out;
+  for (int i = c, t = blockIdx.x + c * gridDim.x; t < tiles; i += 2, t += 2 * gridDim.x) {
+    const int m_blk = t / p.n_tiles, n_blk = t - m_blk * p.n_tiles;
+    float acc[BN];
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    size_t off;
-    if (!tile_row_offset(p.mode, m_blk, r0 + 8 * h, p.M, p.Cout, p.tiles_w, p.tiles_h, p.Hout, p.Wout, off)) continue;
+    for (int q = 0; q < BN; ++q) acc[q] = 0.f;
+    if (t != (int)blockIdx.x) named_bar_sync(1 + c);  // the other consumer finished the previous tile's main loop
+    int it = i * num_kb, prev = -1;
+    for (int kb = 0; kb < num_kb; ++kb, ++it) {
+      const int s = it % STAGES;
+      mbar_wait(&full[s], (it / STAGES) & 1);
+      const uint32_t a = smem_u32(smem + s * Ring::stage_bytes);
+      const uint32_t b = smem_u32(smem + s * Ring::stage_bytes + TC_A_BYTES);
+      wgmma_fence();
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int c = c0 + 8 * j;
-      if (c >= p.Cout) break;  // Cout % 8 == 0: column c + 1 is valid with c
-      const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + c));
-      float o0 = acc[4 * j + 2 * h] + bv.x, o1 = acc[4 * j + 2 * h + 1] + bv.y;
-      if constexpr (RES != 0) {
-        const float2 rv = Pair16<T>::unpack(*reinterpret_cast<const T2*>(res + off + c));
-        if constexpr (RES == 2) {
-          o0 = tc_act<ACT, T>(o0 + rv.x);
-          o1 = tc_act<ACT, T>(o1 + rv.y);
-        } else {
-          o0 = tc_act<ACT, T>(o0) + rv.x;
-          o1 = tc_act<ACT, T>(o1) + rv.y;
-        }
-      } else {
-        o0 = tc_act<ACT, T>(o0);
-        o1 = tc_act<ACT, T>(o1);
+      for (int k = 0; k < TC_BK / 16; ++k) {
+        const uint64_t db = gmma_desc<128>(b + 32 * k);
+        wgmma_16b<T, BN>(acc, gmma_desc<128>(a + 32 * k), db, (uint32_t)(kb | k));
+        wgmma_16b<T, BN>(acc + BN / 2, gmma_desc<128>(a + 64 * 128 + 32 * k), db, (uint32_t)(kb | k));
       }
-      *reinterpret_cast<T2*>(out + off + c) = Pair16<T>::pack(o0, o1);
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous k-block's MMAs are done: its stage goes back to the producer
+      if (prev >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[prev]);
+      }
+      prev = s;
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs<BN>(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[prev]);
+    if (t + (int)gridDim.x < tiles) named_bar_arrive(2 - c);  // the other consumer may start the next tile
+
+    // ===== epilogue: rows 64 mh + 16 warp + lane / 4 (+ 8 h), columns 8 j + 2 (lane % 4) + {0, 1} -> staging tile =====
+    const bool leader = (threadIdx.x & 127) == 0;  // issues and waits for this warpgroup's bulk stores
+    uint8_t* stg = smem + Ring::out_off + c * Ring::out_bytes;
+    if (leader) bulk_wait_read();  // the previous tile's stores have read the staging tile
+    wg_sync(2 + c);                // named barriers 3, 4 (1 and 2 order the main loops)
+    const int c0 = n_blk * BN + 2 * (lane & 3);
+#pragma unroll
+    for (int mh = 0; mh < 2; ++mh) {
+      const float* accm = acc + mh * (BN / 2);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = mh * 64 + warp * 16 + (lane >> 2) + 8 * h;
+        size_t off = 0;
+        if constexpr (RES != 0) {
+          if (!tile_row_offset(p.mode, m_blk, r, p.M, p.Cout, p.tiles_w, p.tiles_h, p.Hout, p.Wout, off)) continue;
+        }
+        const uint32_t swz = RB == 128 ? (uint32_t)(r & 7) : (uint32_t)((r >> 1) & 3);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int cc = c0 + 8 * j;
+          if (cc >= p.Cout) break;  // Cout % 8 == 0: column cc + 1 is valid with cc
+          const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + cc));
+          float o0 = accm[4 * j + 2 * h] + bv.x, o1 = accm[4 * j + 2 * h + 1] + bv.y;
+          if constexpr (RES != 0) {
+            const float2 rv = Pair16<T>::unpack(*reinterpret_cast<const T2*>(res + off + cc));
+            if constexpr (RES == 2) {
+              o0 = tc_act<ACT, T>(o0 + rv.x);
+              o1 = tc_act<ACT, T>(o1 + rv.y);
+            } else {
+              o0 = tc_act<ACT, T>(o0) + rv.x;
+              o1 = tc_act<ACT, T>(o1) + rv.y;
+            }
+          } else {
+            o0 = tc_act<ACT, T>(o0);
+            o1 = tc_act<ACT, T>(o1);
+          }
+          const int col = 8 * j + 2 * (lane & 3), cs = col % SW;  // column within the tile, within its slab
+          const uint32_t o = (uint32_t)(col / SW) * (TC_BM * RB) + (uint32_t)r * RB + ((((uint32_t)cs >> 3) ^ swz) << 4) + (cs & 7) * 2;
+          *reinterpret_cast<T2*>(stg + o) = Pair16<T>::pack(o0, o1);
+        }
+      }
+    }
+    fence_proxy_async();  // generic-proxy writes -> visible to the TMA (async proxy)
+    wg_sync(2 + c);
+    // The TMA clips what lies outside the tensor: the M tail, the parts of a 16 x 8 box beyond the map, the Cout tail.
+    if (leader) {
+#pragma unroll
+      for (int sl = 0; sl < BN / SW; ++sl) {
+        const int col0 = n_blk * BN + sl * SW;
+        if (col0 >= p.Cout) break;
+        if (p.mode == 0) {
+          tma_store_2d(&tmO, stg + sl * TC_BM * RB, col0, m_blk * TC_BM);
+        } else {
+          const int tw = m_blk % p.tiles_w, th = (m_blk / p.tiles_w) % p.tiles_h, b = m_blk / (p.tiles_w * p.tiles_h);
+          tma_store_4d(&tmO, stg + sl * TC_BM * RB, col0, tw * TC_TILE_W, th * TC_TILE_H, b);
+        }
+      }
+      bulk_commit();
     }
   }
+  if ((threadIdx.x & 127) == 0) bulk_wait();
 }
 
 // in-place squeeze-excitation scaling  x[b,p,c] *= s[b,c]  ahead of a tensor-core projection GEMM (T: bf16 or fp16)
@@ -364,10 +456,12 @@ struct TcWeights {
   mutable CUtensorMap mapA, mapB;
   mutable const void* cached_in = nullptr;
   mutable int cached_B = -1;
-  // conv path: tensor maps per (input, batch, N tile) - re-encoding them per launch would sit on the host's launch path
+  // conv path: tensor maps (input, weights, output) per (input, output, batch, N tile) - re-encoding them per launch would
+  // sit on the host's launch path
   struct MapSet {
-    CUtensorMap a, b;
+    CUtensorMap a, b, o;
     const void* in = nullptr;
+    const void* out = nullptr;
     int B = -1, bn = 0;
   };
   mutable std::vector<MapSet> map_sets;
@@ -423,7 +517,7 @@ inline const char* tc_prepare_weights(TcWeights& w, const float* wk, const float
 inline int tc_pick_bn(int cout) { return cout <= 32 ? 32 : cout <= 64 ? 64 : 128; }
 
 template <typename T, int ACT, int RES, int BN>
-inline const char* tc_conv_launch_k(dim3 grid, const CUtensorMap& a, const CUtensorMap& b, const TcConvParams& q, cudaStream_t st) {
+inline const char* tc_conv_launch_k(dim3 grid, const TcWeights::MapSet& ms, const TcConvParams& q, cudaStream_t st) {
   static bool attr_set = false;
   if (!attr_set) {
     if (cudaFuncSetAttribute(tc_conv_kernel<T, ACT, RES, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcRing<BN>::smem_bytes) !=
@@ -431,25 +525,25 @@ inline const char* tc_conv_launch_k(dim3 grid, const CUtensorMap& a, const CUten
       return "cannot raise dynamic shared memory for tc_conv_kernel";
     attr_set = true;
   }
-  launch_k(tc_conv_kernel<T, ACT, RES, BN>, grid, dim3(TC_THREADS), TcRing<BN>::smem_bytes, st, a, b, q);
+  launch_k(tc_conv_kernel<T, ACT, RES, BN>, grid, dim3(TCP_THREADS), TcRing<BN>::smem_bytes, st, ms.a, ms.b, ms.o, q);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 template <typename T, int ACT, int RES>
-inline const char* tc_conv_launch_t(int bn, dim3 grid, const CUtensorMap& a, const CUtensorMap& b, const TcConvParams& q, cudaStream_t st) {
+inline const char* tc_conv_launch_t(int bn, dim3 grid, const TcWeights::MapSet& ms, const TcConvParams& q, cudaStream_t st) {
   switch (bn) {
-    case 32: return tc_conv_launch_k<T, ACT, RES, 32>(grid, a, b, q, st);
-    case 64: return tc_conv_launch_k<T, ACT, RES, 64>(grid, a, b, q, st);
-    default: return tc_conv_launch_k<T, ACT, RES, 128>(grid, a, b, q, st);
+    case 32: return tc_conv_launch_k<T, ACT, RES, 32>(grid, ms, q, st);
+    case 64: return tc_conv_launch_k<T, ACT, RES, 64>(grid, ms, q, st);
+    default: return tc_conv_launch_k<T, ACT, RES, 128>(grid, ms, q, st);
   }
 }
 template <typename T, int ACT>
-inline const char* tc_conv_dispatch_res(int res_mode, int bn, dim3 grid, const CUtensorMap& a, const CUtensorMap& b, const TcConvParams& q,
+inline const char* tc_conv_dispatch_res(int res_mode, int bn, dim3 grid, const TcWeights::MapSet& ms, const TcConvParams& q,
                                         cudaStream_t st) {
   switch (res_mode) {
-    case 0: return tc_conv_launch_t<T, ACT, 0>(bn, grid, a, b, q, st);
-    case 1: return tc_conv_launch_t<T, ACT, 1>(bn, grid, a, b, q, st);
-    default: return tc_conv_launch_t<T, ACT, 2>(bn, grid, a, b, q, st);
+    case 0: return tc_conv_launch_t<T, ACT, 0>(bn, grid, ms, q, st);
+    case 1: return tc_conv_launch_t<T, ACT, 1>(bn, grid, ms, q, st);
+    default: return tc_conv_launch_t<T, ACT, 2>(bn, grid, ms, q, st);
   }
 }
 
@@ -467,19 +561,24 @@ inline const char* tc_conv_launch(const TcWeights& w, const ConvParams& p, bool 
   q.tiles_w = (p.Wout + TC_TILE_W - 1) / TC_TILE_W;
   q.tiles_h = (p.Hout + TC_TILE_H - 1) / TC_TILE_H;
   q.M = p.B * p.Hout * p.Wout;
-  const int m_tiles = q.mode == 0 ? (q.M + TC_BM - 1) / TC_BM : p.B * q.tiles_w * q.tiles_h;
   const int bn = tc_pick_bn(p.Cout);
+  q.m_tiles = q.mode == 0 ? (q.M + TC_BM - 1) / TC_BM : p.B * q.tiles_w * q.tiles_h;
+  q.n_tiles = (p.Cout + bn - 1) / bn;
   const TcWeights::MapSet* ms = nullptr;
   for (const TcWeights::MapSet& c : w.map_sets)
-    if (c.in == p.in && c.B == p.B && c.bn == bn) { ms = &c; break; }
+    if (c.in == p.in && c.out == p.out && c.B == p.B && c.bn == bn) { ms = &c; break; }
   if (!ms) {
     TcWeights::MapSet c;
+    const uint32_t slab = (uint32_t)std::min(bn, 64);  // output box: 64 (SWIZZLE_128B) or 32 (SWIZZLE_64B) channels
     const char* e = q.mode == 0 ? make_tmap_2d<T>(&c.a, p.in, (uint64_t)q.M, (uint64_t)p.Cin, TC_BM)
                                 : make_tmap_nhwc<T>(&c.a, p.in, p.B, p.Hin, p.Win, p.Cin, (uint32_t)p.stride);
     if (e) return e;
     e = make_tmap_2d<T>(&c.b, w.d_w, (uint64_t)p.Cout, (uint64_t)w.taps * p.Cin, (uint32_t)bn);
     if (e) return e;
-    c.in = p.in; c.B = p.B; c.bn = bn;
+    e = q.mode == 0 ? make_tmap_2d<T>(&c.o, p.out, (uint64_t)q.M, (uint64_t)p.Cout, TC_BM, slab)
+                    : make_tmap_nhwc<T>(&c.o, p.out, p.B, p.Hout, p.Wout, p.Cout, 1, slab);
+    if (e) return e;
+    c.in = p.in; c.out = p.out; c.B = p.B; c.bn = bn;
     if (w.map_sets.size() < 16) {
       w.map_sets.push_back(c);
       ms = &w.map_sets.back();
@@ -489,13 +588,13 @@ inline const char* tc_conv_launch(const TcWeights& w, const ConvParams& p, bool 
       ++w.map_rr;
     }
   }
-  const dim3 grid(m_tiles, (p.Cout + bn - 1) / bn);
+  const dim3 grid(std::min(q.m_tiles * q.n_tiles, num_sms()));  // persistent: one CTA per SM
   const int res_mode = p.res ? (res_first ? 2 : 1) : 0;
   switch (p.act) {
-    case ACT_NONE: return tc_conv_dispatch_res<T, ACT_NONE>(res_mode, bn, grid, ms->a, ms->b, q, st);
-    case ACT_SILU: return tc_conv_dispatch_res<T, ACT_SILU>(res_mode, bn, grid, ms->a, ms->b, q, st);
-    case ACT_RELU: return tc_conv_dispatch_res<T, ACT_RELU>(res_mode, bn, grid, ms->a, ms->b, q, st);
-    case ACT_HSWISH: return tc_conv_dispatch_res<T, ACT_HSWISH>(res_mode, bn, grid, ms->a, ms->b, q, st);
+    case ACT_NONE: return tc_conv_dispatch_res<T, ACT_NONE>(res_mode, bn, grid, *ms, q, st);
+    case ACT_SILU: return tc_conv_dispatch_res<T, ACT_SILU>(res_mode, bn, grid, *ms, q, st);
+    case ACT_RELU: return tc_conv_dispatch_res<T, ACT_RELU>(res_mode, bn, grid, *ms, q, st);
+    case ACT_HSWISH: return tc_conv_dispatch_res<T, ACT_HSWISH>(res_mode, bn, grid, *ms, q, st);
     default: return "unsupported activation in the tensor-core epilogue";
   }
 }
