@@ -4,75 +4,300 @@
 ``/root/reference/metrabs_pytorch/backbones/efficientnet.py`` :110-173 MBConv, :176-234 FusedMBConv, :290-293 stem,
 :319-324 last conv, :1127-1161 fixed padding; eval-mode BatchNorm eps 1e-3 :1051) so that a single device launch
 (``mtb_debug_run_op``) can be compared with plain ``torch.nn.functional.conv2d`` arithmetic on identical operands instead
-of with another kernel of this repository.
+of with another kernel of this repository.  The ResNet-50 and MobileNetV3-small layers are those of
+``oracle/port_tf_backbones.py`` (stride / dilation plan, ``_depth``, BN eps, preprocessing, correct_pad).
 
 ``precision``:
 * ``'exact'``  conv -> BN (eval) -> act -> (+res) evaluated in the requested dtype (fp64 on the CPU, fp32 on the GPU with
                TF32 disabled): the bar for the fp32 / 3xTF32 kernels.
-* ``'bf16'``   the SAME arithmetic at the roundings the bf16 tensor-core mode defines: BN folded into the conv weight in
-               fp64 and rounded ONCE to bf16 (``w*gamma/sqrt(var+eps)``), bf16 input (and bf16(scale*x) for a
-               squeeze-excitation projection), wide accumulation, fp32 bias, act, +res; the caller rounds the result to
-               bf16 or allows one bf16 ulp.
+* ``'bf16'``, ``'bf16_simt'``, ``'fp16'``, ``'fp16_simt'``: the SAME arithmetic at the rounding points of that engine mode
+  (csrc/engine.cu ``mtb_finalize_weights`` op loop and ``run_op_t``):
+  - BN is folded in fp64 and the folded weight / bias cast to fp32 (engine.cu:615-624);
+  - the weights of ops that pass ``tc_eligible`` (csrc/tc_gemm.cuh:471-475) are then rounded ONCE to the 16-bit storage
+    type, in the tensor-core AND the CUDA-core mode of that type (engine.cu:625-630); depthwise and stem weights stay fp32;
+  - the squeeze-excitation scaled input ``x*s`` is formed in fp32 and rounded to 16 bits in the tensor-core modes
+    (``se_scale_kernel`` in place ahead of the GEMM, engine.cu:794-801); the CUDA-core modes keep the fp32 product
+    (``conv_igemm_kernel`` a_scale, csrc/conv_simt.cuh:97-99);
+  - everything else is wide; the device rounds the result once to 16 bits.
+  ``layer_bound`` gives the per-element tolerance of that device result; ``'bf16'`` alone keeps its old meaning.
 """
+import math
+
 import torch
 import torch.nn.functional as F
 
 from oracle import port
+from oracle import port_tf_backbones as tfb
+
+# engine mode -> (16-bit storage dtype, tensor-core kernels)
+MODES = {'bf16': (torch.bfloat16, True), 'bf16_simt': (torch.bfloat16, False),
+         'fp16': (torch.float16, True), 'fp16_simt': (torch.float16, False)}
+
+
+def _op(weight, kernel=1, stride=1, pad=(0, 0), dil=1, act=None, depthwise=False, bn=None, eps=port.BN_EPS_EFFNETV2,
+        bias=None, sample=None, res_first=False, pre=None, shift=0):
+    """One engine op.  pad: explicit zero pad (begin, end) on both spatial axes, then VALID; sample: dense conv evaluated
+    at pixels ``shift::stride`` instead (Conv2DDenseSame); pre: per-channel (scale, shift) of the stem input."""
+    return dict(weight=weight, kernel=kernel, stride=stride, pad=pad, dil=dil, act=act, depthwise=depthwise, bn=bn, eps=eps,
+                bias=bias, sample=sample, res_first=res_first, pre=pre, stem=pre is not None, shift=shift, maxpool=False)
+
+
+def _effnet_conv(key, k, stride, shift, act, depthwise=False, stem=False):
+    pb = (k - 1) // 2
+    return _op(key + '.0.weight', k, stride, (pb - shift, k - 1 - pb + shift), act='silu' if act else None,
+               depthwise=depthwise, bn=key + '.1', pre=((2.0,) * 3, (-1.0,) * 3) if stem else None, shift=shift)
 
 
 def effnet_op_table(spec: port.EffNetSpec, prefix='backbone.1'):
-    """engine op name (= reference key prefix of the layer) -> dict(stride, shift, act, depthwise, kernel)."""
-    t = {f'{prefix}.0': dict(stride=2, shift=0, act=True, depthwise=False, kernel=3, stem=True)}
+    """engine op name (= reference key prefix of the layer) -> op dict (see _op)."""
+    t = {f'{prefix}.0': _effnet_conv(f'{prefix}.0', 3, 2, 0, True, stem=True)}
     for b in port.effnet_block_list(spec):
         key = f'{prefix}.{b["key"]}.block'
         if b['block'] == 'fused':
-            t[f'{key}.0'] = dict(stride=b['stride'], shift=b['shift'], act=True, depthwise=False, kernel=b['kernel'])
+            t[f'{key}.0'] = _effnet_conv(f'{key}.0', b['kernel'], b['stride'], b['shift'], True)
             if b['expand'] != 1:
-                t[f'{key}.1'] = dict(stride=1, shift=0, act=False, depthwise=False, kernel=1)
+                t[f'{key}.1'] = _effnet_conv(f'{key}.1', 1, 1, 0, False)
         else:
             i = 0
             if b['expand'] != 1:
-                t[f'{key}.{i}'] = dict(stride=1, shift=0, act=True, depthwise=False, kernel=1)
+                t[f'{key}.{i}'] = _effnet_conv(f'{key}.{i}', 1, 1, 0, True)
                 i += 1
-            t[f'{key}.{i}'] = dict(stride=b['stride'], shift=b['shift'], act=True, depthwise=True, kernel=b['kernel'])
+            t[f'{key}.{i}'] = _effnet_conv(f'{key}.{i}', b['kernel'], b['stride'], b['shift'], True, depthwise=True)
             i += 2  # squeeze-excitation sits between the depthwise conv and the projection
-            t[f'{key}.{i}'] = dict(stride=1, shift=0, act=False, depthwise=False, kernel=1)
-    t[f'{prefix}.{len(spec.stages) + 1}'] = dict(stride=1, shift=0, act=True, depthwise=False, kernel=1)
+            t[f'{key}.{i}'] = _effnet_conv(f'{key}.{i}', 1, 1, 0, False)
+    t[f'{prefix}.{len(spec.stages) + 1}'] = _effnet_conv(f'{prefix}.{len(spec.stages) + 1}', 1, 1, 0, True)
     return t
 
 
-def fold_conv_bn(sd, key, eps=port.BN_EPS_EFFNETV2):
-    """Conv2dNormActivation in eval mode as one affine conv: (w * g/sqrt(v+eps), b - m*g/sqrt(v+eps)), in fp64."""
-    w = sd[key + '.0.weight'].double()
-    g, b = sd[key + '.1.weight'].double(), sd[key + '.1.bias'].double()
-    m, v = sd[key + '.1.running_mean'].double(), sd[key + '.1.running_var'].double()
-    s = g / torch.sqrt(v + eps)
-    return w * s[:, None, None, None], b - m * s
+def resnet50_op_table(cfg: port.PathConfig, prefix='backbone.'):
+    """ResNet50Spec.features (oracle/port_tf_backbones.py): conv bias folded by BN (eps 1e-5), caffe stem, zero-padded
+    max pool, dense-SAME 1x1 convs sampled at shift::stride, dilated 3x3, relu(shortcut + _3_conv)."""
+    e = tfb.RESNET_BN_EPS
+    mean = torch.tensor([103.939, 116.779, 123.68])  # fp32 constants, as in port_tf_backbones and the stem kernel
+    t = {prefix + 'conv1_conv': _op(prefix + 'conv1_conv.weight', 7, 2, (3, 3), act='relu', bn=prefix + 'conv1_bn', eps=e,
+                                    bias=prefix + 'conv1_conv.bias', pre=((255.0,) * 3, tuple((-mean).double().tolist())))}
+    t[prefix + 'pool1_pool'] = dict(_op(None, 3, 2, (1, 1)), maxpool=True)
+    for name, _f, stride, shift, dil, conv_shortcut in tfb.resnet50_blocks(cfg):
+        b = prefix + name
+
+        def cb(j, k=1, **kw):
+            return _op(f'{b}_{j}_conv.weight', k, bn=f'{b}_{j}_bn', eps=e, bias=f'{b}_{j}_conv.bias', **kw)
+        if conv_shortcut:
+            t[f'{b}_0_conv'] = cb(0, stride=stride, sample=shift, shift=shift)
+        t[f'{b}_1_conv'] = cb(1, stride=stride, sample=shift, shift=shift, act='relu')
+        t[f'{b}_2_conv'] = cb(2, 3, pad=(dil, dil), dil=dil, act='relu')
+        t[f'{b}_3_conv'] = cb(3, act='relu', res_first=True)
+    return t
 
 
-def conv_layer_reference(sd, spec, name, x_nhwc, res_nhwc=None, scale=None, precision='exact', dtype=torch.float64):
-    """One conv layer of EfficientNet.features on ``x_nhwc`` [B,H,W,C] (the stem takes NCHW crops in [0,1] and applies
-    PreprocLayer x*2-1, efficientnet.py:1181-1186).  Returns NHWC in ``dtype``."""
-    op = effnet_op_table(spec)[name]
+def mobilenetv3_small_op_table(cfg: port.PathConfig, prefix='backbone.'):
+    """MobileNetV3SmallSpec.features (oracle/port_tf_backbones.py): TF-'same' stem on 2x-1, correct_pad before the
+    stride-2 depthwise convs, ReLU / hard-swish, projection without activation (+ residual), Conv_2 with bias and no BN."""
+    e = tfb.MOBILENET_BN_EPS
+    s = cfg.proc_side
+    pad_total = max(((s + 1) // 2 - 1) * 2 + 3 - s, 0)
+    t = {prefix + 'Conv': _op(prefix + 'Conv.weight', 3, 2, (pad_total // 2, pad_total - pad_total // 2), act='hswish',
+                              bn=prefix + 'Conv.BatchNorm', eps=e, pre=((2.0,) * 3, (-1.0,) * 3))}
+    for bi, (_exp, _filters, k, stride, _se, act, br) in enumerate(tfb.MOBILENETV3_SMALL_ROWS):
+        b = prefix + ('expanded_conv' if bi == 0 else f'expanded_conv_{bi}')
+        act = 'hswish' if act == 'hswish' else 'relu'
+        if bi != 0:
+            t[b + '.expand'] = _op(b + '.expand.weight', act=act, bn=b + '.expand.BatchNorm', eps=e)
+        shift = 1 if (br and cfg.centered_stride and stride == 2) else 0
+        pb = (k - 1) // 2
+        t[b + '.depthwise'] = _op(b + '.depthwise.weight', k, stride, (pb - shift, k - 1 - pb + shift), act=act, depthwise=True,
+                                  bn=b + '.depthwise.BatchNorm', eps=e, shift=shift)
+        t[b + '.project'] = _op(b + '.project.weight', bn=b + '.project.BatchNorm', eps=e)
+    t[prefix + 'Conv_1'] = _op(prefix + 'Conv_1.weight', act='hswish', bn=prefix + 'Conv_1.BatchNorm', eps=e)
+    t[prefix + 'Conv_2'] = _op(prefix + 'Conv_2.weight', act='hswish', bias=prefix + 'Conv_2.bias')
+    return t
+
+
+def op_table(spec):
+    if isinstance(spec, tfb.ResNet50Spec):
+        return resnet50_op_table(spec.cfg)
+    if isinstance(spec, tfb.MobileNetV3SmallSpec):
+        return mobilenetv3_small_op_table(spec.cfg)
+    return effnet_op_table(spec)
+
+
+def _fold(sd, op):
+    """(w, b) of an op with the conv bias folded through BN as (b - mean) * s + beta (engine.cu:609-613), in fp64."""
+    w = sd[op['weight']].double()
+    b = sd[op['bias']].double() if op['bias'] else torch.zeros(w.shape[0], dtype=torch.float64)
+    if op['bn']:
+        k = op['bn']
+        s = sd[k + '.weight'].double() / torch.sqrt(sd[k + '.running_var'].double() + op['eps'])
+        w = w * s[:, None, None, None]
+        b = (b - sd[k + '.running_mean'].double()) * s + sd[k + '.bias'].double()
+    return w, b
+
+
+def tc_eligible(op, cin, cout):
+    """tc_eligible (csrc/tc_gemm.cuh:471-475): the convs whose weights the 16-bit modes round to 16 bits."""
+    return (not op['stem'] and not op['depthwise'] and not op['maxpool'] and cin % 8 == 0 and cout % 8 == 0
+            and op['stride'] in (1, 2) and op['kernel'] in (1, 3))
+
+
+def _act(y, act):
+    if act == 'silu':
+        return F.silu(y)
+    if act == 'relu':
+        return F.relu(y)
+    if act == 'hswish':
+        return tfb.hard_swish(y)
+    if act == 'sigmoid':
+        return torch.sigmoid(y)
+    if act == 'hsigmoid':
+        return tfb.hard_sigmoid(y)
+    return y
+
+
+def _layer(sd, spec, name, x_nhwc, res_nhwc, scale, precision, dtype, magnitude=False):
+    """-> (output NCHW, pre-activation NCHW, products per output).  magnitude: the same layer on |x|, |w|, |b|, |res| with
+    no activation (the pre-activation magnitude that bounds the accumulation error)."""
+    op = op_table(spec)[name]
     dev = x_nhwc.device
-    w, bias = fold_conv_bn(sd, name)
-    if precision == 'bf16' and not op['depthwise'] and not op.get('stem'):
-        w = w.float().bfloat16().double()  # the tensor-core weights; depthwise / stem weights stay fp32 on the device
+    if op['maxpool']:  # zero pad (the pad value takes part in the max), then VALID
+        x = x_nhwc.permute(0, 3, 1, 2).to(dtype)
+        x = x.abs() if magnitude else x
+        y = F.max_pool2d(F.pad(x, op['pad'] * 2), op['kernel'], op['stride'])
+        return y, y, 1
+    w, bias = _fold(sd, op)
+    st = MODES[precision][0] if precision in MODES else None
+    if st is not None:
+        w, bias = w.float().double(), bias.float().double()
+        if tc_eligible(op, w.shape[1], w.shape[0]):
+            w = w.float().to(st).double()
     w, bias = w.to(dev, dtype), bias.to(dev, dtype)
-    if op.get('stem'):
-        x = x_nhwc.to(dtype) * 2 - 1
+    if op['stem']:
+        a, c = (torch.tensor(v, dtype=torch.float32).to(dev, dtype)[None, :, None, None] for v in op['pre'])
+        x = x_nhwc.to(dtype)
+        x = (x * a).abs() + c.abs() if magnitude else x * a + c  # magnitude also bounds the fp32 rounding of x*a + c
     else:
         x = x_nhwc.permute(0, 3, 1, 2).to(dtype)
     if scale is not None:
-        x = x * scale.to(dev, dtype)[:, :, None, None]
-        if precision == 'bf16':
-            x = x.float().bfloat16().to(dtype)
-    if op['kernel'] > 1:
-        x = port._fixed_pad(x, op['kernel'], op['shift'])
-    y = F.conv2d(x, w, bias, stride=op['stride'], groups=x.shape[1] if op['depthwise'] else 1)
-    if op['act']:
-        y = F.silu(y)
-    y = y.permute(0, 2, 3, 1)
+        s = scale.to(dev, dtype)[:, :, None, None]
+        if st is not None and MODES[precision][1] and not magnitude:  # se_scale_kernel: fp32 product, rounded to 16 bits
+            x = (x.float() * s.float()).to(st).to(dtype)
+        else:
+            x = x * s
+    if magnitude:
+        x, w, bias = x.abs(), w.abs(), bias.abs()
+    x = F.pad(x, op['pad'] * 2)
+    groups = x.shape[1] if op['depthwise'] else 1
+    if op['sample'] is not None:
+        z = F.conv2d(x, w, bias, dilation=op['dil'])[:, :, op['sample']::op['stride'], op['sample']::op['stride']]
+    else:
+        z = F.conv2d(x, w, bias, stride=op['stride'], dilation=op['dil'], groups=groups)
+    k = w.shape[1] * w.shape[2] * w.shape[3]
+    res = None
     if res_nhwc is not None:
-        y = y + res_nhwc.to(dtype)
-    return y.contiguous()
+        res = res_nhwc.permute(0, 3, 1, 2).to(dtype)
+        res = res.abs() if magnitude else res
+    if res is not None and op['res_first']:
+        z = z + res
+    y = z if magnitude else _act(z, op['act'])
+    if res is not None and not op['res_first']:
+        y = y + res
+    return y, z, k
+
+
+def conv_layer_reference(sd, spec, name, x_nhwc, res_nhwc=None, scale=None, precision='exact', dtype=torch.float64):
+    """One conv layer (or the max pool) of the backbone on ``x_nhwc`` [B,H,W,C] (the stem takes NCHW crops in [0,1] and
+    applies the model's preprocessing).  Returns NHWC in ``dtype``."""
+    return _layer(sd, spec, name, x_nhwc, res_nhwc, scale, precision, dtype)[0].permute(0, 2, 3, 1).contiguous()
+
+
+# ---------------------------------------------------------------------------------------------- per-element bound
+# Accumulation: any fp32 summation order of n terms errs by at most gamma_n = n*u/(1-n*u) times the sum of |terms|
+# (u = 2^-24 for round-to-nearest).  C_ACC = 2 allows u = 2^-23 (the tensor cores' fp32 accumulate aligns and truncates
+# rather than rounding to nearest) and the 1/(1-n*u) factor; n = products + bias + residual + the fp32 x*s / stem
+# preprocessing products, so K + 4.
+C_ACC = 2.0
+# tanh.approx.f32: maximum relative error 2^-10.987 (PTX ISA, tanh instruction)
+TANH_APPROX_REL = 2.0 ** -10.987
+# sup |act'|: SiLU 1.0998 (x = 2.40), hard-swish 1.5 (x = 3), ReLU / none 1, sigmoid 1/4, hard-sigmoid 1/6
+LIPSCHITZ = {'silu': 1.1, 'hswish': 1.5, 'relu': 1.0, None: 1.0, 'sigmoid': 0.25, 'hsigmoid': 1.0 / 6.0}
+
+
+def _act_error(z, y, act, precision):
+    """|device activation - exact activation| at pre-activation z (y = act(z))."""
+    az, ay = z.abs(), y.abs()
+    if act == 'silu' and precision == 'bf16':
+        # tc_act / fast_act for bf16 outputs: h + h*tanh.approx(h), h = x/2 (csrc/tc_gemm.cuh:169-183, conv_simt.cuh:272-287)
+        h = 0.5 * az
+        return h * torch.tanh(h) * TANH_APPROX_REL + 2.0 ** -22 * (az + ay)
+    if act in ('silu', 'sigmoid'):
+        # silu_f16out (ex2.approx + rcp.approx, csrc/common.cuh:156-166) and act_t (x / (1 + __expf(-x))): the fp32 rounding
+        # of x*log2(e) gives |x|*2^-24 relative error in e^-x, plus a few ulps from ex2 / rcp / mul; |dsig/sig| <= |de/e|
+        return (8.0 + 2.0 * az) * 2.0 ** -24 * ay
+    if act == 'hswish':  # x * sat(x/6 + 0.5): the rounded 1/6, the fma and the product
+        return 2.0 ** -22 * (az + ay)
+    if act == 'hsigmoid':  # min(max(x + 3, 0), 6) * (1/6): the sum, the rounded 1/6 and the product
+        return 2.0 ** -22 * (az + 3.0)
+    return torch.zeros_like(z)
+
+
+def layer_bound(sd, spec, name, x_nhwc, res_nhwc=None, scale=None, precision='fp16'):
+    """-> (ref, tol), NHWC fp64: the exact layer on this mode's rounded operands and the per-element bound on
+    |device - ref| for the device's 16-bit output,
+
+        tol = 2^-p * (|ref| + e) + e + floor,   e = L_act * C_ACC * (K + 4) * 2^-24 * refabs + e_act + 2^-23 * |ref|
+
+    with p = 8 (bf16) / 11 (fp16) (half an ulp of the output, rounded to nearest even), floor = half the fp16 subnormal
+    spacing (2^-25), refabs the pre-activation magnitude (the layer on |x|, |w|, |b|, |res|), e_act the activation's own
+    error (_act_error) and 2^-23 * |ref| the fp32 residual add / epilogue roundings."""
+    st = MODES[precision][0]
+    op = op_table(spec)[name]
+    y, z, k = _layer(sd, spec, name, x_nhwc, res_nhwc, scale, precision, torch.float64)
+    zabs = _layer(sd, spec, name, x_nhwc, res_nhwc, scale, precision, torch.float64, magnitude=True)[1]
+    if op['maxpool']:  # a max of 16-bit values is exact
+        tol = torch.zeros_like(y)
+    else:
+        a = _act(z, op['act'])
+        e = (LIPSCHITZ[op['act']] * C_ACC * (k + 4) * 2.0 ** -24 * zabs + _act_error(z, a, op['act'], precision)
+             + 2.0 ** -23 * y.abs())
+        p = 8 if st == torch.bfloat16 else 11
+        tol = 2.0 ** -p * (y.abs() + e) + e + (2.0 ** -25 if st == torch.float16 else 0.0)
+    nhwc = lambda t: t.permute(0, 2, 3, 1).contiguous()
+    return nhwc(y), nhwc(tol)
+
+
+def overflow_threshold(dtype):
+    """Smallest magnitude that rounds to inf in ``dtype`` (max + half an ulp of max): 65520 for fp16."""
+    fi = torch.finfo(dtype)
+    return fi.max + fi.eps * 2.0 ** math.floor(math.log2(fi.max)) / 2
+
+
+def check_bound(dev, ref, tol, precision):
+    """-> (worst |dev - ref| / tol over the finite device elements, number of violating elements).  Violations: a NaN;
+    an inf where |ref| - tol still overflows the storage type (or a finite value there); an inf of the wrong sign or
+    where |ref| + tol does not reach the overflow threshold; a finite value farther than tol from ref."""
+    dev, ref, tol = dev.double(), ref.double().to(dev.device), tol.double().to(dev.device)
+    top = overflow_threshold(MODES[precision][0])
+    must_inf = ref.abs() - tol >= top
+    may_inf = ref.abs() + tol >= top
+    fin = torch.isfinite(dev)
+    inf_ok = torch.isinf(dev) & may_inf & (torch.sign(dev) == torch.sign(ref))
+    err = torch.where(fin, (dev - ref).abs(), torch.zeros_like(dev))
+    bad = torch.isnan(dev) | (fin & (must_inf | (err > tol))) | (torch.isinf(dev) & ~inf_ok)
+    ratio = torch.where(fin & ~must_inf, err / tol.clamp_min(1e-300), torch.zeros_like(dev))
+    return float(ratio.max()) if ratio.numel() else 0.0, int(bad.sum())
+
+
+def se_fc_bound(x, xabs, n_in, w, b, act, x_err=None):
+    """One squeeze-excitation fc (1x1 conv on [B, Cin], fp32 weights and output: small_io ops are never tc_eligible) on
+    an input ``x`` [B, Cin] whose fp32 evaluation summed ``n_in`` terms of magnitude ``xabs`` per element (the pooled
+    mean of an HxW map: H*W pixels, the partial slices and the 1/(H*W) product; 0 for an exact input), and which may
+    also differ from ``x`` by ``x_err`` (absolute, per element).
+    -> (ref, tol) [B, Cout] fp64: act(x @ w.T + b) and the bound on the device's fp32 result,
+    tol = L_act * (C_ACC * (Cin + n_in + 4) * 2^-24 * (|w| @ xabs + |b|) + |w| @ x_err) + e_act + 2^-23 * |ref|."""
+    w = w.reshape(w.shape[0], -1).float().double().to(x.device)
+    b = b.float().double().to(x.device)
+    z = x.double() @ w.T + b
+    y = _act(z, act)
+    e = C_ACC * (w.shape[1] + n_in + 4) * 2.0 ** -24 * (xabs.double() @ w.abs().T + b.abs())
+    if x_err is not None:
+        e = e + x_err.double() @ w.abs().T
+    return y, LIPSCHITZ[act] * e + _act_error(z, y, act, 'fp32') + 2.0 ** -23 * y.abs()

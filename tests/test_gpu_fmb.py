@@ -7,7 +7,11 @@ launch, the expanded tile never leaves the SM) against
   output plus the propagated ulp flips of the intermediate (1e-2 on ||.||inf/||ref||inf; a descriptor / layout / pipeline
   bug gives O(1) errors);
 * the unfused device path (two tc_conv_kernel launches) on identical inputs: same MMA order and roundings, so equal up to
-  one bf16 ulp."""
+  one bf16 ulp;
+* in bf16 and fp16, element by element: the unfused path's 16-bit intermediate within port_ops.layer_bound of the expand
+  conv, and the fused output within the bound of the projection evaluated on that intermediate.  This assumes the fused
+  kernel's own intermediate is bit-equal to the unfused one (same MMA order, bias, activation and rounding); the test
+  asserts it where it can, by requiring the fused output to be bit-equal to the two-launch output."""
 import pytest
 import torch
 
@@ -26,21 +30,34 @@ def H():
     return helpers
 
 
-def _block_reference(sd, spec, names, i, x):
-    """expand conv -> bf16 -> projection (+ residual x) with conv2d, fp32 accumulate on the GPU."""
-    y = port_ops.conv_layer_reference(sd, spec, names[i], x, precision='bf16', dtype=torch.float32)
-    y = y.bfloat16().float()
-    return port_ops.conv_layer_reference(sd, spec, names[i + 1], y, x, precision='bf16', dtype=torch.float32)
+def _block_reference(sd, spec, names, i, x, precision='bf16'):
+    """expand conv -> 16 bits -> projection (+ residual x) with conv2d, fp32 accumulate on the GPU."""
+    y = port_ops.conv_layer_reference(sd, spec, names[i], x, precision=precision, dtype=torch.float32)
+    y = y.to(port_ops.MODES[precision][0]).float()
+    return port_ops.conv_layer_reference(sd, spec, names[i + 1], y, x, precision=precision, dtype=torch.float32)
+
+
+def _check_elementwise(sd, spec, names, i, x, res, mid, out, precision):
+    """-> worst |dev-ref|/tol of the intermediate and of the fused output (on the device's own intermediate)."""
+    worst = []
+    for nm, xin, res, dev in [(names[i], x, None, mid), (names[i + 1], mid, res, out)]:
+        ref, tol = port_ops.layer_bound(sd, spec, nm, xin.double(), None if res is None else res.double(), None, precision)
+        w, bad = port_ops.check_bound(dev, ref, tol, precision)
+        assert bad == 0, (nm, precision, bad, w)
+        worst.append(w)
+    return worst
 
 
 @pytest.mark.parametrize('name,side,batch', [('efficientnetv2-s', 256, 3), ('efficientnetv2-l', 256, 2), ('efficientnetv2-l', 384, 1),
                                              ('efficientnetv2-m', 192, 2), ('efficientnetv2-tiny', 64, 5),  # tiny: Cin 16, one 64-wide chunk
                                              ('efficientnetv2-l', 32, 3)])  # 8x8 / 4x4 maps, 3 crops: tiles mostly outside the map
-def test_fused_block_vs_conv2d_and_unfused(H, name, side, batch):
+@pytest.mark.parametrize('precision', ['bf16', 'fp16'])
+def test_fused_block_vs_conv2d_and_unfused(H, name, side, batch, precision):
     pcfg = port.PathConfig(proc_side=side)
     spec = port.effnet_spec(name)
     sd = port.make_effnet_state_dict(spec, pcfg, 8, seed=0, calib_batch=1)
-    eng = H.device_model(name, pcfg, 8, sd, precision='bf16').engine()
+    st = port_ops.MODES[precision][0]
+    eng = H.device_model(name, pcfg, 8, sd, precision=precision).engine()
     names = eng.op_names()
     g = torch.Generator().manual_seed(5)
     seen = set()
@@ -51,16 +68,20 @@ def test_fused_block_vs_conv2d_and_unfused(H, name, side, batch):
         if io['in_shape'] in seen:
             continue
         seen.add(io['in_shape'])
-        x = torch.randn((batch,) + io['in_shape'], generator=g).bfloat16().float().cuda()
+        x = torch.randn((batch,) + io['in_shape'], generator=g).to(st).float().cuda()
         out = eng.debug_run_fused_block(i, x)
-        ref = _block_reference(sd, spec, names, i, x)
+        ref = _block_reference(sd, spec, names, i, x, precision)
         err = port.relative_error(out.cpu(), ref.cpu())
         mid = eng.debug_run_op(i, x)
-        two = eng.debug_run_op(i + 1, mid, x if eng.op_io(i + 1)['residual'] else None)
+        res = x if eng.op_io(i + 1)['residual'] else None
+        two = eng.debug_run_op(i + 1, mid, res)
         d = (out - two).abs()
         ulp = two.abs() * 2.0 ** -7 + 2.0 ** -9
-        print(f'{name}@{side} {nm} {io["in_shape"]}: fused vs conv2d {err:.2e}; vs unfused device path: '
-              f'{float((d == 0).float().mean()) * 100:.2f} % bit-equal, max diff {float(d.max()):.3e}')
+        assert bool((d == 0).all()), (nm, float(d.max()))  # the intermediate the bound below is evaluated on
+        w_mid, w_out = _check_elementwise(sd, spec, names, i, x, res, mid, out, precision)
+        print(f'{name}@{side} {nm} {io["in_shape"]} [{precision}]: fused vs conv2d {err:.2e}; vs unfused device path: '
+              f'{float((d == 0).float().mean()) * 100:.2f} % bit-equal, max diff {float(d.max()):.3e}; '
+              f'worst |dev-ref|/tol {w_mid:.3g} (expand), {w_out:.3g} (fused output)')
         assert err < 1e-2, (nm, err)
         assert bool((d <= ulp).all()), (nm, float(d.max()))
     assert seen, 'no fused FusedMBConv block in this model'
