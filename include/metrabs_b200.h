@@ -41,11 +41,13 @@ typedef enum {
 
 typedef enum { MTB_DTYPE_F32 = 0, MTB_DTYPE_BF16 = 1, MTB_DTYPE_F16 = 2, MTB_DTYPE_I64 = 3 } mtb_dtype;
 
-/* Backbone families of BASELINE.json's configs.  EFFNET covers EfficientNetV2-S/M/L and any table in the same
- * block grammar (backbones/efficientnet.py:379-433); RESNET50 / MOBILENETV3_SMALL follow the TF-only
+/* Backbone families.  EFFNET covers EfficientNetV2-S/M/L and any table in the same block grammar
+ * (backbones/efficientnet.py:379-433); the RESNET* values (V1, metrabs_tf/backbones/resnet.py: ResNet-18/34 with the
+ * basic block :322-388, ResNet-50/101/152 with the bottleneck :239-319) and MOBILENETV3_SMALL follow the TF-only
  * metrabs_tf/backbones/{resnet,mobilenet_v3}.py. */
 typedef enum { MTB_ARCH_EFFNET = 0, MTB_ARCH_RESNET50 = 1, MTB_ARCH_MOBILENETV3_SMALL = 2,
-               MTB_ARCH_HEAD_ONLY = 3 } mtb_arch;
+               MTB_ARCH_HEAD_ONLY = 3, MTB_ARCH_RESNET18 = 4, MTB_ARCH_RESNET34 = 5, MTB_ARCH_RESNET101 = 6,
+               MTB_ARCH_RESNET152 = 7 } mtb_arch;
 
 /* Arithmetic of the conv/GEMM kernels.  FP32: CUDA-core fp32 FMA everywhere (the 1e-3 parity mode).
  * BF16_TC: bf16 operands on wgmma tensor cores with fp32 accumulation in registers, bf16 activations in HBM

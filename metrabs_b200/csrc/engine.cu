@@ -367,23 +367,47 @@ void plan_effnet(mtb_handle* h) {
   h->small_c = std::max(P.max_small, 4);
 }
 
-// ResNet-50 V1 at output stride `stride_test` (metrabs_tf/backbones/resnet.py:75-236 stem/pool, :239-319 bottleneck,
-// :601-666 stride/dilation plan; BN eps 1e-5 :71; every conv has a bias :270).  Key schema: Keras layer names,
-// "backbone.<layer>.{weight,bias}" / "backbone.<layer>.{weight,bias,running_mean,running_var}" in torch layout.
-int plan_resnet50(mtb_handle* h) {
-  const mtb_config& c = h->cfg;
-  if (c.stride_test != 8 && c.stride_test != 16 && c.stride_test != 32)
-    return fail(h, MTB_ERR_UNSUPPORTED, "ResNet-50: stride_test must be 8, 16 or 32 (got %d)", c.stride_test);
-  // get_strides_and_dilations(stride_test) (:601-618)
-  int strides[3] = {2, 2, 2}, dil_in[3] = {1, 1, 1}, dil_out[3] = {1, 1, 1};
-  bool brs[3] = {false, false, false};
+// get_strides_and_dilations(output_stride) (metrabs_tf/backbones/resnet.py:601-618), output_stride in {8, 16, 32}
+void resnet_stride_plan(int output_stride, bool centered, int strides[3], int dil_in[3], int dil_out[3], bool brs[3]) {
+  for (int i = 0; i < 3; ++i) { strides[i] = 2; dil_in[i] = dil_out[i] = 1; brs[i] = false; }
   int i_last = 0;
-  for (int s_ = c.stride_test; s_ > 8; s_ >>= 1) ++i_last;  // log2(stride) - 3
-  if (c.centered_stride) brs[i_last] = true;
+  for (int s_ = output_stride; s_ > 8; s_ >>= 1) ++i_last;  // log2(stride) - 3
+  if (centered) brs[i_last] = true;
   for (int i = i_last + 1; i < 3; ++i) {
     strides[i] = 1;
     dil_in[i] = 1 << (i - (i_last + 1));
     dil_out[i] = dil_in[i] * 2;
+  }
+}
+
+// The ResNet V1 family at output stride `stride_test` (metrabs_tf/backbones/resnet.py:75-236 stem/pool, :601-666
+// stride/dilation plan; BN eps 1e-5 :71), `counts` blocks in conv2..conv5:
+// * bottleneck (ResNet-50/101/152, ResNetUnified :621-666): block1_dense :239-319, every conv has a bias (:270);
+// * basic (ResNet-18/34, ResNetUnifiedBasic :669-707): block1_basic_dense :322-388, no conv has a bias (stem included,
+//   :704-707), conv2_block1 has an identity shortcut (conv1_shortcut=False, :689-692).
+// Key schema: Keras layer names, "backbone.<layer>.{weight,bias}" / "backbone.<layer>.{weight,bias,running_mean,running_var}"
+// in torch layout.
+int plan_resnet(mtb_handle* h, const int counts[4], bool basic) {
+  const mtb_config& c = h->cfg;
+  auto valid_stride = [](int s) { return s == 8 || s == 16 || s == 32; };
+  if (!valid_stride(c.stride_test))
+    return fail(h, MTB_ERR_UNSUPPORTED, "ResNet: stride_test must be 8, 16 or 32 (got %d)", c.stride_test);
+  int strides[3], dil_in[3], dil_out[3];
+  bool brs[3];
+  resnet_stride_plan(c.stride_test, c.centered_stride, strides, dil_in, dil_out, brs);
+  // the basic block's second 3x3 has dilation dilation_rate_test * strides / strides_test (:377-383), with `strides`
+  // from the training stride plan
+  int strides_train[3] = {1, 1, 1};
+  if (basic) {
+    if (!valid_stride(c.stride_train))
+      return fail(h, MTB_ERR_UNSUPPORTED, "ResNet-18/34: stride_train must be 8, 16 or 32 (got %d)", c.stride_train);
+    int di[3], dout[3];
+    bool b_[3];
+    resnet_stride_plan(c.stride_train, c.centered_stride, strides_train, di, dout, b_);
+    for (int i = 0; i < 3; ++i)
+      if (dil_out[i] * strides_train[i] / strides[i] < 1)  // the reference truncates 1 * 1 / 2 to a dilation of 0
+        return fail(h, MTB_ERR_UNSUPPORTED, "ResNet-18/34: stride_train %d below stride_test %d gives a dilation of 0",
+                    c.stride_train, c.stride_test);
   }
   Planner P{h, c.proc_side, c.proc_side, 3};
   const std::string pre = "backbone.";
@@ -392,7 +416,7 @@ int plan_resnet50(mtb_handle* h) {
     Op op;
     op.type = OP_STEM;
     op.name = pre + "conv1_conv";
-    op.wkey = op.name + ".weight"; op.biaskey = op.name + ".bias"; op.bnkey = pre + "conv1_bn"; op.bn_eps = eps;
+    op.wkey = op.name + ".weight"; op.biaskey = basic ? "" : op.name + ".bias"; op.bnkey = pre + "conv1_bn"; op.bn_eps = eps;
     op.Hin = op.Win = c.proc_side; op.Cin = 3; op.Cout = 64;
     op.R = op.S = 7; op.stride = 2; op.pad_t = op.pad_l = 3; op.act = ACT_RELU;
     op.Hout = op.Wout = (c.proc_side + 6 - 7) / 2 + 1;
@@ -411,11 +435,11 @@ int plan_resnet50(mtb_handle* h) {
     P.H = mp.Hout; P.W = mp.Wout; P.cur = 1;
     h->ops.push_back(mp);
   }
-  const int counts[4] = {3, 4, 6, 3}, filters[4] = {64, 128, 256, 512};
+  const int filters[4] = {64, 128, 256, 512};
   for (int st = 0; st < 4; ++st) {
     for (int bi = 0; bi < counts[st]; ++bi) {
       const bool first = bi == 0;
-      // V1: stride on the first 1x1 and on the shortcut of block1; the 3x3 uses dil_out of its stack in EVERY block
+      // V1: stride on the first conv and on the shortcut of block1; the 3x3 uses dil_out of its stack in EVERY block
       const int stride = (st > 0 && first) ? strides[st - 1] : 1;
       const int shift = (st > 0 && first && brs[st - 1]) ? 1 : 0;
       const int dil = st == 0 ? dil_in[0] : dil_out[st - 1];
@@ -423,12 +447,14 @@ int plan_resnet50(mtb_handle* h) {
       char nm[64];
       snprintf(nm, sizeof(nm), "conv%d_block%d", st + 2, bi + 1);
       const std::string b = pre + nm;
+      auto bias = [&](int j) { return basic ? std::string() : b + "_" + std::to_string(j) + "_conv.bias"; };
       const int x_in = P.cur;
       const int Hin = P.H, Win = P.W, Cin = P.C;
+      const bool last = st == 3 && bi == counts[3] - 1;
       int sc = x_in;
-      if (first) {  // conv shortcut: strided 1x1 sampled at pixels shift::stride (Conv2DDenseSame semantics)
+      if (first && !(basic && st == 0)) {  // conv shortcut: strided 1x1 sampled at pixels shift::stride (Conv2DDenseSame)
         sc = P.pick({x_in});
-        P.conv_k(b + "_0_conv", b + "_0_conv.weight", b + "_0_conv.bias", b + "_0_bn", 4 * f, 1, stride, -shift, 0, ACT_NONE,
+        P.conv_k(b + "_0_conv", b + "_0_conv.weight", bias(0), b + "_0_bn", basic ? f : 4 * f, 1, stride, -shift, 0, ACT_NONE,
                  x_in, sc, false, 1, eps);
         Op& o = h->ops.back();
         o.Hout = Hin / stride; o.Wout = Win / stride;
@@ -436,8 +462,25 @@ int plan_resnet50(mtb_handle* h) {
         P.H = Hin; P.W = Win; P.C = Cin;  // the main branch restarts from the block input
       }
       int t1 = P.pick({x_in, sc});
-      P.conv_k(b + "_1_conv", b + "_1_conv.weight", b + "_1_conv.bias", b + "_1_bn", f, 1, stride, -shift, 0, ACT_RELU, x_in, t1,
-               false, 1, eps);
+      if (basic) {
+        // _1_conv: dense SAME 3x3 sampled at shift::stride, i.e. a strided conv with begin pad dil - shift
+        P.conv_k(b + "_1_conv", b + "_1_conv.weight", "", b + "_1_bn", f, 3, stride, dil - shift, 2 * dil, ACT_RELU, x_in, t1,
+                 false, dil, eps);
+        Op& o = h->ops.back();
+        o.Hout = Hin / stride; o.Wout = Win / stride;
+        o.flops = 2.0 * o.Hout * o.Wout * o.Cout * Cin * 9;
+        P.H = o.Hout; P.W = o.Wout;
+        const int dil2 = (st > 0 && first) ? dil * strides_train[st - 1] / strides[st - 1] : dil;
+        int t2 = P.pick({sc, t1});
+        Op& o2 = P.conv_k(b + "_2_conv", b + "_2_conv.weight", "", b + "_2_bn", f, 3, 1, dil2, 2 * dil2, ACT_RELU, t1,
+                          last ? BUF_FEATURES : t2, false, dil2, eps);
+        o2.res_buf = sc;
+        o2.res_first = true;  // relu(shortcut + x)
+        P.cur = t2;
+        continue;
+      }
+      P.conv_k(b + "_1_conv", b + "_1_conv.weight", bias(1), b + "_1_bn", f, 1, stride, -shift, 0, ACT_RELU, x_in, t1, false, 1,
+               eps);
       {
         Op& o = h->ops.back();
         o.Hout = Hin / stride; o.Wout = Win / stride;
@@ -445,11 +488,10 @@ int plan_resnet50(mtb_handle* h) {
         P.H = o.Hout; P.W = o.Wout;
       }
       int t2 = P.pick({x_in, sc, t1});
-      P.conv_k(b + "_2_conv", b + "_2_conv.weight", b + "_2_conv.bias", b + "_2_bn", f, 3, 1, dil, 2 * dil, ACT_RELU, t1, t2,
-               false, dil, eps);
+      P.conv_k(b + "_2_conv", b + "_2_conv.weight", bias(2), b + "_2_bn", f, 3, 1, dil, 2 * dil, ACT_RELU, t1, t2, false, dil,
+               eps);
       int t3 = P.pick({sc, t2});
-      const bool last = st == 3 && bi == counts[3] - 1;
-      Op& o3 = P.conv_k(b + "_3_conv", b + "_3_conv.weight", b + "_3_conv.bias", b + "_3_bn", 4 * f, 1, 1, 0, 0, ACT_RELU, t2,
+      Op& o3 = P.conv_k(b + "_3_conv", b + "_3_conv.weight", bias(3), b + "_3_bn", 4 * f, 1, 1, 0, 0, ACT_RELU, t2,
                         last ? BUF_FEATURES : t3, false, 1, eps);
       o3.res_buf = sc;
       o3.res_first = true;  // relu(shortcut + x)
@@ -533,12 +575,23 @@ int plan_mobilenetv3_small(mtb_handle* h) {
   return MTB_OK;
 }
 
+// block counts of conv2..conv5 (resnet.py:746-788)
+struct ResNetArch { int arch; int counts[4]; bool basic; };
+const ResNetArch kResNets[] = {{MTB_ARCH_RESNET18, {2, 2, 2, 2}, true},    {MTB_ARCH_RESNET34, {3, 4, 6, 3}, true},
+                               {MTB_ARCH_RESNET50, {3, 4, 6, 3}, false},   {MTB_ARCH_RESNET101, {3, 4, 23, 3}, false},
+                               {MTB_ARCH_RESNET152, {3, 8, 36, 3}, false}};
+
 int plan(mtb_handle* h) {
   const mtb_config& c = h->cfg;
   h->ops.clear();
-  switch (c.arch) {
+  const ResNetArch* resnet = nullptr;
+  for (const ResNetArch& r : kResNets)
+    if (c.arch == r.arch) resnet = &r;
+  if (resnet) {
+    int rc = plan_resnet(h, resnet->counts, resnet->basic);
+    if (rc) return rc;
+  } else switch (c.arch) {
     case MTB_ARCH_EFFNET: plan_effnet(h); break;
-    case MTB_ARCH_RESNET50: { int rc = plan_resnet50(h); if (rc) return rc; break; }
     case MTB_ARCH_MOBILENETV3_SMALL: { int rc = plan_mobilenetv3_small(h); if (rc) return rc; break; }
     case MTB_ARCH_HEAD_ONLY:
       h->feat_side = c.proc_side / c.stride_test;
