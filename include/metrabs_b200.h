@@ -43,11 +43,12 @@ typedef enum { MTB_DTYPE_F32 = 0, MTB_DTYPE_BF16 = 1, MTB_DTYPE_F16 = 2, MTB_DTY
 
 /* Backbone families.  EFFNET covers EfficientNetV2-S/M/L and any table in the same block grammar
  * (backbones/efficientnet.py:379-433); the RESNET* values (V1, metrabs_tf/backbones/resnet.py: ResNet-18/34 with the
- * basic block :322-388, ResNet-50/101/152 with the bottleneck :239-319) and MOBILENETV3_SMALL follow the TF-only
+ * basic block :322-388, ResNet-50/101/152 with the bottleneck :239-319) and MOBILENETV3_SMALL / _LARGE
+ * (metrabs_tf/backbones/mobilenet_v3.py:348-384 / :387-428, alpha 1, not minimalistic) follow the TF-only
  * metrabs_tf/backbones/{resnet,mobilenet_v3}.py. */
 typedef enum { MTB_ARCH_EFFNET = 0, MTB_ARCH_RESNET50 = 1, MTB_ARCH_MOBILENETV3_SMALL = 2,
                MTB_ARCH_HEAD_ONLY = 3, MTB_ARCH_RESNET18 = 4, MTB_ARCH_RESNET34 = 5, MTB_ARCH_RESNET101 = 6,
-               MTB_ARCH_RESNET152 = 7 } mtb_arch;
+               MTB_ARCH_RESNET152 = 7, MTB_ARCH_MOBILENETV3_LARGE = 8 } mtb_arch;
 
 /* Arithmetic of the conv/GEMM kernels.  FP32: CUDA-core fp32 FMA everywhere (the 1e-3 parity mode).
  * BF16_TC: bf16 operands on wgmma tensor cores with fp32 accumulation in registers, bf16 activations in HBM
@@ -339,6 +340,13 @@ double mtb_backbone_flops_per_crop(const mtb_handle* h);
  * rows per item, row bands per crop (= SE pooling slices) and bytes of one shared-memory stage; all 0 when the shape falls
  * back to the strip kernel. */
 int mtb_debug_dw_plan(int height, int width, int* crops_per_item, int* rows_per_item, int* row_bands, int* stage_bytes);
+/* The kernel mtb_finalize_weights chose for depthwise backbone op `op`: GENERIC is dwconv_kernel (one thread per pixel and
+ * 4 channels; every fp32 / 3xTF32 / _SIMT mode op that no other kernel covers), TMA the TMA-staged 3x3 stride-1 kernel and
+ * STRIP_16B / STRIP_F32 the 3x3 strip kernels (these three also write the SE pooling slices), 5X5_16B the 16-bit 5x5 kernel
+ * of the BF16_TC / F16_TC modes (bit-identical to dwconv_kernel, no pooling).  MTB_ERR_INVALID_ARG for an index out of
+ * range or an op that is not depthwise. */
+typedef enum { MTB_DW_GENERIC = 0, MTB_DW_TMA = 1, MTB_DW_STRIP_16B = 2, MTB_DW_STRIP_F32 = 3, MTB_DW_5X5_16B = 4 } mtb_dw_kernel;
+int mtb_op_dw_kernel(const mtb_handle* h, int op);
 
 #ifdef __cplusplus
 }

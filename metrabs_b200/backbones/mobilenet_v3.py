@@ -1,16 +1,23 @@
-"""MobileNetV3-Small parameter holder for the H100 engine.
+"""MobileNetV3-Small and -Large parameter holders for the H100 engine.
 
-Keras-only in the reference (/root/reference/metrabs_tf/backbones/mobilenet_v3.py:258-296, :348-384, :465-553); key schema
+Keras-only in the reference (/root/reference/metrabs_tf/backbones/mobilenet_v3.py:258-296, :348-428, :465-553); key schema
 defined by this build from the Keras layer names with '/' -> '.': ``backbone.Conv.weight``,
 ``backbone.Conv.BatchNorm.*``, ``backbone.expanded_conv_<i>.{expand,depthwise,project}.weight`` (+ ``.BatchNorm.*``),
-``backbone.expanded_conv_<i>.squeeze_excite.{Conv,Conv_1}.{weight,bias}``, ``backbone.Conv_1.*``, ``backbone.Conv_2.*``."""
+``backbone.expanded_conv_<i>.squeeze_excite.{Conv,Conv_1}.{weight,bias}``, ``backbone.Conv_1.*``, ``backbone.Conv_2.*``.
+Block 0 (``expanded_conv``) has no expand conv.  Alpha 1, not minimalistic (the variants the released models use)."""
 from torch import nn
 
 from metrabs_b200 import _lib
 
-_ROWS = [  # (expanded channels, filters, kernel, has SE)
+_ROWS = [  # MobileNetV3-Small (:364-384): (expanded channels, filters, kernel, has SE)
     (16, 16, 3, True), (72, 24, 3, False), (88, 24, 3, False), (96, 40, 5, True), (240, 40, 5, True), (240, 40, 5, True),
     (120, 48, 5, True), (144, 48, 5, True), (288, 96, 5, True), (576, 96, 5, True), (576, 96, 5, True)]
+_ROWS_LARGE = [  # MobileNetV3-Large (:403-428)
+    (16, 16, 3, False), (64, 24, 3, False), (72, 24, 3, False), (72, 40, 5, True), (120, 40, 5, True), (120, 40, 5, True),
+    (240, 80, 3, False), (200, 80, 3, False), (184, 80, 3, False), (184, 80, 3, False), (480, 112, 3, True),
+    (672, 112, 3, True), (672, 160, 5, True), (960, 160, 5, True), (960, 160, 5, True)]
+# variant -> (arch, rows, last point channels)
+VARIANTS = {'small': (_lib.ARCH_MOBILENETV3_SMALL, _ROWS, 1024), 'large': (_lib.ARCH_MOBILENETV3_LARGE, _ROWS_LARGE, 1280)}
 
 
 def _depth(v, divisor=8):
@@ -28,15 +35,15 @@ def _conv(cin, cout, k, groups=1, bn=True, bias=False):
 
 
 class Features(nn.Module):
-    arch = _lib.ARCH_MOBILENETV3_SMALL
-    last_channel = 1024
     stages = []
 
-    def __init__(self):
+    def __init__(self, variant='small'):
         super().__init__()
+        self.arch, rows, self.last_channel = VARIANTS[variant]
+        self.variant = variant
         self.add_module('Conv', _conv(3, 16, 3))
         cin = 16
-        for i, (cexp, filters, k, se) in enumerate(_ROWS):
+        for i, (cexp, filters, k, se) in enumerate(rows):
             blk = nn.Module()
             if i != 0:
                 blk.add_module('expand', _conv(cin, cexp, 1))
@@ -50,7 +57,7 @@ class Features(nn.Module):
             self.add_module('expanded_conv' if i == 0 else f'expanded_conv_{i}', blk)
             cin = filters
         self.add_module('Conv_1', _conv(cin, _depth(cin * 6), 1))
-        self.add_module('Conv_2', _conv(_depth(cin * 6), 1024, 1, bn=False, bias=True))
+        self.add_module('Conv_2', _conv(_depth(cin * 6), self.last_channel, 1, bn=False, bias=True))
 
     def forward(self, x):
         raise RuntimeError('metrabs_b200 backbones run inside Metrabs.forward (libmetrabs_b200.so)')
@@ -58,4 +65,9 @@ class Features(nn.Module):
 
 def mobilenet_v3_small(**kwargs):
     """Use as ``Metrabs(mobilenet_v3_small(), joint_info)``."""
-    return Features()
+    return Features('small')
+
+
+def mobilenet_v3_large(**kwargs):
+    """Use as ``Metrabs(mobilenet_v3_large(), joint_info)`` (the backbone of metrabs_mob3l_y4 / _y4t)."""
+    return Features('large')

@@ -483,6 +483,93 @@ __global__ void __launch_bounds__(256, 3) dwconv3x3_pool_f32_kernel(ConvParams p
 }
 
 // ----------------------------------------------------------------------------------------------------------
+// depthwise 5x5 (stride 1 or 2) + bias + activation, bf16 or fp16 NHWC, C % 8 == 0: the per-thread layout of
+// dwconv3x3_pool_16b_kernel (8 channels x OW output pixels, 16-byte loads), so each of the (OW-1)*STRIDE + 5 input column vectors of a
+// row is loaded once and feeds every output that uses it (40 / 55 loads per 4 outputs instead of 100).  The arithmetic is
+// dwconv_kernel's, operation for operation: each accumulator starts at the bias, the taps are added with fmaf in row-major
+// order (r outer, s inner), taps outside the map are skipped, the activation is the exact act_t and the result is rounded
+// to nearest even; the outputs are bit-identical to dwconv_kernel's on the same inputs.  It does not pool (the SE squeeze
+// stays a separate pool_mean_kernel pass).  One grid-stride loop over (crop, output row, strip, channel vector), channel
+// vectors fastest: narrow layers (72, 96, 120 channels) fill whole warps.  grid grid_for(items, 256), block 256.
+// ----------------------------------------------------------------------------------------------------------
+template <typename T, int STRIDE, int ACT, int OW = 4>
+__global__ void __launch_bounds__(256) dwconv5x5_16b_kernel(ConvParams p) {
+  constexpr int NCOL = (OW - 1) * STRIDE + 5;  // input columns feeding OW outputs
+  const T* __restrict__ in = reinterpret_cast<const T*>(p.in);
+  T* __restrict__ out = reinterpret_cast<T*>(p.out);
+  const int C = p.Cout;
+  const int cstride = C >> 3;  // uint4 per pixel
+  const int strips_w = (p.Wout + OW - 1) / OW;
+  const size_t total = (size_t)p.B * p.Hout * strips_w * cstride;
+  for (size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
+    const int c = (int)(idx % cstride) * 8;
+    size_t t = idx / cstride;
+    const int ow0 = (int)(t % strips_w) * OW;
+    t /= strips_w;
+    const int oh = (int)(t % p.Hout);
+    const int b = (int)(t / p.Hout);
+    const int iw0 = ow0 * STRIDE - p.pad_l;
+    unsigned colmask = 0;
+#pragma unroll
+    for (int x = 0; x < NCOL; ++x)
+      if (iw0 + x >= 0 && iw0 + x < p.Win) colmask |= 1u << x;
+    float acc[OW][8];
+    {
+      const float4 b0 = *reinterpret_cast<const float4*>(p.bias + c), b1 = *reinterpret_cast<const float4*>(p.bias + c + 4);
+      const float bias[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+#pragma unroll
+      for (int i = 0; i < OW; ++i)
+#pragma unroll
+        for (int k = 0; k < 8; ++k) acc[i][k] = bias[k];
+    }
+#pragma unroll
+    for (int r = 0; r < 5; ++r) {
+      const int ih = oh * STRIDE - p.pad_t + r;
+      if (ih < 0 || ih >= p.Hin) continue;
+      const uint4* rowp = reinterpret_cast<const uint4*>(in + ((size_t)(b * p.Hin + ih) * p.Win) * C + c) + (ptrdiff_t)iw0 * cstride;
+      uint4 raw[NCOL];
+#pragma unroll
+      for (int x = 0; x < NCOL; ++x) raw[x] = (colmask >> x) & 1u ? __ldg(rowp + (ptrdiff_t)x * cstride) : make_uint4(0u, 0u, 0u, 0u);
+      float w[5][8];
+#pragma unroll
+      for (int s_ = 0; s_ < 5; ++s_) {
+        const float* wp = p.w + (size_t)(r * 5 + s_) * C + c;
+        const float4 w0 = __ldg(reinterpret_cast<const float4*>(wp)), w1 = __ldg(reinterpret_cast<const float4*>(wp + 4));
+        w[s_][0] = w0.x; w[s_][1] = w0.y; w[s_][2] = w0.z; w[s_][3] = w0.w;
+        w[s_][4] = w1.x; w[s_][5] = w1.y; w[s_][6] = w1.z; w[s_][7] = w1.w;
+      }
+      // ascending x visits each output's taps in ascending s; a column outside the map is skipped, not added as zero
+#pragma unroll
+      for (int x = 0; x < NCOL; ++x) {
+        if (!((colmask >> x) & 1u)) continue;
+        const unsigned wd[4] = {raw[x].x, raw[x].y, raw[x].z, raw[x].w};
+        float v[8];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) f2_unpack(unpack2_16b<T>(wd[k]), v[2 * k], v[2 * k + 1]);
+#pragma unroll
+        for (int i = 0; i < OW; ++i) {
+          const int s_ = x - i * STRIDE;  // compile-time after unrolling
+          if (s_ >= 0 && s_ < 5) {
+#pragma unroll
+            for (int k = 0; k < 8; ++k) acc[i][k] = fmaf(v[k], w[s_][k], acc[i][k]);
+          }
+        }
+      }
+    }
+    T* orow = out + ((size_t)(b * p.Hout + oh) * p.Wout + ow0) * C + c;
+#pragma unroll
+    for (int i = 0; i < OW; ++i) {
+      if (ow0 + i >= p.Wout) continue;
+      uint4 ov;
+      typename Pair16<T>::type* o2 = reinterpret_cast<typename Pair16<T>::type*>(&ov);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) o2[k] = Pair16<T>::pack(act_t<ACT>(acc[i][2 * k]), act_t<ACT>(acc[i][2 * k + 1]));
+      *reinterpret_cast<uint4*>(orow + (size_t)i * C) = ov;
+    }
+  }
+}
+
+// ----------------------------------------------------------------------------------------------------------
 // stem: direct conv for tiny Cin (3) reading the caller's NCHW fp32 crops, with the per-channel input affine
 // (PreprocLayer x*2-1, backbones/efficientnet.py:1185) applied to in-bounds pixels only (pad happens AFTER
 // preprocessing in the reference), writing NHWC.  w: [R*S*Cin][Cout], one thread per (pixel, 4 out channels).

@@ -10,6 +10,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <iterator>
 #include <map>
 #include <string>
 #include <vector>
@@ -30,8 +31,11 @@ namespace {
 std::string g_error;
 
 enum OpType { OP_STEM = 0, OP_CONV = 1, OP_DW = 2, OP_POOL = 3, OP_MAXPOOL = 4 };
-// depthwise kernels: TMA-staged (dw_tma.cuh), 16-bit (bf16 / fp16) or fp32 strip (SE pooling fused), generic (dwconv_kernel)
-enum DwKernel { DW_GENERIC = 0, DW_TMA = 1, DW_STRIP_16B = 2, DW_STRIP_F32 = 3 };
+// depthwise kernels: TMA-staged (dw_tma.cuh), 16-bit (bf16 / fp16) or fp32 strip (SE pooling fused), generic (dwconv_kernel),
+// 16-bit 5x5 (dwconv5x5_16b_kernel: dwconv_kernel's arithmetic with column reuse, no pooling); values of mtb_dw_kernel
+enum DwKernel { DW_GENERIC = 0, DW_TMA = 1, DW_STRIP_16B = 2, DW_STRIP_F32 = 3, DW_5X5_16B = 4 };
+static_assert((int)DW_GENERIC == (int)MTB_DW_GENERIC && (int)DW_TMA == (int)MTB_DW_TMA && (int)DW_STRIP_16B == (int)MTB_DW_STRIP_16B &&
+              (int)DW_STRIP_F32 == (int)MTB_DW_STRIP_F32 && (int)DW_5X5_16B == (int)MTB_DW_5X5_16B, "DwKernel must match mtb_dw_kernel");
 // kernel classes for the CUDA-event profiler (mtb_profile_begin / mtb_profile_end)
 enum KClass { KC_STEM = 0, KC_IGEMM_SIMT = 1, KC_DWCONV = 2, KC_POOL = 3, KC_SE_FC = 4, KC_TC_GEMM = 5, KC_FMB = 6,
               KC_HEAD_FUSED = 7, KC_HEAD_CONV_SIMT = 8, KC_SOFTARGMAX = 9, KC_RECON = 10, KC_OTHER = 11, KC_SE_SCALE = 12, KC_TC32 = 13,
@@ -505,9 +509,32 @@ int plan_resnet(mtb_handle* h, const int counts[4], bool basic) {
   return MTB_OK;
 }
 
-// MobileNetV3-Small (metrabs_tf/backbones/mobilenet_v3.py:348-384 table, :490-553 block, :465-487 SE, :258-296 stem and
-// Conv_1 / Conv_2, :556-575 correct_pad; preprocessing 255*x then Rescaling(1/127.5, -1) = 2x-1, builder.py:116-117).
-int plan_mobilenetv3_small(mtb_handle* h) {
+// One row of a MobileNetV3 table: _inverted_res_block(x, expansion, filters, kernel, stride, se_ratio, activation, ...)
+// with the expanded width already rounded by _depth
+struct MbV3Row { int exp_ch, filters, k, stride; bool se; int act; bool br; };
+// MobileNetV3-Small (metrabs_tf/backbones/mobilenet_v3.py:364-384)
+const MbV3Row kMobileNetV3Small[] = {
+    {16, 16, 3, 2, true, ACT_RELU, false},     {72, 24, 3, 2, false, ACT_RELU, false},
+    {88, 24, 3, 1, false, ACT_RELU, false},    {96, 40, 5, 2, true, ACT_HSWISH, false},
+    {240, 40, 5, 1, true, ACT_HSWISH, false},  {240, 40, 5, 1, true, ACT_HSWISH, false},
+    {120, 48, 5, 1, true, ACT_HSWISH, false},  {144, 48, 5, 1, true, ACT_HSWISH, false},
+    {288, 96, 5, 2, true, ACT_HSWISH, true},   {576, 96, 5, 1, true, ACT_HSWISH, false},
+    {576, 96, 5, 1, true, ACT_HSWISH, false}};
+// MobileNetV3-Large (:403-428): block 0 has no expand, the ReLU blocks 3-5 use 5x5 kernels with SE
+const MbV3Row kMobileNetV3Large[] = {
+    {16, 16, 3, 1, false, ACT_RELU, false},     {64, 24, 3, 2, false, ACT_RELU, false},
+    {72, 24, 3, 1, false, ACT_RELU, false},     {72, 40, 5, 2, true, ACT_RELU, false},
+    {120, 40, 5, 1, true, ACT_RELU, false},     {120, 40, 5, 1, true, ACT_RELU, false},
+    {240, 80, 3, 2, false, ACT_HSWISH, false},  {200, 80, 3, 1, false, ACT_HSWISH, false},
+    {184, 80, 3, 1, false, ACT_HSWISH, false},  {184, 80, 3, 1, false, ACT_HSWISH, false},
+    {480, 112, 3, 1, true, ACT_HSWISH, false},  {672, 112, 3, 1, true, ACT_HSWISH, false},
+    {672, 160, 5, 2, true, ACT_HSWISH, true},   {960, 160, 5, 1, true, ACT_HSWISH, false},
+    {960, 160, 5, 1, true, ACT_HSWISH, false}};
+
+// MobileNetV3 (metrabs_tf/backbones/mobilenet_v3.py:490-553 block, :465-487 SE, :258-296 stem and Conv_1 / Conv_2,
+// :556-575 correct_pad; preprocessing 255*x then Rescaling(1/127.5, -1) = 2x-1, builder.py:116-117), `n_rows` rows of
+// `rows` and a last point conv (Conv_2) of `last_point_ch` channels: 1024 for Small, 1280 for Large.
+int plan_mobilenetv3(mtb_handle* h, const MbV3Row* rows, int n_rows, int last_point_ch) {
   const mtb_config& c = h->cfg;
   Planner P{h, c.proc_side, c.proc_side, 3};
   const std::string pre = "backbone.";
@@ -528,20 +555,13 @@ int plan_mobilenetv3_small(mtb_handle* h) {
     P.track(P.H, P.W, P.C);
     h->ops.push_back(op);
   }
-  struct Row { int exp_ch, filters, k, stride; bool se; int act; bool br; };
-  const Row rows[11] = {{16, 16, 3, 2, true, ACT_RELU, false},     {72, 24, 3, 2, false, ACT_RELU, false},
-                        {88, 24, 3, 1, false, ACT_RELU, false},    {96, 40, 5, 2, true, ACT_HSWISH, false},
-                        {240, 40, 5, 1, true, ACT_HSWISH, false},  {240, 40, 5, 1, true, ACT_HSWISH, false},
-                        {120, 48, 5, 1, true, ACT_HSWISH, false},  {144, 48, 5, 1, true, ACT_HSWISH, false},
-                        {288, 96, 5, 2, true, ACT_HSWISH, true},   {576, 96, 5, 1, true, ACT_HSWISH, false},
-                        {576, 96, 5, 1, true, ACT_HSWISH, false}};
   auto depth8 = [](double v) {  // _depth (:449-456)
     int nv = std::max(8, (int)(v + 4) / 8 * 8);
     if (nv < 0.9 * v) nv += 8;
     return nv;
   };
-  for (int bi = 0; bi < 11; ++bi) {
-    const Row& r = rows[bi];
+  for (int bi = 0; bi < n_rows; ++bi) {
+    const MbV3Row& r = rows[bi];
     const std::string b = pre + (bi == 0 ? std::string("expanded_conv") : "expanded_conv_" + std::to_string(bi));
     const int x_in = P.cur, cin = P.C;
     int t1 = x_in;
@@ -566,7 +586,8 @@ int plan_mobilenetv3_small(mtb_handle* h) {
   {
     int t1 = P.pick({P.cur});
     P.conv_k(pre + "Conv_1", pre + "Conv_1.weight", "", pre + "Conv_1.BatchNorm", depth8(P.C * 6), 1, 1, 0, 0, ACT_HSWISH, P.cur, t1);
-    P.conv_k(pre + "Conv_2", pre + "Conv_2.weight", pre + "Conv_2.bias", "", 1024, 1, 1, 0, 0, ACT_HSWISH, t1, BUF_FEATURES);
+    P.conv_k(pre + "Conv_2", pre + "Conv_2.weight", pre + "Conv_2.bias", "", last_point_ch, 1, 1, 0, 0, ACT_HSWISH, t1,
+             BUF_FEATURES);
   }
   h->feat_side = P.H;
   h->feat_c = P.C;
@@ -592,7 +613,8 @@ int plan(mtb_handle* h) {
     if (rc) return rc;
   } else switch (c.arch) {
     case MTB_ARCH_EFFNET: plan_effnet(h); break;
-    case MTB_ARCH_MOBILENETV3_SMALL: { int rc = plan_mobilenetv3_small(h); if (rc) return rc; break; }
+    case MTB_ARCH_MOBILENETV3_SMALL: { int rc = plan_mobilenetv3(h, kMobileNetV3Small, (int)std::size(kMobileNetV3Small), 1024); if (rc) return rc; break; }
+    case MTB_ARCH_MOBILENETV3_LARGE: { int rc = plan_mobilenetv3(h, kMobileNetV3Large, (int)std::size(kMobileNetV3Large), 1280); if (rc) return rc; break; }
     case MTB_ARCH_HEAD_ONLY:
       h->feat_side = c.proc_side / c.stride_test;
       h->feat_c = c.feature_channels;
@@ -771,13 +793,28 @@ bool dw_strip_eligible(const Op& op) {
          (op.act == ACT_SILU || op.act == ACT_RELU || op.act == ACT_HSWISH);
 }
 
+// shapes covered by dwconv5x5_16b_kernel
+bool dw5x5_eligible(const Op& op) {
+  return op.type == OP_DW && op.R == 5 && op.S == 5 && op.dil == 1 && op.Cout % 8 == 0 && (op.stride == 1 || op.stride == 2) &&
+         (op.act == ACT_RELU || op.act == ACT_HSWISH);
+}
+
+// the depthwise kernels that also write the SE pooling slices of their output
+bool dw_kernel_pools(DwKernel k) { return k == DW_TMA || k == DW_STRIP_16B || k == DW_STRIP_F32; }
+
 constexpr int kDwOW = 4;  // outputs per thread along W in dwconv3x3_pool_16b_kernel (measured: 4 -> 3.65 ms, 2 -> 4.25 ms per 128 crops)
+constexpr int kDw5OW = 4;  // outputs per thread along W in dwconv5x5_16b_kernel
 
 // Picks the kernel of a depthwise op and the number of partial pooling slices it writes (fc1 sums that many).  bf16 and fp16
-// tensor-core modes: stride-1 ops run the TMA-staged kernel when a plan fits, the rest the 16-bit strip kernel.  3xTF32 mode:
-// the fp32 strip kernel (exact activation).  Other modes and shapes: the generic kernel, which does not pool.
+// tensor-core modes: 5x5 ops run dwconv5x5_16b_kernel, which does not pool; 3x3 stride-1 ops run the TMA-staged kernel when
+// a plan fits, the other 3x3 ops the 16-bit strip kernel.  3xTF32 mode: the fp32 strip kernel (exact activation) for 3x3
+// ops.  Other modes and shapes: the generic kernel, which does not pool.
 void choose_dw_kernel(const mtb_handle* h, Op& op) {
   op.dw_kernel = DW_GENERIC;
+  if (dw5x5_eligible(op)) {
+    if (is_tc16(h)) op.dw_kernel = DW_5X5_16B;
+    return;
+  }
   if (!dw_strip_eligible(op)) return;
   if (is_tc16(h)) {
     if (op.stride == 1 && op.Hin == op.Hout && op.Win == op.Wout) {
@@ -913,6 +950,17 @@ int run_op_t(mtb_handle* h, const Op& op, const float* crops, int B, const Works
           else if (op.act == ACT_RELU) { if (op.stride == 1) MTB_DWF32(1, ACT_RELU); else MTB_DWF32(2, ACT_RELU); }
           else { if (op.stride == 1) MTB_DWF32(1, ACT_HSWISH); else MTB_DWF32(2, ACT_HSWISH); }
 #undef MTB_DWF32
+        } else if (op.dw_kernel == DW_5X5_16B) {
+          if constexpr (!k16) {
+            return fail(h, MTB_ERR_CUDA, "depthwise %s: 16-bit kernel chosen for fp32 storage", op.name.c_str());
+          } else {
+            const size_t items = (size_t)B * op.Hout * ((op.Wout + kDw5OW - 1) / kDw5OW) * (op.Cout / 8);
+            const dim3 grid(grid_for(items, 256));
+#define MTB_DW5(ST, AC) launch_k(dwconv5x5_16b_kernel<T, ST, AC, kDw5OW>, grid, dim3(256), 0, st, p)
+            if (op.act == ACT_RELU) { if (op.stride == 1) MTB_DW5(1, ACT_RELU); else MTB_DW5(2, ACT_RELU); }
+            else { if (op.stride == 1) MTB_DW5(1, ACT_HSWISH); else MTB_DW5(2, ACT_HSWISH); }
+#undef MTB_DW5
+          }
         } else {
           size_t total = (size_t)B * op.Hout * op.Wout * (op.Cout / 4);
           launch_k(dwconv_kernel<T>, dim3(grid_for(total, 256)), dim3(256), 0, st, p);
@@ -1328,7 +1376,7 @@ int mtb_finalize_weights(mtb_handle* h) {
     choose_dw_kernel(h, op);
   }
   for (size_t i = 0; i + 1 < h->ops.size(); ++i)  // the strip and TMA-staged depthwise kernels also pool for the SE block behind them
-    if (h->ops[i].dw_kernel != DW_GENERIC && h->ops[i + 1].type == OP_POOL) h->ops[i].fused_pool = h->ops[i + 1].fused_pool = true;
+    if (dw_kernel_pools(h->ops[i].dw_kernel) && h->ops[i + 1].type == OP_POOL) h->ops[i].fused_pool = h->ops[i + 1].fused_pool = true;
   for (auto& op : h->ops) {
     int rc = prepare_op_weights(h, op);
     if (rc) return rc;
@@ -2105,6 +2153,12 @@ int mtb_debug_run_op(mtb_handle* h, int op_index, const float* in, const float* 
   else copy_to_float(h, src, out, n_out, st);
   CUDA_TRY(h, cudaGetLastError());
   return MTB_OK;
+}
+
+int mtb_op_dw_kernel(const mtb_handle* h, int op) {
+  if (!h || op < 0 || op >= (int)h->ops.size()) return fail(h, MTB_ERR_INVALID_ARG, "op index out of range");
+  if (h->ops[op].type != OP_DW) return fail(h, MTB_ERR_INVALID_ARG, "op %d (%s) is not depthwise", op, h->ops[op].name.c_str());
+  return h->ops[op].dw_kernel;
 }
 
 int mtb_op_is_fused_block(const mtb_handle* h, int op_index) {

@@ -314,6 +314,14 @@ class Engine:
                                      ws.data_ptr(), ws.numel(), _stream_ptr(self.device)), self._h)
         return out
 
+    def op_dw_kernel(self, op):
+        """The kernel finalize chose for depthwise op `op`: one of _lib.DW_GENERIC, DW_TMA, DW_STRIP_16B, DW_STRIP_F32,
+        DW_5X5_16B."""
+        k = lib().mtb_op_dw_kernel(self._h, op)
+        if k < 0:
+            check(k, self._h)
+        return k
+
     def op_is_fused_block(self, op):
         """True when backbone op `op` (3x3 expand) and op + 1 (1x1 projection) run as one fused FusedMBConv kernel."""
         return bool(lib().mtb_op_is_fused_block(self._h, op))
