@@ -4,7 +4,7 @@
 //
 // as ONE kernel: the 128-pixel x Cexp expanded tile never leaves the SM.  Per output tile (16 x 8 pixels, as mode 1 of
 // tc_conv_kernel) and per chunk of 128 expanded channels:
-//   GEMM-1  (3x3 expand, implicit GEMM)   acc1[128 x 128] = shifted input boxes (4D TMA per tap) x W1[chunk rows]^T
+//   GEMM-1  (3x3 expand, implicit GEMM)   acc1[128 x 128] = shifted input boxes x W1[chunk rows]^T
 //   epilogue-1  acc1 -> + folded-BN bias -> SiLU -> bf16 / fp16 -> shared memory in the 128B-swizzled K-major operand layout:
 //           it IS the A operand of GEMM-2 (channels >= Cexp are written as zeros)
 //   GEMM-2  (1x1 projection)  acc2[128 x Cout] += A2 x W2[:, chunk]^T, the W2 slice travelling through the same TMA ring
@@ -12,21 +12,39 @@
 // of the tile in both GEMMs, so the A2 hand-over needs only a warpgroup barrier.  The MMA sequence of every output element
 // (tap-major K of GEMM-1, chunk-major K of GEMM-2, K = 16 per wgmma) and every rounding are those of the two-launch path
 // (tc_conv_kernel twice, with the same activation form per element type), so the fused block reproduces it.
+//
+// Persistent: one CTA per SM walks tiles t = blockIdx.x, blockIdx.x + gridDim.x, ...  The input of a tile is read once, as
+// three column-shifted 16 x 10-pixel boxes per 64-channel k-chunk (tma_load_tap_boxes), kept resident across the tile's
+// expanded-channel chunks; tap (r, s) of GEMM-1 is box s from pixel row r on.  The ring carries only weights: 16 KB stages
+// holding a W1 block [128 expanded channels x 64] or one 64-channel half of the W2 slice [Cout x 64].  The producer streams
+// the k-blocks of the CTA's whole tile sequence, and loads the next tile's boxes as soon as the last GEMM-1 of the current
+// tile has read them, under its last epilogue-1, GEMM-2 and epilogue-2.
 #pragma once
 #include "tc_gemm.cuh"
 
 namespace mtb {
 
-constexpr int FMB_NC = 128;                       // expanded channels per chunk (N of GEMM-1, K of GEMM-2)
-constexpr int FMB_STAGES = 4;
-constexpr int FMB_STAGE_BYTES = TC_A_BYTES + FMB_NC * TC_BK * 2;   // 32 KB: [A 16 KB | W1 block 16 KB] or [W2 slice <= 32 KB]
-constexpr int FMB_A2_OFF = FMB_STAGES * FMB_STAGE_BYTES;
+constexpr int FMB_NC = 128;                                         // expanded channels per chunk (N of GEMM-1, K of GEMM-2)
+constexpr int FMB_BOX_H = TC_TILE_H + 2;                            // the tile's 8 input rows and the row above and below
+constexpr int FMB_BOX_BYTES = TC_TILE_W * FMB_BOX_H * TC_BK * 2;    // 20 KB (a multiple of 1024: every box is swizzle-aligned)
+constexpr int FMB_W_BYTES = FMB_NC * TC_BK * 2;                     // ring stage: W1 block 16 KB, or W2 half BN2 x 128 B <= 16 KB
 constexpr int FMB_A2_BYTES = TC_BM * FMB_NC * 2;  // two 16 KB swizzle tiles (expanded channels 0-63, 64-127 of the chunk)
-constexpr int FMB_BAR_OFF = FMB_A2_OFF + FMB_A2_BYTES;
-constexpr int FMB_SMEM_BYTES = FMB_BAR_OFF + 256 + 1024 /*align slack*/;
+
+// Shared memory per BN2 (= tc_pick_bn(Cout), Cout = Cin): [3 x kchunks boxes | ring | A2 | barriers].  Cin <= 64 is one
+// 64-channel k-chunk (BN2 <= 64): 60 KB of boxes + 8 x 16 KB ring + 32 KB = 221 KB; Cin 80 / 96 is two (BN2 = 128): 120 KB of
+// boxes + 4 x 16 KB + 32 KB = 216 KB.
+template <int BN2>
+struct FmbSmem {
+  static constexpr int kchunks = BN2 == 128 ? 2 : 1;
+  static constexpr int stages = BN2 == 128 ? 4 : 8;
+  static constexpr int ring_off = 3 * kchunks * FMB_BOX_BYTES;
+  static constexpr int a2_off = ring_off + stages * FMB_W_BYTES;
+  static constexpr int bar_off = a2_off + FMB_A2_BYTES;
+  static constexpr int smem_bytes = bar_off + 256 + 1024 /*align slack*/;
+};
 
 struct FmbParams {
-  TcConvParams g;           // geometry of the 3x3 expand conv (mode 1); g.res = x (residual), g.out = block output
+  TcConvParams g;           // geometry of the 3x3 expand conv (mode 1); g.res = x (residual), g.out = block output, g.m_tiles tiles
   const float* bias1;       // [Cexp]
   int Cexp, nch, has_res;
 };
@@ -35,10 +53,14 @@ template <typename T, int BN2>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 fmb_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW1, const __grid_constant__ CUtensorMap tmW2,
            const FmbParams p) {
+  using L = FmbSmem<BN2>;
+  constexpr int STAGES = L::stages, KCH = L::kchunks, NUM_KB = 9 * KCH;
   extern __shared__ uint8_t tc_smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)tc_smem_raw + 1023) & ~(uintptr_t)1023);
-  uint64_t* full = (uint64_t*)(smem + FMB_BAR_OFF);
-  uint64_t* empty = full + FMB_STAGES;
+  uint64_t* full = (uint64_t*)(smem + L::bar_off);
+  uint64_t* empty = full + STAGES;
+  uint64_t* box_full = empty + STAGES;
+  uint64_t* box_empty = box_full + 1;
   const TcConvParams& g = p.g;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -46,34 +68,38 @@ fmb_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmW1);
     tma_prefetch_desc(&tmW2);
-    for (int i = 0; i < FMB_STAGES; ++i) {
+    for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full[i], 1);
       mbar_init(&empty[i], TC_CONSUMER_WARPS);
     }
+    mbar_init(box_full, 1);
+    mbar_init(box_empty, TC_CONSUMER_WARPS);
     fence_barrier_init();
   }
   __syncthreads();
 
-  const int m_blk = blockIdx.x;
-  const int num_kb = g.taps * g.kchunks;
   if (warp == TC_CONSUMER_WARPS) {
-    // ===== TMA producer: per chunk, num_kb (input box, W1 block) stages, then one W2 stage =====
+    // ===== TMA producer: per tile the input boxes, then per chunk NUM_KB W1 blocks and the two W2 halves =====
     if (lane == 0) {
-      int it = 0;
-      for (int c = 0; c < p.nch; ++c) {
-        for (int kb = 0; kb <= num_kb; ++kb, ++it) {
-          const int s = it % FMB_STAGES;
-          mbar_wait(&empty[s], ((it / FMB_STAGES) & 1) ^ 1);
-          uint8_t* st = smem + s * FMB_STAGE_BYTES;
-          if (kb < num_kb) {
-            const int tap = kb / g.kchunks, kc = kb - tap * g.kchunks;
-            mbar_expect_tx(&full[s], FMB_STAGE_BYTES);
-            tma_load_a_tile<TC_BK>(st, &tmA, &full[s], g, m_blk, kb);
-            tma_load_2d(st + TC_A_BYTES, &tmW1, &full[s], tap * g.Cin + kc * TC_BK, c * FMB_NC);
-          } else {
-            mbar_expect_tx(&full[s], 2 * BN2 * TC_BK * 2);
-            tma_load_2d(st, &tmW2, &full[s], c * FMB_NC, 0);
-            tma_load_2d(st + BN2 * TC_BK * 2, &tmW2, &full[s], c * FMB_NC + TC_BK, 0);
+      int it = 0, n = 0;
+      for (int t = blockIdx.x; t < g.m_tiles; t += gridDim.x, ++n) {
+        mbar_wait(box_empty, (n & 1) ^ 1);
+        mbar_expect_tx(box_full, 3 * KCH * FMB_BOX_BYTES);
+#pragma unroll
+        for (int kc = 0; kc < KCH; ++kc) tma_load_tap_boxes(smem + 3 * kc * FMB_BOX_BYTES, FMB_BOX_BYTES, &tmA, box_full, g, t, kc);
+        for (int c = 0; c < p.nch; ++c) {
+          for (int kb = 0; kb < NUM_KB + 2; ++kb, ++it) {
+            const int s = it % STAGES;
+            mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
+            uint8_t* st = smem + L::ring_off + s * FMB_W_BYTES;
+            if (kb < NUM_KB) {
+              const int tap = kb / KCH, kc = kb - tap * KCH;
+              mbar_expect_tx(&full[s], FMB_W_BYTES);
+              tma_load_2d(st, &tmW1, &full[s], tap * g.Cin + kc * TC_BK, c * FMB_NC);
+            } else {
+              mbar_expect_tx(&full[s], BN2 * TC_BK * 2);
+              tma_load_2d(st, &tmW2, &full[s], c * FMB_NC + (kb - NUM_KB) * TC_BK, 0);
+            }
           }
         }
       }
@@ -81,100 +107,110 @@ fmb_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
     return;
   }
   const int wg = warp >> 2;
-  const uint32_t a2 = smem_u32(smem + FMB_A2_OFF);
+  const uint32_t boxes = smem_u32(smem) + wg * 64 * 128, ring = smem_u32(smem + L::ring_off), a2 = smem_u32(smem + L::a2_off);
   const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // fragment rows r0, r0 + 8; columns 8 j + 2 (lane % 4) + {0, 1}
-  float acc2[BN2 / 2];
-#pragma unroll
-  for (int i = 0; i < BN2 / 2; ++i) acc2[i] = 0.f;
-  int it = 0;
-  for (int c = 0; c < p.nch; ++c) {
-    // ---- GEMM-1 ----
-    float acc1[FMB_NC / 2];
-#pragma unroll
-    for (int i = 0; i < FMB_NC / 2; ++i) acc1[i] = 0.f;
-    int prev = -1;
-    for (int kb = 0; kb < num_kb; ++kb, ++it) {
-      const int s = it % FMB_STAGES;
-      mbar_wait(&full[s], (it / FMB_STAGES) & 1);
-      const uint32_t a = smem_u32(smem + s * FMB_STAGE_BYTES) + wg * 64 * 128;
-      const uint32_t b = smem_u32(smem + s * FMB_STAGE_BYTES + TC_A_BYTES);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < TC_BK / 16; ++k)
-        wgmma_16b<T, FMB_NC>(acc1, gmma_desc<128>(a + 32 * k), gmma_desc<128>(b + 32 * k), (uint32_t)(kb | k));
-      wgmma_commit();
-      wgmma_wait<1>();
-      if (prev >= 0) {
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty[prev]);
-      }
-      prev = s;
-    }
-    wgmma_wait<0>();
-    wgmma_fence_regs<FMB_NC / 2>(acc1);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[prev]);
-    // ---- epilogue-1: + bias, SiLU, 16-bit -> A2 (this warpgroup's rows; 16-byte chunk j of row r at j ^ (r & 7)) ----
-#pragma unroll
-    for (int j = 0; j < FMB_NC / 8; ++j) {
-      const int cc = 8 * j + 2 * (lane & 3);  // column within the chunk
-      const int col = c * FMB_NC + cc;
-      float2 bv = make_float2(0.f, 0.f);
-      if (col < p.Cexp) bv = __ldg(reinterpret_cast<const float2*>(p.bias1 + col));  // Cexp % 16 == 0: col + 1 valid with col
-      const uint32_t sub = (uint32_t)(cc >> 6) * (TC_BM * 128), kc = (uint32_t)(cc & 63);
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int r = r0 + 8 * h;
-        typename Pair16<T>::type v = Pair16<T>::pack(0.f, 0.f);
-        if (col < p.Cexp)
-          v = Pair16<T>::pack(tc_act<ACT_SILU, T>(acc1[4 * j + 2 * h] + bv.x), tc_act<ACT_SILU, T>(acc1[4 * j + 2 * h + 1] + bv.y));
-        const uint32_t off = sub + (uint32_t)r * 128 + ((((kc >> 3) ^ (uint32_t)(r & 7))) << 4) + (kc & 7) * 2;
-        *reinterpret_cast<typename Pair16<T>::type*>(smem + FMB_A2_OFF + off) = v;
-      }
-    }
-    fence_proxy_async();  // generic-proxy writes -> visible to the tensor core (async proxy)
-    wg_sync(wg);
-    // ---- GEMM-2: acc2 += A2 x W2[:, chunk]^T ----
-    {
-      const int s = it % FMB_STAGES;
-      mbar_wait(&full[s], (it / FMB_STAGES) & 1);
-      const uint32_t b = smem_u32(smem + s * FMB_STAGE_BYTES);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < FMB_NC / 16; ++k) {
-        const uint32_t sub = (uint32_t)(k >> 2), ko = (uint32_t)(k & 3) * 32;
-        wgmma_16b<T, BN2>(acc2, gmma_desc<128>(a2 + sub * (TC_BM * 128) + wg * 64 * 128 + ko), gmma_desc<128>(b + sub * (BN2 * 128) + ko),
-                        (uint32_t)(c | k));
-      }
-      wgmma_commit();
-      wgmma_wait<0>();  // A2 is rewritten by the next chunk's epilogue-1
-      wgmma_fence_regs<BN2 / 2>(acc2);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty[s]);
-      ++it;
-    }
-  }
-  // ---- epilogue-2: + bias, + residual x, 16-bit store ----
   typedef typename Pair16<T>::type T2;
   const T* __restrict__ res = (const T*)g.res;
   T* __restrict__ out = (T*)g.out;
-  const int c0 = 2 * (lane & 3);
+  int it = 0, n = 0;
+  for (int t = blockIdx.x; t < g.m_tiles; t += gridDim.x, ++n) {
+    float acc2[BN2 / 2];
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    size_t off;
-    if (!tile_row_offset(1, m_blk, r0 + 8 * h, g.M, g.Cout, g.tiles_w, g.tiles_h, g.Hout, g.Wout, off)) continue;
+    for (int i = 0; i < BN2 / 2; ++i) acc2[i] = 0.f;
+    mbar_wait(box_full, n & 1);
+    for (int c = 0; c < p.nch; ++c) {
+      // ---- GEMM-1 ----
+      float acc1[FMB_NC / 2];
 #pragma unroll
-    for (int j = 0; j < BN2 / 8; ++j) {
-      const int cidx = c0 + 8 * j;
-      if (cidx >= g.Cout) break;
-      const float2 bv = __ldg(reinterpret_cast<const float2*>(g.bias + cidx));
-      float o0 = acc2[4 * j + 2 * h] + bv.x, o1 = acc2[4 * j + 2 * h + 1] + bv.y;
-      if (p.has_res) {
-        const float2 rv = Pair16<T>::unpack(*reinterpret_cast<const T2*>(res + off + cidx));
-        o0 += rv.x;
-        o1 += rv.y;
+      for (int i = 0; i < FMB_NC / 2; ++i) acc1[i] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < NUM_KB; ++kb, ++it) {
+        const int s = it % STAGES;
+        mbar_wait(&full[s], (it / STAGES) & 1);
+        const int tap = kb / KCH, kc = kb - tap * KCH, r = tap / 3, sx = tap - 3 * r;
+        const uint32_t a = boxes + (uint32_t)(3 * kc + sx) * FMB_BOX_BYTES + (uint32_t)r * (TC_TILE_W * 128);
+        const uint32_t b = ring + s * FMB_W_BYTES;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < TC_BK / 16; ++k)
+          wgmma_16b<T, FMB_NC>(acc1, gmma_desc<128>(a + 32 * k), gmma_desc<128>(b + 32 * k), (uint32_t)(kb | k));
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty[prev]);
+        }
+        prev = s;
       }
-      *reinterpret_cast<T2*>(out + off + cidx) = Pair16<T>::pack(o0, o1);
+      wgmma_wait<0>();
+      wgmma_fence_regs<FMB_NC / 2>(acc1);
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(&empty[prev]);
+        if (c == p.nch - 1) mbar_arrive(box_empty);  // the tile's last read of its input boxes
+      }
+      // ---- epilogue-1: + bias, SiLU, 16-bit -> A2 (this warpgroup's rows; 16-byte chunk j of row r at j ^ (r & 7)) ----
+#pragma unroll
+      for (int j = 0; j < FMB_NC / 8; ++j) {
+        const int cc = 8 * j + 2 * (lane & 3);  // column within the chunk
+        const int col = c * FMB_NC + cc;
+        float2 bv = make_float2(0.f, 0.f);
+        if (col < p.Cexp) bv = __ldg(reinterpret_cast<const float2*>(p.bias1 + col));  // Cexp % 16 == 0: col + 1 valid with col
+        const uint32_t sub = (uint32_t)(cc >> 6) * (TC_BM * 128), kc = (uint32_t)(cc & 63);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = r0 + 8 * h;
+          T2 v = Pair16<T>::pack(0.f, 0.f);
+          if (col < p.Cexp)
+            v = Pair16<T>::pack(tc_act<ACT_SILU, T>(acc1[4 * j + 2 * h] + bv.x), tc_act<ACT_SILU, T>(acc1[4 * j + 2 * h + 1] + bv.y));
+          const uint32_t off = sub + (uint32_t)r * 128 + ((((kc >> 3) ^ (uint32_t)(r & 7))) << 4) + (kc & 7) * 2;
+          *reinterpret_cast<T2*>(smem + L::a2_off + off) = v;
+        }
+      }
+      fence_proxy_async();  // generic-proxy writes -> visible to the tensor core (async proxy)
+      wg_sync(wg);
+      // ---- GEMM-2: acc2 += A2 x W2[:, chunk]^T, the two 64-channel halves of the W2 slice in consecutive stages ----
+      {
+        const int s0 = it % STAGES, s1 = (it + 1) % STAGES;
+        mbar_wait(&full[s0], (it / STAGES) & 1);
+        mbar_wait(&full[s1], ((it + 1) / STAGES) & 1);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < FMB_NC / 16; ++k) {
+          const uint32_t sub = (uint32_t)(k >> 2), ko = (uint32_t)(k & 3) * 32;
+          const uint32_t b = ring + (sub ? s1 : s0) * FMB_W_BYTES;
+          wgmma_16b<T, BN2>(acc2, gmma_desc<128>(a2 + sub * (TC_BM * 128) + wg * 64 * 128 + ko), gmma_desc<128>(b + ko), (uint32_t)(c | k));
+        }
+        wgmma_commit();
+        wgmma_wait<0>();  // A2 is rewritten by the next chunk's epilogue-1
+        wgmma_fence_regs<BN2 / 2>(acc2);
+        __syncwarp();
+        if (lane == 0) {
+          mbar_arrive(&empty[s0]);
+          mbar_arrive(&empty[s1]);
+        }
+        it += 2;
+      }
+    }
+    // ---- epilogue-2: + bias, + residual x, 16-bit store ----
+    const int c0 = 2 * (lane & 3);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      size_t off;
+      if (!tile_row_offset(1, t, r0 + 8 * h, g.M, g.Cout, g.tiles_w, g.tiles_h, g.Hout, g.Wout, off)) continue;
+#pragma unroll
+      for (int j = 0; j < BN2 / 8; ++j) {
+        const int cidx = c0 + 8 * j;
+        if (cidx >= g.Cout) break;
+        const float2 bv = __ldg(reinterpret_cast<const float2*>(g.bias + cidx));
+        float o0 = acc2[4 * j + 2 * h] + bv.x, o1 = acc2[4 * j + 2 * h + 1] + bv.y;
+        if (p.has_res) {
+          const float2 rv = Pair16<T>::unpack(*reinterpret_cast<const T2*>(res + off + cidx));
+          o0 += rv.x;
+          o1 += rv.y;
+        }
+        *reinterpret_cast<T2*>(out + off + cidx) = Pair16<T>::pack(o0, o1);
+      }
     }
   }
 }
@@ -186,7 +222,7 @@ struct FmbWeights {
   const TcWeights* w2 = nullptr;  // the projection's [Cout][Cexp] + bias
   int Cin = 0, Cexp = 0, Cout = 0, bn2 = 0;
   CUtensorMap mapW1, mapW2;
-  mutable CUtensorMap mapA;
+  mutable CUtensorMap mapA;       // the block input, 16 x 10-pixel boxes (tma_load_tap_boxes)
   mutable const void* cached_in = nullptr;
   mutable int cached_B = -1;
 };
@@ -216,12 +252,13 @@ inline const char* fmb_prepare(FmbWeights& f, const TcWeights& w1, const TcWeigh
 template <typename T, int BN2>
 inline const char* fmb_launch_k(int grid, const FmbWeights& f, const FmbParams& q, cudaStream_t st) {
   static bool attr_set = false;
+  if (q.g.kchunks != FmbSmem<BN2>::kchunks) return "fmb_kernel: k-chunks do not match the output width";
   if (!attr_set) {
-    if (cudaFuncSetAttribute(fmb_kernel<T, BN2>, cudaFuncAttributeMaxDynamicSharedMemorySize, FMB_SMEM_BYTES) != cudaSuccess)
+    if (cudaFuncSetAttribute(fmb_kernel<T, BN2>, cudaFuncAttributeMaxDynamicSharedMemorySize, FmbSmem<BN2>::smem_bytes) != cudaSuccess)
       return "cannot raise dynamic shared memory for fmb_kernel";
     attr_set = true;
   }
-  launch_k(fmb_kernel<T, BN2>, dim3(grid), dim3(TC_THREADS), FMB_SMEM_BYTES, st, f.mapA, f.mapW1, f.mapW2, q);
+  launch_k(fmb_kernel<T, BN2>, dim3(grid), dim3(TC_THREADS), FmbSmem<BN2>::smem_bytes, st, f.mapA, f.mapW1, f.mapW2, q);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
@@ -246,12 +283,13 @@ inline const char* fmb_launch(const FmbWeights& f, const void* in, void* out, in
   q.nch = (f.Cexp + FMB_NC - 1) / FMB_NC;
   q.has_res = has_res ? 1 : 0;
   if (f.cached_in != in || f.cached_B != B) {
-    const char* e = make_tmap_nhwc<T>(&f.mapA, in, B, H, W, f.Cin, 1);
+    const char* e = make_tmap_nhwc<T>(&f.mapA, in, B, H, W, f.Cin, 1, TC_BK, TC_TILE_W, FMB_BOX_H);
     if (e) return e;
     f.cached_in = in;
     f.cached_B = B;
   }
-  const int grid = B * g.tiles_w * g.tiles_h;
+  g.m_tiles = B * g.tiles_w * g.tiles_h;
+  const int grid = std::min(g.m_tiles, num_sms());  // persistent: one CTA per SM
   switch (f.bn2) {
     case 32: return fmb_launch_k<T, 32>(grid, f, q, st);
     case 64: return fmb_launch_k<T, 64>(grid, f, q, st);

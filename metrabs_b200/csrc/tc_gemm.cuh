@@ -209,6 +209,20 @@ __device__ __forceinline__ void tma_load_a_tile(void* dst, const CUtensorMap* ma
   }
 }
 
+// The p.S column-shifted input boxes of a stride-1, dilation-1 RxS conv for output tile m_blk and channel chunk kc: box s
+// (at dst + s * box_bytes) holds TC_TILE_W x (TC_TILE_H + R - 1) pixels from input row th * TC_TILE_H - pad_t and column
+// tw * TC_TILE_W - pad_l + s (map: make_tmap_nhwc with tile_h = TC_TILE_H + R - 1).  The A tile of tap (r, s) is then box s
+// from pixel row r on, r * TC_TILE_W * 128 bytes in: a multiple of 1024, so it keeps the SWIZZLE_128B phase and the
+// descriptors of a 1024-byte-aligned tile, and holds what tma_load_a_tile loads for that tap.  One load per column offset
+// instead of one per tap: R x fewer boxes and (TC_TILE_H + R - 1) / (R x TC_TILE_H) of the bytes.
+template <typename P>
+__device__ __forceinline__ void tma_load_tap_boxes(uint8_t* dst, int box_bytes, const CUtensorMap* map, uint64_t* bar, const P& p, int m_blk,
+                                                   int kc) {
+  const int tw = m_blk % p.tiles_w, th = (m_blk / p.tiles_w) % p.tiles_h, b = m_blk / (p.tiles_w * p.tiles_h);
+  for (int s = 0; s < p.S; ++s)
+    tma_load_4d(dst + s * box_bytes, map, bar, kc * TC_BK, tw * TC_TILE_W - p.pad_l + s, th * TC_TILE_H - p.pad_t, b);
+}
+
 // Persistent conv / GEMM kernel.  ACT: epilogue activation; RES: 0 no residual, 1 residual added AFTER the activation
 // (EfficientNet), 2 BEFORE (ResNet); BN: output channels per tile (wgmma N); T: operand and activation element type
 // (__nv_bfloat16 or __half).
