@@ -5,6 +5,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <map>
+#include <mutex>
 #include <type_traits>
 #include <utility>
 
@@ -24,13 +26,46 @@ inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, siz
 
 // streaming multiprocessors of the current device (grid sizes of the persistent / grid-stride kernels)
 inline int num_sms() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = 132;
-  }
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
+    n = 132;
   return n;
+}
+
+// Raises `kernel`'s dynamic shared-memory limit on the current device to `bytes`, unless an earlier call already raised it
+// that far there.  The limit belongs to the device's context: a process with handles on two devices needs it on both.
+inline cudaError_t smem_opt_in(const void* kernel, int bytes) {
+  static std::mutex mu;
+  static std::map<std::pair<int, const void*>, int> raised;  // (device, kernel) -> limit set
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  std::lock_guard<std::mutex> lock(mu);
+  int& limit = raised[{dev, kernel}];
+  if (limit >= bytes) return cudaSuccess;
+  e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e == cudaSuccess) limit = bytes;
+  return e;
+}
+
+// launch_k for kernels that may take more than 48 KB of dynamic shared memory; nullptr on success, else the CUDA error
+template <typename... KArgs, typename... Args>
+inline const char* launch_smem(void (*kernel)(KArgs...), dim3 grid, dim3 block, int smem, cudaStream_t st, Args&&... args) {
+  cudaError_t e = smem_opt_in((const void*)kernel, smem);
+  if (e == cudaSuccess) {
+    launch_k(kernel, grid, block, (size_t)smem, st, std::forward<Args>(args)...);
+    e = cudaGetLastError();
+  }
+  return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+}
+
+// Calls f(std::integral_constant<int, V>{}) for the V of Vs equal to v and returns its result, or `none` when v is not listed.
+// Each call site lists the values it launches with, so only those kernel instances are compiled.
+template <int... Vs, typename R, typename F>
+inline R with_const(int v, R none, F&& f) {
+  R r = none;
+  (void)((v == Vs && (r = f(std::integral_constant<int, Vs>{}), true)) || ...);
+  return r;
 }
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + __expf(-x)); }

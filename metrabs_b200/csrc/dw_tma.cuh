@@ -68,23 +68,6 @@ inline DwTmaPlan dw_tma_plan(int H, int W) {
   return best;
 }
 
-// rank-4 16-bit NHWC tensor [B][H][W][C]; box = 64 channels (128 bytes) x (W+2) x (BH+2) x G, no swizzle (quarter-warps read
-// whole 128-byte pixel rows: conflict-free as is)
-template <typename T>
-inline const char* make_tmap_dw(CUtensorMap* m, const void* ptr, uint64_t B, uint64_t H, uint64_t W, uint64_t C, uint32_t pw,
-                                uint32_t ph, uint32_t g) {
-  tmap_encode_fn enc = get_tmap_encode();
-  if (!enc) return "cuTensorMapEncodeTiled unavailable";
-  cuuint64_t dims[4] = {C, W, H, B};
-  cuuint64_t strides[3] = {C * 2, W * C * 2, H * W * C * 2};
-  cuuint32_t box[4] = {DWT_CG, pw, ph, g};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(m, tmap_dtype<T>(), 4, const_cast<void*>(ptr), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? nullptr : "cuTensorMapEncodeTiled(dw) failed";
-}
-
 // activation of a pair; SiLU(x) = h + h * tanh(h), h = x / 2 for bf16 outputs, silu_f16out for fp16 ones (same arithmetic as
 // fast_act<ACT_SILU, T>)
 template <int ACT, typename T>
@@ -279,14 +262,8 @@ dw3x3s1_tma_kernel(const __grid_constant__ CUtensorMap tmIn, const DwTmaParams p
   }
 }
 
-struct DwTmaCache {
-  CUtensorMap map;
-  const void* in = nullptr;
-  int B = -1;
-};
-
 template <typename T>
-inline const char* dw_tma_launch(DwTmaCache& cache, const DwTmaPlan& plan, const void* in, void* out, const float* w, const float* bias,
+inline const char* dw_tma_launch(TmapCache& cache, const DwTmaPlan& plan, const void* in, void* out, const float* w, const float* bias,
                                  float* pooled, int B, int H, int W, int C, int pad_t, int pad_l, int act, cudaStream_t st) {
   DwTmaParams p;
   p.out = out; p.w = w; p.bias = bias; p.pooled = pooled;
@@ -300,36 +277,19 @@ inline const char* dw_tma_launch(DwTmaCache& cache, const DwTmaPlan& plan, const
   p.nstrips = plan.G * p.bands * p.strips_w;
   p.stage_bytes = 128 * (W + 2) * (plan.BH + 2) * plan.G;
   p.inv_hw = 1.0f / (float)(H * W);
-  if (cache.in != in || cache.B != B) {
-    const char* e = make_tmap_dw<T>(&cache.map, in, (uint64_t)B, (uint64_t)H, (uint64_t)W, (uint64_t)C, (uint32_t)(W + 2),
-                                 (uint32_t)(plan.BH + 2), (uint32_t)plan.G);
-    if (e) return e;
-    cache.in = in;
-    cache.B = B;
-  }
+  // input box: 64 channels (128 bytes) x (W+2) x (BH+2) pixels x G crops, unswizzled (quarter-warps read whole 128-byte pixel
+  // rows: conflict-free as is)
+  const CUtensorMap* m = nullptr;
+  const char* e = cache.get(&m, [&](CUtensorMap* c) {
+    return make_tmap_nhwc<T>(c, in, B, H, W, C, DWT_CG, W + 2, plan.BH + 2, plan.G, 1, CU_TENSOR_MAP_SWIZZLE_NONE);
+  }, in, B, H, W, C, plan.BH, plan.G);
+  if (e) return e;
   // + one pixel row of slack: the last strip of a ragged row may read (never use) a few pixels past the patch
-  const size_t smem = (size_t)DWT_STAGES * p.stage_bytes + 128 + 8 * 128;
+  const int smem = DWT_STAGES * p.stage_bytes + 128 + 8 * 128;
   const int grid = std::min(p.items, 2 * num_sms());
-#define MTB_DWT_LAUNCH(A)                                                                                                  \
-  {                                                                                                                        \
-    static bool attr_set = false;                                                                                          \
-    if (!attr_set) {                                                                                                       \
-      if (cudaFuncSetAttribute(dw3x3s1_tma_kernel<T, A>, cudaFuncAttributeMaxDynamicSharedMemorySize,                          \
-                               DWT_STAGES * DWT_MAX_STAGE + 128 + 8 * 128) != cudaSuccess)                                 \
-        return "cannot raise dynamic shared memory for dw3x3s1_tma_kernel";                                                \
-      attr_set = true;                                                                                                     \
-    }                                                                                                                      \
-    launch_k(dw3x3s1_tma_kernel<T, A>, dim3(grid), dim3(DWT_THREADS), smem, st, cache.map, p);                                 \
-  }
-  switch (act) {
-    case ACT_SILU: MTB_DWT_LAUNCH(ACT_SILU); break;
-    case ACT_RELU: MTB_DWT_LAUNCH(ACT_RELU); break;
-    case ACT_HSWISH: MTB_DWT_LAUNCH(ACT_HSWISH); break;
-    default: return "unsupported activation in dw3x3s1_tma_kernel";
-  }
-#undef MTB_DWT_LAUNCH
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+  return with_const<ACT_SILU, ACT_RELU, ACT_HSWISH>(act, "unsupported activation in dw3x3s1_tma_kernel", [&](auto a) {
+    return launch_smem(dw3x3s1_tma_kernel<T, a>, dim3(grid), dim3(DWT_THREADS), smem, st, m[0], p);
+  });
 }
 
 }  // namespace mtb

@@ -83,7 +83,7 @@ struct Op {
   TcWeights tc;             // 16-bit (bf16 / fp16) K-major copy + TMA descriptor state for the wgmma path
   Tc32Weights tc32;         // fp32 K-major copy + TMA descriptor state for the 3xTF32 wgmma path (MTB_PRECISION_TF32X3)
   FmbWeights fmb;           // 16-bit tensor-core modes: this 3x3 expand conv and the NEXT op (1x1 projection) run as one fmb_kernel launch
-  mutable DwTmaCache dw_cache;  // input tensor map of the TMA-staged depthwise kernel
+  mutable TmapCache dw_maps;    // DW_TMA: its input tensor maps
   double flops = 0;         // 2*MACs per crop
   int stage = 0;            // EfficientNet stage (1-based; 0 = stem / last conv / other backbones)
 };
@@ -191,12 +191,18 @@ inline bool is_tc16(const mtb_handle* h) {
 }
 // calls f((T*)nullptr) with T the storage element type of the handle's mode
 template <typename F>
-int with_storage(const mtb_handle* h, F&& f) {
+auto with_storage(const mtb_handle* h, F&& f) {
   switch (storage(h)) {
     case ST_BF16: return f((__nv_bfloat16*)nullptr);
     case ST_F16: return f((__half*)nullptr);
     default: return f((float*)nullptr);
   }
+}
+// with_storage for the code that only exists for 16-bit storage (the tensor-core kernels): T is __half in the fp16 modes,
+// __nv_bfloat16 otherwise
+template <typename F>
+auto with_storage16(const mtb_handle* h, F&& f) {
+  return storage(h) == ST_F16 ? f((__half*)nullptr) : f((__nv_bfloat16*)nullptr);
 }
 // points the head decodes and the reconstruction solves for: the latents of a latent-point model, cfg.n_joints otherwise
 inline int head_points(const mtb_handle* h) { return h->n_latents > 0 ? h->n_latents : h->cfg.n_joints; }
@@ -646,10 +652,8 @@ const HostTensor* find(const mtb_handle* h, const std::string& k) {
 }
 
 int upload(mtb_handle* h, const void* host, size_t bytes, void** dev) {
-  CUDA_TRY(h, cudaMalloc(dev, bytes));
-  h->dev_allocs.push_back(*dev);
-  CUDA_TRY(h, cudaMemcpy(*dev, host, bytes, cudaMemcpyHostToDevice));
-  return MTB_OK;
+  const char* e = upload_dev(h->dev_allocs, dev, host, bytes);
+  return e ? fail(h, MTB_ERR_CUDA, "weight upload: %s", e) : MTB_OK;
 }
 
 int prepare_op_weights(mtb_handle* h, Op& op) {
@@ -708,8 +712,10 @@ int prepare_op_weights(mtb_handle* h, Op& op) {
   rc = upload(h, bias.data(), bias.size() * 4, (void**)&op.d_bias);
   if (rc) return rc;
   if (is_tc16(h) && tc_like) {
-    const char* e = storage(h) == ST_F16 ? tc_prepare_weights<__half>(op.tc, wk.data(), bias.data(), K, op.Cout, op.R, op.S, op.Cin, h->dev_allocs)
-                                         : tc_prepare_weights<__nv_bfloat16>(op.tc, wk.data(), bias.data(), K, op.Cout, op.R, op.S, op.Cin, h->dev_allocs);
+    const char* e = with_storage16(h, [&](auto* tag) {
+      return tc_prepare_weights<std::remove_pointer_t<decltype(tag)>>(op.tc, wk.data(), bias.data(), K, op.Cout, op.R, op.S, op.Cin,
+                                                                      h->dev_allocs);
+    });
     if (e) return fail(h, MTB_ERR_CUDA, "tensor-core weight prep for '%s': %s", op.name.c_str(), e);
   }
   if (h->cfg.precision == MTB_PRECISION_TF32X3 &&
@@ -804,6 +810,14 @@ bool dw_kernel_pools(DwKernel k) { return k == DW_TMA || k == DW_STRIP_16B || k 
 
 constexpr int kDwOW = 4;  // outputs per thread along W in dwconv3x3_pool_16b_kernel (measured: 4 -> 3.65 ms, 2 -> 4.25 ms per 128 crops)
 constexpr int kDw5OW = 4;  // outputs per thread along W in dwconv5x5_16b_kernel
+
+// f(stride, act) with both compile-time constants (stride 1 or 2, act one of ACTS): the launch of a templated depthwise kernel
+template <int... ACTS, typename F>
+cudaError_t dw_dispatch(const Op& op, F&& f) {
+  return with_const<1, 2>(op.stride, cudaErrorNotSupported, [&](auto s) {
+    return with_const<ACTS...>(op.act, cudaErrorNotSupported, [&](auto a) { return f(s, a); });
+  });
+}
 
 // Picks the kernel of a depthwise op and the number of partial pooling slices it writes (fc1 sums that many).  bf16 and fp16
 // tensor-core modes: 5x5 ops run dwconv5x5_16b_kernel, which does not pool; 3x3 stride-1 ops run the TMA-staged kernel when
@@ -931,35 +945,33 @@ int run_op_t(mtb_handle* h, const Op& op, const float* crops, int B, const Works
           if constexpr (!k16) {
             return fail(h, MTB_ERR_CUDA, "depthwise %s: 16-bit kernel chosen for fp32 storage", op.name.c_str());
           } else if (op.dw_kernel == DW_TMA) {
-            const char* e = dw_tma_launch<T>(op.dw_cache, op.dw_plan, p.in, p.out, op.d_w, op.d_bias, pooled, B, op.Hout, op.Wout,
+            const char* e = dw_tma_launch<T>(op.dw_maps, op.dw_plan, p.in, p.out, op.d_w, op.d_bias, pooled, B, op.Hout, op.Wout,
                                              op.Cout, op.pad_t, op.pad_l, op.act, st);
             if (e) return fail(h, MTB_ERR_CUDA, "depthwise (TMA) launch %s: %s", op.name.c_str(), e);
           } else {
-            dim3 grid((op.Cout / 8 + 31) / 32, op.pool_slices, B), block(32, 8);
-#define MTB_DW16(ST, AC) launch_k(dwconv3x3_pool_16b_kernel<T, ST, AC, kDwOW>, dim3(grid), dim3(block), 0, st, p, pooled)
-            if (op.act == ACT_SILU) { if (op.stride == 1) MTB_DW16(1, ACT_SILU); else MTB_DW16(2, ACT_SILU); }
-            else if (op.act == ACT_RELU) { if (op.stride == 1) MTB_DW16(1, ACT_RELU); else MTB_DW16(2, ACT_RELU); }
-            else { if (op.stride == 1) MTB_DW16(1, ACT_HSWISH); else MTB_DW16(2, ACT_HSWISH); }
-#undef MTB_DW16
+            const dim3 grid((op.Cout / 8 + 31) / 32, op.pool_slices, B), block(32, 8);
+            const cudaError_t e = dw_dispatch<ACT_SILU, ACT_RELU, ACT_HSWISH>(op, [&](auto s, auto a) {
+              return launch_k(dwconv3x3_pool_16b_kernel<T, s, a, kDwOW>, grid, block, 0, st, p, pooled);
+            });
+            if (e != cudaSuccess) return fail(h, MTB_ERR_CUDA, "depthwise launch %s: %s", op.name.c_str(), cudaGetErrorString(e));
           }
         } else if (op.dw_kernel == DW_STRIP_F32) {
           // fp32 strip kernel: 4 channels x 4 pixels per thread, SE squeeze fused (partial slices summed by fc1)
-          dim3 grid((op.Cout / 4 + 31) / 32, op.pool_slices, B), block(32, 8);
-#define MTB_DWF32(ST, AC) launch_k(dwconv3x3_pool_f32_kernel<ST, AC, kDwOW>, dim3(grid), dim3(block), 0, st, p, pooled)
-          if (op.act == ACT_SILU) { if (op.stride == 1) MTB_DWF32(1, ACT_SILU); else MTB_DWF32(2, ACT_SILU); }
-          else if (op.act == ACT_RELU) { if (op.stride == 1) MTB_DWF32(1, ACT_RELU); else MTB_DWF32(2, ACT_RELU); }
-          else { if (op.stride == 1) MTB_DWF32(1, ACT_HSWISH); else MTB_DWF32(2, ACT_HSWISH); }
-#undef MTB_DWF32
+          const dim3 grid((op.Cout / 4 + 31) / 32, op.pool_slices, B), block(32, 8);
+          const cudaError_t e = dw_dispatch<ACT_SILU, ACT_RELU, ACT_HSWISH>(op, [&](auto s, auto a) {
+            return launch_k(dwconv3x3_pool_f32_kernel<s, a, kDwOW>, grid, block, 0, st, p, pooled);
+          });
+          if (e != cudaSuccess) return fail(h, MTB_ERR_CUDA, "depthwise launch %s: %s", op.name.c_str(), cudaGetErrorString(e));
         } else if (op.dw_kernel == DW_5X5_16B) {
           if constexpr (!k16) {
             return fail(h, MTB_ERR_CUDA, "depthwise %s: 16-bit kernel chosen for fp32 storage", op.name.c_str());
           } else {
             const size_t items = (size_t)B * op.Hout * ((op.Wout + kDw5OW - 1) / kDw5OW) * (op.Cout / 8);
             const dim3 grid(grid_for(items, 256));
-#define MTB_DW5(ST, AC) launch_k(dwconv5x5_16b_kernel<T, ST, AC, kDw5OW>, grid, dim3(256), 0, st, p)
-            if (op.act == ACT_RELU) { if (op.stride == 1) MTB_DW5(1, ACT_RELU); else MTB_DW5(2, ACT_RELU); }
-            else { if (op.stride == 1) MTB_DW5(1, ACT_HSWISH); else MTB_DW5(2, ACT_HSWISH); }
-#undef MTB_DW5
+            const cudaError_t e = dw_dispatch<ACT_RELU, ACT_HSWISH>(op, [&](auto s, auto a) {
+              return launch_k(dwconv5x5_16b_kernel<T, s, a, kDw5OW>, grid, dim3(256), 0, st, p);
+            });
+            if (e != cudaSuccess) return fail(h, MTB_ERR_CUDA, "depthwise launch %s: %s", op.name.c_str(), cudaGetErrorString(e));
           }
         } else {
           size_t total = (size_t)B * op.Hout * op.Wout * (op.Cout / 4);
@@ -1029,8 +1041,9 @@ int run_fused_block(mtb_handle* h, const Op& a, const Op& b, int B, const Worksp
   void* out = buf_ptr(ws, b.out_buf, features);
   const double bytes = 2.0 * B * a.Hin * a.Win * (a.Cin + b.Cout) + 2.0 * (9.0 * a.Cin * a.Cout + (double)b.Cin * b.Cout);
   ProfScope prof(h, KC_FMB, (a.flops + b.flops) * B, bytes, st);
-  const char* e = storage(h) == ST_F16 ? fmb_launch<__half>(a.fmb, in, out, B, a.Hin, a.Win, a.pad_t, a.pad_l, b.res_buf != BUF_NONE, st)
-                                       : fmb_launch<__nv_bfloat16>(a.fmb, in, out, B, a.Hin, a.Win, a.pad_t, a.pad_l, b.res_buf != BUF_NONE, st);
+  const char* e = with_storage16(h, [&](auto* tag) {
+    return fmb_launch<std::remove_pointer_t<decltype(tag)>>(a.fmb, in, out, B, a.Hin, a.Win, a.pad_t, a.pad_l, b.res_buf != BUF_NONE, st);
+  });
   if (e) return fail(h, MTB_ERR_CUDA, "fused FusedMBConv launch %s: %s", a.name.c_str(), e);
   h->launches++;
   return MTB_OK;
@@ -1086,16 +1099,10 @@ DecodeScale make_scale(const mtb_config& c) {
 }
 
 template <typename T>
-int launch_softargmax_bhwn(const void* logits, float* out2d, float* out3d, int B, int J, int D, int H, int W,
-                           int ld, DecodeScale sc, cudaStream_t st) {
-  const int N = J * (1 + D);
-  size_t smem = ((size_t)N + 4 * 128) * sizeof(float4);
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(softargmax_bhwn_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return (int)e;
-  }
-  launch_k(softargmax_bhwn_kernel<T>, dim3(B), dim3(512), smem, st, (const T*)logits, out2d, out3d, J, D, H, W, ld, sc);
-  return (int)cudaGetLastError();
+const char* launch_softargmax_bhwn(const void* logits, float* out2d, float* out3d, int B, int J, int D, int H, int W,
+                                   int ld, DecodeScale sc, cudaStream_t st) {
+  const int smem = (J * (1 + D) + 4 * 128) * (int)sizeof(float4);
+  return launch_smem(softargmax_bhwn_kernel<T>, dim3(B), dim3(512), smem, st, (const T*)logits, out2d, out3d, J, D, H, W, ld, sc);
 }
 
 int head_decode_impl(mtb_handle* h, const void* features, int B, float* c2d, float* c3d, const Workspace& ws,
@@ -1109,10 +1116,10 @@ int head_decode_impl(mtb_handle* h, const void* features, int B, float* c2d, flo
   if (op.tc.ready) {
     // fused: 1x1-conv GEMM on the tensor cores with the soft-argmax reduction in the epilogue; logits never reach HBM
     ProfScope prof(h, KC_HEAD_FUSED, op.flops * B, feat_bytes + (double)op.Cin * op.Cout * 2 + out_bytes, st);
-    const char* e = storage(h) == ST_F16 ? tc_head_launch<__half>(op.tc, features, B, h->feat_side, h->feat_side, J, c.depth,
-                                                                  make_scale(c), c2d, c3d, ws.base + ws.off_logits, st)
-                                         : tc_head_launch<__nv_bfloat16>(op.tc, features, B, h->feat_side, h->feat_side, J, c.depth,
-                                                                         make_scale(c), c2d, c3d, ws.base + ws.off_logits, st);
+    const char* e = with_storage16(h, [&](auto* tag) {
+      return tc_head_launch<std::remove_pointer_t<decltype(tag)>>(op.tc, features, B, h->feat_side, h->feat_side, J, c.depth,
+                                                                  make_scale(c), c2d, c3d, ws.base + ws.off_logits, st);
+    });
     if (e) return fail(h, MTB_ERR_CUDA, "fused head: %s", e);
     h->launches += 2;
     return MTB_OK;
@@ -1131,14 +1138,12 @@ int head_decode_impl(mtb_handle* h, const void* features, int B, float* c2d, flo
     e = cudaSuccess;
   } else {
     ProfScope prof(h, KC_HEAD_CONV_SIMT, op.flops * B, feat_bytes + (double)op.Cin * op.Cout * 4 + logit_bytes, st);
-    e = storage(h) == ST_BF16  ? launch_conv_igemm<__nv_bfloat16, float>(p, st)
-        : storage(h) == ST_F16 ? launch_conv_igemm<__half, float>(p, st)
-                               : launch_conv_igemm<float, float>(p, st);
+    e = with_storage(h, [&](auto* tag) { return launch_conv_igemm<std::remove_pointer_t<decltype(tag)>, float>(p, st); });
   }
   if (e != cudaSuccess) return fail(h, MTB_ERR_CUDA, "head conv: %s", cudaGetErrorString(e));
   ProfScope prof(h, KC_SOFTARGMAX, 0.0, logit_bytes + out_bytes, st);
-  int rc = launch_softargmax_bhwn<float>(p.out, c2d, c3d, B, J, c.depth, op.Hin, op.Win, op.Cout, make_scale(c), st);
-  if (rc) return fail(h, MTB_ERR_CUDA, "softargmax: %s", cudaGetErrorString((cudaError_t)rc));
+  const char* se = launch_softargmax_bhwn<float>(p.out, c2d, c3d, B, J, c.depth, op.Hin, op.Win, op.Cout, make_scale(c), st);
+  if (se) return fail(h, MTB_ERR_CUDA, "softargmax: %s", se);
   h->launches += 2;
   return MTB_OK;
 }
@@ -1204,19 +1209,19 @@ __global__ void from_float_kernel(const float* in, T* out, size_t n) {
 
 // storage -> fp32 copy of n elements (a plain copy for fp32 storage)
 void copy_to_float(const mtb_handle* h, const void* src, float* out, size_t n, cudaStream_t st) {
-  switch (storage(h)) {
-    case ST_BF16: launch_k(to_float_kernel<__nv_bfloat16>, dim3(grid_for(n, 256)), dim3(256), 0, st, (const __nv_bfloat16*)src, out, n); break;
-    case ST_F16: launch_k(to_float_kernel<__half>, dim3(grid_for(n, 256)), dim3(256), 0, st, (const __half*)src, out, n); break;
-    default: cudaMemcpyAsync(out, src, n * 4, cudaMemcpyDeviceToDevice, st); break;
-  }
+  with_storage(h, [&](auto* tag) {
+    using T = std::remove_pointer_t<decltype(tag)>;
+    if constexpr (std::is_same<T, float>::value) return cudaMemcpyAsync(out, src, n * 4, cudaMemcpyDeviceToDevice, st);
+    else return launch_k(to_float_kernel<T>, dim3(grid_for(n, 256)), dim3(256), 0, st, (const T*)src, out, n);
+  });
 }
 // fp32 -> storage copy of n elements
 void copy_from_float(const mtb_handle* h, const float* src, void* out, size_t n, cudaStream_t st) {
-  switch (storage(h)) {
-    case ST_BF16: launch_k(from_float_kernel<__nv_bfloat16>, dim3(grid_for(n, 256)), dim3(256), 0, st, src, (__nv_bfloat16*)out, n); break;
-    case ST_F16: launch_k(from_float_kernel<__half>, dim3(grid_for(n, 256)), dim3(256), 0, st, src, (__half*)out, n); break;
-    default: cudaMemcpyAsync(out, src, n * 4, cudaMemcpyDeviceToDevice, st); break;
-  }
+  with_storage(h, [&](auto* tag) {
+    using T = std::remove_pointer_t<decltype(tag)>;
+    if constexpr (std::is_same<T, float>::value) return cudaMemcpyAsync(out, src, n * 4, cudaMemcpyDeviceToDevice, st);
+    else return launch_k(from_float_kernel<T>, dim3(grid_for(n, 256)), dim3(256), 0, st, src, (T*)out, n);
+  });
 }
 
 // [b,J,2] + [b,J,3] -> [b,J,5] (what travels in the all-gather) and back
@@ -1392,8 +1397,7 @@ int mtb_finalize_weights(mtb_handle* h) {
     if (b.R != 1 || b.stride != 1 || b.act != ACT_NONE || b.scale_buf != BUF_NONE || b.res_first || b.in_buf != a.out_buf) continue;
     if (b.res_buf != BUF_NONE && b.res_buf != a.in_buf) continue;
     if (a.Hin != a.Hout || a.Win != a.Wout || b.out_buf == a.in_buf) continue;
-    const char* e = storage(h) == ST_F16 ? fmb_prepare<__half>(a.fmb, a.tc, b.tc) : fmb_prepare<__nv_bfloat16>(a.fmb, a.tc, b.tc);
-    if (e) return fail(h, MTB_ERR_CUDA, "fused FusedMBConv weight prep for '%s': %s", a.name.c_str(), e);
+    fmb_prepare(a.fmb, a.tc, b.tc);
   }
   {
     Op& hd = h->head;
@@ -1449,8 +1453,9 @@ int mtb_finalize_weights(mtb_handle* h) {
           b0[n] = find(h, hd.biaskey)->data[n];
           for (int cc = 0; cc < hd.Cin; ++cc) w0[(size_t)n * hd.Cin + cc] = w->data[(size_t)n * hd.Cin + cc];
         }
-        const char* e = storage(h) == ST_F16 ? tc_prepare_head<__half>(hd.tc, w0.data(), b0.data(), hd.Cin, n_real, h->dev_allocs)
-                                             : tc_prepare_head<__nv_bfloat16>(hd.tc, w0.data(), b0.data(), hd.Cin, n_real, h->dev_allocs);
+        const char* e = with_storage16(h, [&](auto* tag) {
+          return tc_prepare_head<std::remove_pointer_t<decltype(tag)>>(hd.tc, w0.data(), b0.data(), hd.Cin, n_real, h->dev_allocs);
+        });
         if (e) return fail(h, MTB_ERR_CUDA, "tensor-core head weight prep: %s", e);
       }
     }
@@ -1554,23 +1559,18 @@ int mtb_softargmax(const void* logits, int dtype, int layout_, int batch, int n_
     int hw_shift = 0, w_shift = 0;
     while ((1 << hw_shift) < hw) ++hw_shift;
     while ((1 << w_shift) < width) ++w_shift;
-#define MTB_SA_LAUNCH(TT, VV, PP)                                                                                        \
-  launch_k(softargmax_bdjhw_kernel<TT, VV, PP>, dim3(rows), dim3(256), 0, st, (const TT*)logits, out, n_joints, D, height, \
-           width, (int)two_d, hw_shift, w_shift)
-    if (dtype == MTB_DTYPE_F32) {
-      if (vec && pow2) MTB_SA_LAUNCH(float, 4, true);
-      else if (vec) MTB_SA_LAUNCH(float, 4, false);
-      else MTB_SA_LAUNCH(float, 1, false);
-    } else if (dtype == MTB_DTYPE_BF16) {
-      if (vec && pow2) MTB_SA_LAUNCH(__nv_bfloat16, 8, true);
-      else if (vec) MTB_SA_LAUNCH(__nv_bfloat16, 8, false);
-      else MTB_SA_LAUNCH(__nv_bfloat16, 1, false);
-    } else {  // fp16: what the reference's head emits under its autocast (multiperson_model.py:241, models/metrabs.py:80)
-      if (vec && pow2) MTB_SA_LAUNCH(__half, 8, true);
-      else if (vec) MTB_SA_LAUNCH(__half, 8, false);
-      else MTB_SA_LAUNCH(__half, 1, false);
-    }
-#undef MTB_SA_LAUNCH
+    // loads: 0 scalar, 1 vector, 2 vector with power-of-two shapes (shift indexing)
+    const int loads = vec ? (pow2 ? 2 : 1) : 0;
+    auto launch = [&](auto* tag) {
+      using TT = std::remove_pointer_t<decltype(tag)>;
+      with_const<0, 1, 2>(loads, cudaErrorNotSupported, [&](auto l) {
+        return launch_k(softargmax_bdjhw_kernel<TT, l == 0 ? 1 : 16 / (int)sizeof(TT), l == 2>, dim3(rows), dim3(256), 0, st,
+                        (const TT*)logits, out, n_joints, D, height, width, (int)two_d, hw_shift, w_shift);
+      });
+    };
+    if (dtype == MTB_DTYPE_F32) launch((float*)nullptr);
+    else if (dtype == MTB_DTYPE_BF16) launch((__nv_bfloat16*)nullptr);
+    else launch((__half*)nullptr);  // fp16: what the reference's head emits under its autocast (multiperson_model.py:241, models/metrabs.py:80)
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(nullptr, MTB_ERR_CUDA, "softargmax launch: %s", cudaGetErrorString(e));
     return MTB_OK;
@@ -1578,10 +1578,10 @@ int mtb_softargmax(const void* logits, int dtype, int layout_, int batch, int n_
   if (layout_ == MTB_LAYOUT_BHWN) {
     DecodeScale sc{};
     sc.apply = 0;
-    int rc = dtype == MTB_DTYPE_F32
+    const char* e = dtype == MTB_DTYPE_F32
                  ? launch_softargmax_bhwn<float>(logits, out2d, out3d, batch, n_joints, depth, height, width, n_joints * (1 + depth), sc, st)
                  : launch_softargmax_bhwn<__nv_bfloat16>(logits, out2d, out3d, batch, n_joints, depth, height, width, n_joints * (1 + depth), sc, st);
-    if (rc) return fail(nullptr, MTB_ERR_CUDA, "softargmax launch: %s", cudaGetErrorString((cudaError_t)rc));
+    if (e) return fail(nullptr, MTB_ERR_CUDA, "softargmax launch: %s", e);
     return MTB_OK;
   }
   return fail(nullptr, MTB_ERR_INVALID_ARG, "unknown layout %d", layout_);
@@ -2141,10 +2141,6 @@ int mtb_debug_run_op(mtb_handle* h, int op_index, const float* in, const float* 
   if (res) { o.res_buf = 1; put(res, 1, n_out, false); }
   if (scale) { o.scale_buf = BUF_SMALL0 + 2; put(scale, o.scale_buf, (size_t)batch * o.Cin, true); }
   o.out_buf = (o.type == OP_POOL || o.small_io) ? BUF_SMALL0 + 1 : 2;
-  o.tc.cached_in = nullptr;  // the copy must not reuse a tensor map encoded for other buffers
-  o.tc.map_sets.clear();
-  o.tc32.map_sets.clear();
-  o.dw_cache = DwTmaCache();
   o.fused_pool = false;      // in isolation a depthwise op does not pool and a pool op runs its own kernel
   rc = run_op(h, o, crops, batch, ws, nullptr, st);
   if (rc) return rc;
@@ -2180,7 +2176,6 @@ int mtb_debug_run_fused_block(mtb_handle* h, int op_index, const float* in, int 
   copy_from_float(h, in, buf_ptr(ws, 0, nullptr), n_in, st);
   a.in_buf = 0; a.out_buf = 1; b.in_buf = 1; b.out_buf = 2;
   if (b.res_buf != BUF_NONE) b.res_buf = 0;
-  a.fmb.cached_in = nullptr;  // the copy must not reuse a tensor map encoded for other buffers
   rc = run_fused_block(h, a, b, batch, ws, nullptr, st);
   if (rc) return rc;
   copy_to_float(h, buf_ptr(ws, 2, nullptr), out, n_out, st);

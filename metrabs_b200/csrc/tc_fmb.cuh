@@ -221,10 +221,7 @@ struct FmbWeights {
   const TcWeights* w1 = nullptr;  // the expand conv's 16-bit K-major weights [Cexp][9*Cin] + bias
   const TcWeights* w2 = nullptr;  // the projection's [Cout][Cexp] + bias
   int Cin = 0, Cexp = 0, Cout = 0, bn2 = 0;
-  CUtensorMap mapW1, mapW2;
-  mutable CUtensorMap mapA;       // the block input, 16 x 10-pixel boxes (tma_load_tap_boxes)
-  mutable const void* cached_in = nullptr;
-  mutable int cached_B = -1;
+  mutable TmapCache maps;         // (block input in 16 x 10-pixel boxes for tma_load_tap_boxes, W1, W2)
 };
 
 // shapes the fused kernel covers: 3x3 stride-1 expand (SiLU) + 1x1 projection, Cin = Cout (identity-shaped block)
@@ -232,35 +229,13 @@ inline bool fmb_shape_ok(int cin, int cexp, int cout) {
   return cin % 16 == 0 && cin >= 16 && cin <= 96 && cout == cin && cexp % 16 == 0 && cexp >= 32 && cexp <= 512;
 }
 
-template <typename T>
-inline const char* fmb_prepare(FmbWeights& f, const TcWeights& w1, const TcWeights& w2) {
+inline void fmb_prepare(FmbWeights& f, const TcWeights& w1, const TcWeights& w2) {
   f.ready = false;
-  if (!fmb_shape_ok(w1.Cin, w1.Cout, w2.Cout) || w2.Cin != w1.Cout || w1.taps != 9) return nullptr;
+  if (!fmb_shape_ok(w1.Cin, w1.Cout, w2.Cout) || w2.Cin != w1.Cout || w1.taps != 9) return;
   f.w1 = &w1; f.w2 = &w2;
   f.Cin = w1.Cin; f.Cexp = w1.Cout; f.Cout = w2.Cout;
   f.bn2 = tc_pick_bn(f.Cout);
-  const char* e = make_tmap_2d<T>(&f.mapW1, w1.d_w, (uint64_t)f.Cexp, (uint64_t)9 * f.Cin, FMB_NC);
-  if (e) return e;
-  e = make_tmap_2d<T>(&f.mapW2, w2.d_w, (uint64_t)f.Cout, (uint64_t)f.Cexp, (uint32_t)f.bn2);
-  if (e) return e;
-  f.cached_in = nullptr;
-  f.cached_B = -1;
   f.ready = true;
-  return nullptr;
-}
-
-template <typename T, int BN2>
-inline const char* fmb_launch_k(int grid, const FmbWeights& f, const FmbParams& q, cudaStream_t st) {
-  static bool attr_set = false;
-  if (q.g.kchunks != FmbSmem<BN2>::kchunks) return "fmb_kernel: k-chunks do not match the output width";
-  if (!attr_set) {
-    if (cudaFuncSetAttribute(fmb_kernel<T, BN2>, cudaFuncAttributeMaxDynamicSharedMemorySize, FmbSmem<BN2>::smem_bytes) != cudaSuccess)
-      return "cannot raise dynamic shared memory for fmb_kernel";
-    attr_set = true;
-  }
-  launch_k(fmb_kernel<T, BN2>, dim3(grid), dim3(TC_THREADS), FmbSmem<BN2>::smem_bytes, st, f.mapA, f.mapW1, f.mapW2, q);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 
 template <typename T>
@@ -282,19 +257,20 @@ inline const char* fmb_launch(const FmbWeights& f, const void* in, void* out, in
   q.Cexp = f.Cexp;
   q.nch = (f.Cexp + FMB_NC - 1) / FMB_NC;
   q.has_res = has_res ? 1 : 0;
-  if (f.cached_in != in || f.cached_B != B) {
-    const char* e = make_tmap_nhwc<T>(&f.mapA, in, B, H, W, f.Cin, 1, TC_BK, TC_TILE_W, FMB_BOX_H);
-    if (e) return e;
-    f.cached_in = in;
-    f.cached_B = B;
-  }
+  const CUtensorMap* m = nullptr;  // block input, W1, W2
+  const char* e = f.maps.get(&m, [&](CUtensorMap* c) {
+    const CUtensorMapSwizzle sw = CU_TENSOR_MAP_SWIZZLE_128B;
+    const char* r = make_tmap_nhwc<T>(&c[0], in, B, H, W, f.Cin, TC_BK, TC_TILE_W, FMB_BOX_H, 1, 1, sw);
+    if (!r) r = make_tmap_2d<T>(&c[1], f.w1->d_w, f.Cexp, (uint64_t)9 * f.Cin, FMB_NC, TC_BK, sw);
+    return r ? r : make_tmap_2d<T>(&c[2], f.w2->d_w, f.Cout, f.Cexp, f.bn2, TC_BK, sw);
+  }, in, f.w1->d_w, f.w2->d_w, B, H, W, f.Cin, f.Cexp, f.Cout, f.bn2);
+  if (e) return e;
   g.m_tiles = B * g.tiles_w * g.tiles_h;
   const int grid = std::min(g.m_tiles, num_sms());  // persistent: one CTA per SM
-  switch (f.bn2) {
-    case 32: return fmb_launch_k<T, 32>(grid, f, q, st);
-    case 64: return fmb_launch_k<T, 64>(grid, f, q, st);
-    default: return fmb_launch_k<T, 128>(grid, f, q, st);
-  }
+  return with_const<32, 64, 128>(f.bn2, "unsupported N tile", [&](auto bn2) {
+    if (q.g.kchunks != FmbSmem<bn2>::kchunks) return "fmb_kernel: k-chunks do not match the output width";
+    return launch_smem(fmb_kernel<T, bn2>, dim3(grid), dim3(TC_THREADS), FmbSmem<bn2>::smem_bytes, st, m[0], m[1], m[2], q);
+  });
 }
 
 }  // namespace mtb

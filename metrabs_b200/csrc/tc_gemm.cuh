@@ -211,7 +211,7 @@ __device__ __forceinline__ void tma_load_a_tile(void* dst, const CUtensorMap* ma
 
 // The p.S column-shifted input boxes of a stride-1, dilation-1 RxS conv for output tile m_blk and channel chunk kc: box s
 // (at dst + s * box_bytes) holds TC_TILE_W x (TC_TILE_H + R - 1) pixels from input row th * TC_TILE_H - pad_t and column
-// tw * TC_TILE_W - pad_l + s (map: make_tmap_nhwc with tile_h = TC_TILE_H + R - 1).  The A tile of tap (r, s) is then box s
+// tw * TC_TILE_W - pad_l + s (map: make_tmap_nhwc with box_h = TC_TILE_H + R - 1).  The A tile of tap (r, s) is then box s
 // from pixel row r on, r * TC_TILE_W * 128 bytes in: a multiple of 1024, so it keeps the SWIZZLE_128B phase and the
 // descriptors of a 1024-byte-aligned tile, and holds what tma_load_a_tile loads for that tap.  One load per column offset
 // instead of one per tap: R x fewer boxes and (TC_TILE_H + R - 1) / (R x TC_TILE_H) of the bytes.
@@ -423,41 +423,88 @@ inline tmap_encode_fn get_tmap_encode() {
 
 template <typename T>
 constexpr CUtensorMapDataType tmap_dtype() {
-  return std::is_same<T, __half>::value ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  return std::is_same<T, float>::value    ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+         : std::is_same<T, __half>::value ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
+                                          : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
 }
 
-// rank-2 16-bit tensor [rows][cols] (cols contiguous), box [box_rows][64], 128B swizzle, OOB -> 0
-template <typename T = __nv_bfloat16>
-inline const char* make_tmap_2d(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows,
-                                uint32_t box_cols = TC_BK) {
+// Encodes the tensor map of a dense T tensor (float, bf16 or fp16) with `rank` dims, innermost first, and a box of
+// box[i] elements taken every estr[i] elements along dim i (to load N elements with traversal stride s, box = N * s).
+// Out-of-bounds elements read as 0.  The swizzle is the caller's: it must match how the kernel addresses the box in shared
+// memory, and cannot be derived from the box's row bytes (dw3x3s1_tma_kernel reads 128-byte rows unswizzled).
+template <typename T>
+inline const char* make_tmap(CUtensorMap* m, const void* ptr, int rank, const uint64_t* dims, const uint32_t* box, const uint32_t* estr,
+                             CUtensorMapSwizzle swizzle) {
   tmap_encode_fn enc = get_tmap_encode();
   if (!enc) return "cuTensorMapEncodeTiled unavailable";
-  cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {cols * 2};
-  cuuint32_t box[2] = {box_cols, box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(m, tmap_dtype<T>(), 2, const_cast<void*>(ptr), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, box_cols == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? nullptr : "cuTensorMapEncodeTiled(2d) failed";
+  cuuint64_t strides[3];
+  for (int i = 1; i < rank; ++i) strides[i - 1] = (i == 1 ? sizeof(T) : strides[i - 2]) * dims[i - 1];
+  CUresult r = enc(m, tmap_dtype<T>(), rank, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
+                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? nullptr : "cuTensorMapEncodeTiled failed";
 }
-// rank-4 16-bit NHWC tensor [B][H][W][C]; box = 64 channels x (TILE_W x TILE_H) pixels sampled every `stride` pixels
-// (element strides: to load N elements along a dimension with traversal stride s, boxDim = N*s)
-template <typename T = __nv_bfloat16>
-inline const char* make_tmap_nhwc(CUtensorMap* m, const void* ptr, uint64_t B, uint64_t H, uint64_t W, uint64_t C, uint32_t stride,
-                                  uint32_t box_c = TC_BK, uint32_t tile_w = TC_TILE_W, uint32_t tile_h = TC_TILE_H) {
-  tmap_encode_fn enc = get_tmap_encode();
-  if (!enc) return "cuTensorMapEncodeTiled unavailable";
-  cuuint64_t dims[4] = {C, W, H, B};
-  cuuint64_t strides[3] = {C * 2, W * C * 2, H * W * C * 2};
-  cuuint32_t box[4] = {box_c, tile_w * stride, tile_h * stride, 1};
-  cuuint32_t estr[4] = {1, stride, stride, 1};
-  CUresult r = enc(m, tmap_dtype<T>(), 4, const_cast<void*>(ptr), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, box_c == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? nullptr : "cuTensorMapEncodeTiled(4d) failed";
+// row-major matrix [rows][cols], box [box_rows][box_cols]
+template <typename T>
+inline const char* make_tmap_2d(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows, uint32_t box_cols,
+                             CUtensorMapSwizzle swizzle) {
+  const uint64_t dims[2] = {cols, rows};
+  const uint32_t box[2] = {box_cols, box_rows}, estr[2] = {1, 1};
+  return make_tmap<T>(m, ptr, 2, dims, box, estr, swizzle);
+}
+// NHWC tensor [B][H][W][C], box box_c channels x box_w x box_h pixels sampled every `stride` pixels x box_b images
+template <typename T>
+inline const char* make_tmap_nhwc(CUtensorMap* m, const void* ptr, uint64_t B, uint64_t H, uint64_t W, uint64_t C, uint32_t box_c,
+                             uint32_t box_w, uint32_t box_h, uint32_t box_b, uint32_t stride, CUtensorMapSwizzle swizzle) {
+  const uint64_t dims[4] = {C, W, H, B};
+  const uint32_t box[4] = {box_c, box_w * stride, box_h * stride, box_b}, estr[4] = {1, stride, stride, 1};
+  return make_tmap<T>(m, ptr, 4, dims, box, estr, swizzle);
+}
+
+// The tensor maps one kernel's launches take, for one weight set.  An entry's key holds every device pointer and size its
+// maps encode, plus the kernel variant, so an entry is only ever reused for the buffers and shapes it was encoded for: a
+// copied Op that runs on other buffers encodes its own.  Encoding on every launch would sit on the host's launch path; a
+// handle alternates between a few (workspace, batch) pairs, and past kEntries the oldest entry is replaced.
+struct TmapCache {
+  static constexpr int kEntries = 16, kKeyWords = 14;
+  struct Entry {
+    uint64_t key[kKeyWords];
+    CUtensorMap map[3];
+  };
+  std::vector<Entry> entries;
+  size_t replaced = 0;
+
+  // *maps = the maps of `key` (device pointers and integers); on a miss encode(CUtensorMap*) makes them (nullptr on success)
+  template <typename Encode, typename... K>
+  const char* get(const CUtensorMap** maps, Encode&& encode, K... key) {
+    static_assert(sizeof...(K) <= kKeyWords, "TmapCache key too long");
+    Entry n = {};
+    int i = 0;
+    ((n.key[i++] = key_word(key)), ...);
+    for (const Entry& e : entries)
+      if (std::equal(e.key, e.key + kKeyWords, n.key)) {
+        *maps = e.map;
+        return nullptr;
+      }
+    if (const char* err = encode(n.map)) return err;
+    Entry& slot = entries.size() < kEntries ? entries.emplace_back(n) : (entries[replaced++ % kEntries] = n);
+    *maps = slot.map;
+    return nullptr;
+  }
+  template <typename X>
+  static uint64_t key_word(X x) {
+    if constexpr (std::is_pointer<X>::value) return (uint64_t)(uintptr_t)x;
+    else return (uint64_t)x;
+  }
+};
+
+// cudaMalloc, record the allocation in `allocs` (freed with the handle) and copy `bytes` from the host; nullptr on success
+inline const char* upload_dev(std::vector<void*>& allocs, void** dev, const void* host, size_t bytes) {
+  cudaError_t e = cudaMalloc(dev, bytes);
+  if (e == cudaSuccess) {
+    allocs.push_back(*dev);
+    e = cudaMemcpy(*dev, host, bytes, cudaMemcpyHostToDevice);
+  }
+  return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 
 struct TcWeights {
@@ -465,21 +512,8 @@ struct TcWeights {
   void* d_w = nullptr;           // [Cout][taps*Cin] K-major, bf16 or fp16 (the mode's storage type)
   float* d_bias = nullptr;       // [Cout]
   int Cout = 0, Cin = 0, taps = 1, S = 1;
-  // head
-  int n_real = 0;
-  mutable CUtensorMap mapA, mapB;
-  mutable const void* cached_in = nullptr;
-  mutable int cached_B = -1;
-  // conv path: tensor maps (input, weights, output) per (input, output, batch, N tile) - re-encoding them per launch would
-  // sit on the host's launch path
-  struct MapSet {
-    CUtensorMap a, b, o;
-    const void* in = nullptr;
-    const void* out = nullptr;
-    int B = -1, bn = 0;
-  };
-  mutable std::vector<MapSet> map_sets;
-  mutable size_t map_rr = 0;
+  int n_real = 0;                // head
+  mutable TmapCache maps;        // conv: (input, weights, output); head: (weights, features)
 };
 
 inline bool tc_eligible(bool is_conv, bool depthwise, bool small_io, int k, int stride, int cin, int cout) {
@@ -514,52 +548,16 @@ inline const char* tc_prepare_weights(TcWeights& w, const float* wk, const float
   std::vector<T> t((size_t)K * cout);
   for (int k = 0; k < K; ++k)
     for (int n = 0; n < cout; ++n) t[(size_t)n * K + k] = host_16b<T>(wk[(size_t)k * cout + n]);
-  if (cudaMalloc(&w.d_w, t.size() * 2) != cudaSuccess) return "cudaMalloc failed";
-  allocs.push_back(w.d_w);
-  if (cudaMemcpy(w.d_w, t.data(), t.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess) return "cudaMemcpy failed";
-  if (cudaMalloc((void**)&w.d_bias, (size_t)cout * 4) != cudaSuccess) return "cudaMalloc failed";
-  allocs.push_back(w.d_bias);
-  if (cudaMemcpy(w.d_bias, bias, (size_t)cout * 4, cudaMemcpyHostToDevice) != cudaSuccess) return "cudaMemcpy failed";
+  const char* e = upload_dev(allocs, &w.d_w, t.data(), t.size() * sizeof(T));
+  if (!e) e = upload_dev(allocs, (void**)&w.d_bias, bias, (size_t)cout * 4);
+  if (e) return e;
   w.Cout = cout; w.Cin = cin; w.taps = R * S; w.S = S;
   w.ready = true;
-  w.cached_in = nullptr;
-  w.cached_B = -1;
   return nullptr;
 }
 
 // N-tile width: the narrowest wgmma N in {32, 64, 128} that covers Cout, else 128 (Cout > 128 runs several N tiles)
 inline int tc_pick_bn(int cout) { return cout <= 32 ? 32 : cout <= 64 ? 64 : 128; }
-
-template <typename T, int ACT, int RES, int BN>
-inline const char* tc_conv_launch_k(dim3 grid, const TcWeights::MapSet& ms, const TcConvParams& q, cudaStream_t st) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    if (cudaFuncSetAttribute(tc_conv_kernel<T, ACT, RES, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcRing<BN>::smem_bytes) !=
-        cudaSuccess)
-      return "cannot raise dynamic shared memory for tc_conv_kernel";
-    attr_set = true;
-  }
-  launch_k(tc_conv_kernel<T, ACT, RES, BN>, grid, dim3(TCP_THREADS), TcRing<BN>::smem_bytes, st, ms.a, ms.b, ms.o, q);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
-}
-template <typename T, int ACT, int RES>
-inline const char* tc_conv_launch_t(int bn, dim3 grid, const TcWeights::MapSet& ms, const TcConvParams& q, cudaStream_t st) {
-  switch (bn) {
-    case 32: return tc_conv_launch_k<T, ACT, RES, 32>(grid, ms, q, st);
-    case 64: return tc_conv_launch_k<T, ACT, RES, 64>(grid, ms, q, st);
-    default: return tc_conv_launch_k<T, ACT, RES, 128>(grid, ms, q, st);
-  }
-}
-template <typename T, int ACT>
-inline const char* tc_conv_dispatch_res(int res_mode, int bn, dim3 grid, const TcWeights::MapSet& ms, const TcConvParams& q,
-                                        cudaStream_t st) {
-  switch (res_mode) {
-    case 0: return tc_conv_launch_t<T, ACT, 0>(bn, grid, ms, q, st);
-    case 1: return tc_conv_launch_t<T, ACT, 1>(bn, grid, ms, q, st);
-    default: return tc_conv_launch_t<T, ACT, 2>(bn, grid, ms, q, st);
-  }
-}
 
 // T: the storage type the weights were prepared in (tc_prepare_weights<T>)
 template <typename T>
@@ -578,39 +576,29 @@ inline const char* tc_conv_launch(const TcWeights& w, const ConvParams& p, bool 
   const int bn = tc_pick_bn(p.Cout);
   q.m_tiles = q.mode == 0 ? (q.M + TC_BM - 1) / TC_BM : p.B * q.tiles_w * q.tiles_h;
   q.n_tiles = (p.Cout + bn - 1) / bn;
-  const TcWeights::MapSet* ms = nullptr;
-  for (const TcWeights::MapSet& c : w.map_sets)
-    if (c.in == p.in && c.out == p.out && c.B == p.B && c.bn == bn) { ms = &c; break; }
-  if (!ms) {
-    TcWeights::MapSet c;
+  const CUtensorMap* m = nullptr;  // input, weights, output
+  const char* e = w.maps.get(&m, [&](CUtensorMap* c) {
+    const CUtensorMapSwizzle sw = CU_TENSOR_MAP_SWIZZLE_128B;
     const uint32_t slab = (uint32_t)std::min(bn, 64);  // output box: 64 (SWIZZLE_128B) or 32 (SWIZZLE_64B) channels
-    const char* e = q.mode == 0 ? make_tmap_2d<T>(&c.a, p.in, (uint64_t)q.M, (uint64_t)p.Cin, TC_BM)
-                                : make_tmap_nhwc<T>(&c.a, p.in, p.B, p.Hin, p.Win, p.Cin, (uint32_t)p.stride);
-    if (e) return e;
-    e = make_tmap_2d<T>(&c.b, w.d_w, (uint64_t)p.Cout, (uint64_t)w.taps * p.Cin, (uint32_t)bn);
-    if (e) return e;
-    e = q.mode == 0 ? make_tmap_2d<T>(&c.o, p.out, (uint64_t)q.M, (uint64_t)p.Cout, TC_BM, slab)
-                    : make_tmap_nhwc<T>(&c.o, p.out, p.B, p.Hout, p.Wout, p.Cout, 1, slab);
-    if (e) return e;
-    c.in = p.in; c.out = p.out; c.B = p.B; c.bn = bn;
-    if (w.map_sets.size() < 16) {
-      w.map_sets.push_back(c);
-      ms = &w.map_sets.back();
-    } else {
-      w.map_sets[w.map_rr % 16] = c;
-      ms = &w.map_sets[w.map_rr % 16];
-      ++w.map_rr;
-    }
-  }
+    const CUtensorMapSwizzle out_sw = slab == 64 ? sw : CU_TENSOR_MAP_SWIZZLE_64B;
+    const char* r = q.mode == 0 ? make_tmap_2d<T>(&c[0], p.in, q.M, p.Cin, TC_BM, TC_BK, sw)
+                                : make_tmap_nhwc<T>(&c[0], p.in, p.B, p.Hin, p.Win, p.Cin, TC_BK, TC_TILE_W, TC_TILE_H, 1, p.stride, sw);
+    if (!r) r = make_tmap_2d<T>(&c[1], w.d_w, p.Cout, (uint64_t)w.taps * p.Cin, bn, TC_BK, sw);
+    if (!r)
+      r = q.mode == 0 ? make_tmap_2d<T>(&c[2], p.out, q.M, p.Cout, TC_BM, slab, out_sw)
+                      : make_tmap_nhwc<T>(&c[2], p.out, p.B, p.Hout, p.Wout, p.Cout, slab, TC_TILE_W, TC_TILE_H, 1, 1, out_sw);
+    return r;
+  }, p.in, p.out, w.d_w, p.B, p.Hin, p.Win, p.Cin, p.Hout, p.Wout, p.Cout, w.taps, p.stride, bn);
+  if (e) return e;
   const dim3 grid(std::min(q.m_tiles * q.n_tiles, num_sms()));  // persistent: one CTA per SM
   const int res_mode = p.res ? (res_first ? 2 : 1) : 0;
-  switch (p.act) {
-    case ACT_NONE: return tc_conv_dispatch_res<T, ACT_NONE>(res_mode, bn, grid, *ms, q, st);
-    case ACT_SILU: return tc_conv_dispatch_res<T, ACT_SILU>(res_mode, bn, grid, *ms, q, st);
-    case ACT_RELU: return tc_conv_dispatch_res<T, ACT_RELU>(res_mode, bn, grid, *ms, q, st);
-    case ACT_HSWISH: return tc_conv_dispatch_res<T, ACT_HSWISH>(res_mode, bn, grid, *ms, q, st);
-    default: return "unsupported activation in the tensor-core epilogue";
-  }
+  return with_const<ACT_NONE, ACT_SILU, ACT_RELU, ACT_HSWISH>(p.act, "unsupported activation in the tensor-core epilogue", [&](auto act) {
+    return with_const<0, 1, 2>(res_mode, "unsupported residual mode", [&](auto res) {
+      return with_const<32, 64, 128>(bn, "unsupported N tile", [&](auto bn_) {
+        return launch_smem(tc_conv_kernel<T, act, res, bn_>, grid, dim3(TCP_THREADS), TcRing<bn_>::smem_bytes, st, m[0], m[1], m[2], q);
+      });
+    });
+  });
 }
 
 template <typename T>
@@ -847,20 +835,11 @@ inline const char* tc_prepare_head(TcWeights& w, const float* wt, const float* b
   if (C % 8 != 0) return nullptr;
   std::vector<T> t((size_t)n_out * C);
   for (size_t i = 0; i < t.size(); ++i) t[i] = host_16b<T>(wt[i]);
-  if (cudaMalloc(&w.d_w, t.size() * 2) != cudaSuccess) return "cudaMalloc failed";
-  allocs.push_back(w.d_w);
-  if (cudaMemcpy(w.d_w, t.data(), t.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess) return "cudaMemcpy failed";
-  if (cudaMalloc((void**)&w.d_bias, (size_t)n_out * 4) != cudaSuccess) return "cudaMalloc failed";
-  allocs.push_back(w.d_bias);
-  if (cudaMemcpy(w.d_bias, bias, (size_t)n_out * 4, cudaMemcpyHostToDevice) != cudaSuccess) return "cudaMemcpy failed";
-  if (cudaFuncSetAttribute(tc_head_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, TCH_SMEM_BYTES) != cudaSuccess)
-    return "cannot raise dynamic shared memory for tc_head_kernel";
-  const char* e = make_tmap_2d<T>(&w.mapA, w.d_w, (uint64_t)n_out, (uint64_t)C, TC_BM);
+  const char* e = upload_dev(allocs, &w.d_w, t.data(), t.size() * sizeof(T));
+  if (!e) e = upload_dev(allocs, (void**)&w.d_bias, bias, (size_t)n_out * 4);
   if (e) return e;
   w.Cout = n_out; w.Cin = C; w.n_real = n_out;
   w.ready = true;
-  w.cached_in = nullptr;
-  w.cached_B = -1;
   return nullptr;
 }
 
@@ -889,16 +868,16 @@ inline const char* tc_head_launch(const TcWeights& w, const void* features, int 
   const int n_groups = q.cpt > 0 ? (B + q.cpt - 1) / q.cpt : B;
   q.m_tiles = (q.n_out + TC_BM - 1) / TC_BM;
   q.kblocks = (q.C + TC_BK - 1) / TC_BK;
-  if (w.cached_in != features || w.cached_B != B) {
-    const char* e = make_tmap_2d<T>(&w.mapB, features, (uint64_t)B * q.P, (uint64_t)q.C, (uint32_t)q.bnp);
-    if (e) return e;
-    w.cached_in = features;
-    w.cached_B = B;
-  }
-  launch_k(tc_head_kernel<T>, dim3(n_groups * q.m_tiles), dim3(TC_THREADS), TCH_SMEM_BYTES, st, w.mapA, w.mapB, q);
+  const CUtensorMap* m = nullptr;  // weights, features
+  const char* e = w.maps.get(&m, [&](CUtensorMap* c) {
+    const char* r = make_tmap_2d<T>(&c[0], w.d_w, q.n_out, q.C, TC_BM, TC_BK, CU_TENSOR_MAP_SWIZZLE_128B);
+    return r ? r : make_tmap_2d<T>(&c[1], features, (uint64_t)B * q.P, q.C, q.bnp, TC_BK, CU_TENSOR_MAP_SWIZZLE_128B);
+  }, w.d_w, features, B, H, W, q.C, q.n_out);
+  if (!e) e = launch_smem(tc_head_kernel<T>, dim3(n_groups * q.m_tiles), dim3(TC_THREADS), TCH_SMEM_BYTES, st, m[0], m[1], q);
+  if (e) return e;
   launch_k(head_finalize_kernel, dim3(B), dim3(128), 0, st, q.states, c2d, c3d, J, D, H, W, sc);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+  const cudaError_t ce = cudaGetLastError();
+  return ce == cudaSuccess ? nullptr : cudaGetErrorString(ce);
 }
 
 }  // namespace mtb

@@ -246,46 +246,12 @@ tc32_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-// rank-2 fp32 tensor [rows][cols] (cols contiguous), box [box_rows][box_cols], swizzle = row bytes, OOB -> 0
-inline const char* make_tmap_2d_f32(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows, uint32_t box_cols) {
-  tmap_encode_fn enc = get_tmap_encode();
-  if (!enc) return "cuTensorMapEncodeTiled unavailable";
-  cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {cols * 4};
-  cuuint32_t box[2] = {box_cols, box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   box_cols == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? nullptr : "cuTensorMapEncodeTiled(2d, f32) failed";
-}
-// rank-4 fp32 NHWC tensor; box = box_c channels x (16 x 8) pixels sampled every `stride` pixels
-inline const char* make_tmap_nhwc_f32(CUtensorMap* m, const void* ptr, uint64_t B, uint64_t H, uint64_t W, uint64_t C, uint32_t stride,
-                                      uint32_t box_c) {
-  tmap_encode_fn enc = get_tmap_encode();
-  if (!enc) return "cuTensorMapEncodeTiled unavailable";
-  cuuint64_t dims[4] = {C, W, H, B};
-  cuuint64_t strides[3] = {C * 4, W * C * 4, H * W * C * 4};
-  cuuint32_t box[4] = {box_c, TC_TILE_W * stride, TC_TILE_H * stride, 1};
-  cuuint32_t estr[4] = {1, stride, stride, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   box_c == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? nullptr : "cuTensorMapEncodeTiled(4d, f32) failed";
-}
-
 struct Tc32Weights {
   bool ready = false;
   float* d_w = nullptr;     // fp32 [2][Cout][taps*Cin] K-major (BN folded): hi plane, lo plane
   float* d_bias = nullptr;  // [Cout]
   int Cout = 0, Cin = 0, taps = 1, S = 1;
-  struct MapSet {
-    CUtensorMap a, b;
-    const void* in = nullptr;
-    int B = -1, bn = 0, rb = 0;
-  };
-  mutable std::vector<MapSet> map_sets;
-  mutable size_t map_rr = 0;
+  mutable TmapCache maps;   // (input, weights)
 };
 
 // wk: fp32 [K = taps*Cin][Cout] (BN folded) -> two K-major planes [2][Cout][K]: hi = tf32(w) (round to nearest, as
@@ -304,15 +270,11 @@ inline const char* tc32_prepare_weights(Tc32Weights& w, const float* wk, const f
       t[(size_t)n * K + k] = hi;
       t[(size_t)cout * K + (size_t)n * K + k] = x - hi;
     }
-  if (cudaMalloc((void**)&w.d_w, t.size() * 4) != cudaSuccess) return "cudaMalloc failed";
-  allocs.push_back(w.d_w);
-  if (cudaMemcpy(w.d_w, t.data(), t.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess) return "cudaMemcpy failed";
-  if (cudaMalloc((void**)&w.d_bias, (size_t)cout * 4) != cudaSuccess) return "cudaMalloc failed";
-  allocs.push_back(w.d_bias);
-  if (cudaMemcpy(w.d_bias, bias, (size_t)cout * 4, cudaMemcpyHostToDevice) != cudaSuccess) return "cudaMemcpy failed";
+  const char* e = upload_dev(allocs, (void**)&w.d_w, t.data(), t.size() * 4);
+  if (!e) e = upload_dev(allocs, (void**)&w.d_bias, bias, (size_t)cout * 4);
+  if (e) return e;
   w.Cout = cout; w.Cin = cin; w.taps = R * S; w.S = S;
   w.ready = true;
-  w.map_sets.clear();
   return nullptr;
 }
 
@@ -321,36 +283,6 @@ inline bool tc32_eligible(bool is_conv, bool depthwise, bool small_io, int k, in
   if (!is_conv || depthwise || small_io) return false;
   if (cin % 4 != 0 || cout % 4 != 0) return false;
   return (stride == 1 || stride == 2) && (k == 1 || k == 3);
-}
-
-template <int ACT, int RES, int BN>
-inline const char* tc32_launch_k(dim3 grid, const CUtensorMap& a, const CUtensorMap& b, const Tc32Params& q, cudaStream_t st) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    if (cudaFuncSetAttribute(tc32_conv_kernel<ACT, RES, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, T32Ring<BN>::smem_bytes) !=
-        cudaSuccess)
-      return "cannot raise dynamic shared memory for tc32_conv_kernel";
-    attr_set = true;
-  }
-  launch_k(tc32_conv_kernel<ACT, RES, BN>, grid, dim3(TC_THREADS), T32Ring<BN>::smem_bytes, st, a, b, q);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
-}
-template <int ACT>
-inline const char* tc32_dispatch_res(int res_mode, int bn, dim3 grid, const CUtensorMap& a, const CUtensorMap& b, const Tc32Params& q,
-                                     cudaStream_t st) {
-  if (bn == 32) {
-    switch (res_mode) {
-      case 0: return tc32_launch_k<ACT, 0, 32>(grid, a, b, q, st);
-      case 1: return tc32_launch_k<ACT, 1, 32>(grid, a, b, q, st);
-      default: return tc32_launch_k<ACT, 2, 32>(grid, a, b, q, st);
-    }
-  }
-  switch (res_mode) {
-    case 0: return tc32_launch_k<ACT, 0, 64>(grid, a, b, q, st);
-    case 1: return tc32_launch_k<ACT, 1, 64>(grid, a, b, q, st);
-    default: return tc32_launch_k<ACT, 2, 64>(grid, a, b, q, st);
-  }
 }
 
 inline const char* tc32_conv_launch(const Tc32Weights& w, const ConvParams& p, bool res_first, cudaStream_t st) {
@@ -370,35 +302,23 @@ inline const char* tc32_conv_launch(const Tc32Weights& w, const ConvParams& p, b
   q.kchunks = (p.Cin + T32_BK - 1) / T32_BK;
   const int m_tiles = q.mode == 0 ? (q.M + TC_BM - 1) / TC_BM : p.B * q.tiles_w * q.tiles_h;
   const int bn = p.Cout <= 32 ? 32 : 64;
-  const Tc32Weights::MapSet* ms = nullptr;
-  for (const Tc32Weights::MapSet& c : w.map_sets)
-    if (c.in == p.in && c.B == p.B && c.bn == bn) { ms = &c; break; }
-  if (!ms) {
-    Tc32Weights::MapSet c;
-    const char* e = q.mode == 0 ? make_tmap_2d_f32(&c.a, p.in, (uint64_t)q.M, (uint64_t)p.Cin, TC_BM, (uint32_t)T32_BK)
-                                : make_tmap_nhwc_f32(&c.a, p.in, p.B, p.Hin, p.Win, p.Cin, (uint32_t)p.stride, (uint32_t)T32_BK);
-    if (e) return e;
-    e = make_tmap_2d_f32(&c.b, w.d_w, (uint64_t)2 * p.Cout, (uint64_t)w.taps * p.Cin, (uint32_t)bn, (uint32_t)T32_BK);
-    if (e) return e;
-    c.in = p.in; c.B = p.B; c.bn = bn;
-    if (w.map_sets.size() < 16) {
-      w.map_sets.push_back(c);
-      ms = &w.map_sets.back();
-    } else {
-      w.map_sets[w.map_rr % 16] = c;
-      ms = &w.map_sets[w.map_rr % 16];
-      ++w.map_rr;
-    }
-  }
+  const CUtensorMap* m = nullptr;  // input, weights
+  const char* e = w.maps.get(&m, [&](CUtensorMap* c) {
+    const CUtensorMapSwizzle sw = CU_TENSOR_MAP_SWIZZLE_128B;  // T32_BK fp32 = 128-byte rows
+    const char* r = q.mode == 0 ? make_tmap_2d<float>(&c[0], p.in, q.M, p.Cin, TC_BM, T32_BK, sw)
+                                : make_tmap_nhwc<float>(&c[0], p.in, p.B, p.Hin, p.Win, p.Cin, T32_BK, TC_TILE_W, TC_TILE_H, 1, p.stride, sw);
+    return r ? r : make_tmap_2d<float>(&c[1], w.d_w, (uint64_t)2 * p.Cout, (uint64_t)w.taps * p.Cin, bn, T32_BK, sw);
+  }, p.in, w.d_w, p.B, p.Hin, p.Win, p.Cin, p.Hout, p.Wout, p.Cout, w.taps, p.stride, bn);
+  if (e) return e;
   const dim3 grid(m_tiles, (p.Cout + bn - 1) / bn);
   const int res_mode = p.res ? (res_first ? 2 : 1) : 0;
-  switch (p.act) {
-    case ACT_NONE: return tc32_dispatch_res<ACT_NONE>(res_mode, bn, grid, ms->a, ms->b, q, st);
-    case ACT_SILU: return tc32_dispatch_res<ACT_SILU>(res_mode, bn, grid, ms->a, ms->b, q, st);
-    case ACT_RELU: return tc32_dispatch_res<ACT_RELU>(res_mode, bn, grid, ms->a, ms->b, q, st);
-    case ACT_HSWISH: return tc32_dispatch_res<ACT_HSWISH>(res_mode, bn, grid, ms->a, ms->b, q, st);
-    default: return "unsupported activation in the 3xTF32 epilogue";
-  }
+  return with_const<ACT_NONE, ACT_SILU, ACT_RELU, ACT_HSWISH>(p.act, "unsupported activation in the 3xTF32 epilogue", [&](auto act) {
+    return with_const<0, 1, 2>(res_mode, "unsupported residual mode", [&](auto res) {
+      return with_const<32, 64>(bn, "unsupported N tile", [&](auto bn_) {
+        return launch_smem(tc32_conv_kernel<act, res, bn_>, grid, dim3(TC_THREADS), T32Ring<bn_>::smem_bytes, st, m[0], m[1], q);
+      });
+    });
+  });
 }
 
 }  // namespace mtb
