@@ -41,14 +41,16 @@ typedef enum {
 
 typedef enum { MTB_DTYPE_F32 = 0, MTB_DTYPE_BF16 = 1, MTB_DTYPE_F16 = 2, MTB_DTYPE_I64 = 3 } mtb_dtype;
 
-/* Backbone families.  EFFNET covers EfficientNetV2-S/M/L and any table in the same block grammar
- * (backbones/efficientnet.py:379-433); the RESNET* values (V1, metrabs_tf/backbones/resnet.py: ResNet-18/34 with the
+/* Backbone families.  EFFNET covers EfficientNetV2-S/M/L, EfficientNet-B5/B6/B7 and any table in the same block grammar
+ * (backbones/efficientnet.py:379-433) with BatchNorm epsilon 1e-3; EFFNET_EPS1E5 is the same grammar with torchvision's
+ * default epsilon 1e-5, for EfficientNet-B0..B4 (:753-960), and takes MBConv rows only (kernel 3 or 5, stride 1 or 2;
+ * anything else fails with MTB_ERR_UNSUPPORTED); the RESNET* values (V1, metrabs_tf/backbones/resnet.py: ResNet-18/34 with the
  * basic block :322-388, ResNet-50/101/152 with the bottleneck :239-319) and MOBILENETV3_SMALL / _LARGE
  * (metrabs_tf/backbones/mobilenet_v3.py:348-384 / :387-428, alpha 1, not minimalistic) follow the TF-only
  * metrabs_tf/backbones/{resnet,mobilenet_v3}.py. */
 typedef enum { MTB_ARCH_EFFNET = 0, MTB_ARCH_RESNET50 = 1, MTB_ARCH_MOBILENETV3_SMALL = 2,
                MTB_ARCH_HEAD_ONLY = 3, MTB_ARCH_RESNET18 = 4, MTB_ARCH_RESNET34 = 5, MTB_ARCH_RESNET101 = 6,
-               MTB_ARCH_RESNET152 = 7, MTB_ARCH_MOBILENETV3_LARGE = 8 } mtb_arch;
+               MTB_ARCH_RESNET152 = 7, MTB_ARCH_MOBILENETV3_LARGE = 8, MTB_ARCH_EFFNET_EPS1E5 = 9 } mtb_arch;
 
 /* Arithmetic of the conv/GEMM kernels.  FP32: CUDA-core fp32 FMA everywhere (the 1e-3 parity mode).
  * BF16_TC: bf16 operands on wgmma tensor cores with fp32 accumulation in registers, bf16 activations in HBM
@@ -81,7 +83,7 @@ typedef enum {
 typedef struct {
   int32_t block;       /* 0 = FusedMBConv (:176-234), 1 = MBConv (:110-173) */
   int32_t expand;      /* expand_ratio */
-  int32_t kernel;      /* 3 */
+  int32_t kernel;      /* 3 or 5 */
   int32_t stride;      /* stride of the first block of the stage */
   int32_t cin, cout;
   int32_t layers;
@@ -104,8 +106,8 @@ typedef struct {
   float box_size_mm;
   float mix_3d_inside_fov;            /* < 0 means None (ptu3d.py:28) */
   int32_t weak_perspective;           /* must be 0: the reference's weak-perspective solve crashes (ptu.py:30) */
-  int32_t n_stages;                   /* EFFNET only */
-  int32_t last_channel;               /* EFFNET only: 1280 */
+  int32_t n_stages;                   /* EFFNET / EFFNET_EPS1E5 only */
+  int32_t last_channel;               /* EFFNET / EFFNET_EPS1E5 only: 1280 (V2), 4 * last cout (B0-B7) */
   mtb_stage stages[MTB_MAX_STAGES];
 } mtb_config;
 
@@ -343,9 +345,11 @@ int mtb_debug_dw_plan(int height, int width, int* crops_per_item, int* rows_per_
 /* The kernel mtb_finalize_weights chose for depthwise backbone op `op`: GENERIC is dwconv_kernel (one thread per pixel and
  * 4 channels; every fp32 / 3xTF32 / _SIMT mode op that no other kernel covers), TMA the TMA-staged 3x3 stride-1 kernel and
  * STRIP_16B / STRIP_F32 the 3x3 strip kernels (these three also write the SE pooling slices), 5X5_16B the 16-bit 5x5 kernel
- * of the BF16_TC / F16_TC modes (bit-identical to dwconv_kernel, no pooling).  MTB_ERR_INVALID_ARG for an index out of
- * range or an op that is not depthwise. */
-typedef enum { MTB_DW_GENERIC = 0, MTB_DW_TMA = 1, MTB_DW_STRIP_16B = 2, MTB_DW_STRIP_F32 = 3, MTB_DW_5X5_16B = 4 } mtb_dw_kernel;
+ * of the BF16_TC / F16_TC modes for ReLU / hard-swish (bit-identical to dwconv_kernel, no pooling), 5X5_POOL_16B the same
+ * kernel for SiLU (bit-identical outputs, and it also writes the SE pooling slices of the stored outputs).
+ * MTB_ERR_INVALID_ARG for an index out of range or an op that is not depthwise. */
+typedef enum { MTB_DW_GENERIC = 0, MTB_DW_TMA = 1, MTB_DW_STRIP_16B = 2, MTB_DW_STRIP_F32 = 3, MTB_DW_5X5_16B = 4,
+               MTB_DW_5X5_POOL_16B = MTB_DW_5X5_16B + 1 /* 5 */ } mtb_dw_kernel;
 int mtb_op_dw_kernel(const mtb_handle* h, int op);
 
 #ifdef __cplusplus

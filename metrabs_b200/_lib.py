@@ -9,7 +9,8 @@ MTB_MAX_STAGES = 16
 ARCH_EFFNET, ARCH_RESNET50, ARCH_MOBILENETV3_SMALL, ARCH_HEAD_ONLY = 0, 1, 2, 3
 ARCH_RESNET18, ARCH_RESNET34, ARCH_RESNET101, ARCH_RESNET152 = 4, 5, 6, 7
 ARCH_MOBILENETV3_LARGE = 8
-DW_GENERIC, DW_TMA, DW_STRIP_16B, DW_STRIP_F32, DW_5X5_16B = 0, 1, 2, 3, 4  # mtb_op_dw_kernel
+ARCH_EFFNET_EPS1E5 = 9  # the EFFNET grammar with BatchNorm eps 1e-5 (EfficientNet-B0..B4)
+DW_GENERIC, DW_TMA, DW_STRIP_16B, DW_STRIP_F32, DW_5X5_16B, DW_5X5_POOL_16B = 0, 1, 2, 3, 4, 5  # mtb_op_dw_kernel
 PRECISION_FP32, PRECISION_BF16_TC, PRECISION_BF16_SIMT, PRECISION_TF32X3, PRECISION_F16_TC, PRECISION_F16_SIMT = 0, 1, 2, 3, 4, 5
 DTYPE_F32, DTYPE_BF16, DTYPE_F16, DTYPE_I64 = 0, 1, 2, 3
 LAYOUT_BDJHW, LAYOUT_BHWN = 0, 1

@@ -1,12 +1,15 @@
-"""EfficientNetV2 backbones for the H100 engine.
+"""EfficientNetV2 and EfficientNet-B0..B7 backbones for the H100 engine.
 
 Mirrors the constructor surface of /root/reference/metrabs_pytorch/backbones/efficientnet.py
-(``efficientnet_v2_{s,m,l}()`` returning an object whose ``.features`` is used, and ``PreprocLayer``; model
+(``efficientnet_v2_{s,m,l}()`` and ``efficientnet_b0()`` .. ``efficientnet_b7()`` returning an object whose ``.features``
+is used, and ``PreprocLayer``; model
 assembly recipe scripts/demo_image.py:59-74).  The modules built here only HOLD parameters under the reference's
 ``state_dict`` key schema (``<stage>.<block>.block.<i>.{0.weight,1.weight,1.bias,1.running_mean,...}``); the
 arithmetic runs in libmetrabs_b200.so (stem / FusedMBConv / MBConv / SE kernels), which receives the block table
 (efficientnet.py:379-433) through ``mtb_config.stages``.
 """
+import math
+
 import torch
 from torch import nn
 
@@ -28,6 +31,35 @@ _TABLES = {
 }
 
 
+# EfficientNet-B base table (efficientnet.py:388-396): (expand, kernel, stride, cin, cout, layers, bottomright on the last
+# strided stage under centered_stride), scaled per variant by (width, depth) and built with BatchNorm eps (:753-1013;
+# B0-B4 keep torchvision's default 1e-5, B5-B7 pass 1e-3)
+_B_BASE = [(1, 3, 1, 32, 16, 1), (6, 3, 2, 16, 24, 2), (6, 5, 2, 24, 40, 2), (6, 3, 2, 40, 80, 3), (6, 5, 1, 80, 112, 3),
+           (6, 5, 2, 112, 192, 4, True), (6, 3, 1, 192, 320, 1)]
+_B_VARIANTS = {'b0': (1.0, 1.0, 1e-5), 'b1': (1.0, 1.1, 1e-5), 'b2': (1.1, 1.2, 1e-5), 'b3': (1.2, 1.4, 1e-5),
+               'b4': (1.4, 1.8, 1e-5), 'b5': (1.6, 2.2, 1e-3), 'b6': (1.8, 2.6, 1e-3), 'b7': (2.0, 3.1, 1e-3)}
+# BatchNorm eps -> mtb_arch of the block grammar
+_ARCH_BY_EPS = {1e-3: _lib.ARCH_EFFNET, 1e-5: _lib.ARCH_EFFNET_EPS1E5}
+
+
+def _make_divisible(v, divisor=8):
+    """torchvision.models._utils._make_divisible with min_value = divisor (MBConvConfig.adjust_channels)."""
+    new_v = max(divisor, int(v + divisor / 2) // divisor * divisor)
+    return new_v + divisor if new_v < 0.9 * v else new_v
+
+
+def b_stage_table(variant, centered_stride=None):
+    """-> (stages, last_channel, bn_eps) of EfficientNet-``variant`` ('b0'..'b7'): channels _make_divisible(c * width, 8),
+    layers ceil(layers * depth) (MBConvConfig :62-93), last conv 4 * the last stage's cout (:320)."""
+    if centered_stride is None:
+        centered_stride = get_config().centered_stride
+    width, depth, eps = _B_VARIANTS[variant]
+    stages = [dict(block='mb', expand=r[0], kernel=r[1], stride=r[2], cin=_make_divisible(r[3] * width),
+                   cout=_make_divisible(r[4] * width), layers=int(math.ceil(r[5] * depth)),
+                   bottomright=bool(len(r) > 6 and r[6] and centered_stride)) for r in _B_BASE]
+    return stages, 4 * stages[-1]['cout'], eps
+
+
 def stage_table(size, centered_stride=None):
     if centered_stride is None:
         centered_stride = get_config().centered_stride
@@ -37,9 +69,9 @@ def stage_table(size, centered_stride=None):
     return stages, last
 
 
-def _conv_bn(cin, cout, k, groups=1):
+def _conv_bn(cin, cout, k, groups=1, eps=1e-3):
     """Parameter holder with the key layout of torchvision's Conv2dNormActivation: '0' conv (no bias), '1' BN."""
-    return nn.Sequential(nn.Conv2d(cin, cout, k, groups=groups, bias=False), nn.BatchNorm2d(cout, eps=1e-3))
+    return nn.Sequential(nn.Conv2d(cin, cout, k, groups=groups, bias=False), nn.BatchNorm2d(cout, eps=eps))
 
 
 class _SE(nn.Module):
@@ -58,14 +90,19 @@ class _Block(nn.Module):
 
 
 class Features(nn.Module):
-    """Parameter tree of ``EfficientNet.features`` (children '0' stem, '1'..'n' stages, 'n+1' last conv)."""
-    arch = _lib.ARCH_EFFNET
+    """Parameter tree of ``EfficientNet.features`` (children '0' stem, '1'..'n' stages, 'n+1' last conv), every BatchNorm
+    with epsilon ``bn_eps``: 1e-3 (EfficientNetV2, B5-B7) runs as ``ARCH_EFFNET``, 1e-5 (B0-B4) as ``ARCH_EFFNET_EPS1E5``."""
 
-    def __init__(self, stages, last_channel):
+    def __init__(self, stages, last_channel, bn_eps=1e-3):
         super().__init__()
+        if bn_eps not in _ARCH_BY_EPS:
+            raise ValueError(f'BatchNorm eps {bn_eps} is not built: 1e-3 or 1e-5')
         self.stages = stages
         self.last_channel = last_channel
-        self.add_module('0', _conv_bn(3, stages[0]['cin'], 3))
+        self.bn_eps = bn_eps
+        self.arch = _ARCH_BY_EPS[bn_eps]
+        bn = lambda cin, cout, k, groups=1: _conv_bn(cin, cout, k, groups, bn_eps)  # noqa: E731
+        self.add_module('0', bn(3, stages[0]['cin'], 3))
         for si, st in enumerate(stages):
             blocks = []
             for bi in range(st['layers']):
@@ -73,16 +110,16 @@ class Features(nn.Module):
                 cexp = cin * st['expand']
                 if st['block'] == 'fused':
                     if st['expand'] != 1:
-                        layers = [_conv_bn(cin, cexp, st['kernel']), _conv_bn(cexp, st['cout'], 1)]
+                        layers = [bn(cin, cexp, st['kernel']), bn(cexp, st['cout'], 1)]
                     else:
-                        layers = [_conv_bn(cin, st['cout'], st['kernel'])]
+                        layers = [bn(cin, st['cout'], st['kernel'])]
                 else:
-                    layers = [_conv_bn(cin, cexp, 1)] if st['expand'] != 1 else []
-                    layers += [_conv_bn(cexp, cexp, st['kernel'], groups=cexp), _SE(cexp, max(1, cin // 4)),
-                               _conv_bn(cexp, st['cout'], 1)]
+                    layers = [bn(cin, cexp, 1)] if st['expand'] != 1 else []
+                    layers += [bn(cexp, cexp, st['kernel'], groups=cexp), _SE(cexp, max(1, cin // 4)),
+                               bn(cexp, st['cout'], 1)]
                 blocks.append(_Block(layers))
             self.add_module(str(si + 1), nn.Sequential(*blocks))
-        self.add_module(str(len(stages) + 1), _conv_bn(stages[-1]['cout'], last_channel, 1))
+        self.add_module(str(len(stages) + 1), bn(stages[-1]['cout'], last_channel, 1))
 
     def forward(self, x):
         raise RuntimeError('metrabs_b200 backbones run inside Metrabs.forward (libmetrabs_b200.so); wrap this in '
@@ -90,11 +127,16 @@ class Features(nn.Module):
 
 
 class EfficientNet(nn.Module):
+    """``size``: a V2 table ('s', 'm', 'l', 'tiny') or a B variant ('b0'..'b7')."""
+
     def __init__(self, size):
         super().__init__()
-        stages, last = stage_table(size)
+        if size in _B_VARIANTS:
+            stages, last, eps = b_stage_table(size)
+        else:
+            (stages, last), eps = stage_table(size), 1e-3
         self.size = size
-        self.features = Features(stages, last)
+        self.features = Features(stages, last, eps)
 
 
 class PreprocLayer(nn.Module):
@@ -118,3 +160,35 @@ def efficientnet_v2_l(**kwargs):
 
 def efficientnet_v2_tiny(**kwargs):
     return EfficientNet('tiny')
+
+
+def efficientnet_b0(**kwargs):
+    return EfficientNet('b0')
+
+
+def efficientnet_b1(**kwargs):
+    return EfficientNet('b1')
+
+
+def efficientnet_b2(**kwargs):
+    return EfficientNet('b2')
+
+
+def efficientnet_b3(**kwargs):
+    return EfficientNet('b3')
+
+
+def efficientnet_b4(**kwargs):
+    return EfficientNet('b4')
+
+
+def efficientnet_b5(**kwargs):
+    return EfficientNet('b5')
+
+
+def efficientnet_b6(**kwargs):
+    return EfficientNet('b6')
+
+
+def efficientnet_b7(**kwargs):
+    return EfficientNet('b7')

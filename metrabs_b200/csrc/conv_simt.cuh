@@ -488,26 +488,63 @@ __global__ void __launch_bounds__(256, 3) dwconv3x3_pool_f32_kernel(ConvParams p
 // row is loaded once and feeds every output that uses it (40 / 55 loads per 4 outputs instead of 100).  The arithmetic is
 // dwconv_kernel's, operation for operation: each accumulator starts at the bias, the taps are added with fmaf in row-major
 // order (r outer, s inner), taps outside the map are skipped, the activation is the exact act_t and the result is rounded
-// to nearest even; the outputs are bit-identical to dwconv_kernel's on the same inputs.  It does not pool (the SE squeeze
-// stays a separate pool_mean_kernel pass).  One grid-stride loop over (crop, output row, strip, channel vector), channel
-// vectors fastest: narrow layers (72, 96, 120 channels) fill whole warps.  grid grid_for(items, 256), block 256.
+// to nearest even; the outputs are bit-identical to dwconv_kernel's on the same inputs.
+// POOL = false: no pooling (the SE squeeze stays a separate pool_mean_kernel pass).  One grid-stride loop over (crop, output
+// row, strip, channel vector), channel vectors fastest: narrow layers (72, 96, 120 channels) fill whole warps.
+// grid grid_for(items, 256), block 256; `pooled` is unused.
+// POOL = true: also the SE squeeze of the outputs AS STORED (rounded to T), as the partial slices pooled[blockIdx.y][b][c]
+// already divided by Hout*Wout, like dwconv3x3_pool_16b_kernel; fc1 sums the slices in a fixed order (deterministic, no
+// atomics).  grid (channel chunks, slices, B); a block is blockDim.x / cb groups of cb = ceil(C/8 / gridDim.x) channel
+// vectors, group g of slice y walks the strips y*groups + g, += gridDim.y*groups of crop blockIdx.z.  `pooled` may be null.
 // ----------------------------------------------------------------------------------------------------------
-template <typename T, int STRIDE, int ACT, int OW = 4>
-__global__ void __launch_bounds__(256) dwconv5x5_16b_kernel(ConvParams p) {
+template <typename T, int STRIDE, int ACT, int OW = 4, bool POOL = false>
+__global__ void __launch_bounds__(256) dwconv5x5_16b_kernel(ConvParams p, float* __restrict__ pooled) {
   constexpr int NCOL = (OW - 1) * STRIDE + 5;  // input columns feeding OW outputs
   const T* __restrict__ in = reinterpret_cast<const T*>(p.in);
   T* __restrict__ out = reinterpret_cast<T*>(p.out);
   const int C = p.Cout;
   const int cstride = C >> 3;  // uint4 per pixel
   const int strips_w = (p.Wout + OW - 1) / OW;
-  const size_t total = (size_t)p.B * p.Hout * strips_w * cstride;
-  for (size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
-    const int c = (int)(idx % cstride) * 8;
-    size_t t = idx / cstride;
-    const int ow0 = (int)(t % strips_w) * OW;
-    t /= strips_w;
-    const int oh = (int)(t % p.Hout);
-    const int b = (int)(t / p.Hout);
+  // POOL: thread (g, cv) of the block is channel vector cv of group g, and its loop index is a strip (oh * strips_w + ow0 / OW)
+  // of crop blockIdx.z.  The if-constexpr forms below leave the POOL = false kernel exactly as it was before pooling existed.
+  struct PoolThread { int cb, groups, g, cv; float psum[8]; };
+  struct NoPool {};
+  std::conditional_t<POOL, PoolThread, NoPool> pt;
+  if constexpr (POOL) {
+    pt.cb = (cstride + gridDim.x - 1) / gridDim.x;
+    pt.groups = blockDim.x / pt.cb;
+    pt.g = threadIdx.x / pt.cb;
+    pt.cv = blockIdx.x * pt.cb + threadIdx.x % pt.cb;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) pt.psum[k] = 0.f;
+  }
+  const size_t total = [&] {
+    if constexpr (POOL) return pt.g < pt.groups && pt.cv < cstride ? (size_t)strips_w * p.Hout : (size_t)0;
+    else return (size_t)p.B * p.Hout * strips_w * cstride;
+  }();
+  const size_t first = [&] {
+    if constexpr (POOL) return (size_t)blockIdx.y * pt.groups + pt.g;
+    else return (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  }();
+  const size_t step = [&] {
+    if constexpr (POOL) return (size_t)gridDim.y * pt.groups;
+    else return (size_t)gridDim.x * blockDim.x;
+  }();
+  for (size_t idx = first; idx < total; idx += step) {
+    int c, ow0, oh, b;
+    if constexpr (POOL) {
+      c = pt.cv * 8;
+      oh = (int)(idx / strips_w);
+      ow0 = (int)(idx - (size_t)oh * strips_w) * OW;
+      b = blockIdx.z;
+    } else {
+      c = (int)(idx % cstride) * 8;
+      size_t t = idx / cstride;
+      ow0 = (int)(t % strips_w) * OW;
+      t /= strips_w;
+      oh = (int)(t % p.Hout);
+      b = (int)(t / p.Hout);
+    }
     const int iw0 = ow0 * STRIDE - p.pad_l;
     unsigned colmask = 0;
 #pragma unroll
@@ -565,6 +602,37 @@ __global__ void __launch_bounds__(256) dwconv5x5_16b_kernel(ConvParams p) {
 #pragma unroll
       for (int k = 0; k < 4; ++k) o2[k] = Pair16<T>::pack(act_t<ACT>(acc[i][2 * k]), act_t<ACT>(acc[i][2 * k + 1]));
       *reinterpret_cast<uint4*>(orow + (size_t)i * C) = ov;
+      if constexpr (POOL) {  // the values as stored
+        const unsigned wd[4] = {ov.x, ov.y, ov.z, ov.w};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          float v0, v1;
+          f2_unpack(unpack2_16b<T>(wd[k]), v0, v1);
+          pt.psum[2 * k] += v0;
+          pt.psum[2 * k + 1] += v1;
+        }
+      }
+    }
+  }
+  if constexpr (POOL) {
+    if (pooled) {
+      __shared__ float red[256][9];
+#pragma unroll
+      for (int k = 0; k < 8; ++k) red[threadIdx.x][k] = pt.psum[k];
+      __syncthreads();
+      if (pt.g == 0 && pt.cv < cstride) {
+        const float inv = 1.0f / (float)(p.Hout * p.Wout);
+        float t[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+          t[k] = 0.f;
+          for (int y = 0; y < pt.groups; ++y) t[k] += red[y * pt.cb + threadIdx.x][k];
+          t[k] *= inv;
+        }
+        float* dst = pooled + ((size_t)blockIdx.y * gridDim.z + blockIdx.z) * C + pt.cv * 8;
+        *reinterpret_cast<float4*>(dst) = make_float4(t[0], t[1], t[2], t[3]);
+        *reinterpret_cast<float4*>(dst + 4) = make_float4(t[4], t[5], t[6], t[7]);
+      }
     }
   }
 }

@@ -32,10 +32,12 @@ std::string g_error;
 
 enum OpType { OP_STEM = 0, OP_CONV = 1, OP_DW = 2, OP_POOL = 3, OP_MAXPOOL = 4 };
 // depthwise kernels: TMA-staged (dw_tma.cuh), 16-bit (bf16 / fp16) or fp32 strip (SE pooling fused), generic (dwconv_kernel),
-// 16-bit 5x5 (dwconv5x5_16b_kernel: dwconv_kernel's arithmetic with column reuse, no pooling); values of mtb_dw_kernel
-enum DwKernel { DW_GENERIC = 0, DW_TMA = 1, DW_STRIP_16B = 2, DW_STRIP_F32 = 3, DW_5X5_16B = 4 };
+// 16-bit 5x5 (dwconv5x5_16b_kernel: dwconv_kernel's arithmetic with column reuse; without pooling for ReLU / hard-swish,
+// with SE pooling for SiLU); values of mtb_dw_kernel
+enum DwKernel { DW_GENERIC = 0, DW_TMA = 1, DW_STRIP_16B = 2, DW_STRIP_F32 = 3, DW_5X5_16B = 4, DW_5X5_POOL_16B = 5 };
 static_assert((int)DW_GENERIC == (int)MTB_DW_GENERIC && (int)DW_TMA == (int)MTB_DW_TMA && (int)DW_STRIP_16B == (int)MTB_DW_STRIP_16B &&
-              (int)DW_STRIP_F32 == (int)MTB_DW_STRIP_F32 && (int)DW_5X5_16B == (int)MTB_DW_5X5_16B, "DwKernel must match mtb_dw_kernel");
+              (int)DW_STRIP_F32 == (int)MTB_DW_STRIP_F32 && (int)DW_5X5_16B == (int)MTB_DW_5X5_16B &&
+              (int)DW_5X5_POOL_16B == (int)MTB_DW_5X5_POOL_16B, "DwKernel must match mtb_dw_kernel");
 // kernel classes for the CUDA-event profiler (mtb_profile_begin / mtb_profile_end)
 enum KClass { KC_STEM = 0, KC_IGEMM_SIMT = 1, KC_DWCONV = 2, KC_POOL = 3, KC_SE_FC = 4, KC_TC_GEMM = 5, KC_FMB = 6,
               KC_HEAD_FUSED = 7, KC_HEAD_CONV_SIMT = 8, KC_SOFTARGMAX = 9, KC_RECON = 10, KC_OTHER = 11, KC_SE_SCALE = 12, KC_TC32 = 13,
@@ -70,7 +72,7 @@ struct Op {
   bool fused_pool = false;  // this depthwise op also produces the SE pooled means (next op is skipped)
   DwKernel dw_kernel = DW_GENERIC;  // depthwise: the kernel that runs it (set by mtb_finalize_weights)
   DwTmaPlan dw_plan;                // DW_TMA: its tiling plan
-  int pool_slices = 1;              // DW_TMA / DW_STRIP_*: partial pooling slices it leaves (= its gridDim.y / dw_plan.n_rb)
+  int pool_slices = 1;              // DW_TMA / DW_STRIP_* / DW_5X5_POOL_16B: partial pooling slices it leaves (= its gridDim.y / dw_plan.n_rb)
   bool res_first = false;  // residual added BEFORE the activation (ResNet); EfficientNet adds it after
   int pool_src = -1;       // fc1: index of the OP_POOL op that produces its input (fused pooling leaves partial slices)
   int ksplit = 1;          // split-K (squeeze-excitation fc1): raw sums, bias/act deferred to the consumer
@@ -292,8 +294,9 @@ struct Planner {
   }
 };
 
-void plan_effnet(mtb_handle* h) {
-  // EfficientNet.features (backbones/efficientnet.py:286-324) with PreprocLayer (:1181-1186) folded in the stem
+// EfficientNet.features (backbones/efficientnet.py:286-324) with PreprocLayer (:1181-1186) folded in the stem, every BatchNorm
+// with epsilon `bn_eps`: 1e-3 for EfficientNetV2 (:1051) and B5-B7 (:973, :1011), torchvision's default 1e-5 for B0-B4
+void plan_effnet(mtb_handle* h, float bn_eps) {
   const mtb_config& c = h->cfg;
   Planner P{h, c.proc_side, c.proc_side, 3};
   const std::string pre = "backbone.1";
@@ -371,6 +374,7 @@ void plan_effnet(mtb_handle* h) {
     snprintf(key, sizeof(key), "%s.%d", pre.c_str(), c.n_stages + 1);
     P.conv(key, c.last_channel, 1, 1, 0, 0, ACT_SILU, P.cur, BUF_FEATURES);  // :319-324
   }
+  for (Op& op : h->ops) op.bn_eps = bn_eps;
   h->feat_side = P.H;
   h->feat_c = P.C;
   h->big_elems_per_crop = P.max_elems;
@@ -618,7 +622,8 @@ int plan(mtb_handle* h) {
     int rc = plan_resnet(h, resnet->counts, resnet->basic);
     if (rc) return rc;
   } else switch (c.arch) {
-    case MTB_ARCH_EFFNET: plan_effnet(h); break;
+    case MTB_ARCH_EFFNET: plan_effnet(h, 1e-3f); break;
+    case MTB_ARCH_EFFNET_EPS1E5: plan_effnet(h, 1e-5f); break;
     case MTB_ARCH_MOBILENETV3_SMALL: { int rc = plan_mobilenetv3(h, kMobileNetV3Small, (int)std::size(kMobileNetV3Small), 1024); if (rc) return rc; break; }
     case MTB_ARCH_MOBILENETV3_LARGE: { int rc = plan_mobilenetv3(h, kMobileNetV3Large, (int)std::size(kMobileNetV3Large), 1280); if (rc) return rc; break; }
     case MTB_ARCH_HEAD_ONLY:
@@ -802,14 +807,26 @@ bool dw_strip_eligible(const Op& op) {
 // shapes covered by dwconv5x5_16b_kernel
 bool dw5x5_eligible(const Op& op) {
   return op.type == OP_DW && op.R == 5 && op.S == 5 && op.dil == 1 && op.Cout % 8 == 0 && (op.stride == 1 || op.stride == 2) &&
-         (op.act == ACT_RELU || op.act == ACT_HSWISH);
+         (op.act == ACT_SILU || op.act == ACT_RELU || op.act == ACT_HSWISH);
 }
 
 // the depthwise kernels that also write the SE pooling slices of their output
-bool dw_kernel_pools(DwKernel k) { return k == DW_TMA || k == DW_STRIP_16B || k == DW_STRIP_F32; }
+bool dw_kernel_pools(DwKernel k) { return k == DW_TMA || k == DW_STRIP_16B || k == DW_STRIP_F32 || k == DW_5X5_POOL_16B; }
 
 constexpr int kDwOW = 4;  // outputs per thread along W in dwconv3x3_pool_16b_kernel (measured: 4 -> 3.65 ms, 2 -> 4.25 ms per 128 crops)
 constexpr int kDw5OW = 4;  // outputs per thread along W in dwconv5x5_16b_kernel
+
+// block shape of the pooling dwconv5x5_16b_kernel for C channels: gridDim.x chunks of cb channel vectors, `groups` groups of
+// cb threads per block.  The fewest chunks that keep at least 192 of a block's 256 threads busy (C = 1152: 2 chunks of 72
+// vectors x 3 groups = 216 threads instead of 144 x 1).
+struct Dw5PoolShape { int chunks, cb, groups; };
+Dw5PoolShape dw5_pool_shape(int C) {
+  const int cv = C / 8;
+  for (int n = (cv + 255) / 256;; ++n) {
+    const int cb = (cv + n - 1) / n, groups = 256 / cb;
+    if (cb * groups >= 192 || n >= cv) return {n, cb, groups};
+  }
+}
 
 // f(stride, act) with both compile-time constants (stride 1 or 2, act one of ACTS): the launch of a templated depthwise kernel
 template <int... ACTS, typename F>
@@ -820,13 +837,22 @@ cudaError_t dw_dispatch(const Op& op, F&& f) {
 }
 
 // Picks the kernel of a depthwise op and the number of partial pooling slices it writes (fc1 sums that many).  bf16 and fp16
-// tensor-core modes: 5x5 ops run dwconv5x5_16b_kernel, which does not pool; 3x3 stride-1 ops run the TMA-staged kernel when
-// a plan fits, the other 3x3 ops the 16-bit strip kernel.  3xTF32 mode: the fp32 strip kernel (exact activation) for 3x3
-// ops.  Other modes and shapes: the generic kernel, which does not pool.
+// tensor-core modes: 5x5 ops run dwconv5x5_16b_kernel, which pools for SiLU (EfficientNet-B) and does not pool for ReLU /
+// hard-swish (MobileNetV3); 3x3 stride-1 ops run the TMA-staged kernel when a plan fits, the other 3x3 ops the 16-bit strip
+// kernel.  3xTF32 mode: the fp32 strip kernel (exact activation) for 3x3 ops.  Other modes and shapes: the generic kernel,
+// which does not pool.
 void choose_dw_kernel(const mtb_handle* h, Op& op) {
   op.dw_kernel = DW_GENERIC;
   if (dw5x5_eligible(op)) {
-    if (is_tc16(h)) op.dw_kernel = DW_5X5_16B;
+    if (!is_tc16(h)) return;
+    if (op.act != ACT_SILU) {
+      op.dw_kernel = DW_5X5_16B;
+      return;
+    }
+    op.dw_kernel = DW_5X5_POOL_16B;
+    const int strips = op.Hout * ((op.Wout + kDw5OW - 1) / kDw5OW);
+    const int groups = dw5_pool_shape(op.Cout).groups;
+    op.pool_slices = std::min((strips + groups - 1) / groups, kPoolSlices);
     return;
   }
   if (!dw_strip_eligible(op)) return;
@@ -962,15 +988,24 @@ int run_op_t(mtb_handle* h, const Op& op, const float* crops, int B, const Works
             return launch_k(dwconv3x3_pool_f32_kernel<s, a, kDwOW>, grid, block, 0, st, p, pooled);
           });
           if (e != cudaSuccess) return fail(h, MTB_ERR_CUDA, "depthwise launch %s: %s", op.name.c_str(), cudaGetErrorString(e));
-        } else if (op.dw_kernel == DW_5X5_16B) {
+        } else if (op.dw_kernel == DW_5X5_16B || op.dw_kernel == DW_5X5_POOL_16B) {
           if constexpr (!k16) {
             return fail(h, MTB_ERR_CUDA, "depthwise %s: 16-bit kernel chosen for fp32 storage", op.name.c_str());
           } else {
-            const size_t items = (size_t)B * op.Hout * ((op.Wout + kDw5OW - 1) / kDw5OW) * (op.Cout / 8);
-            const dim3 grid(grid_for(items, 256));
-            const cudaError_t e = dw_dispatch<ACT_RELU, ACT_HSWISH>(op, [&](auto s, auto a) {
-              return launch_k(dwconv5x5_16b_kernel<T, s, a, kDw5OW>, grid, dim3(256), 0, st, p);
-            });
+            cudaError_t e;
+            if (op.dw_kernel == DW_5X5_16B) {
+              const size_t items = (size_t)B * op.Hout * ((op.Wout + kDw5OW - 1) / kDw5OW) * (op.Cout / 8);
+              const dim3 grid(grid_for(items, 256));
+              e = dw_dispatch<ACT_RELU, ACT_HSWISH>(op, [&](auto s, auto a) {
+                return launch_k(dwconv5x5_16b_kernel<T, s, a, kDw5OW>, grid, dim3(256), 0, st, p, nullptr);
+              });
+            } else {
+              const Dw5PoolShape sh = dw5_pool_shape(op.Cout);
+              const dim3 grid(sh.chunks, op.pool_slices, B), block(sh.cb * sh.groups);
+              e = dw_dispatch<ACT_SILU>(op, [&](auto s, auto a) {
+                return launch_k(dwconv5x5_16b_kernel<T, s, a, kDw5OW, true>, grid, block, 0, st, p, pooled);
+              });
+            }
             if (e != cudaSuccess) return fail(h, MTB_ERR_CUDA, "depthwise launch %s: %s", op.name.c_str(), cudaGetErrorString(e));
           }
         } else {
@@ -1274,8 +1309,16 @@ int mtb_create(const mtb_config* cfg, mtb_handle** out) {
   if (cfg->n_joints <= 0 || cfg->depth < 1 || cfg->proc_side <= 0 || cfg->stride_test <= 0 || cfg->stride_train <= 0)
     return fail(nullptr, MTB_ERR_INVALID_ARG, "invalid geometry (n_joints=%d depth=%d proc_side=%d stride=%d)", cfg->n_joints,
                 cfg->depth, cfg->proc_side, cfg->stride_test);
-  if (cfg->arch == MTB_ARCH_EFFNET && (cfg->n_stages <= 0 || cfg->n_stages > MTB_MAX_STAGES))
+  const bool effnet = cfg->arch == MTB_ARCH_EFFNET || cfg->arch == MTB_ARCH_EFFNET_EPS1E5;
+  if (effnet && (cfg->n_stages <= 0 || cfg->n_stages > MTB_MAX_STAGES))
     return fail(nullptr, MTB_ERR_INVALID_ARG, "n_stages out of range");
+  if (cfg->arch == MTB_ARCH_EFFNET_EPS1E5)  // the EfficientNet-B grammar: MBConv rows with 3x3 or 5x5 kernels
+    for (int i = 0; i < cfg->n_stages; ++i) {
+      const mtb_stage& s = cfg->stages[i];
+      if (s.block != 1 || (s.kernel != 3 && s.kernel != 5) || (s.stride != 1 && s.stride != 2))
+        return fail(nullptr, MTB_ERR_UNSUPPORTED, "MTB_ARCH_EFFNET_EPS1E5 stage %d: only MBConv rows with kernel 3 or 5 and "
+                    "stride 1 or 2 (got block %d, kernel %d, stride %d)", i, s.block, s.kernel, s.stride);
+    }
   if (cfg->precision < MTB_PRECISION_FP32 || cfg->precision > MTB_PRECISION_F16_SIMT)
     return fail(nullptr, MTB_ERR_INVALID_ARG, "unknown precision %d", cfg->precision);
   int ndev = 0;

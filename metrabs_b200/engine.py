@@ -316,7 +316,7 @@ class Engine:
 
     def op_dw_kernel(self, op):
         """The kernel finalize chose for depthwise op `op`: one of _lib.DW_GENERIC, DW_TMA, DW_STRIP_16B, DW_STRIP_F32,
-        DW_5X5_16B."""
+        DW_5X5_16B, DW_5X5_POOL_16B."""
         k = lib().mtb_op_dw_kernel(self._h, op)
         if k < 0:
             check(k, self._h)
