@@ -351,6 +351,13 @@ int mtb_debug_dw_plan(int height, int width, int* crops_per_item, int* rows_per_
 typedef enum { MTB_DW_GENERIC = 0, MTB_DW_TMA = 1, MTB_DW_STRIP_16B = 2, MTB_DW_STRIP_F32 = 3, MTB_DW_5X5_16B = 4,
                MTB_DW_5X5_POOL_16B = MTB_DW_5X5_16B + 1 /* 5 */ } mtb_dw_kernel;
 int mtb_op_dw_kernel(const mtb_handle* h, int op);
+/* The tensor-core kernel that runs backbone op `op` of the BF16_TC / F16_TC modes (on the forward, and in isolation with
+ * mtb_debug_run_op): CONV is tc_conv_kernel; CONV3X3S1 is tc_conv3x3s1_kernel, which takes the 3x3 stride-1 undilated
+ * convs with Cin and Cout <= 64 and SiLU or ReLU, from input boxes and weights resident in shared memory.  The profiler
+ * reports both under the class "tc_conv_kernel".  Ops of a fused FusedMBConv block report the kernel that runs them in
+ * isolation.  MTB_ERR_INVALID_ARG for an index out of range or an op without 16-bit tensor-core weights. */
+typedef enum { MTB_TC_CONV = 0, MTB_TC_CONV3X3S1 = 1 } mtb_tc_kernel;
+int mtb_op_tc_kernel(const mtb_handle* h, int op);
 
 #ifdef __cplusplus
 }

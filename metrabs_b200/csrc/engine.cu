@@ -2200,6 +2200,13 @@ int mtb_op_dw_kernel(const mtb_handle* h, int op) {
   return h->ops[op].dw_kernel;
 }
 
+int mtb_op_tc_kernel(const mtb_handle* h, int op) {
+  if (!h || op < 0 || op >= (int)h->ops.size()) return fail(h, MTB_ERR_INVALID_ARG, "op index out of range");
+  const Op& o = h->ops[op];
+  if (!o.tc.ready) return fail(h, MTB_ERR_INVALID_ARG, "op %d (%s) has no 16-bit tensor-core weights", op, o.name.c_str());
+  return tc3x3s1_eligible(o.R, o.S, o.stride, o.dil, o.Cin, o.Cout, o.act) ? MTB_TC_CONV3X3S1 : MTB_TC_CONV;  // as tc_conv_launch
+}
+
 int mtb_op_is_fused_block(const mtb_handle* h, int op_index) {
   return (h && op_index >= 0 && op_index + 1 < (int)h->ops.size() && h->ops[op_index].fmb.ready) ? 1 : 0;
 }

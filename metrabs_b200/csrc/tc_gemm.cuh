@@ -6,6 +6,9 @@
 //                    of the NHWC input fetched by a 4D TMA (out-of-bounds = the reference's explicit zero padding,
 //                    backbones/efficientnet.py:1127-1161)                                             (mode 1)
 //                    epilogue: registers -> + folded-BN bias, activation, + residual, 16-bit NHWC store.
+//   tc_conv3x3s1_kernel  3x3 stride-1 conv with Cin, Cout <= 64 (EfficientNetV2 stage 1, ResNet conv2_x): the input of a
+//                    tile as three column-shifted boxes instead of one box per tap, the weights resident; same MMA order
+//                    and the same epilogue as tc_conv_kernel.
 //   tc_head_kernel   MetrabsHeads (models/metrabs.py:75-85): swapped operands, D[channel, pixel] = W[N, C] * F^T, so every
 //                    epilogue thread owns one (d,j) channel and reduces its pixels in registers: the J x D x H x W logits
 //                    never leave the SM.
@@ -223,6 +226,78 @@ __device__ __forceinline__ void tma_load_tap_boxes(uint8_t* dst, int box_bytes, 
     tma_load_4d(dst + s * box_bytes, map, bar, kc * TC_BK, tw * TC_TILE_W - p.pad_l + s, th * TC_TILE_H - p.pad_t, b);
 }
 
+// Epilogue of one 128-row x BN-column output tile held by consumer warpgroup c (rows [0, 64) in acc, [64, 128) in
+// acc + BN/2, as two m64nBNk16 wgmma accumulators): + folded-BN bias, activation, + residual read from global, rounded to
+// 16 bits into the warpgroup's staging tile stg in the TMA's swizzled layout ([BN / SW slabs][128 rows][SW columns], SW =
+// min(BN, 64)), then one thread stores the slabs with the TMA (2D box for mode 0, 4D 16 x 8-pixel box for mode 1).  The
+// TMA clips what lies outside the tensor: the M tail, the parts of a 16 x 8 box beyond the map, the Cout tail.  Uses the
+// named barrier 3 + c; the staging tile is rewritten only after the warpgroup's previous stores have read it.
+template <typename T, int ACT, int RES, int BN>
+__device__ __forceinline__ void tc_tile_epilogue(const float* acc, uint8_t* stg, const CUtensorMap* tmO, const TcConvParams& p, int m_blk,
+                                                 int n_blk, int c) {
+  constexpr int SW = BN < 64 ? BN : 64, RB = SW * 2;  // staging slab: columns, bytes per row
+  typedef typename Pair16<T>::type T2;
+  const T* __restrict__ res = (const T*)p.res;
+  const int warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  // rows 64 mh + 16 warp + lane / 4 (+ 8 h), columns 8 j + 2 (lane % 4) + {0, 1} -> staging tile
+  const bool leader = (threadIdx.x & 127) == 0;  // issues and waits for this warpgroup's bulk stores
+  if (leader) bulk_wait_read();  // the previous tile's stores have read the staging tile
+  wg_sync(2 + c);                // named barriers 3, 4 (1 and 2 order tc_conv_kernel's main loops)
+  const int c0 = n_blk * BN + 2 * (lane & 3);
+#pragma unroll
+  for (int mh = 0; mh < 2; ++mh) {
+    const float* accm = acc + mh * (BN / 2);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = mh * 64 + warp * 16 + (lane >> 2) + 8 * h;
+      size_t off = 0;
+      if constexpr (RES != 0) {
+        if (!tile_row_offset(p.mode, m_blk, r, p.M, p.Cout, p.tiles_w, p.tiles_h, p.Hout, p.Wout, off)) continue;
+      }
+      const uint32_t swz = RB == 128 ? (uint32_t)(r & 7) : (uint32_t)((r >> 1) & 3);
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int cc = c0 + 8 * j;
+        if (cc >= p.Cout) break;  // Cout % 8 == 0: column cc + 1 is valid with cc
+        const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + cc));
+        float o0 = accm[4 * j + 2 * h] + bv.x, o1 = accm[4 * j + 2 * h + 1] + bv.y;
+        if constexpr (RES != 0) {
+          const float2 rv = Pair16<T>::unpack(*reinterpret_cast<const T2*>(res + off + cc));
+          if constexpr (RES == 2) {
+            o0 = tc_act<ACT, T>(o0 + rv.x);
+            o1 = tc_act<ACT, T>(o1 + rv.y);
+          } else {
+            o0 = tc_act<ACT, T>(o0) + rv.x;
+            o1 = tc_act<ACT, T>(o1) + rv.y;
+          }
+        } else {
+          o0 = tc_act<ACT, T>(o0);
+          o1 = tc_act<ACT, T>(o1);
+        }
+        const int col = 8 * j + 2 * (lane & 3), cs = col % SW;  // column within the tile, within its slab
+        const uint32_t o = (uint32_t)(col / SW) * (TC_BM * RB) + (uint32_t)r * RB + ((((uint32_t)cs >> 3) ^ swz) << 4) + (cs & 7) * 2;
+        *reinterpret_cast<T2*>(stg + o) = Pair16<T>::pack(o0, o1);
+      }
+    }
+  }
+  fence_proxy_async();  // generic-proxy writes -> visible to the TMA (async proxy)
+  wg_sync(2 + c);
+  if (leader) {
+#pragma unroll
+    for (int sl = 0; sl < BN / SW; ++sl) {
+      const int col0 = n_blk * BN + sl * SW;
+      if (col0 >= p.Cout) break;
+      if (p.mode == 0) {
+        tma_store_2d(tmO, stg + sl * TC_BM * RB, col0, m_blk * TC_BM);
+      } else {
+        const int tw = m_blk % p.tiles_w, th = (m_blk / p.tiles_w) % p.tiles_h, b = m_blk / (p.tiles_w * p.tiles_h);
+        tma_store_4d(tmO, stg + sl * TC_BM * RB, col0, tw * TC_TILE_W, th * TC_TILE_H, b);
+      }
+    }
+    bulk_commit();
+  }
+}
+
 // Persistent conv / GEMM kernel.  ACT: epilogue activation; RES: 0 no residual, 1 residual added AFTER the activation
 // (EfficientNet), 2 BEFORE (ResNet); BN: output channels per tile (wgmma N); T: operand and activation element type
 // (__nv_bfloat16 or __half).
@@ -245,7 +320,7 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint64_t* full = (uint64_t*)(smem + Ring::bar_off);
   uint64_t* empty = full + STAGES;
 
-  const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
@@ -283,9 +358,6 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   // ===== consumers: warpgroup 1 + c computes the CTA's tiles c, c + 2, ... (rows [0, 64) in acc, [64, 128) in acc + BN/2) =====
   setmaxnreg_inc<232>();
   const int c = wg - 1;
-  constexpr int SW = Ring::slab_cols, RB = SW * 2;  // staging slab: columns, bytes per row
-  typedef typename Pair16<T>::type T2;
-  const T* __restrict__ res = (const T*)p.res;
   for (int i = c, t = blockIdx.x + c * gridDim.x; t < tiles; i += 2, t += 2 * gridDim.x) {
     const int m_blk = t / p.n_tiles, n_blk = t - m_blk * p.n_tiles;
     float acc[BN];
@@ -318,66 +390,123 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[prev]);
     if (t + (int)gridDim.x < tiles) named_bar_arrive(2 - c);  // the other consumer may start the next tile
+    tc_tile_epilogue<T, ACT, RES, BN>(acc, smem + Ring::out_off + c * Ring::out_bytes, &tmO, p, m_blk, n_blk, c);
+  }
+  if ((threadIdx.x & 127) == 0) bulk_wait();
+}
 
-    // ===== epilogue: rows 64 mh + 16 warp + lane / 4 (+ 8 h), columns 8 j + 2 (lane % 4) + {0, 1} -> staging tile =====
-    const bool leader = (threadIdx.x & 127) == 0;  // issues and waits for this warpgroup's bulk stores
-    uint8_t* stg = smem + Ring::out_off + c * Ring::out_bytes;
-    if (leader) bulk_wait_read();  // the previous tile's stores have read the staging tile
-    wg_sync(2 + c);                // named barriers 3, 4 (1 and 2 order the main loops)
-    const int c0 = n_blk * BN + 2 * (lane & 3);
-#pragma unroll
-    for (int mh = 0; mh < 2; ++mh) {
-      const float* accm = acc + mh * (BN / 2);
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int r = mh * 64 + warp * 16 + (lane >> 2) + 8 * h;
-        size_t off = 0;
-        if constexpr (RES != 0) {
-          if (!tile_row_offset(p.mode, m_blk, r, p.M, p.Cout, p.tiles_w, p.tiles_h, p.Hout, p.Wout, off)) continue;
-        }
-        const uint32_t swz = RB == 128 ? (uint32_t)(r & 7) : (uint32_t)((r >> 1) & 3);
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          const int cc = c0 + 8 * j;
-          if (cc >= p.Cout) break;  // Cout % 8 == 0: column cc + 1 is valid with cc
-          const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + cc));
-          float o0 = accm[4 * j + 2 * h] + bv.x, o1 = accm[4 * j + 2 * h + 1] + bv.y;
-          if constexpr (RES != 0) {
-            const float2 rv = Pair16<T>::unpack(*reinterpret_cast<const T2*>(res + off + cc));
-            if constexpr (RES == 2) {
-              o0 = tc_act<ACT, T>(o0 + rv.x);
-              o1 = tc_act<ACT, T>(o1 + rv.y);
-            } else {
-              o0 = tc_act<ACT, T>(o0) + rv.x;
-              o1 = tc_act<ACT, T>(o1) + rv.y;
-            }
-          } else {
-            o0 = tc_act<ACT, T>(o0);
-            o1 = tc_act<ACT, T>(o1);
-          }
-          const int col = 8 * j + 2 * (lane & 3), cs = col % SW;  // column within the tile, within its slab
-          const uint32_t o = (uint32_t)(col / SW) * (TC_BM * RB) + (uint32_t)r * RB + ((((uint32_t)cs >> 3) ^ swz) << 4) + (cs & 7) * 2;
-          *reinterpret_cast<T2*>(stg + o) = Pair16<T>::pack(o0, o1);
-        }
+// ------------------------------------------------------------------- 3x3 stride-1 conv with Cin, Cout <= 64
+// tc_conv3x3s1_kernel's shared memory for K per tap = N tile = CK (32: 64-byte rows, SWIZZLE_64B; 64: 128-byte rows,
+// SWIZZLE_128B): the 9 taps' [CK][CK] weight blocks, resident for the CTA's whole tile sequence; per consumer warpgroup
+// `sets` sets of the three 16 x 10-pixel input boxes of a tile; one output staging tile per consumer warpgroup.
+// CK = 32: 18 KB + 4 x 30 KB + 2 x 8 KB = 154 KB; CK = 64: 72 KB + 2 x 60 KB + 2 x 16 KB = 224 KB.
+template <int CK>
+struct Tc3x3Smem {
+  static constexpr int RB = CK * 2;                              // bytes per pixel of a box, per output channel of a weight block
+  static constexpr int w_tap_bytes = CK * RB;
+  static constexpr int box_bytes = TC_TILE_W * (TC_TILE_H + 2) * RB;  // 10 / 20 KB, a multiple of 1024
+  static constexpr int sets = CK == 32 ? 2 : 1;
+  static constexpr int box_off = 9 * w_tap_bytes;
+  static constexpr int out_bytes = TC_BM * CK * 2;
+  static constexpr int out_off = box_off + 2 * sets * 3 * box_bytes;
+  static constexpr int bar_off = out_off + 2 * out_bytes;
+  static constexpr int smem_bytes = bar_off + 256 /*barriers*/ + 1024 /*align slack*/;
+};
+
+// Shapes tc_conv3x3s1_kernel takes: 3x3, stride 1, dilation 1, Cin and Cout multiples of 8 up to 64, SiLU or ReLU (the
+// stage-1 convs of EfficientNetV2, the conv2_x 3x3 convs of the ResNets); its K per tap and N tile is 32 when Cin and Cout
+// fit in 32, else 64.
+inline bool tc3x3s1_eligible(int R, int S, int stride, int dil, int cin, int cout, int act) {
+  return R == 3 && S == 3 && stride == 1 && dil == 1 && cin <= 64 && cout <= 64 && cin % 8 == 0 && cout % 8 == 0 &&
+         (act == ACT_SILU || act == ACT_RELU);
+}
+inline int tc3x3s1_width(int cin, int cout) { return std::max(cin, cout) <= 32 ? 32 : 64; }
+
+// Persistent 3x3 stride-1 conv, one N tile (BN = CK >= Cout), mode-1 16 x 8-pixel output tiles.  The input of a tile is
+// loaded once, as the three column-shifted 16 x 10-pixel boxes of tma_load_tap_boxes with CK channels (those beyond Cin
+// are zeros from the TMA); the A tile of tap (r, s) is box s from pixel row r on, r x 16 x RB bytes in, a multiple of
+// the swizzle atom, so its descriptors are those of an aligned per-tap tile.  The weights are loaded once per CTA.  At
+// Cin < CK the 32-column weight block of tap t also holds the first weights of tap t + 1 (of the last tap: the map's
+// out-of-bounds zeros); they meet zero A channels.
+//
+// Warpgroup 0 (one thread) loads the weights, then the boxes of the CTA's tiles; consumer warpgroups 1 and 2 take
+// alternate tiles, each into box sets of its own, so both may be in their MMAs at once.  A box set goes back to the producer
+// once its tile's last wgmma has retired, before the epilogue.  The MMA sequence of every output element is that of
+// tc_conv_kernel (taps in order, channels ascending, K = 16 per wgmma, fp32 accumulators) without the k16 steps whose A
+// columns are all zeros (channels >= 32 at Cin <= 32), and the epilogue is tc_conv_kernel's.
+template <typename T, int ACT, int RES, int CK>
+__global__ void __launch_bounds__(TCP_THREADS, 1)
+tc_conv3x3s1_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                    const __grid_constant__ CUtensorMap tmO, const TcConvParams p) {
+  using L = Tc3x3Smem<CK>;
+  constexpr int BN = CK, SETS = L::sets, RB = L::RB;
+  extern __shared__ uint8_t tc_smem_raw[];
+  uint8_t* smem = (uint8_t*)(((uintptr_t)tc_smem_raw + 1023) & ~(uintptr_t)1023);
+  uint64_t* w_full = (uint64_t*)(smem + L::bar_off);
+  uint64_t* box_full = w_full + 1;           // [consumer][set]
+  uint64_t* box_empty = box_full + 2 * SETS;
+
+  const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    tma_prefetch_desc(&tmO);
+    mbar_init(w_full, 1);
+    for (int i = 0; i < 2 * SETS; ++i) {
+      mbar_init(&box_full[i], 1);   // the producer's arrive.expect_tx
+      mbar_init(&box_empty[i], 4);  // one arrive per warp of the consuming warpgroup
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  const int tiles = p.m_tiles;
+  if (wg == 0) {
+    // ===== TMA producer: the weights, then tile n's boxes into set (n / 2) % SETS of consumer n % 2 =====
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      mbar_expect_tx(w_full, 9 * L::w_tap_bytes);
+      for (int tap = 0; tap < 9; ++tap) tma_load_2d(smem + tap * L::w_tap_bytes, &tmB, w_full, tap * p.Cin, 0);
+      int n = 0;
+      for (int t = blockIdx.x; t < tiles; t += gridDim.x, ++n) {
+        const int j = n >> 1, b = (n & 1) * SETS + j % SETS;
+        mbar_wait(&box_empty[b], ((j / SETS) & 1) ^ 1);
+        mbar_expect_tx(&box_full[b], 3 * L::box_bytes);
+        tma_load_tap_boxes(smem + L::box_off + b * 3 * L::box_bytes, L::box_bytes, &tmA, &box_full[b], p, t, 0);
       }
     }
-    fence_proxy_async();  // generic-proxy writes -> visible to the TMA (async proxy)
-    wg_sync(2 + c);
-    // The TMA clips what lies outside the tensor: the M tail, the parts of a 16 x 8 box beyond the map, the Cout tail.
-    if (leader) {
+    return;
+  }
+  // ===== consumers: warpgroup 1 + c computes the CTA's tiles c, c + 2, ... =====
+  setmaxnreg_inc<232>();
+  const int c = wg - 1;
+  const uint32_t wts = smem_u32(smem);
+  mbar_wait(w_full, 0);
+  for (int j = 0, t = blockIdx.x + c * gridDim.x; t < tiles; ++j, t += 2 * gridDim.x) {
+    const int b = c * SETS + j % SETS;
+    float acc[BN];
 #pragma unroll
-      for (int sl = 0; sl < BN / SW; ++sl) {
-        const int col0 = n_blk * BN + sl * SW;
-        if (col0 >= p.Cout) break;
-        if (p.mode == 0) {
-          tma_store_2d(&tmO, stg + sl * TC_BM * RB, col0, m_blk * TC_BM);
-        } else {
-          const int tw = m_blk % p.tiles_w, th = (m_blk / p.tiles_w) % p.tiles_h, b = m_blk / (p.tiles_w * p.tiles_h);
-          tma_store_4d(&tmO, stg + sl * TC_BM * RB, col0, tw * TC_TILE_W, th * TC_TILE_H, b);
-        }
+    for (int q = 0; q < BN; ++q) acc[q] = 0.f;
+    mbar_wait(&box_full[b], (j / SETS) & 1);
+    const uint32_t box = smem_u32(smem + L::box_off + b * 3 * L::box_bytes);
+    wgmma_fence();
+#pragma unroll
+    for (int tap = 0; tap < 9; ++tap) {
+      const int r = tap / 3, s = tap - 3 * r;
+      const uint32_t a = box + s * L::box_bytes + r * TC_TILE_W * RB, w = wts + tap * L::w_tap_bytes;
+#pragma unroll
+      for (int k = 0; k < CK / 16; ++k) {
+        const uint64_t db = gmma_desc<RB>(w + 32 * k);
+        wgmma_16b<T, BN>(acc, gmma_desc<RB>(a + 32 * k), db, (uint32_t)(tap | k));
+        wgmma_16b<T, BN>(acc + BN / 2, gmma_desc<RB>(a + 64 * RB + 32 * k), db, (uint32_t)(tap | k));
       }
-      bulk_commit();
     }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs<BN>(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&box_empty[b]);  // the boxes go back to the producer under the epilogue
+    tc_tile_epilogue<T, ACT, RES, BN>(acc, smem + L::out_off + c * L::out_bytes, &tmO, p, t, 0, c);
   }
   if ((threadIdx.x & 127) == 0) bulk_wait();
 }
@@ -573,7 +702,9 @@ inline const char* tc_conv_launch(const TcWeights& w, const ConvParams& p, bool 
   q.tiles_w = (p.Wout + TC_TILE_W - 1) / TC_TILE_W;
   q.tiles_h = (p.Hout + TC_TILE_H - 1) / TC_TILE_H;
   q.M = p.B * p.Hout * p.Wout;
-  const int bn = tc_pick_bn(p.Cout);
+  // tc_conv3x3s1_kernel for the shapes it takes (bn: its K per tap and N tile), tc_conv_kernel for every other conv
+  const bool s1 = tc3x3s1_eligible(p.R, p.S, p.stride, p.dil, p.Cin, p.Cout, p.act);
+  const int bn = s1 ? tc3x3s1_width(p.Cin, p.Cout) : tc_pick_bn(p.Cout);
   q.m_tiles = q.mode == 0 ? (q.M + TC_BM - 1) / TC_BM : p.B * q.tiles_w * q.tiles_h;
   q.n_tiles = (p.Cout + bn - 1) / bn;
   const CUtensorMap* m = nullptr;  // input, weights, output
@@ -581,17 +712,32 @@ inline const char* tc_conv_launch(const TcWeights& w, const ConvParams& p, bool 
     const CUtensorMapSwizzle sw = CU_TENSOR_MAP_SWIZZLE_128B;
     const uint32_t slab = (uint32_t)std::min(bn, 64);  // output box: 64 (SWIZZLE_128B) or 32 (SWIZZLE_64B) channels
     const CUtensorMapSwizzle out_sw = slab == 64 ? sw : CU_TENSOR_MAP_SWIZZLE_64B;
-    const char* r = q.mode == 0 ? make_tmap_2d<T>(&c[0], p.in, q.M, p.Cin, TC_BM, TC_BK, sw)
-                                : make_tmap_nhwc<T>(&c[0], p.in, p.B, p.Hin, p.Win, p.Cin, TC_BK, TC_TILE_W, TC_TILE_H, 1, p.stride, sw);
-    if (!r) r = make_tmap_2d<T>(&c[1], w.d_w, p.Cout, (uint64_t)w.taps * p.Cin, bn, TC_BK, sw);
+    const char* r;
+    if (s1) {  // 16 x 10-pixel input boxes and [bn][bn] weight blocks, both with rows of bn channels like the output box
+      r = make_tmap_nhwc<T>(&c[0], p.in, p.B, p.Hin, p.Win, p.Cin, bn, TC_TILE_W, TC_TILE_H + 2, 1, 1, out_sw);
+      if (!r) r = make_tmap_2d<T>(&c[1], w.d_w, p.Cout, (uint64_t)w.taps * p.Cin, bn, bn, out_sw);
+    } else {
+      r = q.mode == 0 ? make_tmap_2d<T>(&c[0], p.in, q.M, p.Cin, TC_BM, TC_BK, sw)
+                      : make_tmap_nhwc<T>(&c[0], p.in, p.B, p.Hin, p.Win, p.Cin, TC_BK, TC_TILE_W, TC_TILE_H, 1, p.stride, sw);
+      if (!r) r = make_tmap_2d<T>(&c[1], w.d_w, p.Cout, (uint64_t)w.taps * p.Cin, bn, TC_BK, sw);
+    }
     if (!r)
       r = q.mode == 0 ? make_tmap_2d<T>(&c[2], p.out, q.M, p.Cout, TC_BM, slab, out_sw)
                       : make_tmap_nhwc<T>(&c[2], p.out, p.B, p.Hout, p.Wout, p.Cout, slab, TC_TILE_W, TC_TILE_H, 1, 1, out_sw);
     return r;
-  }, p.in, p.out, w.d_w, p.B, p.Hin, p.Win, p.Cin, p.Hout, p.Wout, p.Cout, w.taps, p.stride, bn);
+  }, p.in, p.out, w.d_w, p.B, p.Hin, p.Win, p.Cin, p.Hout, p.Wout, p.Cout, w.taps, p.stride, bn, s1);
   if (e) return e;
   const dim3 grid(std::min(q.m_tiles * q.n_tiles, num_sms()));  // persistent: one CTA per SM
   const int res_mode = p.res ? (res_first ? 2 : 1) : 0;
+  if (s1)
+    return with_const<ACT_SILU, ACT_RELU>(p.act, "unsupported activation in tc_conv3x3s1_kernel", [&](auto act) {
+      return with_const<0, 1, 2>(res_mode, "unsupported residual mode", [&](auto res) {
+        return with_const<32, 64>(bn, "unsupported width of tc_conv3x3s1_kernel", [&](auto ck) {
+          return launch_smem(tc_conv3x3s1_kernel<T, act, res, ck>, grid, dim3(TCP_THREADS), Tc3x3Smem<ck>::smem_bytes, st, m[0], m[1], m[2],
+                             q);
+        });
+      });
+    });
   return with_const<ACT_NONE, ACT_SILU, ACT_RELU, ACT_HSWISH>(p.act, "unsupported activation in the tensor-core epilogue", [&](auto act) {
     return with_const<0, 1, 2>(res_mode, "unsupported residual mode", [&](auto res) {
       return with_const<32, 64, 128>(bn, "unsupported N tile", [&](auto bn_) {

@@ -322,6 +322,14 @@ class Engine:
             check(k, self._h)
         return k
 
+    def op_tc_kernel(self, op):
+        """The 16-bit tensor-core kernel that runs op `op`: _lib.TC_CONV (tc_conv_kernel) or _lib.TC_CONV3X3S1
+        (tc_conv3x3s1_kernel, the 3x3 stride-1 convs with Cin, Cout <= 64)."""
+        k = lib().mtb_op_tc_kernel(self._h, op)
+        if k < 0:
+            check(k, self._h)
+        return k
+
     def op_is_fused_block(self, op):
         """True when backbone op `op` (3x3 expand) and op + 1 (1x1 projection) run as one fused FusedMBConv kernel."""
         return bool(lib().mtb_op_is_fused_block(self._h, op))
