@@ -255,28 +255,41 @@ __device__ __forceinline__ void tc_tile_epilogue(const float* acc, uint8_t* stg,
         if (!tile_row_offset(p.mode, m_blk, r, p.M, p.Cout, p.tiles_w, p.tiles_h, p.Hout, p.Wout, off)) continue;
       }
       const uint32_t swz = RB == 128 ? (uint32_t)(r & 7) : (uint32_t)((r >> 1) & 3);
+      // The residual pairs of up to 64 columns are loaded ahead of their arithmetic: loaded inside the column loop, behind
+      // the previous column's staging store, each load waited out its full latency before the next one was issued.  A whole
+      // row at BN = 128 would not fit next to the accumulators in the 168 registers of __launch_bounds__.
+      constexpr int JB = BN / 8 < 8 ? BN / 8 : 8;
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int cc = c0 + 8 * j;
-        if (cc >= p.Cout) break;  // Cout % 8 == 0: column cc + 1 is valid with cc
-        const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + cc));
-        float o0 = accm[4 * j + 2 * h] + bv.x, o1 = accm[4 * j + 2 * h + 1] + bv.y;
+      for (int j0 = 0; j0 < BN / 8; j0 += JB) {
+        T2 rv2[RES != 0 ? JB : 1];
         if constexpr (RES != 0) {
-          const float2 rv = Pair16<T>::unpack(*reinterpret_cast<const T2*>(res + off + cc));
-          if constexpr (RES == 2) {
-            o0 = tc_act<ACT, T>(o0 + rv.x);
-            o1 = tc_act<ACT, T>(o1 + rv.y);
-          } else {
-            o0 = tc_act<ACT, T>(o0) + rv.x;
-            o1 = tc_act<ACT, T>(o1) + rv.y;
-          }
-        } else {
-          o0 = tc_act<ACT, T>(o0);
-          o1 = tc_act<ACT, T>(o1);
+#pragma unroll
+          for (int jj = 0; jj < JB; ++jj)
+            if (c0 + 8 * (j0 + jj) < p.Cout) rv2[jj] = *reinterpret_cast<const T2*>(res + off + c0 + 8 * (j0 + jj));
         }
-        const int col = 8 * j + 2 * (lane & 3), cs = col % SW;  // column within the tile, within its slab
-        const uint32_t o = (uint32_t)(col / SW) * (TC_BM * RB) + (uint32_t)r * RB + ((((uint32_t)cs >> 3) ^ swz) << 4) + (cs & 7) * 2;
-        *reinterpret_cast<T2*>(stg + o) = Pair16<T>::pack(o0, o1);
+#pragma unroll
+        for (int j = j0; j < j0 + JB; ++j) {
+          const int cc = c0 + 8 * j;
+          if (cc >= p.Cout) break;  // Cout % 8 == 0: column cc + 1 is valid with cc
+          const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + cc));
+          float o0 = accm[4 * j + 2 * h] + bv.x, o1 = accm[4 * j + 2 * h + 1] + bv.y;
+          if constexpr (RES != 0) {
+            const float2 rv = Pair16<T>::unpack(rv2[j - j0]);
+            if constexpr (RES == 2) {
+              o0 = tc_act<ACT, T>(o0 + rv.x);
+              o1 = tc_act<ACT, T>(o1 + rv.y);
+            } else {
+              o0 = tc_act<ACT, T>(o0) + rv.x;
+              o1 = tc_act<ACT, T>(o1) + rv.y;
+            }
+          } else {
+            o0 = tc_act<ACT, T>(o0);
+            o1 = tc_act<ACT, T>(o1);
+          }
+          const int col = 8 * j + 2 * (lane & 3), cs = col % SW;  // column within the tile, within its slab
+          const uint32_t o = (uint32_t)(col / SW) * (TC_BM * RB) + (uint32_t)r * RB + ((((uint32_t)cs >> 3) ^ swz) << 4) + (cs & 7) * 2;
+          *reinterpret_cast<T2*>(stg + o) = Pair16<T>::pack(o0, o1);
+        }
       }
     }
   }
