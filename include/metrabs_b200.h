@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define MTB_ABI_VERSION 1
+#define MTB_ABI_VERSION 2
 
 typedef enum {
   MTB_OK = 0,
@@ -88,6 +88,10 @@ typedef struct {
   int32_t cin, cout;
   int32_t layers;
   int32_t bottomright; /* bottomright_stride: pad (pb-1, pe+1) on the first block (:140-141, :195-196) */
+  int32_t dilation_in;  /* dilation of the first block's depthwise conv (`din` of metrabs_tf effnetv2_configs.py), 1..8 */
+  int32_t dilation_out; /* dilation of the later blocks (`dout`); both 1 in the stride-32 tables.  A table whose output
+                         * stride (2 x the product of the stage strides) is below 32 must equal stride_test, and dilates
+                         * MBConv rows only (the reference's efficientnetv2-{s,l}-stride{16,8}, :163-228) */
 } mtb_stage;
 
 /* Frozen copy of the get_config() keys the path reads (util.py:41-57; config/config_l.yaml:1-21). */
@@ -346,10 +350,13 @@ int mtb_debug_dw_plan(int height, int width, int* crops_per_item, int* rows_per_
  * 4 channels; every fp32 / 3xTF32 / _SIMT mode op that no other kernel covers), TMA the TMA-staged 3x3 stride-1 kernel and
  * STRIP_16B / STRIP_F32 the 3x3 strip kernels (these three also write the SE pooling slices), 5X5_16B the 16-bit 5x5 kernel
  * of the BF16_TC / F16_TC modes for ReLU / hard-swish (bit-identical to dwconv_kernel, no pooling), 5X5_POOL_16B the same
- * kernel for SiLU (bit-identical outputs, and it also writes the SE pooling slices of the stored outputs).
+ * kernel for SiLU (bit-identical outputs, and it also writes the SE pooling slices of the stored outputs), TMA_DIL the
+ * TMA-staged kernel for the 3x3 stride-1 SiLU ops with dilation 2 or 4 of the BF16_TC / F16_TC modes (one undilated pass per
+ * phase of the dilation, same arithmetic per output as TMA, also writes the SE pooling slices).
  * MTB_ERR_INVALID_ARG for an index out of range or an op that is not depthwise. */
 typedef enum { MTB_DW_GENERIC = 0, MTB_DW_TMA = 1, MTB_DW_STRIP_16B = 2, MTB_DW_STRIP_F32 = 3, MTB_DW_5X5_16B = 4,
-               MTB_DW_5X5_POOL_16B = MTB_DW_5X5_16B + 1 /* 5 */ } mtb_dw_kernel;
+               MTB_DW_5X5_POOL_16B = MTB_DW_5X5_16B + 1 /* 5 */,
+               MTB_DW_TMA_DIL = MTB_DW_5X5_POOL_16B + 1 /* 6 */ } mtb_dw_kernel;
 int mtb_op_dw_kernel(const mtb_handle* h, int op);
 /* The tensor-core kernel that runs backbone op `op` of the BF16_TC / F16_TC modes (on the forward, and in isolation with
  * mtb_debug_run_op): CONV is tc_conv_kernel; CONV3X3S1 is tc_conv3x3s1_kernel, which takes the 3x3 stride-1 undilated

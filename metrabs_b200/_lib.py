@@ -3,14 +3,14 @@ shared library is missing or cannot be loaded, importing the compute entry point
 import ctypes as C
 import os
 
-MTB_ABI_VERSION = 1
+MTB_ABI_VERSION = 2
 MTB_MAX_STAGES = 16
 
 ARCH_EFFNET, ARCH_RESNET50, ARCH_MOBILENETV3_SMALL, ARCH_HEAD_ONLY = 0, 1, 2, 3
 ARCH_RESNET18, ARCH_RESNET34, ARCH_RESNET101, ARCH_RESNET152 = 4, 5, 6, 7
 ARCH_MOBILENETV3_LARGE = 8
 ARCH_EFFNET_EPS1E5 = 9  # the EFFNET grammar with BatchNorm eps 1e-5 (EfficientNet-B0..B4)
-DW_GENERIC, DW_TMA, DW_STRIP_16B, DW_STRIP_F32, DW_5X5_16B, DW_5X5_POOL_16B = 0, 1, 2, 3, 4, 5  # mtb_op_dw_kernel
+DW_GENERIC, DW_TMA, DW_STRIP_16B, DW_STRIP_F32, DW_5X5_16B, DW_5X5_POOL_16B, DW_TMA_DIL = 0, 1, 2, 3, 4, 5, 6  # mtb_op_dw_kernel
 TC_CONV, TC_CONV3X3S1 = 0, 1  # mtb_op_tc_kernel
 PRECISION_FP32, PRECISION_BF16_TC, PRECISION_BF16_SIMT, PRECISION_TF32X3, PRECISION_F16_TC, PRECISION_F16_SIMT = 0, 1, 2, 3, 4, 5
 DTYPE_F32, DTYPE_BF16, DTYPE_F16, DTYPE_I64 = 0, 1, 2, 3
@@ -21,7 +21,8 @@ LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'libmetrabs_
 
 class MtbStage(C.Structure):
     _fields_ = [('block', C.c_int32), ('expand', C.c_int32), ('kernel', C.c_int32), ('stride', C.c_int32),
-                ('cin', C.c_int32), ('cout', C.c_int32), ('layers', C.c_int32), ('bottomright', C.c_int32)]
+                ('cin', C.c_int32), ('cout', C.c_int32), ('layers', C.c_int32), ('bottomright', C.c_int32),
+                ('dilation_in', C.c_int32), ('dilation_out', C.c_int32)]
 
 
 class MtbConfig(C.Structure):

@@ -56,16 +56,53 @@ def b_stage_table(variant, centered_stride=None):
     width, depth, eps = _B_VARIANTS[variant]
     stages = [dict(block='mb', expand=r[0], kernel=r[1], stride=r[2], cin=_make_divisible(r[3] * width),
                    cout=_make_divisible(r[4] * width), layers=int(math.ceil(r[5] * depth)),
-                   bottomright=bool(len(r) > 6 and r[6] and centered_stride)) for r in _B_BASE]
+                   bottomright=bool(len(r) > 6 and r[6] and centered_stride), dilation_in=1, dilation_out=1)
+               for r in _B_BASE]
     return stages, 4 * stages[-1]['cout'], eps
 
 
-def stage_table(size, centered_stride=None):
+# output strides below 32 that the reference defines tables for (metrabs_tf effnetv2_configs.py:163-228); stride 4 would
+# dilate FusedMBConv stages and is not built
+_DILATED_SIZES = ('s', 'l', 'tiny')
+_OUTPUT_STRIDES = (8, 16, 32)
+
+
+def dilate_stages(stages, output_stride, centered_stride):
+    """The stride-32 table ``stages`` re-strided to ``output_stride`` (the reference's ``efficientnetv2-{s,l}-stride{16,8}``
+    tables, effnetv2_configs.py:163-228): with a running stride from 2 after the stem and a running dilation d = 1, a
+    stride-2 row that would take the stride past ``output_stride`` becomes stride 1 with ``dilation_in`` d, then d doubles
+    and is its ``dilation_out``; every other row gets d for both.  The bottom-right shift moves to the last row that still
+    strides, under ``centered_stride`` only (:45)."""
+    out, running, d = [], 2, 1
+    for st in stages:
+        st = dict(st, bottomright=False)
+        if st['stride'] == 2 and running * 2 > output_stride:
+            st.update(stride=1, dilation_in=d, dilation_out=2 * d)
+            d *= 2
+        else:
+            running *= st['stride']
+            st.update(dilation_in=d, dilation_out=d)
+        out.append(st)
+    last_strided = max(i for i, st in enumerate(out) if st['stride'] == 2)
+    out[last_strided]['bottomright'] = bool(centered_stride)
+    return out
+
+
+def stage_table(size, centered_stride=None, output_stride=32):
+    """-> (stages, last_channel) of EfficientNetV2-``size`` at ``output_stride`` 32, or 16 / 8 for 's', 'l' and 'tiny'."""
     if centered_stride is None:
         centered_stride = get_config().centered_stride
+    if output_stride not in _OUTPUT_STRIDES:
+        raise ValueError(f'EfficientNetV2 output stride {output_stride} is not built: 32, 16 or 8')
+    if output_stride != 32 and size not in _DILATED_SIZES:
+        raise ValueError(f'EfficientNetV2-{size} has no table at output stride {output_stride}: only '
+                         f'{", ".join(_DILATED_SIZES)} run at 16 or 8')
     rows, last = _TABLES[size]
     stages = [dict(block=r[0], expand=r[1], kernel=r[2], stride=r[3], cin=r[4], cout=r[5], layers=r[6],
-                   bottomright=bool(len(r) > 7 and r[7] and centered_stride)) for r in rows]
+                   bottomright=bool(len(r) > 7 and r[7] and centered_stride), dilation_in=1, dilation_out=1)
+              for r in rows]
+    if output_stride != 32:
+        stages = dilate_stages(stages, output_stride, centered_stride)
     return stages, last
 
 
@@ -101,6 +138,7 @@ class Features(nn.Module):
         self.last_channel = last_channel
         self.bn_eps = bn_eps
         self.arch = _ARCH_BY_EPS[bn_eps]
+        self.output_stride = 2 * math.prod(st['stride'] for st in stages)
         bn = lambda cin, cout, k, groups=1: _conv_bn(cin, cout, k, groups, bn_eps)  # noqa: E731
         self.add_module('0', bn(3, stages[0]['cin'], 3))
         for si, st in enumerate(stages):
@@ -127,14 +165,17 @@ class Features(nn.Module):
 
 
 class EfficientNet(nn.Module):
-    """``size``: a V2 table ('s', 'm', 'l', 'tiny') or a B variant ('b0'..'b7')."""
+    """``size``: a V2 table ('s', 'm', 'l', 'tiny') or a B variant ('b0'..'b7').  ``output_stride`` 16 or 8 builds the
+    dilated V2-S / V2-L (and 'tiny') tables; the model's ``Config.stride_test`` must then equal it."""
 
-    def __init__(self, size):
+    def __init__(self, size, output_stride=32):
         super().__init__()
         if size in _B_VARIANTS:
+            if output_stride != 32:
+                raise ValueError(f'EfficientNet-{size.upper()} has no table at output stride {output_stride}: only 32')
             stages, last, eps = b_stage_table(size)
         else:
-            (stages, last), eps = stage_table(size), 1e-3
+            (stages, last), eps = stage_table(size, output_stride=output_stride), 1e-3
         self.size = size
         self.features = Features(stages, last, eps)
 
@@ -146,20 +187,20 @@ class PreprocLayer(nn.Module):
         return inp
 
 
-def efficientnet_v2_s(**kwargs):
-    return EfficientNet('s')
+def efficientnet_v2_s(output_stride=32, **kwargs):
+    return EfficientNet('s', output_stride)
 
 
 def efficientnet_v2_m(**kwargs):
     return EfficientNet('m')
 
 
-def efficientnet_v2_l(**kwargs):
-    return EfficientNet('l')
+def efficientnet_v2_l(output_stride=32, **kwargs):
+    return EfficientNet('l', output_stride)
 
 
-def efficientnet_v2_tiny(**kwargs):
-    return EfficientNet('tiny')
+def efficientnet_v2_tiny(output_stride=32, **kwargs):
+    return EfficientNet('tiny', output_stride)
 
 
 def efficientnet_b0(**kwargs):

@@ -33,11 +33,12 @@ std::string g_error;
 enum OpType { OP_STEM = 0, OP_CONV = 1, OP_DW = 2, OP_POOL = 3, OP_MAXPOOL = 4 };
 // depthwise kernels: TMA-staged (dw_tma.cuh), 16-bit (bf16 / fp16) or fp32 strip (SE pooling fused), generic (dwconv_kernel),
 // 16-bit 5x5 (dwconv5x5_16b_kernel: dwconv_kernel's arithmetic with column reuse; without pooling for ReLU / hard-swish,
-// with SE pooling for SiLU); values of mtb_dw_kernel
-enum DwKernel { DW_GENERIC = 0, DW_TMA = 1, DW_STRIP_16B = 2, DW_STRIP_F32 = 3, DW_5X5_16B = 4, DW_5X5_POOL_16B = 5 };
+// with SE pooling for SiLU), TMA-staged dilated 3x3 (dw_tma.cuh, one undilated pass per phase); values of mtb_dw_kernel
+enum DwKernel { DW_GENERIC = 0, DW_TMA = 1, DW_STRIP_16B = 2, DW_STRIP_F32 = 3, DW_5X5_16B = 4, DW_5X5_POOL_16B = 5, DW_TMA_DIL = 6 };
 static_assert((int)DW_GENERIC == (int)MTB_DW_GENERIC && (int)DW_TMA == (int)MTB_DW_TMA && (int)DW_STRIP_16B == (int)MTB_DW_STRIP_16B &&
               (int)DW_STRIP_F32 == (int)MTB_DW_STRIP_F32 && (int)DW_5X5_16B == (int)MTB_DW_5X5_16B &&
-              (int)DW_5X5_POOL_16B == (int)MTB_DW_5X5_POOL_16B, "DwKernel must match mtb_dw_kernel");
+              (int)DW_5X5_POOL_16B == (int)MTB_DW_5X5_POOL_16B && (int)DW_TMA_DIL == (int)MTB_DW_TMA_DIL,
+              "DwKernel must match mtb_dw_kernel");
 // kernel classes for the CUDA-event profiler (mtb_profile_begin / mtb_profile_end)
 enum KClass { KC_STEM = 0, KC_IGEMM_SIMT = 1, KC_DWCONV = 2, KC_POOL = 3, KC_SE_FC = 4, KC_TC_GEMM = 5, KC_FMB = 6,
               KC_HEAD_FUSED = 7, KC_HEAD_CONV_SIMT = 8, KC_SOFTARGMAX = 9, KC_RECON = 10, KC_OTHER = 11, KC_SE_SCALE = 12, KC_TC32 = 13,
@@ -71,8 +72,8 @@ struct Op {
   float pre_scale[3] = {2.f, 2.f, 2.f}, pre_shift[3] = {-1.f, -1.f, -1.f};  // stem input affine (PreprocLayer: x*2-1)
   bool fused_pool = false;  // this depthwise op also produces the SE pooled means (next op is skipped)
   DwKernel dw_kernel = DW_GENERIC;  // depthwise: the kernel that runs it (set by mtb_finalize_weights)
-  DwTmaPlan dw_plan;                // DW_TMA: its tiling plan
-  int pool_slices = 1;              // DW_TMA / DW_STRIP_* / DW_5X5_POOL_16B: partial pooling slices it leaves (= its gridDim.y / dw_plan.n_rb)
+  DwTmaPlan dw_plan;                // DW_TMA / DW_TMA_DIL: its tiling plan (DW_TMA_DIL: of one phase of the dilation)
+  int pool_slices = 1;              // DW_TMA* / DW_STRIP_* / DW_5X5_POOL_16B: partial pooling slices it leaves (= its gridDim.y / dw_plan.n_rb)
   bool res_first = false;  // residual added BEFORE the activation (ResNet); EfficientNet adds it after
   int pool_src = -1;       // fc1: index of the OP_POOL op that produces its input (fused pooling leaves partial slices)
   int ksplit = 1;          // split-K (squeeze-excitation fc1): raw sums, bias/act deferred to the consumer
@@ -85,7 +86,7 @@ struct Op {
   TcWeights tc;             // 16-bit (bf16 / fp16) K-major copy + TMA descriptor state for the wgmma path
   Tc32Weights tc32;         // fp32 K-major copy + TMA descriptor state for the 3xTF32 wgmma path (MTB_PRECISION_TF32X3)
   FmbWeights fmb;           // 16-bit tensor-core modes: this 3x3 expand conv and the NEXT op (1x1 projection) run as one fmb_kernel launch
-  mutable TmapCache dw_maps;    // DW_TMA: its input tensor maps
+  mutable TmapCache dw_maps;    // DW_TMA / DW_TMA_DIL: its input tensor maps
   double flops = 0;         // 2*MACs per crop
   int stage = 0;            // EfficientNet stage (1-based; 0 = stem / last conv / other backbones)
 };
@@ -326,7 +327,10 @@ void plan_effnet(mtb_handle* h, float bn_eps) {
       const bool residual = stride == 1 && cin == st.cout;
       const int cexp = cin * st.expand;
       const int k = st.kernel;
-      const int pad_beg = (k - 1) / 2 - shift, pad_total = k - 1;  // fixed_padding_layer (:1127-1161)
+      // dilation of the depthwise conv: din on the first block, dout on the rest (metrabs_tf effnetv2_model.py:574-600);
+      // mtb_create admits dilation > 1 on MBConv rows only
+      const int dil = first ? st.dilation_in : st.dilation_out;
+      const int pad_total = (k - 1) * dil, pad_beg = pad_total / 2 - shift;  // fixed_padding_layer (:1127-1161)
       char key[64];
       snprintf(key, sizeof(key), "%s.%d.%d.block", pre.c_str(), si + 1, bi);
       const std::string kb = key;
@@ -354,7 +358,7 @@ void plan_effnet(mtb_handle* h, float bn_eps) {
           ++i;
         }
         int t2 = P.pick({x_in, t1});
-        P.conv(kb + "." + std::to_string(i), cexp, k, stride, pad_beg, pad_total, ACT_SILU, t1, t2, true);
+        P.conv(kb + "." + std::to_string(i), cexp, k, stride, pad_beg, pad_total, ACT_SILU, t1, t2, true, dil);
         ++i;
         // squeeze-excitation: avgpool -> fc1 + SiLU -> fc2 + sigmoid -> scale (folded into the projection's A load)
         const std::string se = kb + "." + std::to_string(i);
@@ -811,7 +815,9 @@ bool dw5x5_eligible(const Op& op) {
 }
 
 // the depthwise kernels that also write the SE pooling slices of their output
-bool dw_kernel_pools(DwKernel k) { return k == DW_TMA || k == DW_STRIP_16B || k == DW_STRIP_F32 || k == DW_5X5_POOL_16B; }
+bool dw_kernel_pools(DwKernel k) {
+  return k == DW_TMA || k == DW_TMA_DIL || k == DW_STRIP_16B || k == DW_STRIP_F32 || k == DW_5X5_POOL_16B;
+}
 
 constexpr int kDwOW = 4;  // outputs per thread along W in dwconv3x3_pool_16b_kernel (measured: 4 -> 3.65 ms, 2 -> 4.25 ms per 128 crops)
 constexpr int kDw5OW = 4;  // outputs per thread along W in dwconv5x5_16b_kernel
@@ -839,10 +845,23 @@ cudaError_t dw_dispatch(const Op& op, F&& f) {
 // Picks the kernel of a depthwise op and the number of partial pooling slices it writes (fc1 sums that many).  bf16 and fp16
 // tensor-core modes: 5x5 ops run dwconv5x5_16b_kernel, which pools for SiLU (EfficientNet-B) and does not pool for ReLU /
 // hard-swish (MobileNetV3); 3x3 stride-1 ops run the TMA-staged kernel when a plan fits, the other 3x3 ops the 16-bit strip
-// kernel.  3xTF32 mode: the fp32 strip kernel (exact activation) for 3x3 ops.  Other modes and shapes: the generic kernel,
-// which does not pool.
+// kernel; 3x3 stride-1 SiLU ops with dilation 2 or 4 and SAME padding (the dilated EfficientNetV2 stages) run the TMA-staged
+// kernel phase by phase when a plan fits.  3xTF32 mode: the fp32 strip kernel (exact activation) for undilated 3x3 ops.  Other
+// modes and shapes: the generic kernel, which does not pool.
 void choose_dw_kernel(const mtb_handle* h, Op& op) {
   op.dw_kernel = DW_GENERIC;
+  if (op.type == OP_DW && op.R == 3 && op.S == 3 && (op.dil == 2 || op.dil == 4)) {
+    if (!is_tc16(h) || op.stride != 1 || op.act != ACT_SILU || op.Cout % 8 != 0 || op.pad_t != op.dil || op.pad_l != op.dil ||
+        op.Hin != op.Hout || op.Win != op.Wout)
+      return;
+    const DwTmaPlan pl = dw_tma_plan((op.Hout + op.dil - 1) / op.dil, (op.Wout + op.dil - 1) / op.dil, op.dil);
+    if (pl.ok && pl.n_rb <= kPoolSlices) {
+      op.dw_kernel = DW_TMA_DIL;
+      op.dw_plan = pl;
+      op.pool_slices = pl.n_rb;
+    }
+    return;
+  }
   if (dw5x5_eligible(op)) {
     if (!is_tc16(h)) return;
     if (op.act != ACT_SILU) {
@@ -967,12 +986,12 @@ int run_op_t(mtb_handle* h, const Op& op, const float* crops, int B, const Works
       p.res_first = op.res_first ? 1 : 0;
       if (op.type == OP_DW) {
         float* pooled = op.fused_pool ? (float*)buf_ptr(ws, BUF_SMALL0, features) : nullptr;
-        if (op.dw_kernel == DW_TMA || op.dw_kernel == DW_STRIP_16B) {
+        if (op.dw_kernel == DW_TMA || op.dw_kernel == DW_TMA_DIL || op.dw_kernel == DW_STRIP_16B) {
           if constexpr (!k16) {
             return fail(h, MTB_ERR_CUDA, "depthwise %s: 16-bit kernel chosen for fp32 storage", op.name.c_str());
-          } else if (op.dw_kernel == DW_TMA) {
+          } else if (op.dw_kernel == DW_TMA || op.dw_kernel == DW_TMA_DIL) {
             const char* e = dw_tma_launch<T>(op.dw_maps, op.dw_plan, p.in, p.out, op.d_w, op.d_bias, pooled, B, op.Hout, op.Wout,
-                                             op.Cout, op.pad_t, op.pad_l, op.act, st);
+                                             op.Cout, op.pad_t, op.pad_l, op.act, op.dw_kernel == DW_TMA ? 1 : op.dil, st);
             if (e) return fail(h, MTB_ERR_CUDA, "depthwise (TMA) launch %s: %s", op.name.c_str(), e);
           } else {
             const dim3 grid((op.Cout / 8 + 31) / 32, op.pool_slices, B), block(32, 8);
@@ -1319,6 +1338,23 @@ int mtb_create(const mtb_config* cfg, mtb_handle** out) {
         return fail(nullptr, MTB_ERR_UNSUPPORTED, "MTB_ARCH_EFFNET_EPS1E5 stage %d: only MBConv rows with kernel 3 or 5 and "
                     "stride 1 or 2 (got block %d, kernel %d, stride %d)", i, s.block, s.kernel, s.stride);
     }
+  if (effnet) {
+    int out_stride = 2;
+    for (int i = 0; i < cfg->n_stages; ++i) {
+      const mtb_stage& s = cfg->stages[i];
+      if (s.dilation_in < 1 || s.dilation_in > 8 || s.dilation_out < 1 || s.dilation_out > 8)
+        return fail(nullptr, MTB_ERR_UNSUPPORTED, "stage %d: dilation %d / %d outside 1..8", i, s.dilation_in, s.dilation_out);
+      if (s.block == 0 && (s.dilation_in > 1 || s.dilation_out > 1))
+        return fail(nullptr, MTB_ERR_UNSUPPORTED, "stage %d: FusedMBConv rows are not dilated (dilation %d / %d); only the "
+                    "output strides 32, 16 and 8 of EfficientNetV2 are built", i, s.dilation_in, s.dilation_out);
+      out_stride *= s.stride;
+    }
+    // stride-32 tables run whatever stride_test says (as before dilation existed); a dilated table decodes its finer heatmap
+    // with the geometry of stride_test, so the two must agree
+    if (out_stride < 32 && out_stride != cfg->stride_test)
+      return fail(nullptr, MTB_ERR_INVALID_ARG, "the stage table has output stride %d but stride_test is %d: set "
+                  "Config(stride_test=%d) for this backbone", out_stride, cfg->stride_test, out_stride);
+  }
   if (cfg->precision < MTB_PRECISION_FP32 || cfg->precision > MTB_PRECISION_F16_SIMT)
     return fail(nullptr, MTB_ERR_INVALID_ARG, "unknown precision %d", cfg->precision);
   int ndev = 0;

@@ -48,6 +48,7 @@ def make_config(cfg, n_joints, stages=None, last_channel=0, arch=_lib.ARCH_EFFNE
         s.expand, s.kernel, s.stride = st['expand'], st['kernel'], st['stride']
         s.cin, s.cout, s.layers = st['cin'], st['cout'], st['layers']
         s.bottomright = int(bool(st['bottomright']))
+        s.dilation_in, s.dilation_out = st.get('dilation_in', 1), st.get('dilation_out', 1)
     return c
 
 
@@ -316,7 +317,7 @@ class Engine:
 
     def op_dw_kernel(self, op):
         """The kernel finalize chose for depthwise op `op`: one of _lib.DW_GENERIC, DW_TMA, DW_STRIP_16B, DW_STRIP_F32,
-        DW_5X5_16B, DW_5X5_POOL_16B."""
+        DW_5X5_16B, DW_5X5_POOL_16B, DW_TMA_DIL."""
         k = lib().mtb_op_dw_kernel(self._h, op)
         if k < 0:
             check(k, self._h)
