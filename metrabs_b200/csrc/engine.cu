@@ -940,8 +940,8 @@ int run_op_t(mtb_handle* h, const Op& op, const float* crops, int B, const Works
              cudaStream_t st) {
   constexpr bool k16 = sizeof(T) == 2;
   if constexpr (k16) {
-    if (op.type == OP_CONV && op.tc.ready && op.scale_buf != BUF_NONE) {
-      // squeeze-excitation scale applied in place ahead of the 16-bit tensor-core conv
+    if (op.type == OP_CONV && op.tc.ready && op.scale_buf != BUF_NONE && !tc_se_in_gemm(op.Cout)) {
+      // squeeze-excitation scale applied in place ahead of a 16-bit tensor-core conv that does not apply it itself
       void* x = buf_ptr(ws, op.in_buf, features);
       const double bytes = 2.0 * B * op.Hin * op.Win * op.Cin * elem_size(h);
       ProfScope ps(h, KC_SE_SCALE, 0.0, bytes, st, false);
@@ -1056,6 +1056,7 @@ int run_op_t(mtb_handle* h, const Op& op, const float* crops, int B, const Works
       } else if (op.tc.ready) {
         if constexpr (!k16) return fail(h, MTB_ERR_CUDA, "%s: tensor-core weights in an fp32 mode", op.name.c_str());
         else {
+          if (!tc_se_in_gemm(op.Cout)) p.a_scale = nullptr;  // already applied by se_scale_kernel
           const char* e = tc_conv_launch<T>(op.tc, p, op.res_first, st);
           if (e) return fail(h, MTB_ERR_CUDA, "tensor-core launch %s: %s", op.name.c_str(), e);
         }

@@ -67,6 +67,14 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if (clock64() - t0 > 8000000000LL) __trap();  // ~4 s at 2 GHz
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+__device__ __forceinline__ uint4 ld_shared_u4(uint32_t addr) {
+  uint4 v;
+  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_shared_u4(uint32_t addr, const uint4& v) {
+  asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 // named barrier of one consumer warpgroup (ids 1, 2; id 0 is __syncthreads)
 __device__ __forceinline__ void wg_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
@@ -99,6 +107,7 @@ __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.comm
 // the shared-memory source of every committed bulk store has been read (it may be overwritten)
 __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+__device__ __forceinline__ void prefetch_l1(const void* p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
@@ -151,7 +160,8 @@ struct TcConvParams {
   int m_tiles, n_tiles;  // tc_conv_kernel's tile grid (tile t = m_blk * n_tiles + n_blk)
 };
 
-// warpgroup register budgets of tc_conv_kernel: 128 x 40 + 256 x 232 = 64512 of the SM's 65536 registers
+// warpgroup register budgets of tc_conv_kernel: 128 x 40 + 256 x 232 = 64512 of the SM's 65536 registers; the SE instances,
+// whose warpgroup 0 also scales the A tiles: 128 x 56 + 256 x 224 = 64512
 template <int R>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 template <int R>
@@ -311,9 +321,99 @@ __device__ __forceinline__ void tc_tile_epilogue(const float* acc, uint8_t* stg,
   }
 }
 
+// Squeeze-excitation scale of the landed mode-0 A tiles (128 rows of the flat [M][Cin] input from row m0, 64 channels per
+// k-block), in place: x[m][k] = round16(x[m][k] * s[m / P][k]), the fp32 product rounded to nearest even, so the wgmma reads
+// the bits a separate in-place pass over the tensor would have stored.  Transform thread u (0..95) owns logical 16-byte chunk
+// L = u % 8 (8 channels) of the contiguous rows [r0, r1) of row block u / 8 (12 blocks of 11 or 10 rows); SWIZZLE_128B puts
+// that chunk at physical chunk L ^ (r & 7) of row r.  A warp's 32 accesses then cover four whole 128-byte rows (no bank
+// conflicts), and a block of 11 rows spans at most two crops, ca and cb, when P >= 10: the thread loads both crops' 8
+// scales before it waits for the stage, and prefetches those of its next k-block into L1.  Crops strictly between them
+// (maps below 10 pixels) load their scales row by row.  Rows m >= M and channels k >= Cin are the TMA's zero fill and are
+// left alone (Cin % 8 == 0: a chunk lies wholly inside or outside Cin).
+struct SeRows {
+  int r0, r1;  // the thread's rows of the tile, r1 clipped to the M tail (r1 <= r0: none)
+  int ca, cb;  // crops of rows r0 and r1 - 1
+};
+__device__ __forceinline__ SeRows se_rows(int u, int m0, int M, int P) {
+  const int g = u >> 3;
+  SeRows w;
+  w.r0 = 10 * g + min(g, 8);
+  w.r1 = min(w.r0 + (g < 8 ? 11 : 10), M - m0);
+  w.ca = (m0 + w.r0) / P;
+  w.cb = (m0 + max(w.r1, w.r0 + 1) - 1) / P;
+  return w;
+}
+template <typename T>
+__device__ __forceinline__ void se_scale_chunk(uint32_t addr, const float4& s0, const float4& s1) {
+  typedef typename Pair16<T>::type T2;
+  uint4 v = ld_shared_u4(addr);
+  T2* v2 = reinterpret_cast<T2*>(&v);
+  float2 f = Pair16<T>::unpack(v2[0]);
+  v2[0] = Pair16<T>::pack(f.x * s0.x, f.y * s0.y);
+  f = Pair16<T>::unpack(v2[1]);
+  v2[1] = Pair16<T>::pack(f.x * s0.z, f.y * s0.w);
+  f = Pair16<T>::unpack(v2[2]);
+  v2[2] = Pair16<T>::pack(f.x * s1.x, f.y * s1.y);
+  f = Pair16<T>::unpack(v2[3]);
+  v2[3] = Pair16<T>::pack(f.x * s1.z, f.y * s1.w);
+  st_shared_u4(addr, v);
+}
+// rows [rb, re) of chunk L with one crop's scales, two rows per step so that their shared-memory loads overlap
+template <typename T>
+__device__ __forceinline__ void se_scale_rows(uint32_t a, int L, int rb, int re, const float4& s0, const float4& s1) {
+  typedef typename Pair16<T>::type T2;
+  int r = rb;
+#pragma unroll 1
+  for (; r + 1 < re; r += 2) {
+    const uint32_t p0 = a + r * 128 + ((L ^ (r & 7)) << 4), p1 = a + (r + 1) * 128 + ((L ^ ((r + 1) & 7)) << 4);
+    uint4 v = ld_shared_u4(p0), w = ld_shared_u4(p1);
+    T2* v2 = reinterpret_cast<T2*>(&v);
+    T2* w2 = reinterpret_cast<T2*>(&w);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float sx = j < 2 ? (j == 0 ? s0.x : s0.z) : (j == 2 ? s1.x : s1.z);
+      const float sy = j < 2 ? (j == 0 ? s0.y : s0.w) : (j == 2 ? s1.y : s1.w);
+      const float2 f = Pair16<T>::unpack(v2[j]), g = Pair16<T>::unpack(w2[j]);
+      v2[j] = Pair16<T>::pack(f.x * sx, f.y * sy);
+      w2[j] = Pair16<T>::pack(g.x * sx, g.y * sy);
+    }
+    st_shared_u4(p0, v);
+    st_shared_u4(p1, w);
+  }
+  if (r < re) se_scale_chunk<T>(a + r * 128 + ((L ^ (r & 7)) << 4), s0, s1);
+}
+// One stage: k-block kb's A tile at shared address a, landing on `full` with parity `ph`; waits for it in every case.
+template <typename T>
+__device__ __forceinline__ void se_scale_a_tile(uint32_t a, uint64_t* full, uint32_t ph, const SeRows& w, const float* __restrict__ s, int m0,
+                                                int P, int Cin, int kb, int u) {
+  const int L = u & 7, k = kb * TC_BK + 8 * L;
+  if (k >= Cin || w.r1 <= w.r0) {
+    mbar_wait(full, ph);
+    return;
+  }
+  const float4* sa = reinterpret_cast<const float4*>(s + (size_t)w.ca * Cin + k);
+  const float4* sb = reinterpret_cast<const float4*>(s + (size_t)w.cb * Cin + k);
+  const float4 a0 = __ldg(sa), a1 = __ldg(sa + 1), b0 = __ldg(sb), b1 = __ldg(sb + 1);
+  if (k + TC_BK < Cin) {  // the next k-block's scales, into L1 a whole stage ahead of their loads
+    prefetch_l1(sa + TC_BK / 4);
+    prefetch_l1(sb + TC_BK / 4);
+  }
+  mbar_wait(full, ph);
+  const int ra = min((w.ca + 1) * P - m0, w.r1);        // first row past crop ca
+  const int rb = max(min(w.cb * P - m0, w.r1), ra);     // first row of crop cb (when cb > ca)
+  se_scale_rows<T>(a, L, w.r0, ra, a0, a1);
+#pragma unroll 1
+  for (int r = ra; r < rb; ++r) {                       // crops between ca and cb: maps of fewer than 10 pixels
+    const float4* sr = reinterpret_cast<const float4*>(s + (size_t)((m0 + r) / P) * Cin + k);
+    se_scale_chunk<T>(a + r * 128 + ((L ^ (r & 7)) << 4), __ldg(sr), __ldg(sr + 1));
+  }
+  se_scale_rows<T>(a, L, rb, w.r1, b0, b1);
+}
+
 // Persistent conv / GEMM kernel.  ACT: epilogue activation; RES: 0 no residual, 1 residual added AFTER the activation
 // (EfficientNet), 2 BEFORE (ResNet); BN: output channels per tile (wgmma N); T: operand and activation element type
-// (__nv_bfloat16 or __half).
+// (__nv_bfloat16 or __half); SE (mode 0 only): scale the A rows by the squeeze-excitation vector of their crop,
+// a_scale [B][Cin] (crop of row m: m / (Hin * Win)), in shared memory before the consumers read them.
 //
 // CTA b walks tiles t = b, b + gridDim.x, ...; tile t is (m_blk, n_blk) = (t / n_tiles, t % n_tiles): N fastest, so the CTAs
 // running at the same time cover every N tile of a few M blocks and each A tile comes from HBM once, the re-reads from L2.
@@ -322,16 +422,24 @@ __device__ __forceinline__ void tc_tile_epilogue(const float* acc, uint8_t* stg,
 // barrier orders their main loops: a consumer starts waiting on its tile's stages only after the other finished the previous
 // tile's, which keeps every mbarrier wait within one phase of the barrier, and lets one warpgroup's epilogue run under the
 // other's MMAs.  Every output element sees the wgmma sequence and the roundings of a one-CTA-per-tile kernel.
-template <typename T, int ACT, int RES, int BN>
+//
+// With SE, warps 1-3 of warpgroup 0 walk the producer's (tile, k-block) sequence too: wait for full[s], scale the stage's A
+// tile in place (se_scale_a_tile), fence the generic-proxy writes for the wgmma's async proxy, and arrive on ready[s] (one
+// arrive per warp); the consumers wait on ready[s] instead of full[s].  The parities stay in phase: full[s] completes phase
+// k + 1 only after the producer saw empty[s] complete phase k, which needs the consumers to have taken ready[s] phase k,
+// which needs every transform warp to have finished phase k; so no barrier runs more than one phase ahead of its waiters.
+template <typename T, int ACT, int RES, int BN, bool SE = false>
 __global__ void __launch_bounds__(TCP_THREADS, 1)
 tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
-               const TcConvParams p) {
+               const TcConvParams p, const float* __restrict__ a_scale) {
   using Ring = TcRing<BN>;
   constexpr int STAGES = Ring::stages;
   extern __shared__ uint8_t tc_smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)tc_smem_raw + 1023) & ~(uintptr_t)1023);  // SWIZZLE_128B needs 1024 B alignment
   uint64_t* full = (uint64_t*)(smem + Ring::bar_off);
   uint64_t* empty = full + STAGES;
+  uint64_t* ready = empty + STAGES;  // SE only: the stage's A tile is scaled
+  uint64_t* landed = SE ? ready : full;  // what the consumers wait for
 
   const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
@@ -341,16 +449,17 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full[i], 1);  // the producer's arrive.expect_tx
       mbar_init(&empty[i], 4); // one arrive per warp of the consuming warpgroup
+      if constexpr (SE) mbar_init(&ready[i], 3);  // one arrive per transform warp
     }
     fence_barrier_init();
   }
   __syncthreads();
 
   const int tiles = p.m_tiles * p.n_tiles;
-  const int num_kb = p.taps * p.kchunks;
+  const int num_kb = SE ? p.kchunks : p.taps * p.kchunks;  // SE: mode 0, one tap; read as is, warpgroup 0 would spill the product
   if (wg == 0) {
     // ===== TMA producer =====
-    setmaxnreg_dec<40>();
+    setmaxnreg_dec<SE ? 56 : 40>();
     if (threadIdx.x == 0) {
       int it = 0;
       for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
@@ -365,11 +474,28 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           tma_load_2d(sa + TC_A_BYTES, &tmB, &full[s], tap * p.Cin + kc * TC_BK, n_blk * BN);
         }
       }
+    } else if constexpr (SE) {
+      if (threadIdx.x >= 32) {
+        // ===== warps 1-3: squeeze-excitation scale of each landed A tile (mode 0: k-block kb = channel chunk kb) =====
+        const int u = threadIdx.x - 32, P = p.Hin * p.Win;
+        int it = 0;
+        for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+          const int m0 = (t / p.n_tiles) * TC_BM;
+          const SeRows w = se_rows(u, m0, p.M, P);
+          for (int kb = 0; kb < num_kb; ++kb, ++it) {
+            const int s = it % STAGES;
+            se_scale_a_tile<T>(smem_u32(smem + s * Ring::stage_bytes), &full[s], (it / STAGES) & 1, w, a_scale, m0, P, p.Cin, kb, u);
+            fence_proxy_async();  // generic-proxy writes -> visible to the wgmma (async proxy)
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&ready[s]);
+          }
+        }
+      }
     }
     return;
   }
   // ===== consumers: warpgroup 1 + c computes the CTA's tiles c, c + 2, ... (rows [0, 64) in acc, [64, 128) in acc + BN/2) =====
-  setmaxnreg_inc<232>();
+  setmaxnreg_inc<SE ? 224 : 232>();
   const int c = wg - 1;
   for (int i = c, t = blockIdx.x + c * gridDim.x; t < tiles; i += 2, t += 2 * gridDim.x) {
     const int m_blk = t / p.n_tiles, n_blk = t - m_blk * p.n_tiles;
@@ -380,7 +506,7 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     int it = i * num_kb, prev = -1;
     for (int kb = 0; kb < num_kb; ++kb, ++it) {
       const int s = it % STAGES;
-      mbar_wait(&full[s], (it / STAGES) & 1);
+      mbar_wait(&landed[s], (it / STAGES) & 1);
       const uint32_t a = smem_u32(smem + s * Ring::stage_bytes);
       const uint32_t b = smem_u32(smem + s * Ring::stage_bytes + TC_A_BYTES);
       wgmma_fence();
@@ -700,6 +826,11 @@ inline const char* tc_prepare_weights(TcWeights& w, const float* wk, const float
 
 // N-tile width: the narrowest wgmma N in {32, 64, 128} that covers Cout, else 128 (Cout > 128 runs several N tiles)
 inline int tc_pick_bn(int cout) { return cout <= 32 ? 32 : cout <= 64 ? 64 : 128; }
+// Where a 1x1 projection's squeeze-excitation scale is applied: inside tc_conv_kernel (SE instances) when the GEMM has at
+// most two N tiles (Cout <= 256), else by se_scale_kernel in place ahead of it.  The GEMM scales its A tile once per N tile,
+// in warps whose throughput bounds the projection: at 2 N tiles that costs less than the separate pass's read and write of
+// the tensor, at 3 and 5 (EfficientNetV2-L stages 6 and 7, Cout 384 and 640) more (DESIGN.md section 2).
+inline bool tc_se_in_gemm(int cout) { return cout <= 256; }
 
 // T: the storage type the weights were prepared in (tc_prepare_weights<T>)
 template <typename T>
@@ -715,6 +846,8 @@ inline const char* tc_conv_launch(const TcWeights& w, const ConvParams& p, bool 
   q.tiles_w = (p.Wout + TC_TILE_W - 1) / TC_TILE_W;
   q.tiles_h = (p.Hout + TC_TILE_H - 1) / TC_TILE_H;
   q.M = p.B * p.Hout * p.Wout;
+  if (p.a_scale && (q.mode != 0 || !tc_se_in_gemm(p.Cout)))
+    return "squeeze-excitation scale outside the 1x1 projections tc_conv_kernel scales (tc_se_in_gemm)";
   // tc_conv3x3s1_kernel for the shapes it takes (bn: its K per tap and N tile), tc_conv_kernel for every other conv
   const bool s1 = tc3x3s1_eligible(p.R, p.S, p.stride, p.dil, p.Cin, p.Cout, p.act);
   const int bn = s1 ? tc3x3s1_width(p.Cin, p.Cout) : tc_pick_bn(p.Cout);
@@ -751,10 +884,20 @@ inline const char* tc_conv_launch(const TcWeights& w, const ConvParams& p, bool 
         });
       });
     });
+  if (p.a_scale)  // the MBConv / MobileNetV3 projections: no activation, residual after it or none
+    return with_const<ACT_NONE>(p.act, "unsupported activation with a squeeze-excitation scale", [&](auto act) {
+      return with_const<0, 1>(res_mode, "unsupported residual mode with a squeeze-excitation scale", [&](auto res) {
+        return with_const<32, 64, 128>(bn, "unsupported N tile", [&](auto bn_) {
+          return launch_smem(tc_conv_kernel<T, act, res, bn_, true>, grid, dim3(TCP_THREADS), TcRing<bn_>::smem_bytes, st, m[0], m[1], m[2],
+                             q, p.a_scale);
+        });
+      });
+    });
   return with_const<ACT_NONE, ACT_SILU, ACT_RELU, ACT_HSWISH>(p.act, "unsupported activation in the tensor-core epilogue", [&](auto act) {
     return with_const<0, 1, 2>(res_mode, "unsupported residual mode", [&](auto res) {
       return with_const<32, 64, 128>(bn, "unsupported N tile", [&](auto bn_) {
-        return launch_smem(tc_conv_kernel<T, act, res, bn_>, grid, dim3(TCP_THREADS), TcRing<bn_>::smem_bytes, st, m[0], m[1], m[2], q);
+        return launch_smem(tc_conv_kernel<T, act, res, bn_>, grid, dim3(TCP_THREADS), TcRing<bn_>::smem_bytes, st, m[0], m[1], m[2], q,
+                           (const float*)nullptr);
       });
     });
   });
