@@ -311,6 +311,12 @@ int mtb_debug_run_ops(mtb_handle* h, const float* crops, int batch, int n_ops, f
 int mtb_op_output_shape(const mtb_handle* h, int op, int* height, int* width, int* channels);
 int mtb_op_input_shape(const mtb_handle* h, int op, int* height, int* width, int* channels, int* has_residual,
                        int* has_scale);
+/* The workspace buffers the forward's planner gave backbone op `op`: its input, its output, its residual and its
+ * squeeze-excitation scale.  Ids: -2 the feature output, -1 none (the stem's input: it reads the crops), 0-3 the large
+ * activation buffers, 4-6 the small [B,C] ones.  An operand of op k is the output of the latest op j < k whose out_buf is that id (not always k - 1: a projection
+ * reads the depthwise output before the SE ops, its residual is the block input), so a test can take an op's operands
+ * from mtb_debug_run_ops prefixes.  Any output pointer may be null.  MTB_ERR_INVALID_ARG for an index out of range. */
+int mtb_debug_op_buffers(const mtb_handle* h, int op, int* in_buf, int* out_buf, int* res_buf, int* scale_buf);
 /* Runs ONE backbone op in isolation on caller-provided fp32 NHWC device tensors (converted to the handle's
  * storage type - fp32, or bf16 / fp16 rounded to nearest even): in [B,Hin,Win,Cin] (the stem takes NCHW crops), optional residual [B,Hout,Wout,Cout] and
  * squeeze-excitation scale [B,Cin]; out receives [B,Hout,Wout,Cout] as fp32.  Lets tests compare the tensor-core

@@ -2248,6 +2248,16 @@ int mtb_op_is_fused_block(const mtb_handle* h, int op_index) {
   return (h && op_index >= 0 && op_index + 1 < (int)h->ops.size() && h->ops[op_index].fmb.ready) ? 1 : 0;
 }
 
+int mtb_debug_op_buffers(const mtb_handle* h, int op, int* in_buf, int* out_buf, int* res_buf, int* scale_buf) {
+  if (!h || op < 0 || op >= (int)h->ops.size()) return fail(h, MTB_ERR_INVALID_ARG, "op index out of range");
+  const Op& o = h->ops[op];
+  if (in_buf) *in_buf = o.in_buf;
+  if (out_buf) *out_buf = o.out_buf;
+  if (res_buf) *res_buf = o.res_buf;
+  if (scale_buf) *scale_buf = o.scale_buf;
+  return MTB_OK;
+}
+
 int mtb_debug_run_fused_block(mtb_handle* h, int op_index, const float* in, int batch, float* out, size_t out_floats, void* workspace,
                               size_t workspace_bytes, void* stream) {
   int rc = check_common(h, batch, workspace_bytes, workspace);

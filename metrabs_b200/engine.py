@@ -301,6 +301,13 @@ class Engine:
         return dict(in_shape=(a[0].value, a[1].value, a[2].value), out_shape=(o[0].value, o[1].value, o[2].value),
                     residual=bool(a[3].value), scale=bool(a[4].value))
 
+    def op_buffers(self, op):
+        """-> dict(input=, output=, residual=, scale=) workspace buffer ids of backbone op `op` in the forward
+        (mtb_debug_op_buffers): _lib.BUF_FEATURES, _lib.BUF_NONE, 0-3 the large buffers, 4-6 the small ones."""
+        a = [C.c_int() for _ in range(4)]
+        check(lib().mtb_debug_op_buffers(self._h, op, *[C.byref(x) for x in a]), self._h)
+        return dict(zip(('input', 'output', 'residual', 'scale'), (x.value for x in a)))
+
     def debug_run_op(self, op, x, res=None, scale=None):
         """One op in isolation on fp32 device tensors (NHWC; the stem takes NCHW crops)."""
         io = self.op_io(op)
