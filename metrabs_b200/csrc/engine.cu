@@ -98,6 +98,7 @@ struct mtb_handle {
   std::map<std::string, HostTensor> raw;
   std::vector<Op> ops;
   Op head;
+  bool head_fused = false;  // tc_head_kernel + head_finalize_kernel (tc_head_plan fits the feature map); else the unfused head
   // latent-point model (mtb_set_latent_recombination): the forward reconstructs head points [0, n_latents) and maps them to
   // n_out joints with recomb [n_latents][n_out]; n_latents == 0 for a plain model
   int n_latents = 0, n_out = 0;
@@ -1168,7 +1169,7 @@ int head_decode_impl(mtb_handle* h, const void* features, int B, float* c2d, flo
   const double feat_bytes = (double)B * P * op.Cin * elem_size(h);
   const int J = head_points(h);
   const double out_bytes = (double)B * J * 5 * 4;
-  if (op.tc.ready) {
+  if (h->head_fused) {
     // fused: 1x1-conv GEMM on the tensor cores with the soft-argmax reduction in the epilogue; logits never reach HBM
     ProfScope prof(h, KC_HEAD_FUSED, op.flops * B, feat_bytes + (double)op.Cin * op.Cout * 2 + out_bytes, st);
     const char* e = with_storage16(h, [&](auto* tag) {
@@ -1537,6 +1538,7 @@ int mtb_finalize_weights(mtb_handle* h) {
           return tc_prepare_head<std::remove_pointer_t<decltype(tag)>>(hd.tc, w0.data(), b0.data(), hd.Cin, n_real, h->dev_allocs);
         });
         if (e) return fail(h, MTB_ERR_CUDA, "tensor-core head weight prep: %s", e);
+        h->head_fused = true;
       }
     }
   }

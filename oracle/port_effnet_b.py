@@ -144,17 +144,13 @@ def conv_layer_reference(sd, spec, name, x_nhwc, res_nhwc=None, scale=None, prec
 
 def layer_bound(sd, spec, name, x_nhwc, res_nhwc=None, scale=None, precision='fp16'):
     """port_ops.layer_bound for the ops of ``spec``: -> (ref, tol), NHWC fp64, with the same bound
-    tol = 2^-p (|ref| + e) + e + floor, e = L_act C_ACC (K + 4) 2^-24 refabs + e_act + 2^-23 |ref|.
-    (port_mobilenet._layer is the op-dict form of port_ops._layer: no max pool or dilation, residual after the activation,
+    tol = 2^-p (|ref| + e) + e + floor, e = L_act C_ACC (K + 4) 2^-24 refabs + e_act + 2^-23 |ref| (any engine mode:
+    port_ops.bound_from_parts).  (port_mobilenet._layer is the op-dict form of port_ops._layer: no max pool or dilation, residual after the activation,
     which is also what an MBConv op needs.)"""
-    st = port_ops.MODES[precision][0]
     op = op_table(spec)[name]
     y, z, k = port_mobilenet._layer(sd, op, x_nhwc, res_nhwc, scale, precision, torch.float64)
     zabs = port_mobilenet._layer(sd, op, x_nhwc, res_nhwc, scale, precision, torch.float64, magnitude=True)[1]
-    a = port_ops._act(z, op['act'])
-    e = (port_ops.LIPSCHITZ[op['act']] * port_ops.C_ACC * (k + 4) * 2.0 ** -24 * zabs
-         + port_ops._act_error(z, a, op['act'], precision) + 2.0 ** -23 * y.abs())
-    p = 8 if st == torch.bfloat16 else 11
-    tol = 2.0 ** -p * (y.abs() + e) + e + (2.0 ** -25 if st == torch.float16 else 0.0)
+    tc32 = precision == 'tf32x3' and port_ops.tc32_eligible(op, x_nhwc.shape[-1], y.shape[1])
+    tol = port_ops.bound_from_parts(z, y, zabs, k, op['act'], precision, tc32)
     nhwc = lambda t: t.permute(0, 2, 3, 1).contiguous()  # noqa: E731
     return nhwc(y), nhwc(tol)

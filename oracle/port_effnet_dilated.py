@@ -207,7 +207,6 @@ def op_table(spec, prefix='backbone.1'):
 def dw_layer_bound(sd, spec, name, x_nhwc, precision='fp16'):
     """port_ops.layer_bound for a (dilated) depthwise op of ``spec``: the exact layer on this mode's rounded operands and
     the same per-element bound, tol = 2^-p (|ref| + e) + e + floor.  -> (ref, tol), NHWC fp64."""
-    st = port_ops.MODES[precision][0]
     op = op_table(spec)[name]
     assert op['depthwise'] and op['act'] == 'silu', name
     w, bias = (t.float().double().to(x_nhwc.device) for t in port_ops._fold(sd, op))
@@ -217,9 +216,6 @@ def dw_layer_bound(sd, spec, name, x_nhwc, precision='fp16'):
     zabs = conv(x.abs(), w.abs(), bias.abs())
     y = port_ops._act(z, 'silu')
     k = w.shape[2] * w.shape[3]
-    e = (port_ops.LIPSCHITZ['silu'] * port_ops.C_ACC * (k + 4) * 2.0 ** -24 * zabs + port_ops._act_error(z, y, 'silu', precision)
-         + 2.0 ** -23 * y.abs())
-    p = 8 if st == torch.bfloat16 else 11
-    tol = 2.0 ** -p * (y.abs() + e) + e + (2.0 ** -25 if st == torch.float16 else 0.0)
+    tol = port_ops.bound_from_parts(z, y, zabs, k, 'silu', precision)
     nhwc = lambda t: t.permute(0, 2, 3, 1).contiguous()  # noqa: E731
     return nhwc(y), nhwc(tol)

@@ -153,9 +153,9 @@ def _layer(sd, op, x_nhwc, res_nhwc, scale, precision, dtype, magnitude=False):
     dev = x_nhwc.device
     w, bias = port_ops._fold(sd, op)
     st = port_ops.MODES[precision][0] if precision in port_ops.MODES else None
-    if st is not None:  # folded in fp64, cast to fp32, GEMM weights rounded once to 16 bits
+    if st is not None or precision in port_ops.WIDE_MODES:  # folded in fp64, cast to fp32, GEMM weights rounded once to 16 bits
         w, bias = w.float().double(), bias.float().double()
-        if port_ops.tc_eligible(op, w.shape[1], w.shape[0]):
+        if st is not None and port_ops.tc_eligible(op, w.shape[1], w.shape[0]):
             w = w.float().to(st).double()
     w, bias = w.to(dev, dtype), bias.to(dev, dtype)
     if op['stem']:
@@ -168,6 +168,8 @@ def _layer(sd, op, x_nhwc, res_nhwc, scale, precision, dtype, magnitude=False):
         s = scale.to(dev, dtype)[:, :, None, None]
         if st is not None and port_ops.MODES[precision][1] and not magnitude:  # se_scale_kernel: fp32 product, rounded
             x = (x.float() * s.float()).to(st).to(dtype)
+        elif precision in port_ops.WIDE_MODES and not magnitude:  # fp32 product, no further rounding
+            x = (x.float() * s.float()).to(dtype)
         else:
             x = x * s
     if magnitude:
@@ -188,15 +190,12 @@ def conv_layer_reference(sd, spec, name, x_nhwc, res_nhwc=None, scale=None, prec
 
 def layer_bound(sd, spec, name, x_nhwc, res_nhwc=None, scale=None, precision='fp16'):
     """port_ops.layer_bound for the ops of ``spec`` (either variant): -> (ref, tol), NHWC fp64, with the same bound
-    tol = 2^-p (|ref| + e) + e + floor, e = L_act C_ACC (K + 4) 2^-24 refabs + e_act + 2^-23 |ref|."""
-    st = port_ops.MODES[precision][0]
+    tol = 2^-p (|ref| + e) + e + floor, e = L_act C_ACC (K + 4) 2^-24 refabs + e_act + 2^-23 |ref| (any engine mode:
+    port_ops.bound_from_parts)."""
     op = op_table(spec)[name]
     y, z, k = _layer(sd, op, x_nhwc, res_nhwc, scale, precision, torch.float64)
     zabs = _layer(sd, op, x_nhwc, res_nhwc, scale, precision, torch.float64, magnitude=True)[1]
-    a = port_ops._act(z, op['act'])
-    e = (port_ops.LIPSCHITZ[op['act']] * port_ops.C_ACC * (k + 4) * 2.0 ** -24 * zabs
-         + port_ops._act_error(z, a, op['act'], precision) + 2.0 ** -23 * y.abs())
-    p = 8 if st == torch.bfloat16 else 11
-    tol = 2.0 ** -p * (y.abs() + e) + e + (2.0 ** -25 if st == torch.float16 else 0.0)
+    tc32 = precision == 'tf32x3' and port_ops.tc32_eligible(op, x_nhwc.shape[-1], y.shape[1])
+    tol = port_ops.bound_from_parts(z, y, zabs, k, op['act'], precision, tc32)
     nhwc = lambda t: t.permute(0, 2, 3, 1).contiguous()  # noqa: E731
     return nhwc(y), nhwc(tol)

@@ -20,6 +20,9 @@ of with another kernel of this repository.  The ResNet-50 and MobileNetV3-small 
     (``conv_igemm_kernel`` a_scale, csrc/conv_simt.cuh:97-99);
   - everything else is wide; the device rounds the result once to 16 bits.
   ``layer_bound`` gives the per-element tolerance of that device result; ``'bf16'`` alone keeps its old meaning.
+* ``'fp32'``, ``'tf32x3'``: the fp32-storage modes.  The folded weights are cast to fp32 and not rounded further (the
+  3xTF32 kernel splits them into hi / lo planes whose sum is the fp32 weight, tc_tf32.cuh tc32_prepare_weights); the SE
+  product ``x*s`` is formed in fp32 (``t32_split_a`` and ``conv_igemm_kernel`` a_scale) and not rounded further.
 """
 import math
 
@@ -32,6 +35,13 @@ from oracle import port_tf_backbones as tfb
 # engine mode -> (16-bit storage dtype, tensor-core kernels)
 MODES = {'bf16': (torch.bfloat16, True), 'bf16_simt': (torch.bfloat16, False),
          'fp16': (torch.float16, True), 'fp16_simt': (torch.float16, False)}
+# the fp32-storage modes: 'fp32' (CUDA-core FMA) and 'tf32x3' (tc32_conv_kernel on its eligible convs, CUDA cores elsewhere)
+WIDE_MODES = {'fp32': (torch.float32, False), 'tf32x3': (torch.float32, True)}
+
+
+def storage(precision):
+    """activation storage dtype of an engine mode (16-bit or fp32)"""
+    return (MODES.get(precision) or WIDE_MODES[precision])[0]
 
 
 def _op(weight, kernel=1, stride=1, pad=(0, 0), dil=1, act=None, depthwise=False, bn=None, eps=port.BN_EPS_EFFNETV2,
@@ -139,6 +149,14 @@ def tc_eligible(op, cin, cout):
             and op['stride'] in (1, 2) and op['kernel'] in (1, 3))
 
 
+def tc32_eligible(op, cin, cout):
+    """tc32_eligible (csrc/tc_tf32.cuh:282) for the ops of an op table: the convs that 'tf32x3' runs on tc32_conv_kernel
+    (the others on CUDA cores).  The engine's rule also excludes its small_io ops, the squeeze-excitation fcs; those are
+    not in the op tables (se_fc_bound covers them), so stem / depthwise / max pool stand in for is_conv / depthwise here."""
+    return (not op['stem'] and not op['depthwise'] and not op['maxpool'] and cin % 4 == 0 and cout % 4 == 0
+            and op['stride'] in (1, 2) and op['kernel'] in (1, 3))
+
+
 def _act(y, act):
     if act == 'silu':
         return F.silu(y)
@@ -165,9 +183,9 @@ def _layer(sd, spec, name, x_nhwc, res_nhwc, scale, precision, dtype, magnitude=
         return y, y, 1
     w, bias = _fold(sd, op)
     st = MODES[precision][0] if precision in MODES else None
-    if st is not None:
+    if st is not None or precision in WIDE_MODES:
         w, bias = w.float().double(), bias.float().double()
-        if tc_eligible(op, w.shape[1], w.shape[0]):
+        if st is not None and tc_eligible(op, w.shape[1], w.shape[0]):
             w = w.float().to(st).double()
     w, bias = w.to(dev, dtype), bias.to(dev, dtype)
     if op['stem']:
@@ -180,6 +198,8 @@ def _layer(sd, spec, name, x_nhwc, res_nhwc, scale, precision, dtype, magnitude=
         s = scale.to(dev, dtype)[:, :, None, None]
         if st is not None and MODES[precision][1] and not magnitude:  # se_scale_kernel: fp32 product, rounded to 16 bits
             x = (x.float() * s.float()).to(st).to(dtype)
+        elif precision in WIDE_MODES and not magnitude:  # fp32 product, no further rounding
+            x = (x.float() * s.float()).to(dtype)
         else:
             x = x * s
     if magnitude:
@@ -215,6 +235,13 @@ def conv_layer_reference(sd, spec, name, x_nhwc, res_nhwc=None, scale=None, prec
 # rather than rounding to nearest) and the 1/(1-n*u) factor; n = products + bias + residual + the fp32 x*s / stem
 # preprocessing products, so K + 4.
 C_ACC = 2.0
+# 3xTF32 products (tc_tf32.cuh): x = hi + lo with hi = RN_tf32(x), so |lo| <= 2^-11 |x|; the tensor core reads the lo
+# operands (the split activations and the host lo weight plane) as tf32, truncating: |lo - tf32(lo)| < 2^-10 |lo| <= 2^-21 |x|;
+# the lo*lo product is dropped: <= 2^-22 |x w|.  Per product |x*w - (hi_x hi_w + lo_x' hi_w + hi_x lo_w')|
+# <= (2^-22 + 2 * 2^-21 (1 + 2^-11)) |x| |w| <= 5 * 2^-22 * (1 + 2^-10) |x| |w|.
+TC32_SPLIT = 5.0 * 2.0 ** -22 * (1.0 + 2.0 ** -10)
+# smallest normal fp32: the MUFU approximations (ex2 / rcp .ftz) flush subnormal results to zero
+FP32_FLOOR = 2.0 ** -126
 # tanh.approx.f32: maximum relative error 2^-10.987 (PTX ISA, tanh instruction)
 TANH_APPROX_REL = 2.0 ** -10.987
 # sup |act'|: SiLU 1.0998 (x = 2.40), hard-swish 1.5 (x = 3), ReLU / none 1, sigmoid 1/4, hard-sigmoid 1/6
@@ -229,8 +256,10 @@ def _act_error(z, y, act, precision):
         h = 0.5 * az
         return h * torch.tanh(h) * TANH_APPROX_REL + 2.0 ** -22 * (az + ay)
     if act in ('silu', 'sigmoid'):
-        # silu_f16out (ex2.approx + rcp.approx, csrc/common.cuh:156-166) and act_t (x / (1 + __expf(-x))): the fp32 rounding
-        # of x*log2(e) gives |x|*2^-24 relative error in e^-x, plus a few ulps from ex2 / rcp / mul; |dsig/sig| <= |de/e|
+        # silu_f16out and t32_act<ACT_SILU> (ex2.approx.ftz + rcp.approx.ftz, csrc/common.cuh:156-166, tc_tf32.cuh:74-83) and
+        # act_t (x / (1 + __expf(-x)), IEEE divide): the fp32 rounding of x*log2(e) gives |x|*2^-24 relative error in e^-x,
+        # ex2 2 ulp, 1 + e 1/2 ulp, rcp 1 ulp (or the divide 1/2 ulp), the product 1/2 ulp: (8 + |x|) * 2^-24 relative, as
+        # |dsig/sig| <= |de/e|
         return (8.0 + 2.0 * az) * 2.0 ** -24 * ay
     if act == 'hswish':  # x * sat(x/6 + 0.5): the rounded 1/6, the fma and the product
         return 2.0 ** -22 * (az + ay)
@@ -239,27 +268,39 @@ def _act_error(z, y, act, precision):
     return torch.zeros_like(z)
 
 
+def bound_from_parts(z, y, zabs, k, act, precision, tc32=False):
+    """The per-element tolerance of a device result from the exact layer: pre-activation z, output y (after the
+    residual), pre-activation magnitude zabs and k products per output; tc32 adds the 3xTF32 split term per product.
+
+        16-bit modes: tol = 2^-p * (|y| + e) + e + floor16,  fp32 modes: tol = e + 2^-126,
+        e = L_act * (C_ACC * (K + 4) * 2^-24 + [TC32_SPLIT]) * zabs + e_act + 2^-23 * |y|"""
+    rate = C_ACC * (k + 4) * 2.0 ** -24 + (TC32_SPLIT if tc32 else 0.0)
+    e = LIPSCHITZ[act] * rate * zabs + _act_error(z, _act(z, act), act, precision) + 2.0 ** -23 * y.abs()
+    st = storage(precision)
+    if st == torch.float32:
+        return e + FP32_FLOOR
+    p = 8 if st == torch.bfloat16 else 11
+    return 2.0 ** -p * (y.abs() + e) + e + (2.0 ** -25 if st == torch.float16 else 0.0)
+
+
 def layer_bound(sd, spec, name, x_nhwc, res_nhwc=None, scale=None, precision='fp16'):
     """-> (ref, tol), NHWC fp64: the exact layer on this mode's rounded operands and the per-element bound on
-    |device - ref| for the device's 16-bit output,
+    |device - ref| (bound_from_parts),
 
         tol = 2^-p * (|ref| + e) + e + floor,   e = L_act * C_ACC * (K + 4) * 2^-24 * refabs + e_act + 2^-23 * |ref|
 
     with p = 8 (bf16) / 11 (fp16) (half an ulp of the output, rounded to nearest even), floor = half the fp16 subnormal
     spacing (2^-25), refabs the pre-activation magnitude (the layer on |x|, |w|, |b|, |res|), e_act the activation's own
-    error (_act_error) and 2^-23 * |ref| the fp32 residual add / epilogue roundings."""
-    st = MODES[precision][0]
+    error (_act_error) and 2^-23 * |ref| the fp32 residual add / epilogue roundings.  In the fp32-storage modes there is
+    no output rounding (tol = e + 2^-126), and a 'tf32x3' op that reaches tc32_conv_kernel adds TC32_SPLIT * refabs."""
     op = op_table(spec)[name]
     y, z, k = _layer(sd, spec, name, x_nhwc, res_nhwc, scale, precision, torch.float64)
     zabs = _layer(sd, spec, name, x_nhwc, res_nhwc, scale, precision, torch.float64, magnitude=True)[1]
-    if op['maxpool']:  # a max of 16-bit values is exact
+    if op['maxpool']:  # a max of stored values is exact
         tol = torch.zeros_like(y)
     else:
-        a = _act(z, op['act'])
-        e = (LIPSCHITZ[op['act']] * C_ACC * (k + 4) * 2.0 ** -24 * zabs + _act_error(z, a, op['act'], precision)
-             + 2.0 ** -23 * y.abs())
-        p = 8 if st == torch.bfloat16 else 11
-        tol = 2.0 ** -p * (y.abs() + e) + e + (2.0 ** -25 if st == torch.float16 else 0.0)
+        tc32 = precision == 'tf32x3' and tc32_eligible(op, x_nhwc.shape[-1], y.shape[1])
+        tol = bound_from_parts(z, y, zabs, k, op['act'], precision, tc32)
     nhwc = lambda t: t.permute(0, 2, 3, 1).contiguous()
     return nhwc(y), nhwc(tol)
 
@@ -275,7 +316,7 @@ def check_bound(dev, ref, tol, precision):
     an inf where |ref| - tol still overflows the storage type (or a finite value there); an inf of the wrong sign or
     where |ref| + tol does not reach the overflow threshold; a finite value farther than tol from ref."""
     dev, ref, tol = dev.double(), ref.double().to(dev.device), tol.double().to(dev.device)
-    top = overflow_threshold(MODES[precision][0])
+    top = overflow_threshold(storage(precision))
     must_inf = ref.abs() - tol >= top
     may_inf = ref.abs() + tol >= top
     fin = torch.isfinite(dev)
@@ -301,3 +342,87 @@ def se_fc_bound(x, xabs, n_in, w, b, act, x_err=None):
     if x_err is not None:
         e = e + x_err.double() @ w.abs().T
     return y, LIPSCHITZ[act] * e + _act_error(z, y, act, 'fp32') + 2.0 ** -23 * y.abs()
+
+
+def pool_mean_bound(x_nhwc):
+    """pool_mean_kernel (csrc/conv_simt.cuh:821): the mean over H*W of x [B,H,W,C], summed in fp32 (a strided per-thread sum,
+    then an 8-way tree) and multiplied by the rounded 1/(H*W).  -> (mean, tol) [B, C] fp64, tol = C_ACC (P + 2) 2^-24 mean|x|."""
+    x = x_nhwc.double()
+    n = x.shape[1] * x.shape[2]
+    return x.mean(dim=(1, 2)), C_ACC * (n + 2) * 2.0 ** -24 * x.abs().mean(dim=(1, 2)) + FP32_FLOOR
+
+
+# ------------------------------------------------------------------------------------------ soft-argmax decode bound
+def head_logit_delta(feats_nchw, w, b, tc32=False):
+    """Per-logit bound on |device logit - exact logit| of the head's 1x1 conv on features [B,C,H,W] with weight w
+    [N,C,1,1] and bias b [N] (the operands the device multiplies: 16-bit features and weights for the fused 16-bit head,
+    fp32 otherwise): C_ACC (C + 2) 2^-24 (|w| |f| + |b|), the fp32 accumulation of exact products (tc_head_kernel,
+    conv_igemm_kernel), plus TC32_SPLIT |w| |f| for the 3xTF32 head GEMM."""
+    mag = F.conv2d(feats_nchw.abs(), w.abs())
+    c = feats_nchw.shape[1]
+    return C_ACC * (c + 2) * 2.0 ** -24 * (mag + b.abs()[None, :, None, None]) + (TC32_SPLIT * mag if tc32 else 0.0)
+
+
+def _soft_argmax_bound(logits, delta, dims):
+    """-> (coords [..., len(dims)] in [0,1] heatmap units, tol of the same shape) of port.soft_argmax over ``dims`` for
+    device logits within ``delta`` (absolute, per logit) of ``logits``, decoded by softargmax_bhwn_kernel or the fused
+    head's epilogue (online softmax in fp32, exp2 on the MUFU):
+
+        |c' - c| <= e^Dmax * sum_i p_i (e^D_i - 1) |x_i - c|  +  (2 gamma_n + 3 * 2^-24) |c|  +  n * 2^-120
+
+    p the exact softmax, x_i the linspace coordinate of element i on that axis, and D_i = delta_i + the decode's own
+    error in the weight of element i: the rounding of its exponent argument, in either form ((v - m) * log2e, or
+    v * log2e - m * log2e with the bias folded in) 8 * 2^-24 (|v_i| + |m|) as a natural-log error, and one ex2 (2 ulp) and
+    one product (1/2 ulp) per running-max rescale or merge it passes through (at most n_exp = P + D + 4).  gamma_n =
+    C_ACC (n + n_exp + 4) 2^-24 covers the fp32 sums s, sx, sy, sz (n = P in 2D, P * D in 3D), and 3 * 2^-24 the two
+    divisions; n * 2^-120 the weights ex2.approx.ftz flushes to zero."""
+    dims = tuple(d if d >= 0 else logits.ndim + d for d in dims)
+    n = 1
+    for d in dims:
+        n *= logits.shape[d]
+    spatial = logits.shape[dims[0]] * logits.shape[dims[1]]
+    depth = logits.shape[dims[2]] if len(dims) > 2 else 0
+    n_exp = spatial + depth + 4
+    mx = torch.amax(logits, dim=dims, keepdim=True)
+    e = torch.exp(logits - mx)
+    p = e / e.sum(dim=dims, keepdim=True)
+    dmax_all = torch.amax(delta, dim=dims, keepdim=True)
+    big = 8.0 * 2.0 ** -24 * (logits.abs() + mx.abs() + 2 * dmax_all) + n_exp * (2.0 ** -22 + 2.0 ** -24)
+    dtot = delta + big
+    dmax = torch.amax(dtot, dim=dims, keepdim=True)
+    gamma = C_ACC * (n + n_exp + 4) * 2.0 ** -24
+    coords, tols = [], []
+    for d in dims:
+        shape = [1] * logits.ndim
+        shape[d] = logits.shape[d]
+        x = port.linspace01(logits.shape[d], torch.float64).reshape(shape)
+        c = (p * x).sum(dim=dims, keepdim=True)
+        t = torch.exp(dmax) * (p * torch.expm1(dtot) * (x - c).abs()).sum(dim=dims, keepdim=True)
+        t = t + (2 * gamma + 3 * 2.0 ** -24) * c.abs() + n * 2.0 ** -120
+        for hd in sorted(dims, reverse=True):
+            c, t = c.squeeze(hd), t.squeeze(hd)
+        coords.append(c)
+        tols.append(t)
+    return torch.stack(coords, dim=-1), torch.stack(tols, dim=-1)
+
+
+def decode_bound(logits, delta, cfg, n_joints):
+    """The head's decode on exact fp64 logits [B, J + D*J, H, W] (CPU) with per-logit device tolerance ``delta`` (same
+    shape) -> (coords2d px [B,J,2], tol2d, coords3d_rel mm [B,J,3], tol3d): port.heads' soft-argmax and
+    heatmap_to_image / heatmap_to_metric, each coordinate with the bound of _soft_argmax_bound carried through the
+    device's fmaf scale (c * mul + add with mul, add rounded to fp32: 4 * 2^-24 (|c mul| + |add|))."""
+    l2, l3 = port.split_logits(logits, n_joints, cfg.depth)
+    d2, d3 = port.split_logits(delta, n_joints, cfg.depth)
+    c2, t2 = _soft_argmax_bound(l2, d2, dims=(3, 2))
+    c3, t3 = _soft_argmax_bound(l3, d3, dims=(4, 3, 1))
+    last = cfg.proc_side - 1
+    mul = float(last - last % cfg.stride_test)
+    add = float(cfg.stride_test // 2) * (int(cfg.centered_stride) + int(cfg.legacy_centered_stride_bug))
+    mm = cfg.box_size_mm / cfg.proc_side
+    px2 = port.heatmap_to_image(c2, cfg)
+    tol2 = mul * t2 + 4 * 2.0 ** -24 * (mul * c2.abs() + abs(add))
+    mm3 = port.heatmap_to_metric(c3, cfg)
+    scale3 = torch.tensor([mul * mm, mul * mm, cfg.box_size_mm], dtype=torch.float64)
+    add3 = torch.tensor([add * mm, add * mm, 0.0], dtype=torch.float64)
+    tol3 = scale3 * t3 + 4 * 2.0 ** -24 * (scale3 * c3.abs() + add3.abs())
+    return px2, tol2, mm3, tol3

@@ -161,9 +161,9 @@ def _layer(sd, op, x_nhwc, res_nhwc, precision, dtype, magnitude=False):
         return y, y, 1
     dev = x_nhwc.device
     w, bias = port_ops._fold(sd, op)
-    if precision in port_ops.MODES:  # folded in fp64, cast to fp32, GEMM weights rounded once to 16 bits
-        w, bias = w.float().double(), bias.float().double()
-        if port_ops.tc_eligible(op, w.shape[1], w.shape[0]):
+    if precision in port_ops.MODES or precision in port_ops.WIDE_MODES:  # folded in fp64, cast to fp32, GEMM weights
+        w, bias = w.float().double(), bias.float().double()                 # rounded once to 16 bits
+        if precision in port_ops.MODES and port_ops.tc_eligible(op, w.shape[1], w.shape[0]):
             w = w.float().to(port_ops.MODES[precision][0]).double()
     w, bias = w.to(dev, dtype), bias.to(dev, dtype)
     if op['stem']:
@@ -194,17 +194,13 @@ def conv_layer_reference(sd, spec, name, x_nhwc, res_nhwc=None, precision='exact
 def layer_bound(sd, spec, name, x_nhwc, res_nhwc=None, precision='fp16'):
     """port_ops.layer_bound for the ops of ``spec`` (any depth): -> (ref, tol), NHWC fp64, with the same bound
     tol = 2^-p (|ref| + e) + e + floor, e = L_act C_ACC (K + 4) 2^-24 refabs + e_act + 2^-23 |ref|."""
-    st = port_ops.MODES[precision][0]
     op = op_table(spec)[name]
     y, z, k = _layer(sd, op, x_nhwc, res_nhwc, precision, torch.float64)
     zabs = _layer(sd, op, x_nhwc, res_nhwc, precision, torch.float64, magnitude=True)[1]
-    if op['maxpool']:  # a max of 16-bit values is exact
+    if op['maxpool']:  # a max of stored values is exact
         tol = torch.zeros_like(y)
     else:
-        a = port_ops._act(z, op['act'])
-        e = (port_ops.LIPSCHITZ[op['act']] * port_ops.C_ACC * (k + 4) * 2.0 ** -24 * zabs
-             + port_ops._act_error(z, a, op['act'], precision) + 2.0 ** -23 * y.abs())
-        p = 8 if st == torch.bfloat16 else 11
-        tol = 2.0 ** -p * (y.abs() + e) + e + (2.0 ** -25 if st == torch.float16 else 0.0)
+        tc32 = precision == 'tf32x3' and port_ops.tc32_eligible(op, x_nhwc.shape[-1], y.shape[1])
+        tol = port_ops.bound_from_parts(z, y, zabs, k, op['act'], precision, tc32)
     nhwc = lambda t: t.permute(0, 2, 3, 1).contiguous()  # noqa: E731
     return nhwc(y), nhwc(tol)

@@ -15,6 +15,8 @@ import torch.distributed as dist
 import torch.multiprocessing as mp
 
 from oracle import port
+from tests.test_gpu_forward_ops16 import check_head_per_coordinate
+from tests.test_gpu_tc import head_operands, tc_head_plan_fits
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -141,9 +143,12 @@ def test_f16_fused_depthwise_pooling_matches_separate_pool(H):
     (2048, 32, 24, 32, 2),
     (64, 6, 8, 8, 7),
     (1024, 8, 8, 8, 4),
+    (1280, 6, 24, 8, 256),
+    (1280, 7, 24, 8, 5),
 ])
 def test_f16_fused_head_vs_oracle(H, channels, hw, j, depth, batch):
-    """The geometries of test_gpu_tc.test_fused_head_vs_oracle, with features and head weights rounded to fp16."""
+    """The geometries of test_gpu_tc.test_fused_head_vs_oracle, with features and head weights rounded to fp16: 2e-4 of
+    the largest coordinate, and every coordinate within port_ops.decode_bound."""
     import metrabs_b200
     from metrabs_b200 import _lib
     from metrabs_b200.engine import Engine, make_config
@@ -159,10 +164,17 @@ def test_f16_fused_head_vs_oracle(H, channels, hw, j, depth, batch):
         cfg = metrabs_b200.Config(proc_side=side, stride_test=stride, depth=depth, precision=prec)
         eng = Engine(make_config(cfg, j, arch=_lib.ARCH_HEAD_ONLY, feature_channels=channels))
         eng.load_state_dict(sd)
-        c2d, c3d = eng.head_decode(feats.permute(0, 2, 3, 1).contiguous().half().cuda())
+        f16 = feats.permute(0, 2, 3, 1).contiguous().half().cuda()
+        eng.profile_begin()
+        c2d, c3d = eng.head_decode(f16)
+        head_cls = set(eng.profile_end())
+        fused = prec == 'fp16' and tc_head_plan_fits(hw * hw)
+        assert head_cls == ({'tc_head_softargmax_kernel'} if fused
+                            else {'head_conv(conv_igemm_kernel)', 'softargmax_bhwn_kernel'}), (prec, head_cls)
         e2, e3 = H.rel_err(c2d, ref2d), H.rel_err(c3d, ref3d)
-        print(f'[{prec}] C={channels} hw={hw} J={j} D={depth}: coords2d {e2:.2e} coords3d {e3:.2e} '
-              f'launches {eng.last_launch_count}')
+        w2, w3 = check_head_per_coordinate(head_operands(sd, torch.float16), f16, pcfg, c2d, c3d, False, j)
+        print(f'[{prec}] C={channels} hw={hw} J={j} D={depth} x{batch}: coords2d {e2:.2e} coords3d {e3:.2e}, '
+              f'worst |dev-ref|/tol {w2:.3f} / {w3:.3f}, launches {eng.last_launch_count}')
         assert e2 < 2e-4 and e3 < 2e-4, (prec, e2, e3)
 
 

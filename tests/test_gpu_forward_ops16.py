@@ -16,7 +16,8 @@ reads (Engine.op_buffers).  Those stay cached while they are live, so every pref
 * SE fc1 / fc2: port_ops.se_fc_bound on the depthwise output and fc1 output the forward stored, as
   test_gpu_ops16_vs_conv2d.py::test_fused_se_squeeze_on_the_forward.
 * every stored tensor finite; head_decode on the forward's features against port.heads with the head weight rounded to
-  the mode's type (2e-4, the bar of test_gpu_tc.py::test_fused_head_vs_oracle); backbone() bit-equal to the full prefix;
+  the mode's type (2e-4, the bar of test_gpu_tc.py::test_fused_head_vs_oracle) and every coordinate within
+  port_ops.decode_bound; backbone() bit-equal to the full prefix;
   three forward() calls on the same buffers (eager run, graph capture, graph replay) give identical joints.
 * what each configuration reached is asserted (kernel classes, depthwise and tensor-core kernels, SE projection widths),
   and the worst |dev-ref|/tol per kernel kind and the wall time are printed."""
@@ -47,13 +48,13 @@ CONFIGS = [('efficientnetv2-l', 256), ('efficientnetv2-s-os8', 256), ('efficient
 
 
 def build(H, config, precision):
-    """-> (pcfg, state dict, engine, op table, bound(name, x, res, scale) -> (ref, tol), SE activations (fc1, fc2))."""
+    """-> (pcfg, spec, state dict, engine, op table, bound(name, x, res, scale) -> (ref, tol), SE activations (fc1, fc2))."""
     if config == 'efficientnetv2-l':
         pcfg = port.PathConfig(proc_side=256)
         spec = port.effnet_spec(config)
         sd = port.make_effnet_state_dict(spec, pcfg, J, seed=0, calib_batch=1)
         eng = H.device_model(config, pcfg, J, sd, precision=precision).engine()
-        return (pcfg, sd, eng, port_ops.effnet_op_table(spec),
+        return (pcfg, spec, sd, eng, port_ops.effnet_op_table(spec),
                 lambda nm, x, res, sc: port_ops.layer_bound(sd, spec, nm, x, res, sc, precision), ('silu', 'sigmoid'))
     if config == 'efficientnetv2-s-os8':
         from tests.test_gpu_effnet_dilated import device_model, model_and_weights
@@ -65,12 +66,12 @@ def build(H, config, precision):
             if table[nm]['depthwise']:
                 return D.dw_layer_bound(sd, spec, nm, x, precision)
             return port_ops.layer_bound(sd, spec, nm, x, res, sc, precision)
-        return pcfg, sd, eng, table, bound, ('silu', 'sigmoid')
+        return pcfg, spec, sd, eng, table, bound, ('silu', 'sigmoid')
     if config.startswith('efficientnet-b'):
         from tests.test_gpu_effnet_b import device_model, model
         pcfg, spec, sd = model(config, 256, j=J)
         eng = device_model(H, config, pcfg, J, sd, precision).engine()
-        return (pcfg, sd, eng, port_effnet_b.op_table(spec),
+        return (pcfg, spec, sd, eng, port_effnet_b.op_table(spec),
                 lambda nm, x, res, sc: port_effnet_b.layer_bound(sd, spec, nm, x, res, sc, precision), ('silu', 'sigmoid'))
     if config == 'mobilenetv3-large':
         from tests.test_gpu_mobilenet_large import device_model
@@ -78,14 +79,14 @@ def build(H, config, precision):
         spec = port_mobilenet.MobileNetV3Spec(pcfg, 'large')
         sd = tfb.make_state_dict(spec, pcfg, J, seed=0, calib_batch=1)
         eng = device_model(H, 'large', pcfg, J, sd, precision).engine()
-        return (pcfg, sd, eng, port_mobilenet.op_table(spec),
+        return (pcfg, spec, sd, eng, port_mobilenet.op_table(spec),
                 lambda nm, x, res, sc: port_mobilenet.layer_bound(sd, spec, nm, x, res, sc, precision), ('relu', 'hsigmoid'))
     assert config == 'resnet50-s8'  # resnet_step.py's stride-8 configuration: D = 32
     pcfg = port.PathConfig(proc_side=256, stride_test=8, depth=32)
     spec = tfb.ResNet50Spec(pcfg)
     sd = tfb.make_state_dict(spec, pcfg, J, seed=0, calib_batch=1)
     eng = H.device_model_tf('resnet50', pcfg, J, sd, precision=precision).engine()
-    return (pcfg, sd, eng, port_ops.op_table(spec),
+    return (pcfg, spec, sd, eng, port_ops.op_table(spec),
             lambda nm, x, res, sc: port_ops.layer_bound(sd, spec, nm, x, res, sc, precision), None)
 
 
@@ -118,6 +119,23 @@ def check_se_fc(sd, nm, out, x, xabs, n_in, x_err, act, precision):
     return r
 
 
+def check_head_per_coordinate(sd, feats, pcfg, c2d, c3d, tc32, n_joints=J):
+    """head_decode's coordinates within port_ops.decode_bound, each one: the exact fp64 logits of the head's 1x1 conv on
+    the features the device decoded (on the device), their per-logit bound port_ops.head_logit_delta, the decode on the
+    host.  sd holds the head weight and bias as the device multiplies them (on the device), feats is NHWC.  -> (worst 2D, worst 3D |dev-ref|/tol)"""
+    w, b = sd['heatmap_heads.conv_final.weight'], sd['heatmap_heads.conv_final.bias']
+    f = feats.double().permute(0, 3, 1, 2)
+    logits = torch.nn.functional.conv2d(f, w, b).cpu()
+    delta = port_ops.head_logit_delta(f, w, b, tc32).cpu()
+    r2, t2, r3, t3 = port_ops.decode_bound(logits, delta, pcfg, n_joints)
+    e2, e3 = (c2d.double().cpu() - r2).abs(), (c3d.double().cpu() - r3).abs()
+    w2, w3 = float((e2 / t2).max()), float((e3 / t3).max())
+    assert bool((e2 <= t2).all()) and bool((e3 <= t3).all()), (
+        f'head decode outside the per-coordinate bound: 2D {w2:.2f} (max {float(e2.max()):.2e} px), 3D {w3:.2f} '
+        f'(max {float(e3.max()):.2e} mm)')
+    return w2, w3
+
+
 def heads_reference(sd, feats, pcfg):
     """port.heads with the head's 1x1 conv evaluated in fp64 on the device (ResNet-50 at stride 8: 2048 channels on 32x32
     maps) and the soft-argmax decode on the host, where port.heads keeps its coordinate grids."""
@@ -131,7 +149,7 @@ def heads_reference(sd, feats, pcfg):
 @pytest.mark.parametrize('config,batch', CONFIGS)
 def test_forward_ops_vs_conv2d(H, config, batch, precision):
     t0 = time.perf_counter()
-    pcfg, sd, eng, table, bound, se_acts = build(H, config, precision)
+    pcfg, _spec, sd, eng, table, bound, se_acts = build(H, config, precision)
     st = port_ops.MODES[precision][0]
     p = 8 if st == torch.bfloat16 else 11
     crops, intr = (t.cuda() for t in port.synthetic_inputs(batch, pcfg.proc_side, seed=5))
@@ -221,6 +239,7 @@ def test_forward_ops_vs_conv2d(H, config, batch, precision):
     ref2d, ref3d = heads_reference(head, feats, pcfg)
     e2, e3 = H.rel_err(c2d, ref2d), H.rel_err(c3d, ref3d)
     assert e2 < 2e-4 and e3 < 2e-4, (e2, e3)
+    worst['head 2D'], worst['head 3D'] = check_head_per_coordinate(head, feats, pcfg, c2d, c3d, tc32=False)
     # eager run, graph capture, graph replay (mtb_forward keys its graphs on buffers, batch and stream)
     o = torch.empty(batch, eng.n_out, 3, device=crops.device)
     joints = []

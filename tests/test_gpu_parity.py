@@ -247,6 +247,27 @@ def test_batch_global_rms_is_reproduced(H):
         ref = port.reconstruct_absolute(c2d[sl], c3d[sl], k[sl], pcfg)
         out = ptu3d.reconstruct_absolute(c2d[sl].cuda(), c3d[sl].cuda(), k[sl].cuda(), mix_3d_inside_fov=0.5)
         assert H.rel_err(out, ref) < 2e-5
+    # batches past one CTA's strided reduction (128 threads), joints past one pass of the crop loop, crops whose joints
+    # are all outside the field of view, joints exactly on its inclusive bounds, mixing on and off: per crop, max |dev-ref|
+    # over its joints relative to its largest joint, against the fp64 reconstruction on the same fp32 inputs
+    lo, hi = pcfg.stride_train * 0.75, pcfg.proc_side - pcfg.stride_train * 0.75  # is_within_fov, centered stride
+    worst = 0.0
+    for b, j in ((129, 24), (256, 129), (1000, 24), (256, 1024)):
+        c2d = 40 + 170 * torch.rand(b, j, 2, generator=g)
+        c3d = torch.randn(b, j, 3, generator=g) * 300
+        c3d[..., 2] += 3000
+        c2d[1] = 300 + 10 * torch.rand(j, 2, generator=g)  # every joint of crop 1 outside the field of view
+        c2d[2, :, 0] = lo                                   # crop 2 on the lower bound in x, the upper in y
+        c2d[2, :, 1] = hi
+        c2d[b - 1, ::2] = hi                                # half of the last crop's joints on the upper corner
+        _, k = port.synthetic_inputs(b, 256, seed=b + j)
+        for mix in (0.5, None):
+            ref = port.reconstruct_absolute(c2d.double(), c3d.double(), k.double(), pcfg, mix_3d_inside_fov=mix)
+            out = ptu3d.reconstruct_absolute(c2d.cuda(), c3d.cuda(), k.cuda(), mix_3d_inside_fov=mix).double().cpu()
+            per_crop = (out - ref).abs().amax(dim=(1, 2)) / ref.abs().amax(dim=(1, 2))
+            worst = max(worst, float(per_crop.max()))
+            assert float(per_crop.max()) < 2e-5, (b, j, mix, int(per_crop.argmax()), float(per_crop.max()))
+    print(f'reconstruction per crop: worst max|dev-ref| / max|ref| {worst:.1e}')
 
 
 def test_errors_are_loud(H):

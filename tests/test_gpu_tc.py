@@ -8,6 +8,7 @@ import pytest
 import torch
 
 from oracle import port
+from tests.test_gpu_forward_ops16 import check_head_per_coordinate
 
 pytestmark = pytest.mark.gpu
 
@@ -112,8 +113,12 @@ def test_fused_depthwise_pooling_matches_separate_pool(H):
     (2048, 32, 24, 32, 2),    # c2/c5b geometry: N=792, D=32
     (64, 6, 8, 8, 7),         # P=36: crop boundaries inside a 16-column chunk (element-wise path)
     (1024, 8, 8, 8, 4),       # c1 geometry
+    (1280, 6, 24, 8, 256),    # P=36 at the benchmark batch: crop-straddling chunks over 256 crops
+    (1280, 7, 24, 8, 5),      # P=49: no fused plan (tc_head_plan), the 16-bit unfused fallback
 ])
 def test_fused_head_vs_oracle(H, channels, hw, j, depth, batch):
+    """bf16 head against port.heads (2e-4 of the largest coordinate) and, coordinate by coordinate, against
+    port_ops.decode_bound on the operands the device multiplies (bf16 features and weight, fp32 bias)."""
     import metrabs_b200
     from metrabs_b200 import _lib
     from metrabs_b200.engine import Engine, make_config
@@ -124,17 +129,40 @@ def test_fused_head_vs_oracle(H, channels, hw, j, depth, batch):
     feats, sd = port.head_only_inputs(batch, channels, hw, j, depth, seed=1)
     eng = Engine(make_config(cfg, j, arch=_lib.ARCH_HEAD_ONLY, feature_channels=channels))
     eng.load_state_dict(sd)
-    c2d, c3d = eng.head_decode(feats.permute(0, 2, 3, 1).contiguous().bfloat16().cuda())
+    f16 = feats.permute(0, 2, 3, 1).contiguous().bfloat16().cuda()
+    eng.profile_begin()
+    c2d, c3d = eng.head_decode(f16)
+    head_cls = set(eng.profile_end())
+    fused = tc_head_plan_fits(hw * hw)
+    assert head_cls == ({'tc_head_softargmax_kernel'} if fused
+                        else {'head_conv(conv_igemm_kernel)', 'softargmax_bhwn_kernel'}), head_cls
     ref2d, ref3d = port.heads(sd, feats, pcfg, j)
     e2, e3 = H.rel_err(c2d, ref2d), H.rel_err(c3d, ref3d)
-    print(f'C={channels} hw={hw} J={j} D={depth}: coords2d {e2:.2e} coords3d {e3:.2e} launches {eng.last_launch_count}')
+    w2, w3 = check_head_per_coordinate(head_operands(sd, torch.bfloat16), f16, pcfg, c2d, c3d, False, j)
+    print(f'C={channels} hw={hw} J={j} D={depth} x{batch} ({"fused" if fused else "unfused"}): coords2d {e2:.2e} '
+          f'coords3d {e3:.2e}, worst |dev-ref|/tol {w2:.3f} / {w3:.3f}, launches {eng.last_launch_count}')
     assert e2 < 2e-4 and e3 < 2e-4
     # the CUDA-core head on the same bf16 operands agrees too
     cfg_s = metrabs_b200.Config(proc_side=side, stride_test=stride, depth=depth, precision='bf16_simt')
     eng_s = Engine(make_config(cfg_s, j, arch=_lib.ARCH_HEAD_ONLY, feature_channels=channels))
     eng_s.load_state_dict(sd)
-    s2d, s3d = eng_s.head_decode(feats.permute(0, 2, 3, 1).contiguous().bfloat16().cuda())
+    s2d, s3d = eng_s.head_decode(f16)
     assert H.rel_err(s2d, ref2d) < 2e-4 and H.rel_err(s3d, ref3d) < 2e-4
+    check_head_per_coordinate(head_operands(sd, torch.bfloat16), f16, pcfg, s2d, s3d, False, j)
+
+
+def tc_head_plan_fits(P):
+    """tc_head_plan (csrc/tc_gemm.cuh): a fused head tile of c whole crops with c*P % 16 == 0 (P <= 256), or whole
+    256-pixel tiles of one crop."""
+    if P <= 256:
+        return any(c * P % 16 == 0 for c in range(1, 256 // P + 1))
+    return P % 256 == 0
+
+
+def head_operands(sd, st):
+    """the head weight rounded to the 16-bit type and the fp32 bias, fp64 on the device"""
+    return {'heatmap_heads.conv_final.weight': sd['heatmap_heads.conv_final.weight'].float().to(st).double().cuda(),
+            'heatmap_heads.conv_final.bias': sd['heatmap_heads.conv_final.bias'].float().double().cuda()}
 
 
 def test_bf16_forward_deviation_is_reported(H):
