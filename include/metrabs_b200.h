@@ -352,25 +352,49 @@ double mtb_backbone_flops_per_crop(const mtb_handle* h);
  * rows per item, row bands per crop (= SE pooling slices) and bytes of one shared-memory stage; all 0 when the shape falls
  * back to the strip kernel. */
 int mtb_debug_dw_plan(int height, int width, int* crops_per_item, int* rows_per_item, int* row_bands, int* stage_bytes);
-/* The kernel mtb_finalize_weights chose for depthwise backbone op `op`: GENERIC is dwconv_kernel (one thread per pixel and
- * 4 channels; every fp32 / 3xTF32 / _SIMT mode op that no other kernel covers), TMA the TMA-staged 3x3 stride-1 kernel and
- * STRIP_16B / STRIP_F32 the 3x3 strip kernels (these three also write the SE pooling slices), 5X5_16B the 16-bit 5x5 kernel
- * of the BF16_TC / F16_TC modes for ReLU / hard-swish (bit-identical to dwconv_kernel, no pooling), 5X5_POOL_16B the same
- * kernel for SiLU (bit-identical outputs, and it also writes the SE pooling slices of the stored outputs), TMA_DIL the
- * TMA-staged kernel for the 3x3 stride-1 SiLU ops with dilation 2 or 4 of the BF16_TC / F16_TC modes (one undilated pass per
- * phase of the dilation, same arithmetic per output as TMA, also writes the SE pooling slices).
- * MTB_ERR_INVALID_ARG for an index out of range or an op that is not depthwise. */
-typedef enum { MTB_DW_GENERIC = 0, MTB_DW_TMA = 1, MTB_DW_STRIP_16B = 2, MTB_DW_STRIP_F32 = 3, MTB_DW_5X5_16B = 4,
-               MTB_DW_5X5_POOL_16B = MTB_DW_5X5_16B + 1 /* 5 */,
-               MTB_DW_TMA_DIL = MTB_DW_5X5_POOL_16B + 1 /* 6 */ } mtb_dw_kernel;
-int mtb_op_dw_kernel(const mtb_handle* h, int op);
-/* The tensor-core kernel that runs backbone op `op` of the BF16_TC / F16_TC modes (on the forward, and in isolation with
- * mtb_debug_run_op): CONV is tc_conv_kernel; CONV3X3S1 is tc_conv3x3s1_kernel, which takes the 3x3 stride-1 undilated
- * convs with Cin and Cout <= 64 and SiLU or ReLU, from input boxes and weights resident in shared memory.  The profiler
- * reports both under the class "tc_conv_kernel".  Ops of a fused FusedMBConv block report the kernel that runs them in
- * isolation.  MTB_ERR_INVALID_ARG for an index out of range or an op without 16-bit tensor-core weights. */
-typedef enum { MTB_TC_CONV = 0, MTB_TC_CONV3X3S1 = 1 } mtb_tc_kernel;
-int mtb_op_tc_kernel(const mtb_handle* h, int op);
+/* The kernel mtb_finalize_weights chose for each op; the profiler class its launches count under is in brackets.
+ * Stem [stem_conv_kernel]: STEM_3X3S2 is stem3x3s2_kernel, EfficientNet's 3x3 stride-2 stem with 24 or 32 output channels
+ * (bit-identical to the generic kernels; the environment variable MTB_STEM_FAST=0, read once per process, turns it off for
+ * tests); STEM_WIDE is stem_conv_wide_kernel, for a multiple of 32, 24 or 16 output channels; STEM_GENERIC is
+ * stem_conv_kernel for any other width.
+ * MAXPOOL is maxpool_kernel [other].  POOL_MEAN is pool_mean_kernel [pool_mean_kernel], the squeeze-excitation (SE) mean;
+ * POOL_FUSED launches nothing, because the depthwise kernel before it wrote the SE pooling slices (fc1 sums them).
+ * SE_FC is conv_igemm_kernel on the SE fully-connected layers, plus se_reduce_kernel when fc1 splits K [se_fc(...)].
+ * IGEMM is conv_igemm_kernel [conv_igemm_kernel], every conv of the FP32 and _SIMT modes and what no other kernel takes.
+ * Tensor cores, BF16_TC / F16_TC [tc_conv_kernel]: TC_CONV is tc_conv_kernel; TC_CONV_SE is tc_conv_kernel scaling its A
+ * tiles by the SE scale (the 1x1 projections to at most 256 channels); SE_SCALE_TC_CONV is se_scale_kernel
+ * [se_scale_kernel] applying the scale in place, then tc_conv_kernel (the wider projections); TC_CONV3X3S1 is
+ * tc_conv3x3s1_kernel, which takes the 3x3 stride-1 undilated convs with Cin and Cout <= 64 and SiLU or ReLU from input
+ * boxes and weights resident in shared memory.  TC32 is tc32_conv_kernel [tc32_conv_kernel], the TF32X3 mode's GEMMs.
+ * Depthwise [dwconv_kernel]: DW_GENERIC is dwconv_kernel (one thread per pixel and 4 channels; every fp32 / 3xTF32 / _SIMT
+ * mode op that no other kernel covers), DW_TMA the TMA-staged 3x3 stride-1 kernel and DW_STRIP_16B / DW_STRIP_F32 the 3x3
+ * strip kernels (these three also write the SE pooling slices), DW_5X5_16B the 16-bit 5x5 kernel of the BF16_TC / F16_TC
+ * modes for ReLU / hard-swish (bit-identical to dwconv_kernel, no pooling), DW_5X5_POOL_16B the same kernel for SiLU
+ * (bit-identical outputs, and it also writes the SE pooling slices of the stored outputs), DW_TMA_DIL the TMA-staged kernel
+ * for the 3x3 stride-1 SiLU ops with dilation 2 or 4 of the BF16_TC / F16_TC modes (one undilated pass per phase of the
+ * dilation, same arithmetic per output as DW_TMA, also writes the SE pooling slices).
+ * Head (mtb_head_decode and the forward): HEAD_FUSED is tc_head_kernel + head_finalize_kernel
+ * [tc_head_softargmax_kernel], the BF16_TC / F16_TC modes when a fused tile fits the feature map; HEAD_TC32 is
+ * tc32_conv_kernel [tc32_conv_kernel] and HEAD_IGEMM conv_igemm_kernel [head_conv(...)], both followed by
+ * softargmax_bhwn_kernel [softargmax_bhwn_kernel].
+ * The two ops of a fused FusedMBConv block (mtb_op_is_fused_block) run as one fmb_kernel launch [fmb_kernel] on the forward;
+ * each reports the kernel that runs it alone, as on a mtb_debug_run_ops prefix that ends after the first.  In isolation
+ * (mtb_debug_run_op) a depthwise op writes no pooling slices and a POOL_FUSED op runs pool_mean_kernel. */
+typedef enum {
+  /* depthwise values first: their numbers (0-6) are stable for existing callers */
+  MTB_DW_GENERIC = 0, MTB_DW_TMA = 1, MTB_DW_STRIP_16B = 2, MTB_DW_STRIP_F32 = 3, MTB_DW_5X5_16B = 4,
+  MTB_DW_5X5_POOL_16B = MTB_DW_5X5_16B + 1 /* 5 */,
+  MTB_DW_TMA_DIL = MTB_DW_5X5_POOL_16B + 1 /* 6 */,
+  MTB_STEM_3X3S2 = 7, MTB_STEM_WIDE = 8, MTB_STEM_GENERIC = 9,
+  MTB_MAXPOOL = 10, MTB_POOL_MEAN = 11, MTB_POOL_FUSED = 12,
+  MTB_SE_FC = 13, MTB_IGEMM = 14,
+  MTB_TC_CONV = 15, MTB_TC_CONV_SE = 16, MTB_SE_SCALE_TC_CONV = 17, MTB_TC_CONV3X3S1 = 18,
+  MTB_TC32 = 19,
+  MTB_HEAD_FUSED = 20, MTB_HEAD_TC32 = 21, MTB_HEAD_IGEMM = 22
+} mtb_kernel;
+/* The mtb_kernel value of backbone op `op` (the head's is not reported here).  MTB_ERR_NOT_FINALIZED before
+ * mtb_finalize_weights, MTB_ERR_INVALID_ARG for an index out of range. */
+int mtb_op_kernel(const mtb_handle* h, int op);
 
 #ifdef __cplusplus
 }

@@ -10,8 +10,14 @@ ARCH_EFFNET, ARCH_RESNET50, ARCH_MOBILENETV3_SMALL, ARCH_HEAD_ONLY = 0, 1, 2, 3
 ARCH_RESNET18, ARCH_RESNET34, ARCH_RESNET101, ARCH_RESNET152 = 4, 5, 6, 7
 ARCH_MOBILENETV3_LARGE = 8
 ARCH_EFFNET_EPS1E5 = 9  # the EFFNET grammar with BatchNorm eps 1e-5 (EfficientNet-B0..B4)
-DW_GENERIC, DW_TMA, DW_STRIP_16B, DW_STRIP_F32, DW_5X5_16B, DW_5X5_POOL_16B, DW_TMA_DIL = 0, 1, 2, 3, 4, 5, 6  # mtb_op_dw_kernel
-TC_CONV, TC_CONV3X3S1 = 0, 1  # mtb_op_tc_kernel
+# mtb_kernel (mtb_op_kernel): the kernel that runs an op
+DW_GENERIC, DW_TMA, DW_STRIP_16B, DW_STRIP_F32, DW_5X5_16B, DW_5X5_POOL_16B, DW_TMA_DIL = 0, 1, 2, 3, 4, 5, 6
+STEM_3X3S2, STEM_WIDE, STEM_GENERIC = 7, 8, 9
+MAXPOOL, POOL_MEAN, POOL_FUSED = 10, 11, 12
+SE_FC, IGEMM = 13, 14
+TC_CONV, TC_CONV_SE, SE_SCALE_TC_CONV, TC_CONV3X3S1 = 15, 16, 17, 18
+TC32 = 19
+HEAD_FUSED, HEAD_TC32, HEAD_IGEMM = 20, 21, 22
 BUF_FEATURES, BUF_NONE = -2, -1  # mtb_debug_op_buffers; 0-3 the large buffers, 4-6 the small ones
 PRECISION_FP32, PRECISION_BF16_TC, PRECISION_BF16_SIMT, PRECISION_TF32X3, PRECISION_F16_TC, PRECISION_F16_SIMT = 0, 1, 2, 3, 4, 5
 DTYPE_F32, DTYPE_BF16, DTYPE_F16, DTYPE_I64 = 0, 1, 2, 3
@@ -120,8 +126,7 @@ _SIGNATURES = {
                                        C.POINTER(C.c_int)]),
     'mtb_debug_run_op': (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                    C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
-    'mtb_op_dw_kernel': (C.c_int, [C.c_void_p, C.c_int]),
-    'mtb_op_tc_kernel': (C.c_int, [C.c_void_p, C.c_int]),
+    'mtb_op_kernel': (C.c_int, [C.c_void_p, C.c_int]),
     'mtb_op_is_fused_block': (C.c_int, [C.c_void_p, C.c_int]),
     'mtb_debug_run_fused_block': (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p,
                                             C.c_size_t, C.c_void_p]),

@@ -7,6 +7,8 @@
 
 namespace mtb {
 
+// The kernels take it as `const __grid_constant__ ConvParams p` and read it in place: their lambdas take p by reference,
+// and without the qualifier ptxas's register allocation follows the struct's size.
 struct ConvParams {
   const void* in;        // [B,Hin,Win,Cin]
   const void* res;       // optional residual [B,Hout,Wout,Cout]
@@ -14,12 +16,10 @@ struct ConvParams {
   const float* w;        // [R*S*Cin][Cout]  (k = (r*S+s)*Cin + c)
   const float* bias;     // [Cout]
   const float* a_scale;  // optional per-(b,cin) multiplier of the input (squeeze-excitation), [B][Cin]
-  const float* a_bias = nullptr;  // optional per-cin bias + activation applied to the input on load (the producer was a
-  int a_act = 0;                  //   split-K GEMM that left raw sums: squeeze-excitation fc1 -> fc2)
   int res_first = 0;              // 1: add the residual BEFORE the activation (ResNet), 0: after (EfficientNet)
   int ksplit = 1;                 // > 1: blockIdx.z owns a K slice and writes its raw partial sums to out + z*M*Cout (fp32)
-  int a_splits = 1;               // > 1: the input is such a stack of partial-sum slices; they are summed on load (in a
-  size_t a_split_stride = 0;      //   fixed order: deterministic, unlike atomics), then a_bias / a_act apply
+  int a_splits = 1;               // > 1: the input is a stack of partial slices (the pooled means the depthwise kernels
+  size_t a_split_stride = 0;      //   leave for SE fc1); they are summed on load in a fixed order: deterministic
   int B, Hin, Win, Cin, Hout, Wout, Cout, R, S, stride, dil, pad_t, pad_l, act;
 };
 
@@ -28,7 +28,7 @@ struct ConvParams {
 // ----------------------------------------------------------------------------------------------------------
 template <int BM, int BN, int TM, int TN, typename TIn, typename TOut>
 __global__ void __launch_bounds__((BM / TM) * (BN / TN))
-conv_igemm_kernel(ConvParams p) {
+conv_igemm_kernel(const __grid_constant__ ConvParams p) {
   constexpr int BK = 16;
   constexpr int NT = (BM / TM) * (BN / TN);
   constexpr int A_LD = (BM * BK / 4) / NT;  // float4 loads of A per thread per tile
@@ -90,6 +90,7 @@ conv_igemm_kernel(ConvParams p) {
       if (ok) {
         const TIn* ap = in + ((size_t)(a_b[i] * p.Hin + ih) * p.Win + iw) * p.Cin + c;
         v = load4<TIn>(ap);
+#pragma unroll 1  // at most 8 slices; unrolled, the 64x64 fp32 instance (SE fc1) spills
         for (int z = 1; z < p.a_splits; ++z) {
           float4 u = load4<TIn>(ap + (size_t)z * p.a_split_stride);
           v.x += u.x; v.y += u.y; v.z += u.z; v.w += u.w;
@@ -97,11 +98,6 @@ conv_igemm_kernel(ConvParams p) {
         if (p.a_scale) {
           float4 sc = *reinterpret_cast<const float4*>(p.a_scale + (size_t)a_b[i] * p.Cin + c);
           v.x *= sc.x; v.y *= sc.y; v.z *= sc.z; v.w *= sc.w;
-        }
-        if (p.a_bias) {
-          float4 ab = *reinterpret_cast<const float4*>(p.a_bias + c);
-          v.x = apply_act(v.x + ab.x, p.a_act); v.y = apply_act(v.y + ab.y, p.a_act);
-          v.z = apply_act(v.z + ab.z, p.a_act); v.w = apply_act(v.w + ab.w, p.a_act);
         }
       }
       ra[i] = v;
@@ -221,7 +217,7 @@ conv_igemm_kernel(ConvParams p) {
 // depthwise conv, NHWC, one thread per (pixel, 4 channels).  w: [R*S][C], C % 4 == 0.
 // ----------------------------------------------------------------------------------------------------------
 template <typename T>
-__global__ void __launch_bounds__(256) dwconv_kernel(ConvParams p) {
+__global__ void __launch_bounds__(256) dwconv_kernel(const __grid_constant__ ConvParams p) {
   const T* __restrict__ in = reinterpret_cast<const T*>(p.in);
   T* __restrict__ out = reinterpret_cast<T*>(p.out);
   const int C4 = p.Cout >> 2;
@@ -298,7 +294,7 @@ __device__ __forceinline__ f32x2 unpack2_16b(unsigned w) {
 }
 
 template <typename T, int STRIDE, int ACT, int OW = 4>
-__global__ void __launch_bounds__(256, OW == 2 ? 3 : 2) dwconv3x3_pool_16b_kernel(ConvParams p, float* __restrict__ pooled) {
+__global__ void __launch_bounds__(256, OW == 2 ? 3 : 2) dwconv3x3_pool_16b_kernel(const __grid_constant__ ConvParams p, float* __restrict__ pooled) {
   // OW outputs per thread along W; T: element type (__nv_bfloat16 or __half)
   constexpr int NCOL = (OW - 1) * STRIDE + 3;    // input columns feeding them
   const T* __restrict__ in = reinterpret_cast<const T*>(p.in);
@@ -405,7 +401,7 @@ __global__ void __launch_bounds__(256, OW == 2 ? 3 : 2) dwconv3x3_pool_16b_kerne
 // fp32-storage twin of the strip kernel above for the 3xTF32 parity mode: 4 channels (one 16-byte vector) x OW output pixels
 // per thread, exact activation (expf SiLU), the same block-reduced partial pooling slices.  grid (ceil(C/128), slices, B).
 template <int STRIDE, int ACT, int OW = 4>
-__global__ void __launch_bounds__(256, 3) dwconv3x3_pool_f32_kernel(ConvParams p, float* __restrict__ pooled) {
+__global__ void __launch_bounds__(256, 3) dwconv3x3_pool_f32_kernel(const __grid_constant__ ConvParams p, float* __restrict__ pooled) {
   constexpr int NCOL = (OW - 1) * STRIDE + 3;
   const float* __restrict__ in = reinterpret_cast<const float*>(p.in);
   float* __restrict__ out = reinterpret_cast<float*>(p.out);
@@ -498,7 +494,7 @@ __global__ void __launch_bounds__(256, 3) dwconv3x3_pool_f32_kernel(ConvParams p
 // vectors, group g of slice y walks the strips y*groups + g, += gridDim.y*groups of crop blockIdx.z.  `pooled` may be null.
 // ----------------------------------------------------------------------------------------------------------
 template <typename T, int STRIDE, int ACT, int OW = 4, bool POOL = false>
-__global__ void __launch_bounds__(256) dwconv5x5_16b_kernel(ConvParams p, float* __restrict__ pooled) {
+__global__ void __launch_bounds__(256) dwconv5x5_16b_kernel(const __grid_constant__ ConvParams p, float* __restrict__ pooled) {
   constexpr int NCOL = (OW - 1) * STRIDE + 5;  // input columns feeding OW outputs
   const T* __restrict__ in = reinterpret_cast<const T*>(p.in);
   T* __restrict__ out = reinterpret_cast<T*>(p.out);
@@ -858,7 +854,7 @@ __global__ void __launch_bounds__(256) se_reduce_kernel(const float* __restrict_
 // max pool (ResNet stem, metrabs_tf/backbones/resnet.py:187-193), NHWC.  The reference pads with ZeroPadding2D and
 // pools VALID, so an out-of-bounds tap contributes the value 0 to the max.
 template <typename T>
-__global__ void __launch_bounds__(256) maxpool_kernel(ConvParams p) {
+__global__ void __launch_bounds__(256) maxpool_kernel(const __grid_constant__ ConvParams p) {
   const T* __restrict__ in = reinterpret_cast<const T*>(p.in);
   T* __restrict__ out = reinterpret_cast<T*>(p.out);
   const int C4 = p.Cout >> 2;

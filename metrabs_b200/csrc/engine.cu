@@ -31,14 +31,6 @@ namespace {
 std::string g_error;
 
 enum OpType { OP_STEM = 0, OP_CONV = 1, OP_DW = 2, OP_POOL = 3, OP_MAXPOOL = 4 };
-// depthwise kernels: TMA-staged (dw_tma.cuh), 16-bit (bf16 / fp16) or fp32 strip (SE pooling fused), generic (dwconv_kernel),
-// 16-bit 5x5 (dwconv5x5_16b_kernel: dwconv_kernel's arithmetic with column reuse; without pooling for ReLU / hard-swish,
-// with SE pooling for SiLU), TMA-staged dilated 3x3 (dw_tma.cuh, one undilated pass per phase); values of mtb_dw_kernel
-enum DwKernel { DW_GENERIC = 0, DW_TMA = 1, DW_STRIP_16B = 2, DW_STRIP_F32 = 3, DW_5X5_16B = 4, DW_5X5_POOL_16B = 5, DW_TMA_DIL = 6 };
-static_assert((int)DW_GENERIC == (int)MTB_DW_GENERIC && (int)DW_TMA == (int)MTB_DW_TMA && (int)DW_STRIP_16B == (int)MTB_DW_STRIP_16B &&
-              (int)DW_STRIP_F32 == (int)MTB_DW_STRIP_F32 && (int)DW_5X5_16B == (int)MTB_DW_5X5_16B &&
-              (int)DW_5X5_POOL_16B == (int)MTB_DW_5X5_POOL_16B && (int)DW_TMA_DIL == (int)MTB_DW_TMA_DIL,
-              "DwKernel must match mtb_dw_kernel");
 // kernel classes for the CUDA-event profiler (mtb_profile_begin / mtb_profile_end)
 enum KClass { KC_STEM = 0, KC_IGEMM_SIMT = 1, KC_DWCONV = 2, KC_POOL = 3, KC_SE_FC = 4, KC_TC_GEMM = 5, KC_FMB = 6,
               KC_HEAD_FUSED = 7, KC_HEAD_CONV_SIMT = 8, KC_SOFTARGMAX = 9, KC_RECON = 10, KC_OTHER = 11, KC_SE_SCALE = 12, KC_TC32 = 13,
@@ -48,6 +40,28 @@ const char* kKClassNames[KC_COUNT] = {"stem_conv_kernel", "conv_igemm_kernel", "
                                       "tc_head_softargmax_kernel", "head_conv(conv_igemm_kernel)",
                                       "softargmax_bhwn_kernel", "recon_pass1+2_kernel", "other", "se_scale_kernel", "tc32_conv_kernel",
                                       "combine_points_kernel"};
+// One row per mtb_kernel value: the profiler class of its launches, whether it exists for 16-bit storage only (bf16 /
+// fp16), and whether it also writes the SE pooling slices of its output (depthwise)
+struct KernelTraits { mtb_kernel kernel; KClass cls; bool only16, pools; };
+constexpr KernelTraits kKernels[] = {
+    {MTB_DW_GENERIC, KC_DWCONV, false, false},        {MTB_DW_TMA, KC_DWCONV, true, true},
+    {MTB_DW_STRIP_16B, KC_DWCONV, true, true},        {MTB_DW_STRIP_F32, KC_DWCONV, false, true},
+    {MTB_DW_5X5_16B, KC_DWCONV, true, false},         {MTB_DW_5X5_POOL_16B, KC_DWCONV, true, true},
+    {MTB_DW_TMA_DIL, KC_DWCONV, true, true},          {MTB_STEM_3X3S2, KC_STEM, false, false},
+    {MTB_STEM_WIDE, KC_STEM, false, false},           {MTB_STEM_GENERIC, KC_STEM, false, false},
+    {MTB_MAXPOOL, KC_OTHER, false, false},            {MTB_POOL_MEAN, KC_POOL, false, false},
+    {MTB_POOL_FUSED, KC_POOL, false, false},          {MTB_SE_FC, KC_SE_FC, false, false},
+    {MTB_IGEMM, KC_IGEMM_SIMT, false, false},         {MTB_TC_CONV, KC_TC_GEMM, true, false},
+    {MTB_TC_CONV_SE, KC_TC_GEMM, true, false},        {MTB_SE_SCALE_TC_CONV, KC_TC_GEMM, true, false},
+    {MTB_TC_CONV3X3S1, KC_TC_GEMM, true, false},      {MTB_TC32, KC_TC32, false, false},
+    {MTB_HEAD_FUSED, KC_HEAD_FUSED, true, false},     {MTB_HEAD_TC32, KC_TC32, false, false},
+    {MTB_HEAD_IGEMM, KC_HEAD_CONV_SIMT, false, false}};
+constexpr bool kernel_rows_in_order() {
+  for (int i = 0; i < (int)std::size(kKernels); ++i)
+    if (kKernels[i].kernel != i) return false;
+  return std::size(kKernels) == MTB_HEAD_IGEMM + 1;
+}
+static_assert(kernel_rows_in_order(), "kKernels: one row per mtb_kernel value, in order");
 constexpr int kMaxCombinePoints = 4096;  // n_in and n_out of combine_points_kernel (its shared memory holds n_in * 3 floats)
 enum { BUF_FEATURES = -2, BUF_NONE = -1, BUF_SMALL0 = 4 };  // 0..3 big activation buffers, 4..6 small [B,C]
 constexpr int kNumBig = 4, kNumSmall = 3;
@@ -70,15 +84,13 @@ struct Op {
   bool depthwise = false;
   bool small_io = false;  // squeeze-excitation FCs on [B,1,1,C] fp32 tensors
   float pre_scale[3] = {2.f, 2.f, 2.f}, pre_shift[3] = {-1.f, -1.f, -1.f};  // stem input affine (PreprocLayer: x*2-1)
-  bool fused_pool = false;  // this depthwise op also produces the SE pooled means (next op is skipped)
-  DwKernel dw_kernel = DW_GENERIC;  // depthwise: the kernel that runs it (set by mtb_finalize_weights)
+  mtb_kernel kernel = MTB_IGEMM;  // the kernel that runs it (choose_kernels, at mtb_finalize_weights)
+  bool fused_pool = false;  // depthwise: also writes the SE pooling slices of the pool op behind it (MTB_POOL_FUSED)
   DwTmaPlan dw_plan;                // DW_TMA / DW_TMA_DIL: its tiling plan (DW_TMA_DIL: of one phase of the dilation)
   int pool_slices = 1;              // DW_TMA* / DW_STRIP_* / DW_5X5_POOL_16B: partial pooling slices it leaves (= its gridDim.y / dw_plan.n_rb)
   bool res_first = false;  // residual added BEFORE the activation (ResNet); EfficientNet adds it after
   int pool_src = -1;       // fc1: index of the OP_POOL op that produces its input (fused pooling leaves partial slices)
   int ksplit = 1;          // split-K (squeeze-excitation fc1): raw sums, bias/act deferred to the consumer
-  int a_bias_from = -1;    // op index whose bias (+ a_act) is applied to THIS op's input on load
-  int a_act = ACT_NONE;
   bool pad_ok = false;    // weight tensor may be smaller than [Cout,Cin]: channels zero-padded to a multiple of 4
   float bn_eps = 1e-3f;
   float* d_w = nullptr;     // fp32 [R*S*Cin][Cout]  (dw: [R*S][C])
@@ -88,7 +100,6 @@ struct Op {
   FmbWeights fmb;           // 16-bit tensor-core modes: this 3x3 expand conv and the NEXT op (1x1 projection) run as one fmb_kernel launch
   mutable TmapCache dw_maps;    // DW_TMA / DW_TMA_DIL: its input tensor maps
   double flops = 0;         // 2*MACs per crop
-  int stage = 0;            // EfficientNet stage (1-based; 0 = stem / last conv / other backbones)
 };
 
 }  // namespace
@@ -98,7 +109,6 @@ struct mtb_handle {
   std::map<std::string, HostTensor> raw;
   std::vector<Op> ops;
   Op head;
-  bool head_fused = false;  // tc_head_kernel + head_finalize_kernel (tc_head_plan fits the feature map); else the unfused head
   // latent-point model (mtb_set_latent_recombination): the forward reconstructs head points [0, n_latents) and maps them to
   // n_out joints with recomb [n_latents][n_out]; n_latents == 0 for a plain model
   int n_latents = 0, n_out = 0;
@@ -319,7 +329,6 @@ void plan_effnet(mtb_handle* h, float bn_eps) {
   }
   for (int si = 0; si < c.n_stages; ++si) {
     const mtb_stage& st = c.stages[si];
-    const size_t stage_first_op = h->ops.size();
     for (int bi = 0; bi < st.layers; ++bi) {
       const bool first = bi == 0;
       const int cin = first ? st.cin : st.cout;
@@ -372,7 +381,6 @@ void plan_effnet(mtb_handle* h, float bn_eps) {
         P.cur = t3;
       }
     }
-    for (size_t k = stage_first_op; k < h->ops.size(); ++k) h->ops[k].stage = si + 1;
   }
   {
     char key[64];
@@ -721,15 +729,15 @@ int prepare_op_weights(mtb_handle* h, Op& op) {
   if (rc) return rc;
   rc = upload(h, bias.data(), bias.size() * 4, (void**)&op.d_bias);
   if (rc) return rc;
-  if (is_tc16(h) && tc_like) {
+  // the tensor-core kernels' own weight copies (the fused head prepares its own in mtb_finalize_weights)
+  if (kKernels[op.kernel].cls == KC_TC_GEMM) {
     const char* e = with_storage16(h, [&](auto* tag) {
       return tc_prepare_weights<std::remove_pointer_t<decltype(tag)>>(op.tc, wk.data(), bias.data(), K, op.Cout, op.R, op.S, op.Cin,
                                                                       h->dev_allocs);
     });
     if (e) return fail(h, MTB_ERR_CUDA, "tensor-core weight prep for '%s': %s", op.name.c_str(), e);
   }
-  if (h->cfg.precision == MTB_PRECISION_TF32X3 &&
-      tc32_eligible(op.type == OP_CONV, op.depthwise, op.small_io, op.R, op.stride, op.Cin, op.Cout)) {
+  if (kKernels[op.kernel].cls == KC_TC32) {
     const char* e = tc32_prepare_weights(op.tc32, wk.data(), bias.data(), K, op.Cout, op.R, op.S, op.Cin, h->dev_allocs);
     if (e) return fail(h, MTB_ERR_CUDA, "3xTF32 weight prep for '%s': %s", op.name.c_str(), e);
   }
@@ -815,11 +823,6 @@ bool dw5x5_eligible(const Op& op) {
          (op.act == ACT_SILU || op.act == ACT_RELU || op.act == ACT_HSWISH);
 }
 
-// the depthwise kernels that also write the SE pooling slices of their output
-bool dw_kernel_pools(DwKernel k) {
-  return k == DW_TMA || k == DW_TMA_DIL || k == DW_STRIP_16B || k == DW_STRIP_F32 || k == DW_5X5_POOL_16B;
-}
-
 constexpr int kDwOW = 4;  // outputs per thread along W in dwconv3x3_pool_16b_kernel (measured: 4 -> 3.65 ms, 2 -> 4.25 ms per 128 crops)
 constexpr int kDw5OW = 4;  // outputs per thread along W in dwconv5x5_16b_kernel
 
@@ -843,73 +846,103 @@ cudaError_t dw_dispatch(const Op& op, F&& f) {
   });
 }
 
+// ---------------------------------------------------------------------------------------------- kernel choice
+bool stem_fast_enabled() {  // MTB_STEM_FAST=0: the generic stem kernel (A/B runs, bit-equality test)
+  static int v = -1;
+  if (v < 0) {
+    const char* e = getenv("MTB_STEM_FAST");
+    v = (e && e[0] == '0') ? 0 : 1;
+  }
+  return v == 1;
+}
+
 // Picks the kernel of a depthwise op and the number of partial pooling slices it writes (fc1 sums that many).  bf16 and fp16
 // tensor-core modes: 5x5 ops run dwconv5x5_16b_kernel, which pools for SiLU (EfficientNet-B) and does not pool for ReLU /
 // hard-swish (MobileNetV3); 3x3 stride-1 ops run the TMA-staged kernel when a plan fits, the other 3x3 ops the 16-bit strip
 // kernel; 3x3 stride-1 SiLU ops with dilation 2 or 4 and SAME padding (the dilated EfficientNetV2 stages) run the TMA-staged
 // kernel phase by phase when a plan fits.  3xTF32 mode: the fp32 strip kernel (exact activation) for undilated 3x3 ops.  Other
 // modes and shapes: the generic kernel, which does not pool.
-void choose_dw_kernel(const mtb_handle* h, Op& op) {
-  op.dw_kernel = DW_GENERIC;
-  if (op.type == OP_DW && op.R == 3 && op.S == 3 && (op.dil == 2 || op.dil == 4)) {
+mtb_kernel choose_dw(const mtb_handle* h, Op& op) {
+  if (op.R == 3 && op.S == 3 && (op.dil == 2 || op.dil == 4)) {
     if (!is_tc16(h) || op.stride != 1 || op.act != ACT_SILU || op.Cout % 8 != 0 || op.pad_t != op.dil || op.pad_l != op.dil ||
         op.Hin != op.Hout || op.Win != op.Wout)
-      return;
+      return MTB_DW_GENERIC;
     const DwTmaPlan pl = dw_tma_plan((op.Hout + op.dil - 1) / op.dil, (op.Wout + op.dil - 1) / op.dil, op.dil);
-    if (pl.ok && pl.n_rb <= kPoolSlices) {
-      op.dw_kernel = DW_TMA_DIL;
-      op.dw_plan = pl;
-      op.pool_slices = pl.n_rb;
-    }
-    return;
+    if (!pl.ok || pl.n_rb > kPoolSlices) return MTB_DW_GENERIC;
+    op.dw_plan = pl;
+    op.pool_slices = pl.n_rb;
+    return MTB_DW_TMA_DIL;
   }
   if (dw5x5_eligible(op)) {
-    if (!is_tc16(h)) return;
-    if (op.act != ACT_SILU) {
-      op.dw_kernel = DW_5X5_16B;
-      return;
-    }
-    op.dw_kernel = DW_5X5_POOL_16B;
+    if (!is_tc16(h)) return MTB_DW_GENERIC;
+    if (op.act != ACT_SILU) return MTB_DW_5X5_16B;
     const int strips = op.Hout * ((op.Wout + kDw5OW - 1) / kDw5OW);
     const int groups = dw5_pool_shape(op.Cout).groups;
     op.pool_slices = std::min((strips + groups - 1) / groups, kPoolSlices);
-    return;
+    return MTB_DW_5X5_POOL_16B;
   }
-  if (!dw_strip_eligible(op)) return;
-  if (is_tc16(h)) {
-    if (op.stride == 1 && op.Hin == op.Hout && op.Win == op.Wout) {
-      const DwTmaPlan pl = dw_tma_plan(op.Hout, op.Wout);
-      if (pl.ok && pl.n_rb <= kPoolSlices) {
-        op.dw_kernel = DW_TMA;
-        op.dw_plan = pl;
-        op.pool_slices = pl.n_rb;
-        return;
-      }
+  if (!dw_strip_eligible(op) || !(is_tc16(h) || h->cfg.precision == MTB_PRECISION_TF32X3)) return MTB_DW_GENERIC;
+  if (is_tc16(h) && op.stride == 1 && op.Hin == op.Hout && op.Win == op.Wout) {
+    const DwTmaPlan pl = dw_tma_plan(op.Hout, op.Wout);
+    if (pl.ok && pl.n_rb <= kPoolSlices) {
+      op.dw_plan = pl;
+      op.pool_slices = pl.n_rb;
+      return MTB_DW_TMA;
     }
-    op.dw_kernel = DW_STRIP_16B;
-  } else if (h->cfg.precision == MTB_PRECISION_TF32X3) {
-    op.dw_kernel = DW_STRIP_F32;
-  } else {
-    return;
   }
   const int strips = op.Hout * ((op.Wout + kDwOW - 1) / kDwOW);
   op.pool_slices = std::min((strips + 7) / 8, kPoolSlices);
+  return is_tc16(h) ? MTB_DW_STRIP_16B : MTB_DW_STRIP_F32;
 }
 
-int op_class(const Op& op) {
-  switch (op.type) {
-    case OP_STEM: return KC_STEM;
-    case OP_DW: return KC_DWCONV;
-    case OP_POOL: return KC_POOL;
-    case OP_MAXPOOL: return KC_OTHER;
-    default: break;
+// A conv or GEMM op: the SE fully-connected layers run conv_igemm_kernel in fp32; the bf16 and fp16 tensor-core modes run
+// tc_conv_kernel where tc_eligible, with the SE scale inside the GEMM or in se_scale_kernel ahead of it (tc_se_in_gemm), or
+// tc_conv3x3s1_kernel for the shapes it takes; the 3xTF32 mode runs tc32_conv_kernel where tc32_eligible; everything else
+// runs conv_igemm_kernel.
+mtb_kernel choose_conv(const mtb_handle* h, const Op& op) {
+  if (op.small_io) return MTB_SE_FC;
+  if (is_tc16(h) && tc_eligible(true, op.depthwise, op.small_io, op.R, op.stride, op.Cin, op.Cout)) {
+    if (op.scale_buf != BUF_NONE) return tc_se_in_gemm(op.Cout) ? MTB_TC_CONV_SE : MTB_SE_SCALE_TC_CONV;
+    return tc3x3s1_eligible(op.R, op.S, op.stride, op.dil, op.Cin, op.Cout, op.act) ? MTB_TC_CONV3X3S1 : MTB_TC_CONV;
   }
-  if (op.small_io) return KC_SE_FC;
-  if (op.fmb.ready) return KC_FMB;
-  if (op.tc.ready) return KC_TC_GEMM;  // one class per kernel: every tensor-core conv/GEMM launch is tc_conv_kernel
-  if (op.tc32.ready) return KC_TC32;
-  return KC_IGEMM_SIMT;
+  if (h->cfg.precision == MTB_PRECISION_TF32X3 && tc32_eligible(true, op.depthwise, op.small_io, op.R, op.stride, op.Cin, op.Cout))
+    return MTB_TC32;
+  return MTB_IGEMM;
 }
+
+// Sets Op::kernel of every backbone op and of the head, and which depthwise ops pool for the SE op behind them.  (Whether a
+// FusedMBConv pair runs as one fmb_kernel launch is decided once its tensor-core weights exist, in mtb_finalize_weights.)
+void choose_kernels(mtb_handle* h) {
+  for (size_t i = 0; i < h->ops.size(); ++i) {
+    Op& op = h->ops[i];
+    switch (op.type) {
+      case OP_STEM: {
+        // stem3x3s2_kernel: EfficientNet's 3x3 stride-2 stem with 24 or 32 channels; stem_conv_wide_kernel: a multiple of 32,
+        // 24 or 16 channels
+        const bool s2 = op.R == 3 && op.S == 3 && op.Cin == 3 && op.stride == 2 && (op.Cout == 32 || op.Cout == 24);
+        op.kernel = s2 && stem_fast_enabled()                                  ? MTB_STEM_3X3S2
+                    : op.Cout % 32 == 0 || op.Cout % 24 == 0 || op.Cout % 16 == 0 ? MTB_STEM_WIDE
+                                                                                 : MTB_STEM_GENERIC;
+        break;
+      }
+      case OP_MAXPOOL: op.kernel = MTB_MAXPOOL; break;
+      case OP_POOL: op.kernel = i > 0 && h->ops[i - 1].fused_pool ? MTB_POOL_FUSED : MTB_POOL_MEAN; break;
+      case OP_DW: op.kernel = choose_dw(h, op); break;
+      case OP_CONV: op.kernel = choose_conv(h, op); break;
+    }
+    op.fused_pool = kKernels[op.kernel].pools && i + 1 < h->ops.size() && h->ops[i + 1].type == OP_POOL;
+  }
+  // the head: tc_head_kernel when a fused tile fits the feature map, else a GEMM into logits (tc32_conv_kernel where a conv
+  // of its shape runs it) and softargmax_bhwn_kernel
+  Op& hd = h->head;
+  int bnp, cpt, npt;
+  if (is_tc16(h) && tc_head_plan(h->feat_side * h->feat_side, &bnp, &cpt, &npt)) hd.kernel = MTB_HEAD_FUSED;
+  else if (choose_conv(h, hd) == MTB_TC32) hd.kernel = MTB_HEAD_TC32;
+  else hd.kernel = MTB_HEAD_IGEMM;
+}
+
+// profiler class of a backbone op: fmb_kernel for the first op of a fused FusedMBConv block
+int op_class(const Op& op) { return op.fmb.ready ? KC_FMB : kKernels[op.kernel].cls; }
 
 double op_weight_bytes(const Op& op) {
   if (op.type == OP_POOL || op.type == OP_MAXPOOL) return 0.0;
@@ -926,167 +959,143 @@ double op_bytes(const mtb_handle* h, const Op& op, int B) {
 }
 
 // ---------------------------------------------------------------------------------------------- executor
-bool stem_fast_enabled() {  // MTB_STEM_FAST=0: the generic stem kernel (A/B runs, bit-equality test)
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("MTB_STEM_FAST");
-    v = (e && e[0] == '0') ? 0 : 1;
+const char* cuda_msg(cudaError_t e) { return e == cudaSuccess ? nullptr : cudaGetErrorString(e); }
+
+// op.kernel's launch for the kernels that exist for every storage element type T (float, __nv_bfloat16 or __half);
+// nullptr on success
+template <typename T>
+const char* launch_op(mtb_handle* h, const Op& op, ConvParams p, const float* crops, float* pooled, const Workspace& ws,
+                      void* features, cudaStream_t st) {
+  const size_t pixels = (size_t)p.B * op.Hout * op.Wout;
+  switch (op.kernel) {
+    case MTB_STEM_3X3S2:
+    case MTB_STEM_WIDE:
+    case MTB_STEM_GENERIC: {
+      StemParams s;
+      s.in = crops;
+      s.out = p.out; s.w = op.d_w; s.bias = op.d_bias;
+      for (int i = 0; i < 3; ++i) { s.pre_scale[i] = op.pre_scale[i]; s.pre_shift[i] = op.pre_shift[i]; }
+      s.pre_scale[3] = 1.f; s.pre_shift[3] = 0.f;
+      s.B = p.B; s.Hin = op.Hin; s.Win = op.Win; s.Cin = op.Cin; s.Hout = op.Hout; s.Wout = op.Wout; s.Cout = op.Cout;
+      s.R = op.R; s.S = op.S; s.stride = op.stride; s.pad_t = op.pad_t; s.pad_l = op.pad_l; s.act = op.act;
+      const size_t smem = ((size_t)op.R * op.S * op.Cin + 1) * op.Cout * 4;
+      const bool s2 = op.kernel == MTB_STEM_3X3S2, wide = op.kernel == MTB_STEM_WIDE;
+      if (s2 && op.Cout == 32) launch_k(stem3x3s2_kernel<T, 32>, dim3(grid_for(pixels, 128)), dim3(128), (size_t)28 * 32 * 4, st, s);
+      else if (s2) launch_k(stem3x3s2_kernel<T, 24>, dim3(grid_for(pixels, 128)), dim3(128), (size_t)28 * 24 * 4, st, s);
+      else if (wide && op.Cout % 32 == 0) launch_k(stem_conv_wide_kernel<T, 32>, dim3(grid_for(pixels * (op.Cout / 32), 128)), dim3(128), smem, st, s);
+      else if (wide && op.Cout % 24 == 0) launch_k(stem_conv_wide_kernel<T, 24>, dim3(grid_for(pixels * (op.Cout / 24), 128)), dim3(128), smem, st, s);
+      else if (wide) launch_k(stem_conv_wide_kernel<T, 16>, dim3(grid_for(pixels * (op.Cout / 16), 128)), dim3(128), smem, st, s);
+      else launch_k(stem_conv_kernel<T>, dim3(grid_for(pixels * (op.Cout / 4), 256)), dim3(256), smem, st, s);
+      return nullptr;
+    }
+    case MTB_MAXPOOL:
+      launch_k(maxpool_kernel<T>, dim3(grid_for(pixels * (op.Cout / 4), 256)), dim3(256), 0, st, p);
+      return nullptr;
+    case MTB_POOL_MEAN:
+      launch_k(pool_mean_kernel<T>, dim3((op.Cin + 127) / 128, p.B), dim3(32, 8), 0, st, (const T*)p.in, (float*)p.out,
+               op.Hin * op.Win, op.Cin);
+      return nullptr;
+    case MTB_SE_FC: {
+      if (op.pool_src > 0 && h->ops[op.pool_src].kernel == MTB_POOL_FUSED) {  // input = partial pooling slices of the depthwise kernel
+        p.a_splits = h->ops[op.pool_src - 1].pool_slices;
+        p.a_split_stride = (size_t)p.B * op.Cin;
+      }
+      if (op.ksplit == 1) return cuda_msg(launch_conv_igemm<float, float>(p, st));
+      // split-K partial slices go to the (still unused) scale buffer, then one tiny reduce kernel
+      float* final_out = (float*)p.out;
+      p.ksplit = op.ksplit;
+      p.out = buf_ptr(ws, BUF_SMALL0 + 2, features);
+      if (const char* e = cuda_msg(launch_conv_igemm<float, float>(p, st))) return e;
+      const int n = p.B * op.Cout;
+      launch_k(se_reduce_kernel, dim3((n + 255) / 256), dim3(256), 0, st, (const float*)p.out, (const float*)op.d_bias, final_out, n,
+               op.Cout, op.ksplit, op.act);
+      h->launches++;
+      return nullptr;
+    }
+    case MTB_IGEMM: return cuda_msg(launch_conv_igemm<T, T>(p, st));
+    case MTB_TC32: return tc32_conv_launch(op.tc32, p, op.res_first, st);  // SE scale (p.a_scale) applied by the splitter warps
+    case MTB_DW_GENERIC:
+      launch_k(dwconv_kernel<T>, dim3(grid_for(pixels * (op.Cout / 4), 256)), dim3(256), 0, st, p);
+      return nullptr;
+    case MTB_DW_STRIP_F32:  // 4 channels x 4 pixels per thread, SE squeeze fused (partial slices summed by fc1)
+      return cuda_msg(dw_dispatch<ACT_SILU, ACT_RELU, ACT_HSWISH>(op, [&](auto s, auto a) {
+        return launch_k(dwconv3x3_pool_f32_kernel<s, a, kDwOW>, dim3((op.Cout / 4 + 31) / 32, op.pool_slices, p.B), dim3(32, 8), 0,
+                        st, p, pooled);
+      }));
+    default: return "not a backbone kernel";
   }
-  return v == 1;
 }
 
-// T: the storage element type (float, __nv_bfloat16 or __half); the tensor-core and TMA kernels only exist for the 16-bit types
+// op.kernel's launch for the kernels that exist for 16-bit storage only (T: __nv_bfloat16 or __half): the tensor-core and
+// 16-bit depthwise kernels; nullptr on success
 template <typename T>
-int run_op_t(mtb_handle* h, const Op& op, const float* crops, int B, const Workspace& ws, void* features,
-             cudaStream_t st) {
-  constexpr bool k16 = sizeof(T) == 2;
-  if constexpr (k16) {
-    if (op.type == OP_CONV && op.tc.ready && op.scale_buf != BUF_NONE && !tc_se_in_gemm(op.Cout)) {
-      // squeeze-excitation scale applied in place ahead of a 16-bit tensor-core conv that does not apply it itself
-      void* x = buf_ptr(ws, op.in_buf, features);
-      const double bytes = 2.0 * B * op.Hin * op.Win * op.Cin * elem_size(h);
-      ProfScope ps(h, KC_SE_SCALE, 0.0, bytes, st, false);
-      const char* e = tc_se_scale_launch<T>(x, (const float*)buf_ptr(ws, op.scale_buf, features), B, op.Hin * op.Win, op.Cin, st);
-      if (e) return fail(h, MTB_ERR_CUDA, "se scale %s: %s", op.name.c_str(), e);
-      h->launches++;
+const char* launch_op16(const Op& op, const ConvParams& p, float* pooled, cudaStream_t st) {
+  switch (op.kernel) {
+    case MTB_TC_CONV:
+    case MTB_TC_CONV_SE:
+    case MTB_SE_SCALE_TC_CONV: return tc_conv_launch<T>(op.tc, p, op.res_first, false, st);
+    case MTB_TC_CONV3X3S1: return tc_conv_launch<T>(op.tc, p, op.res_first, true, st);
+    case MTB_DW_TMA:
+    case MTB_DW_TMA_DIL:
+      return dw_tma_launch<T>(op.dw_maps, op.dw_plan, p.in, p.out, op.d_w, op.d_bias, pooled, p.B, op.Hout, op.Wout, op.Cout,
+                              op.pad_t, op.pad_l, op.act, op.kernel == MTB_DW_TMA ? 1 : op.dil, st);
+    case MTB_DW_STRIP_16B:
+      return cuda_msg(dw_dispatch<ACT_SILU, ACT_RELU, ACT_HSWISH>(op, [&](auto s, auto a) {
+        return launch_k(dwconv3x3_pool_16b_kernel<T, s, a, kDwOW>, dim3((op.Cout / 8 + 31) / 32, op.pool_slices, p.B), dim3(32, 8),
+                        0, st, p, pooled);
+      }));
+    case MTB_DW_5X5_16B: {
+      const size_t items = (size_t)p.B * op.Hout * ((op.Wout + kDw5OW - 1) / kDw5OW) * (op.Cout / 8);
+      return cuda_msg(dw_dispatch<ACT_RELU, ACT_HSWISH>(op, [&](auto s, auto a) {
+        return launch_k(dwconv5x5_16b_kernel<T, s, a, kDw5OW>, dim3(grid_for(items, 256)), dim3(256), 0, st, p, nullptr);
+      }));
     }
+    case MTB_DW_5X5_POOL_16B: {
+      const Dw5PoolShape sh = dw5_pool_shape(op.Cout);
+      return cuda_msg(dw_dispatch<ACT_SILU>(op, [&](auto s, auto a) {
+        return launch_k(dwconv5x5_16b_kernel<T, s, a, kDw5OW, true>, dim3(sh.chunks, op.pool_slices, p.B), dim3(sh.cb * sh.groups),
+                        0, st, p, pooled);
+      }));
+    }
+    default: return "not a 16-bit backbone kernel";
   }
-  ProfScope prof(h, op_class(op), op.flops * B, op_bytes(h, op, B), st);
-  switch (op.type) {
-    case OP_STEM: {
-      StemParams p;
-      p.in = crops;
-      p.out = buf_ptr(ws, op.out_buf, features); p.w = op.d_w; p.bias = op.d_bias;
-      for (int i = 0; i < 3; ++i) { p.pre_scale[i] = op.pre_scale[i]; p.pre_shift[i] = op.pre_shift[i]; }
-      p.pre_scale[3] = 1.f; p.pre_shift[3] = 0.f;
-      p.B = B; p.Hin = op.Hin; p.Win = op.Win; p.Cin = op.Cin; p.Hout = op.Hout; p.Wout = op.Wout; p.Cout = op.Cout;
-      p.R = op.R; p.S = op.S; p.stride = op.stride; p.pad_t = op.pad_t; p.pad_l = op.pad_l; p.act = op.act;
-      size_t smem = ((size_t)op.R * op.S * op.Cin + 1) * op.Cout * 4;
-      const size_t pixels = (size_t)B * op.Hout * op.Wout;
-      const bool effnet_stem = op.R == 3 && op.S == 3 && op.Cin == 3 && op.stride == 2 && stem_fast_enabled();
-      if (effnet_stem && op.Cout == 32) launch_k(stem3x3s2_kernel<T, 32>, dim3(grid_for(pixels, 128)), dim3(128), (size_t)28 * 32 * 4, st, p);
-      else if (effnet_stem && op.Cout == 24) launch_k(stem3x3s2_kernel<T, 24>, dim3(grid_for(pixels, 128)), dim3(128), (size_t)28 * 24 * 4, st, p);
-      else if (op.Cout % 32 == 0) launch_k(stem_conv_wide_kernel<T, 32>, dim3(grid_for(pixels * (op.Cout / 32), 128)), dim3(128), smem, st, p);
-      else if (op.Cout % 24 == 0) launch_k(stem_conv_wide_kernel<T, 24>, dim3(grid_for(pixels * (op.Cout / 24), 128)), dim3(128), smem, st, p);
-      else if (op.Cout % 16 == 0) launch_k(stem_conv_wide_kernel<T, 16>, dim3(grid_for(pixels * (op.Cout / 16), 128)), dim3(128), smem, st, p);
-      else launch_k(stem_conv_kernel<T>, dim3(grid_for(pixels * (op.Cout / 4), 256)), dim3(256), smem, st, p);
-      h->launches++;
-      break;
-    }
-    case OP_CONV:
-    case OP_DW:
-    case OP_MAXPOOL: {
-      ConvParams p;
-      p.in = buf_ptr(ws, op.in_buf, features);
-      p.out = buf_ptr(ws, op.out_buf, features);
-      p.res = buf_ptr(ws, op.res_buf, features);
-      p.a_scale = (const float*)buf_ptr(ws, op.scale_buf, features);
-      p.w = op.d_w; p.bias = op.d_bias;
-      p.B = B; p.Hin = op.Hin; p.Win = op.Win; p.Cin = op.Cin; p.Hout = op.Hout; p.Wout = op.Wout; p.Cout = op.Cout;
-      p.R = op.R; p.S = op.S; p.stride = op.stride; p.dil = op.dil; p.pad_t = op.pad_t; p.pad_l = op.pad_l; p.act = op.act;
-      p.res_first = op.res_first ? 1 : 0;
-      if (op.type == OP_DW) {
-        float* pooled = op.fused_pool ? (float*)buf_ptr(ws, BUF_SMALL0, features) : nullptr;
-        if (op.dw_kernel == DW_TMA || op.dw_kernel == DW_TMA_DIL || op.dw_kernel == DW_STRIP_16B) {
-          if constexpr (!k16) {
-            return fail(h, MTB_ERR_CUDA, "depthwise %s: 16-bit kernel chosen for fp32 storage", op.name.c_str());
-          } else if (op.dw_kernel == DW_TMA || op.dw_kernel == DW_TMA_DIL) {
-            const char* e = dw_tma_launch<T>(op.dw_maps, op.dw_plan, p.in, p.out, op.d_w, op.d_bias, pooled, B, op.Hout, op.Wout,
-                                             op.Cout, op.pad_t, op.pad_l, op.act, op.dw_kernel == DW_TMA ? 1 : op.dil, st);
-            if (e) return fail(h, MTB_ERR_CUDA, "depthwise (TMA) launch %s: %s", op.name.c_str(), e);
-          } else {
-            const dim3 grid((op.Cout / 8 + 31) / 32, op.pool_slices, B), block(32, 8);
-            const cudaError_t e = dw_dispatch<ACT_SILU, ACT_RELU, ACT_HSWISH>(op, [&](auto s, auto a) {
-              return launch_k(dwconv3x3_pool_16b_kernel<T, s, a, kDwOW>, grid, block, 0, st, p, pooled);
-            });
-            if (e != cudaSuccess) return fail(h, MTB_ERR_CUDA, "depthwise launch %s: %s", op.name.c_str(), cudaGetErrorString(e));
-          }
-        } else if (op.dw_kernel == DW_STRIP_F32) {
-          // fp32 strip kernel: 4 channels x 4 pixels per thread, SE squeeze fused (partial slices summed by fc1)
-          const dim3 grid((op.Cout / 4 + 31) / 32, op.pool_slices, B), block(32, 8);
-          const cudaError_t e = dw_dispatch<ACT_SILU, ACT_RELU, ACT_HSWISH>(op, [&](auto s, auto a) {
-            return launch_k(dwconv3x3_pool_f32_kernel<s, a, kDwOW>, grid, block, 0, st, p, pooled);
-          });
-          if (e != cudaSuccess) return fail(h, MTB_ERR_CUDA, "depthwise launch %s: %s", op.name.c_str(), cudaGetErrorString(e));
-        } else if (op.dw_kernel == DW_5X5_16B || op.dw_kernel == DW_5X5_POOL_16B) {
-          if constexpr (!k16) {
-            return fail(h, MTB_ERR_CUDA, "depthwise %s: 16-bit kernel chosen for fp32 storage", op.name.c_str());
-          } else {
-            cudaError_t e;
-            if (op.dw_kernel == DW_5X5_16B) {
-              const size_t items = (size_t)B * op.Hout * ((op.Wout + kDw5OW - 1) / kDw5OW) * (op.Cout / 8);
-              const dim3 grid(grid_for(items, 256));
-              e = dw_dispatch<ACT_RELU, ACT_HSWISH>(op, [&](auto s, auto a) {
-                return launch_k(dwconv5x5_16b_kernel<T, s, a, kDw5OW>, grid, dim3(256), 0, st, p, nullptr);
-              });
-            } else {
-              const Dw5PoolShape sh = dw5_pool_shape(op.Cout);
-              const dim3 grid(sh.chunks, op.pool_slices, B), block(sh.cb * sh.groups);
-              e = dw_dispatch<ACT_SILU>(op, [&](auto s, auto a) {
-                return launch_k(dwconv5x5_16b_kernel<T, s, a, kDw5OW, true>, grid, block, 0, st, p, pooled);
-              });
-            }
-            if (e != cudaSuccess) return fail(h, MTB_ERR_CUDA, "depthwise launch %s: %s", op.name.c_str(), cudaGetErrorString(e));
-          }
-        } else {
-          size_t total = (size_t)B * op.Hout * op.Wout * (op.Cout / 4);
-          launch_k(dwconv_kernel<T>, dim3(grid_for(total, 256)), dim3(256), 0, st, p);
-        }
-      } else if (op.type == OP_MAXPOOL) {
-        size_t total = (size_t)B * op.Hout * op.Wout * (op.Cout / 4);
-        launch_k(maxpool_kernel<T>, dim3(grid_for(total, 256)), dim3(256), 0, st, p);
-      } else if (op.small_io) {
-        if (op.pool_src > 0 && h->ops[op.pool_src].fused_pool) {  // input = partial pooling slices of the depthwise kernel
-          p.a_splits = h->ops[op.pool_src - 1].pool_slices;
-          p.a_split_stride = (size_t)B * op.Cin;
-        }
-        float* final_out = (float*)p.out;
-        if (op.ksplit > 1) {  // split-K partial slices go to the (still unused) scale buffer, then one tiny reduce kernel
-          p.ksplit = op.ksplit;
-          p.out = buf_ptr(ws, BUF_SMALL0 + 2, features);
-        }
-        cudaError_t e = launch_conv_igemm<float, float>(p, st);
-        if (e == cudaSuccess && op.ksplit > 1) {
-          const int n = B * op.Cout;
-          launch_k(se_reduce_kernel, dim3((n + 255) / 256), dim3(256), 0, st, (const float*)p.out, (const float*)op.d_bias, final_out, n,
-                   op.Cout, op.ksplit, op.act);
-          h->launches++;
-          e = cudaGetLastError();
-        }
-        if (e != cudaSuccess) return fail(h, MTB_ERR_CUDA, "launch %s: %s", op.name.c_str(), cudaGetErrorString(e));
-      } else if (op.tc.ready) {
-        if constexpr (!k16) return fail(h, MTB_ERR_CUDA, "%s: tensor-core weights in an fp32 mode", op.name.c_str());
-        else {
-          if (!tc_se_in_gemm(op.Cout)) p.a_scale = nullptr;  // already applied by se_scale_kernel
-          const char* e = tc_conv_launch<T>(op.tc, p, op.res_first, st);
-          if (e) return fail(h, MTB_ERR_CUDA, "tensor-core launch %s: %s", op.name.c_str(), e);
-        }
-      } else if (op.tc32.ready) {
-        const char* e = tc32_conv_launch(op.tc32, p, op.res_first, st);  // SE scale (p.a_scale) applied by the splitter warps
-        if (e) return fail(h, MTB_ERR_CUDA, "3xTF32 launch %s: %s", op.name.c_str(), e);
-      } else {
-        cudaError_t e = launch_conv_igemm<T, T>(p, st);
-        if (e != cudaSuccess) return fail(h, MTB_ERR_CUDA, "launch %s: %s", op.name.c_str(), cudaGetErrorString(e));
-      }
-      h->launches++;
-      break;
-    }
-    case OP_POOL: {
-      dim3 grid((op.Cin + 127) / 128, B), block(32, 8);
-      launch_k(pool_mean_kernel<T>, dim3(grid), dim3(block), 0, st, (const T*)buf_ptr(ws, op.in_buf, features),
-                                                   (float*)buf_ptr(ws, op.out_buf, features), op.Hin * op.Win, op.Cin);
-      h->launches++;
-      break;
-    }
-  }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(h, MTB_ERR_CUDA, "launch %s: %s", op.name.c_str(), cudaGetErrorString(e));
-  return MTB_OK;
 }
 
 int run_op(mtb_handle* h, const Op& op, const float* crops, int B, const Workspace& ws, void* features, cudaStream_t st) {
-  if (op.type == OP_POOL && op.fused_pool) return MTB_OK;  // produced by the preceding depthwise kernel
-  return with_storage(h, [&](auto* tag) { return run_op_t<std::remove_pointer_t<decltype(tag)>>(h, op, crops, B, ws, features, st); });
+  if (op.kernel == MTB_POOL_FUSED) return MTB_OK;  // produced by the preceding depthwise kernel
+  const bool only16 = kKernels[op.kernel].only16;
+  if (only16 && !is_16b(h)) return fail(h, MTB_ERR_CUDA, "%s: 16-bit kernel chosen for fp32 storage", op.name.c_str());
+  ConvParams p;
+  p.in = buf_ptr(ws, op.in_buf, features);
+  p.out = buf_ptr(ws, op.out_buf, features);
+  p.res = buf_ptr(ws, op.res_buf, features);
+  p.a_scale = (const float*)buf_ptr(ws, op.scale_buf, features);
+  p.w = op.d_w; p.bias = op.d_bias;
+  p.B = B; p.Hin = op.Hin; p.Win = op.Win; p.Cin = op.Cin; p.Hout = op.Hout; p.Wout = op.Wout; p.Cout = op.Cout;
+  p.R = op.R; p.S = op.S; p.stride = op.stride; p.dil = op.dil; p.pad_t = op.pad_t; p.pad_l = op.pad_l; p.act = op.act;
+  p.res_first = op.res_first ? 1 : 0;
+  if (op.kernel == MTB_SE_SCALE_TC_CONV) {
+    // squeeze-excitation scale applied in place ahead of the tensor-core conv, which then runs without it
+    const double bytes = 2.0 * B * op.Hin * op.Win * op.Cin * elem_size(h);
+    ProfScope ps(h, KC_SE_SCALE, 0.0, bytes, st, false);
+    const char* e = with_storage16(h, [&](auto* tag) {
+      return tc_se_scale_launch<std::remove_pointer_t<decltype(tag)>>(buf_ptr(ws, op.in_buf, features), p.a_scale, B, op.Hin * op.Win,
+                                                                      op.Cin, st);
+    });
+    if (e) return fail(h, MTB_ERR_CUDA, "se scale %s: %s", op.name.c_str(), e);
+    h->launches++;
+    p.a_scale = nullptr;
+  }
+  float* pooled = op.fused_pool ? (float*)buf_ptr(ws, BUF_SMALL0, features) : nullptr;
+  ProfScope prof(h, op_class(op), op.flops * B, op_bytes(h, op, B), st);
+  const char* e = only16 ? with_storage16(h, [&](auto* tag) { return launch_op16<std::remove_pointer_t<decltype(tag)>>(op, p, pooled, st); })
+                         : with_storage(h, [&](auto* tag) {
+                             return launch_op<std::remove_pointer_t<decltype(tag)>>(h, op, p, crops, pooled, ws, features, st);
+                           });
+  if (!e) e = cuda_msg(cudaGetLastError());
+  if (e) return fail(h, MTB_ERR_CUDA, "launch %s: %s", op.name.c_str(), e);
+  h->launches++;
+  return MTB_OK;
 }
 
 // The executor runs every op on the whole batch: running a stage crop chunk by crop chunk (intermediates resident in L2)
@@ -1169,7 +1178,7 @@ int head_decode_impl(mtb_handle* h, const void* features, int B, float* c2d, flo
   const double feat_bytes = (double)B * P * op.Cin * elem_size(h);
   const int J = head_points(h);
   const double out_bytes = (double)B * J * 5 * 4;
-  if (h->head_fused) {
+  if (op.kernel == MTB_HEAD_FUSED) {
     // fused: 1x1-conv GEMM on the tensor cores with the soft-argmax reduction in the epilogue; logits never reach HBM
     ProfScope prof(h, KC_HEAD_FUSED, op.flops * B, feat_bytes + (double)op.Cin * op.Cout * 2 + out_bytes, st);
     const char* e = with_storage16(h, [&](auto* tag) {
@@ -1186,17 +1195,14 @@ int head_decode_impl(mtb_handle* h, const void* features, int B, float* c2d, flo
   p.B = B; p.Hin = p.Hout = op.Hin; p.Win = p.Wout = op.Win; p.Cin = op.Cin; p.Cout = op.Cout;
   p.R = p.S = 1; p.stride = 1; p.dil = 1; p.pad_t = p.pad_l = 0; p.act = ACT_NONE;
   const double logit_bytes = (double)B * P * op.Cout * 4;
-  cudaError_t e;
-  if (op.tc32.ready) {  // 3xTF32 GEMM -> fp32 NHWC logits
-    ProfScope prof(h, KC_TC32, op.flops * B, feat_bytes + (double)op.Cin * op.Cout * 4 + logit_bytes, st);
-    const char* te = tc32_conv_launch(op.tc32, p, false, st);
-    if (te) return fail(h, MTB_ERR_CUDA, "3xTF32 head conv: %s", te);
-    e = cudaSuccess;
-  } else {
-    ProfScope prof(h, KC_HEAD_CONV_SIMT, op.flops * B, feat_bytes + (double)op.Cin * op.Cout * 4 + logit_bytes, st);
-    e = with_storage(h, [&](auto* tag) { return launch_conv_igemm<std::remove_pointer_t<decltype(tag)>, float>(p, st); });
+  {
+    // HEAD_TC32: 3xTF32 GEMM, HEAD_IGEMM: conv_igemm_kernel -> fp32 NHWC logits
+    ProfScope prof(h, kKernels[op.kernel].cls, op.flops * B, feat_bytes + (double)op.Cin * op.Cout * 4 + logit_bytes, st);
+    const char* e = op.kernel == MTB_HEAD_TC32
+                        ? tc32_conv_launch(op.tc32, p, false, st)
+                        : cuda_msg(with_storage(h, [&](auto* tag) { return launch_conv_igemm<std::remove_pointer_t<decltype(tag)>, float>(p, st); }));
+    if (e) return fail(h, MTB_ERR_CUDA, "head conv: %s", e);
   }
-  if (e != cudaSuccess) return fail(h, MTB_ERR_CUDA, "head conv: %s", cudaGetErrorString(e));
   ProfScope prof(h, KC_SOFTARGMAX, 0.0, logit_bytes + out_bytes, st);
   const char* se = launch_softargmax_bhwn<float>(p.out, c2d, c3d, B, J, c.depth, op.Hin, op.Win, op.Cout, make_scale(c), st);
   if (se) return fail(h, MTB_ERR_CUDA, "softargmax: %s", se);
@@ -1457,12 +1463,7 @@ int mtb_finalize_weights(mtb_handle* h) {
   h->graphs.clear();
   for (void* p : h->dev_allocs) cudaFree(p);
   h->dev_allocs.clear();
-  for (auto& op : h->ops) {
-    op.fused_pool = false;
-    choose_dw_kernel(h, op);
-  }
-  for (size_t i = 0; i + 1 < h->ops.size(); ++i)  // the strip and TMA-staged depthwise kernels also pool for the SE block behind them
-    if (dw_kernel_pools(h->ops[i].dw_kernel) && h->ops[i + 1].type == OP_POOL) h->ops[i].fused_pool = h->ops[i + 1].fused_pool = true;
+  choose_kernels(h);
   for (auto& op : h->ops) {
     int rc = prepare_op_weights(h, op);
     if (rc) return rc;
@@ -1525,21 +1526,17 @@ int mtb_finalize_weights(mtb_handle* h) {
     }
     int rc = prepare_op_weights(h, hd);
     if (rc) return rc;
-    if (is_tc16(h)) {
-      int bnp, cpt, npt;
-      if (tc_head_plan(h->feat_side * h->feat_side, &bnp, &cpt, &npt)) {
-        // the ORIGINAL (unpadded) [n_real][C] weight: the fused kernel masks rows itself
-        std::vector<float> w0((size_t)n_real * hd.Cin), b0(n_real);
-        for (int n = 0; n < n_real; ++n) {
-          b0[n] = find(h, hd.biaskey)->data[n];
-          for (int cc = 0; cc < hd.Cin; ++cc) w0[(size_t)n * hd.Cin + cc] = w->data[(size_t)n * hd.Cin + cc];
-        }
-        const char* e = with_storage16(h, [&](auto* tag) {
-          return tc_prepare_head<std::remove_pointer_t<decltype(tag)>>(hd.tc, w0.data(), b0.data(), hd.Cin, n_real, h->dev_allocs);
-        });
-        if (e) return fail(h, MTB_ERR_CUDA, "tensor-core head weight prep: %s", e);
-        h->head_fused = true;
+    if (hd.kernel == MTB_HEAD_FUSED) {
+      // the ORIGINAL (unpadded) [n_real][C] weight: the fused kernel masks rows itself
+      std::vector<float> w0((size_t)n_real * hd.Cin), b0(n_real);
+      for (int n = 0; n < n_real; ++n) {
+        b0[n] = find(h, hd.biaskey)->data[n];
+        for (int cc = 0; cc < hd.Cin; ++cc) w0[(size_t)n * hd.Cin + cc] = w->data[(size_t)n * hd.Cin + cc];
       }
+      const char* e = with_storage16(h, [&](auto* tag) {
+        return tc_prepare_head<std::remove_pointer_t<decltype(tag)>>(hd.tc, w0.data(), b0.data(), hd.Cin, n_real, h->dev_allocs);
+      });
+      if (e) return fail(h, MTB_ERR_CUDA, "tensor-core head weight prep: %s", e);
     }
   }
   h->d_recomb = nullptr;
@@ -2223,7 +2220,8 @@ int mtb_debug_run_op(mtb_handle* h, int op_index, const float* in, const float* 
   if (res) { o.res_buf = 1; put(res, 1, n_out, false); }
   if (scale) { o.scale_buf = BUF_SMALL0 + 2; put(scale, o.scale_buf, (size_t)batch * o.Cin, true); }
   o.out_buf = (o.type == OP_POOL || o.small_io) ? BUF_SMALL0 + 1 : 2;
-  o.fused_pool = false;      // in isolation a depthwise op does not pool and a pool op runs its own kernel
+  o.fused_pool = false;  // in isolation a depthwise op does not pool and a pool op runs its own kernel
+  if (o.kernel == MTB_POOL_FUSED) o.kernel = MTB_POOL_MEAN;
   rc = run_op(h, o, crops, batch, ws, nullptr, st);
   if (rc) return rc;
   void* src = buf_ptr(ws, o.out_buf, nullptr);
@@ -2233,17 +2231,10 @@ int mtb_debug_run_op(mtb_handle* h, int op_index, const float* in, const float* 
   return MTB_OK;
 }
 
-int mtb_op_dw_kernel(const mtb_handle* h, int op) {
+int mtb_op_kernel(const mtb_handle* h, int op) {
   if (!h || op < 0 || op >= (int)h->ops.size()) return fail(h, MTB_ERR_INVALID_ARG, "op index out of range");
-  if (h->ops[op].type != OP_DW) return fail(h, MTB_ERR_INVALID_ARG, "op %d (%s) is not depthwise", op, h->ops[op].name.c_str());
-  return h->ops[op].dw_kernel;
-}
-
-int mtb_op_tc_kernel(const mtb_handle* h, int op) {
-  if (!h || op < 0 || op >= (int)h->ops.size()) return fail(h, MTB_ERR_INVALID_ARG, "op index out of range");
-  const Op& o = h->ops[op];
-  if (!o.tc.ready) return fail(h, MTB_ERR_INVALID_ARG, "op %d (%s) has no 16-bit tensor-core weights", op, o.name.c_str());
-  return tc3x3s1_eligible(o.R, o.S, o.stride, o.dil, o.Cin, o.Cout, o.act) ? MTB_TC_CONV3X3S1 : MTB_TC_CONV;  // as tc_conv_launch
+  if (!h->finalized) return fail(h, MTB_ERR_NOT_FINALIZED, "mtb_finalize_weights has not been called");
+  return h->ops[op].kernel;
 }
 
 int mtb_op_is_fused_block(const mtb_handle* h, int op_index) {

@@ -832,9 +832,10 @@ inline int tc_pick_bn(int cout) { return cout <= 32 ? 32 : cout <= 64 ? 64 : 128
 // the tensor, at 3 and 5 (EfficientNetV2-L stages 6 and 7, Cout 384 and 640) more (DESIGN.md section 2).
 inline bool tc_se_in_gemm(int cout) { return cout <= 256; }
 
-// T: the storage type the weights were prepared in (tc_prepare_weights<T>)
+// T: the storage type the weights were prepared in (tc_prepare_weights<T>).  s1: run tc_conv3x3s1_kernel, for a shape
+// that tc3x3s1_eligible takes; else tc_conv_kernel.
 template <typename T>
-inline const char* tc_conv_launch(const TcWeights& w, const ConvParams& p, bool res_first, cudaStream_t st) {
+inline const char* tc_conv_launch(const TcWeights& w, const ConvParams& p, bool res_first, bool s1, cudaStream_t st) {
   TcConvParams q;
   q.res = p.res; q.bias = w.d_bias; q.out = p.out;
   q.mode = (p.R == 1 && p.stride == 1) ? 0 : 1;
@@ -848,8 +849,7 @@ inline const char* tc_conv_launch(const TcWeights& w, const ConvParams& p, bool 
   q.M = p.B * p.Hout * p.Wout;
   if (p.a_scale && (q.mode != 0 || !tc_se_in_gemm(p.Cout)))
     return "squeeze-excitation scale outside the 1x1 projections tc_conv_kernel scales (tc_se_in_gemm)";
-  // tc_conv3x3s1_kernel for the shapes it takes (bn: its K per tap and N tile), tc_conv_kernel for every other conv
-  const bool s1 = tc3x3s1_eligible(p.R, p.S, p.stride, p.dil, p.Cin, p.Cout, p.act);
+  // tc_conv3x3s1_kernel: bn is its K per tap and N tile
   const int bn = s1 ? tc3x3s1_width(p.Cin, p.Cout) : tc_pick_bn(p.Cout);
   q.m_tiles = q.mode == 0 ? (q.M + TC_BM - 1) / TC_BM : p.B * q.tiles_w * q.tiles_h;
   q.n_tiles = (p.Cout + bn - 1) / bn;

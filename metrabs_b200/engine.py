@@ -322,20 +322,29 @@ class Engine:
                                      ws.data_ptr(), ws.numel(), _stream_ptr(self.device)), self._h)
         return out
 
-    def op_dw_kernel(self, op):
-        """The kernel finalize chose for depthwise op `op`: one of _lib.DW_GENERIC, DW_TMA, DW_STRIP_16B, DW_STRIP_F32,
-        DW_5X5_16B, DW_5X5_POOL_16B, DW_TMA_DIL."""
-        k = lib().mtb_op_dw_kernel(self._h, op)
+    def op_kernel(self, op):
+        """The kernel finalize chose for backbone op `op`: one of the mtb_kernel values of _lib (DW_GENERIC ... HEAD_IGEMM)."""
+        k = lib().mtb_op_kernel(self._h, op)
         if k < 0:
             check(k, self._h)
         return k
 
+    # Narrower views of op_kernel for existing callers: they read the same choice, so they cannot disagree with it.
+    def op_dw_kernel(self, op):
+        """op_kernel of depthwise op `op`: one of _lib.DW_GENERIC ... DW_TMA_DIL; raises for any other op."""
+        k = self.op_kernel(op)
+        if k > _lib.DW_TMA_DIL:
+            raise _lib.MetrabsB200Error(f'op {op} is not depthwise')
+        return k
+
     def op_tc_kernel(self, op):
-        """The 16-bit tensor-core kernel that runs op `op`: _lib.TC_CONV (tc_conv_kernel) or _lib.TC_CONV3X3S1
-        (tc_conv3x3s1_kernel, the 3x3 stride-1 convs with Cin, Cout <= 64)."""
-        k = lib().mtb_op_tc_kernel(self._h, op)
-        if k < 0:
-            check(k, self._h)
+        """The 16-bit tensor-core kernel of op `op`: _lib.TC_CONV (tc_conv_kernel, with or without the SE scale) or
+        _lib.TC_CONV3X3S1; raises for an op that runs neither."""
+        k = self.op_kernel(op)
+        if k in (_lib.TC_CONV, _lib.TC_CONV_SE, _lib.SE_SCALE_TC_CONV):
+            return _lib.TC_CONV
+        if k != _lib.TC_CONV3X3S1:
+            raise _lib.MetrabsB200Error(f'op {op} has no 16-bit tensor-core kernel')
         return k
 
     def op_is_fused_block(self, op):

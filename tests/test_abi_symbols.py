@@ -30,6 +30,17 @@ def test_library_exports_every_declared_symbol():
     assert lib.mtb_version is not None
 
 
+def test_kernel_values_match_the_header():
+    """every value of the header's mtb_kernel enum has its _lib twin of the same name, numbered 0, 1, ... in order"""
+    src = open(os.path.join(ROOT, 'include', 'metrabs_b200.h')).read()
+    body = re.sub(r'/\*.*?\*/', '', re.search(r'typedef enum \{([^}]*)\} mtb_kernel;', src, re.S).group(1), flags=re.S)
+    values = {}
+    for name, expr in re.findall(r'MTB_([A-Z0-9_]+) = ([^,]+)', body):
+        values[name] = eval(re.sub(r'MTB_([A-Z0-9_]+)', lambda m: str(values[m.group(1)]), expr.strip()))
+    assert list(values.values()) == list(range(23)), values
+    assert {k: getattr(_lib, k, None) for k in values} == values
+
+
 @pytest.mark.skipif(torch.cuda.is_available(), reason='checks the no-GPU behaviour')
 def test_no_cpu_fallback():
     if not os.path.exists(_lib.LIB_PATH):

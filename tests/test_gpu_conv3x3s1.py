@@ -1,7 +1,7 @@
 """GPU: tc_conv3x3s1_kernel, the tensor-core kernel of the 3x3 stride-1 convs with Cin, Cout <= 64 (stage 1 of
 EfficientNetV2, conv2_x of the ResNets), in bf16 and fp16.
 
-* Selection: Engine.op_tc_kernel reports tc_conv3x3s1_kernel for exactly the ops it takes (3x3, stride 1, dilation 1,
+* Selection: Engine.op_kernel reports tc_conv3x3s1_kernel for exactly the ops it takes (3x3, stride 1, dilation 1,
   Cin and Cout <= 64, SiLU or ReLU) and tc_conv_kernel for every other tensor-core op: 1x1, stride 2, dilated (ResNets at
   output stride 8), Cin or Cout > 64.  Both report the profiler class tc_conv_kernel.
 * Values: every distinct op it takes, against the CUDA-core twin on identical 16-bit inputs (bf16 1e-2, fp16 1.5e-3 of
@@ -55,9 +55,11 @@ def check(e_tc, e_ref, table, bound_of, batch, dtype, bound, seed, prec, twin, s
         op, io = table[nm], e_tc.op_io(i)
         if not port_ops.tc_eligible(op, io['in_shape'][2], io['out_shape'][2]):
             continue
-        k = e_tc.op_tc_kernel(i)
+        k = e_tc.op_kernel(i)
         if not takes(op, io):
-            assert k == _lib.TC_CONV, (nm, io, k)
+            # tc_conv_kernel, with or without the squeeze-excitation scale of a projection
+            tc_conv = (_lib.TC_CONV_SE, _lib.SE_SCALE_TC_CONV) if io['scale'] else (_lib.TC_CONV,)
+            assert k in tc_conv, (nm, io, k)
             if op['kernel'] == 3:
                 rejected.add('stride 2' if op['stride'] == 2 else 'dilated' if op['dil'] > 1 else
                              'wide' if max(io['in_shape'][2], io['out_shape'][2]) > 64 else 'other')

@@ -1,5 +1,5 @@
 """GPU: EfficientNet-B0..B7 (metrabs_b200.backbones.efficientnet.efficientnet_bN) and the pooling 16-bit 5x5 depthwise
-kernel (dwconv5x5_16b_kernel with SE pooling, mtb_dw_kernel DW_5X5_POOL_16B).
+kernel (dwconv5x5_16b_kernel with SE pooling, mtb_kernel DW_5X5_POOL_16B).
 
 * fp32 and tf32x3: B0, B3@384 (no centered stride) and B5 against the goldens the unmodified reference produced
   (tests/golden/effnetb*.npz) and against the restatement (oracle/port_effnet_b.py); all eight variants in fp32 against the
@@ -138,7 +138,7 @@ def test_ops16_vs_conv2d(H, name, side, centered, batch):
             assert classes[nm] in expected_class(op, io, precision), (nm, classes[nm])
             kind = classes[nm]
             if op['depthwise']:
-                dk = eng.op_dw_kernel(i)
+                dk = eng.op_kernel(i)
                 assert dk in dw_expected(op, precision), (nm, precision, dk)
                 kind += f'/{dk}'
             feats |= {kind, ('shift', op['shift']), ('k', op['kernel'])}
@@ -180,7 +180,7 @@ def test_dw5x5_pool_bit_equal_to_the_generic_kernel(H, v, side):
             if sig in seen:
                 continue
             seen.add(sig)
-            assert tc.op_dw_kernel(i) == _lib.DW_5X5_POOL_16B and simt.op_dw_kernel(i) == _lib.DW_GENERIC, nm
+            assert tc.op_kernel(i) == _lib.DW_5X5_POOL_16B and simt.op_kernel(i) == _lib.DW_GENERIC, nm
             for batch in (1, 3, 5):
                 x = (3 * torch.randn((batch,) + io['in_shape'], generator=g)).to(st).float().cuda()
                 a, b = tc.debug_run_op(i, x), simt.debug_run_op(i, x)
@@ -214,7 +214,7 @@ def test_se_pool_on_the_forward(H, precision, name, side, centered, batch):
     crops = port.synthetic_inputs(batch, side, seed=14)[0].cuda()
     checked, worst = 0, 0.0
     for i, nm in enumerate(names):
-        if not nm.endswith('.avgpool') or eng.op_dw_kernel(i - 1) != _lib.DW_5X5_POOL_16B:
+        if not nm.endswith('.avgpool') or eng.op_kernel(i - 1) != _lib.DW_5X5_POOL_16B:
             continue
         hh, ww, _c = eng.op_io(i - 1)['out_shape']
         d = eng.debug_run_ops(crops, i).double()

@@ -97,7 +97,7 @@ def test_dilated_ops_vs_conv2d(H, precision, name, side, output_stride):
     assert ops and {op['dil'] for _, _, op, _ in ops} == ({2} if output_stride == 16 else {2, 4})
     worst = 0.0
     for i, nm, op, io in ops:
-        assert eng.op_dw_kernel(i) == _lib.DW_TMA_DIL, nm
+        assert eng.op_kernel(i) == _lib.DW_TMA_DIL, nm
         hh, ww, _c = io['out_shape']
         G = dw_plan(-(-hh // op['dil']), -(-ww // op['dil']))[0]
         assert G > 0, (nm, hh, ww)
@@ -149,7 +149,7 @@ def test_phases_equal_the_undilated_kernel(H, precision):
     e8 = device_model('efficientnetv2-tiny', 8, pcfg8, 8, sd8, precision).engine()
     e32 = device_model('efficientnetv2-tiny', 32, pcfg32, 8, sd32, precision).engine()
     i8, i32 = e8.op_names().index(nm), e32.op_names().index(nm)
-    assert e8.op_dw_kernel(i8) == _lib.DW_TMA_DIL and e32.op_dw_kernel(i32) == _lib.DW_TMA
+    assert e8.op_kernel(i8) == _lib.DW_TMA_DIL and e32.op_kernel(i32) == _lib.DW_TMA
     assert e8.op_io(i8)['in_shape'] == (8, 8, 192) and e32.op_io(i32)['in_shape'] == (4, 4, 192)
     g = torch.Generator().manual_seed(5)
     for batch in (1, 3, 9):

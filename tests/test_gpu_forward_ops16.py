@@ -36,8 +36,9 @@ pytestmark = pytest.mark.gpu
 
 J = 8
 CHUNK = 1 << 25  # elements per crop chunk of the fp64 reference (input or output, whichever is larger)
-DW_NAMES = {_lib.DW_GENERIC: 'generic', _lib.DW_TMA: 'tma', _lib.DW_STRIP_16B: 'strip16', _lib.DW_STRIP_F32: 'strip32',
-            _lib.DW_5X5_16B: '5x5', _lib.DW_5X5_POOL_16B: '5x5_pool', _lib.DW_TMA_DIL: 'tma_dil'}
+DW_NAMES = {_lib.DW_GENERIC: 'generic', _lib.DW_TMA: 'tma', _lib.DW_STRIP_16B: 'strip16',
+            _lib.DW_STRIP_F32: 'strip32', _lib.DW_5X5_16B: '5x5', _lib.DW_5X5_POOL_16B: '5x5_pool',
+            _lib.DW_TMA_DIL: 'tma_dil'}
 # depthwise kernels that pool their fp32 activations before rounding them to 16 bits (fc1 sums their slices)
 POOLS_FP32 = {_lib.DW_TMA, _lib.DW_TMA_DIL, _lib.DW_STRIP_16B, _lib.DW_STRIP_F32}
 
@@ -172,7 +173,7 @@ def test_forward_ops_vs_conv2d(H, config, batch, precision):
         elif nm.endswith('.fc1'):
             assert names[k - 1].endswith('.avgpool')
             d = live[eng.op_buffers(k - 1)['input']]  # the depthwise output the forward stored
-            dk = eng.op_dw_kernel(k - 2)
+            dk = eng.op_kernel(k - 2)
             xabs = d.abs().mean(dim=(1, 2), dtype=torch.float64)
             x_err = 2.0 ** -p * (1 + 2.0 ** -p) * xabs if dk in POOLS_FP32 else None
             kind = f'se fc1 after {DW_NAMES[dk]}'
@@ -197,7 +198,7 @@ def test_forward_ops_vs_conv2d(H, config, batch, precision):
                 if op['kernel'] == 3 and op['stride'] == 2 and io['out_shape'][2] in (24, 32):
                     reached.add('stem3x3s2')
             elif op['depthwise']:
-                dk = eng.op_dw_kernel(k)
+                dk = eng.op_kernel(k)
                 kind = f'dwconv_kernel/{DW_NAMES[dk]}' + ('+pool' if names[k + 1].endswith('.avgpool') else '')
                 reached |= {('dw', dk), ('dw dil', dk, op['dil'])}
                 if dk in (_lib.DW_TMA, _lib.DW_TMA_DIL):
@@ -207,7 +208,7 @@ def test_forward_ops_vs_conv2d(H, config, batch, precision):
                 kind = 'fmb_kernel'  # the block output; its input is the unfused expand's output, checked one op before
                 reached.add('fmb')
             elif classes[nm] in ('tc_conv_kernel', 'fmb_kernel'):
-                tk = eng.op_tc_kernel(k)
+                tk = eng.op_kernel(k)
                 kind = 'tc_conv3x3s1_kernel' if tk == _lib.TC_CONV3X3S1 else 'tc_conv_kernel'
                 reached.add(('tc', tk))
                 if eng.op_is_fused_block(k):
@@ -215,7 +216,7 @@ def test_forward_ops_vs_conv2d(H, config, batch, precision):
                 if sc is not None:
                     cin, cout = io['in_shape'][2], io['out_shape'][2]
                     se_proj.append((cin, cout))
-                    kind += ' + SE in GEMM' if cout <= 256 else ' behind se_scale_kernel'
+                    kind += ' + SE in GEMM' if tk == _lib.TC_CONV_SE else ' behind se_scale_kernel'
             else:
                 kind = classes[nm]
             reached |= {('act', op['act']), ('dil', op['dil'])}

@@ -108,7 +108,7 @@ def test_forward_ops_vs_conv2d(H, config, batch, precision):
         assert torch.isfinite(out).all(), f'{nm} [{precision}]: {int((~torch.isfinite(out)).sum())} non-finite outputs'
         r = None
         if nm.endswith('.avgpool'):
-            dk = eng.op_dw_kernel(k - 1)
+            dk = eng.op_kernel(k - 1)
             reached.add(('se after', table[names[k - 1]]['act'], DW_NAMES[dk]))
             if dk == _lib.DW_GENERIC:  # pool_mean_kernel; the fused kernels leave partial slices here (fc1 sums them)
                 assert classes[nm] == 'pool_mean_kernel', (nm, classes[nm])
@@ -118,7 +118,7 @@ def test_forward_ops_vs_conv2d(H, config, batch, precision):
                 assert bool((err <= tol).all()), f'{nm} [{precision}]: |dev-ref|/tol {r:.2f}'
         elif nm.endswith('.fc1'):
             assert names[k - 1].endswith('.avgpool')
-            dk = eng.op_dw_kernel(k - 2)
+            dk = eng.op_kernel(k - 2)
             if dk == _lib.DW_GENERIC:  # on the mean pool_mean_kernel stored
                 x = live[eng.op_buffers(k - 1)['output']][:, 0, 0].double()
                 r = check_se_fc(sd, nm, out, x, x.abs(), 0, None, se_acts[0], precision)
@@ -145,7 +145,7 @@ def test_forward_ops_vs_conv2d(H, config, batch, precision):
                 kind = 'maxpool'
                 reached.add(kind)
             elif op['depthwise']:
-                dk = eng.op_dw_kernel(k)
+                dk = eng.op_kernel(k)
                 kind += f'/{DW_NAMES[dk]}' + ('+pool' if names[k + 1].endswith('.avgpool') else '')
                 reached.add(('dw', dk))
             elif cls == 'tc32_conv_kernel':
@@ -223,11 +223,11 @@ def test_forward_ops_vs_conv2d(H, config, batch, precision):
     assert set(head_prof) == ({'tc32_conv_kernel', 'softargmax_bhwn_kernel'} if precision == 'tf32x3'
                               else {'head_conv(conv_igemm_kernel)', 'softargmax_bhwn_kernel'}), set(head_prof)
     assert 'se_scale_kernel' not in prof and 'tc_conv_kernel' not in prof and 'fmb_kernel' not in prof, set(prof)
-    n_generic_pools = sum(eng.op_dw_kernel(i - 1) == _lib.DW_GENERIC for i, nm in enumerate(names) if nm.endswith('.avgpool'))
+    n_generic_pools = sum(eng.op_kernel(i - 1) == _lib.DW_GENERIC for i, nm in enumerate(names) if nm.endswith('.avgpool'))
     assert prof.get('pool_mean_kernel', {}).get('launches', 0) == n_generic_pools
     if precision == 'fp32':
         assert 'tc32_conv_kernel' not in prof and n_generic_pools == n_pool, set(prof)
-        assert all(eng.op_dw_kernel(i) == _lib.DW_GENERIC for i, nm in enumerate(names) if table.get(nm, {}).get('depthwise'))
+        assert all(eng.op_kernel(i) == _lib.DW_GENERIC for i, nm in enumerate(names) if table.get(nm, {}).get('depthwise'))
     else:
         assert any(t[0] == 'tc32' for t in reached if isinstance(t, tuple)), reached
         if config.startswith('efficientnet'):

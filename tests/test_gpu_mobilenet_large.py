@@ -6,7 +6,7 @@
   projections take the restatement's own SE scale), features and joints within 1e-3, at S=256 and S=224, with and without
   the centered stride.
 * bf16, bf16_simt, fp16, fp16_simt: every distinct op element by element against fp64 conv2d at the mode's rounding points
-  (port_mobilenet.layer_bound, port_ops.check_bound), with its kernel class and depthwise kernel (mtb_op_dw_kernel)
+  (port_mobilenet.layer_bound, port_ops.check_bound), with its kernel class and depthwise kernel (mtb_op_kernel)
   asserted: every GEMM on tc_conv_kernel and every 5x5 depthwise op on dwconv5x5_16b_kernel in the tensor-core modes.
   The SE fc1 / fc2 ops are checked on the device's own forward: fc1 reads a separately pooled mean behind the 5x5 kernel.
 * dwconv5x5_16b_kernel against dwconv_kernel: every distinct 5x5 op shape of Small and Large (stride 1 and 2, the
@@ -155,7 +155,7 @@ def test_large_ops16_vs_conv2d(H, side, centered, batch):
             assert classes[nm] in expected_class(op, io, precision), (nm, classes[nm])
             kind = classes[nm]
             if op['depthwise']:
-                dk = eng.op_dw_kernel(i)
+                dk = eng.op_kernel(i)
                 assert dk in dw_expected(op, precision), (nm, precision, dk)
                 kind += f'/{dk}'
             elif not op['stem'] and precision in ('bf16', 'fp16'):
@@ -201,7 +201,7 @@ def test_large_se_squeeze_on_the_forward(H, precision, side, batch):
         if not nm.endswith('.avgpool'):
             continue
         hh, ww, _c = eng.op_io(i - 1)['out_shape']
-        dk = eng.op_dw_kernel(i - 1)
+        dk = eng.op_kernel(i - 1)
         reached.add(dk)
         d = eng.debug_run_ops(crops, i).double()                     # the depthwise output the device stored
         f1 = eng.debug_run_ops(crops, i + 2)[:, 0, 0].double()       # fc1 on the fused (or separate) pooling
@@ -252,7 +252,7 @@ def test_dw5x5_bit_equal_to_the_generic_kernel(H, variant, side):
             if sig in seen:
                 continue
             seen.add(sig)
-            assert tc.op_dw_kernel(i) == _lib.DW_5X5_16B and simt.op_dw_kernel(i) == _lib.DW_GENERIC, nm
+            assert tc.op_kernel(i) == _lib.DW_5X5_16B and simt.op_kernel(i) == _lib.DW_GENERIC, nm
             for batch in (1, 3, 5):
                 x = (3 * torch.randn((batch,) + io['in_shape'], generator=g)).to(st).float().cuda()
                 a, b = tc.debug_run_op(i, x), simt.debug_run_op(i, x)

@@ -44,7 +44,7 @@ def _check_plan(eng, precision, crops, k):
     else:
         assert any(eng.op_is_fused_block(i) for i in range(len(names)))
         dw = [i - 1 for i, nm in enumerate(names) if nm.endswith('.avgpool')]
-        assert any(eng.op_dw_kernel(i) == _lib.DW_TMA for i in dw)
+        assert any(eng.op_kernel(i) == _lib.DW_TMA for i in dw)
         assert {'fmb_kernel', 'tc_head_softargmax_kernel', 'tc_conv_kernel'} <= set(classes), classes
         assert 'dwconv_kernel' in classes, classes  # the depthwise class, which includes the TMA kernel
 
