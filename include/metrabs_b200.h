@@ -285,7 +285,9 @@ typedef struct {
 int mtb_tta_merge(const mtb_tta_args* args, void* stream);
 
 /* plausibility_check.py:8-119: is_pose_plausible, are_augmentation_results_consistent, is_pose_consistent_with_box and
- * pose_non_max_suppression (similarity threshold 0.4) per image.  At most 128 boxes per image, num_aug <= 16. */
+ * pose_non_max_suppression (similarity threshold 0.4) per image.  num_aug <= 16.  The per-box state of one image lives in
+ * shared memory, 14 B per box sized for n_boxes: at most about 16,000 boxes per call on an H100 (227 KB per block);
+ * above what the device holds the call fails with MTB_ERR_UNSUPPORTED and filters nothing. */
 typedef struct {
   const float* poses3d;          /* [n_boxes, num_aug, J, 3] camera space */
   const float* poses2d;          /* [n_boxes, num_aug, J, 2] */

@@ -2024,9 +2024,21 @@ int mtb_filter_poses(const mtb_filter_args* a, void* stream) {
   p.poses3d = a->poses3d; p.poses2d = a->poses2d; p.boxes = a->boxes; p.box_stride = a->box_stride; p.bones = a->bones;
   p.mean_bones = a->mean_bones; p.n_bones = a->n_bones; p.image_start = a->image_start; p.num_aug = a->num_aug; p.J = a->n_joints;
   p.plausible = a->plausible; p.keep = a->keep; p.scratch = a->scratch;
-  launch_k(pose_filter_kernel, dim3(a->n_images), dim3(128), 0, (cudaStream_t)stream, p);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(nullptr, MTB_ERR_CUDA, "pose filter launch: %s", cudaGetErrorString(e));
+  // every image's box count is at most n_boxes, so per-box state for n_boxes boxes covers the most crowded image
+  p.max_boxes = a->n_boxes;
+  int dev = 0, optin = 0;
+  cudaFuncAttributes fa;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+  if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, pose_filter_kernel);
+  if (e != cudaSuccess) return fail(nullptr, MTB_ERR_CUDA, "pose filter setup: %s", cudaGetErrorString(e));
+  const long long smem = (long long)a->n_boxes * MP_FILTER_SMEM_PER_BOX;
+  if (smem > (long long)optin - (long long)fa.sharedSizeBytes)
+    return fail(nullptr, MTB_ERR_UNSUPPORTED, "pose filter: %d boxes need %lld B of shared memory, the device holds %d B per block "
+                "(at most %d boxes per call)", a->n_boxes, smem, optin - (int)fa.sharedSizeBytes,
+                (optin - (int)fa.sharedSizeBytes) / MP_FILTER_SMEM_PER_BOX);
+  if (const char* err = launch_smem(pose_filter_kernel, dim3(a->n_images), dim3(FILTER_THREADS), (int)smem, (cudaStream_t)stream, p))
+    return fail(nullptr, MTB_ERR_CUDA, "pose filter launch: %s", err);
   return MTB_OK;
 }
 

@@ -390,17 +390,23 @@ struct FilterParams {
   uint8_t* plausible;       // [n] out: the three plausibility checks
   uint8_t* keep;            // [n] out: plausible AND surviving the pose NMS
   float* scratch;           // [n, J, 3] mean-over-aug poses
+  int max_boxes;            // bound on every image's box count: sizes the dynamic shared memory
 };
-constexpr int MP_MAX_BOXES_PER_IMAGE = 128;
+// dynamic shared memory of pose_filter_kernel per box of the largest image: score, sqscale, order, valid, supp
+constexpr int MP_FILTER_SMEM_PER_BOX = 4 + 4 + 4 + 1 + 1;
+constexpr int FILTER_THREADS = 128;
 
 // one CTA per image.  Phase 1 (thread per box): the three checks.  Phase 2: pose similarity on demand + greedy NMS.
-__global__ void __launch_bounds__(128) pose_filter_kernel(const FilterParams p) {
-  __shared__ float score[MP_MAX_BOXES_PER_IMAGE];
-  __shared__ float sqscale[MP_MAX_BOXES_PER_IMAGE];
-  __shared__ int order[MP_MAX_BOXES_PER_IMAGE];
-  __shared__ uint8_t valid[MP_MAX_BOXES_PER_IMAGE], supp[MP_MAX_BOXES_PER_IMAGE];
+__global__ void __launch_bounds__(FILTER_THREADS) pose_filter_kernel(const FilterParams p) {
+  __shared__ float sq_all[MP_MAX_AUG * FILTER_THREADS];
+  extern __shared__ __align__(16) unsigned char filter_smem[];
+  float* score = reinterpret_cast<float*>(filter_smem);
+  float* sqscale = score + p.max_boxes;
+  int* order = reinterpret_cast<int*>(sqscale + p.max_boxes);
+  uint8_t* valid = reinterpret_cast<uint8_t*>(order + p.max_boxes);
+  uint8_t* supp = valid + p.max_boxes;
   const int b0 = p.image_start[blockIdx.x], b1 = p.image_start[blockIdx.x + 1];
-  const int n = min(b1 - b0, MP_MAX_BOXES_PER_IMAGE);
+  const int n = b1 - b0;  // <= max_boxes
   const int J = p.J, A = p.num_aug;
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
     const int b = b0 + i;
@@ -435,13 +441,15 @@ __global__ void __launch_bounds__(128) pose_filter_kernel(const FilterParams p) 
     }
     // are_augmentation_results_consistent (:63-67): scale-align the A poses, per-joint stdev over augmentations (unbiased
     // variance, summed over xyz), more than J//4 joints under 200 mm
-    float sq[MP_MAX_AUG];
+    // per-augmentation square scales in shared memory, not a local array: a stack frame makes ptxas spill around the
+    // IEEE division / square-root calls
+    float* sq = sq_all + threadIdx.x;  // sq[a * FILTER_THREADS]
     float msq = 0.f;
     for (int a = 0; a < A; ++a) {
       float s = 0.f;
       for (int j = 0; j < J * 3; ++j) s += P3[(size_t)a * J * 3 + j] * P3[(size_t)a * J * 3 + j];
-      sq[a] = s / (float)(J * 3);
-      msq += sq[a];
+      sq[a * FILTER_THREADS] = s / (float)(J * 3);
+      msq += sq[a * FILTER_THREADS];
     }
     msq /= A;
     int n_stable = 0;
@@ -449,11 +457,11 @@ __global__ void __launch_bounds__(128) pose_filter_kernel(const FilterParams p) 
       float var = 0.f;
       for (int c = 0; c < 3; ++c) {
         float m = 0.f;
-        for (int a = 0; a < A; ++a) m += P3[((size_t)a * J + j) * 3 + c] * sqrtf(msq / sq[a]);
+        for (int a = 0; a < A; ++a) m += P3[((size_t)a * J + j) * 3 + c] * sqrtf(msq / sq[a * FILTER_THREADS]);
         m /= A;
         float vs = 0.f;
         for (int a = 0; a < A; ++a) {
-          const float d = P3[((size_t)a * J + j) * 3 + c] * sqrtf(msq / sq[a]) - m;
+          const float d = P3[((size_t)a * J + j) * 3 + c] * sqrtf(msq / sq[a * FILTER_THREADS]) - m;
           vs += d * d;
         }
         var += vs / (float)(A - 1);  // torch.var default: unbiased
@@ -526,7 +534,6 @@ __global__ void __launch_bounds__(128) pose_filter_kernel(const FilterParams p) 
   }
   __syncthreads();
   for (int i = threadIdx.x; i < n; i += blockDim.x) p.keep[b0 + i] = (valid[i] && !supp[i]) ? 1 : 0;
-  for (int i = n + threadIdx.x; i < b1 - b0; i += blockDim.x) p.keep[b0 + i] = p.plausible[b0 + i] = 0;  // beyond the per-image cap
 }
 
 }  // namespace mtb

@@ -12,9 +12,13 @@ from metrabs_b200.multiperson.warping import _ptr, _stream
 
 def filter_poses(poses3d, poses2d, boxes, n_box_per_image, joint_edges, mean_bones):
     """poses3d [n,A,J,3] (camera space), poses2d [n,A,J,2], boxes [n,5] (x,y,w,h,score), all on the GPU.
-    -> (plausible [n] bool, keep [n] bool): ``keep`` = plausible and surviving pose_non_max_suppression per image."""
+    -> (plausible [n] bool, keep [n] bool): ``keep`` = plausible and surviving pose_non_max_suppression per image.
+    Any number of boxes per image up to what one block's shared memory holds (about 16,000 per call on an H100); beyond
+    that the call raises ``MetrabsB200Error`` rather than drop boxes."""
     dev = poses3d.device
     n, a, j, _ = poses3d.shape
+    if sum(int(c) for c in n_box_per_image) != n or any(int(c) < 0 for c in n_box_per_image):
+        raise ValueError(f'n_box_per_image {list(n_box_per_image)} does not partition the {n} boxes')
     poses3d = poses3d.float().contiguous()
     poses2d = poses2d.float().contiguous()
     boxes = boxes.float().contiguous()

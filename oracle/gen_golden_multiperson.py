@@ -190,13 +190,7 @@ def main():
     np.savez_compressed(os.path.join(OUT, 'multiperson_pipeline.npz'), **data)
 
     # ---- plausibility filter + pose NMS (plausibility_check.py:8-119)
-    import simplepyutils as spu
-    ji = StubJointInfo(JOINT_NAMES, JOINT_EDGES)
     mean_bones = torch.tensor([120., 120., 420., 420., 480., 180., 180.])
-    spu.FLAGS.bone_length_dataset = None
-    spu.FLAGS.bone_length_file = 'stub'
-    spu.load_pickle = lambda f: mean_bones
-    pc.FLAGS = spu.FLAGS
     g = torch.Generator().manual_seed(21)
     base = torch.tensor([[0., 0, 3000], [-120, 0, 3000], [120, 0, 3000], [-130, 420, 3010], [130, 420, 2990], [0, -480, 3000],
                          [-180, -480, 3000], [180, -480, 3000]])
@@ -227,6 +221,24 @@ def main():
         boxes2.append(box)
     boxes2 = torch.stack(boxes2)
     boxes2[1, 4] = boxes2[0, 4]                                          # equal scores: stable order decides
+    plaus, cons, inbox, keep = reference_filter(pc, poses3d, poses2d, boxes2, n_per_image, JOINT_NAMES, JOINT_EDGES, mean_bones)
+    np.savez_compressed(os.path.join(OUT, 'multiperson_filter.npz'), poses3d=poses3d.numpy(), poses2d=poses2d.numpy(),
+                        boxes=boxes2.numpy(), n_per_image=np.array(n_per_image), bones=np.array(JOINT_EDGES),
+                        mean_bones=mean_bones.numpy(), plausible_bones=plaus.numpy(), consistent=cons.numpy(), in_box=inbox.numpy(),
+                        keep=keep.numpy())
+    print('plausible', plaus.tolist(), '\nconsistent', cons.tolist(), '\nin_box', inbox.tolist(), '\nkeep', keep.tolist())
+    crowd(pc)
+
+
+def reference_filter(pc, poses3d, poses2d, boxes, n_per_image, names, edges, mean_bones):
+    """The reference's plausibility_check on one batch: (plausible bones, consistent augmentations, in box, keep).  Stubs:
+    the mean bone lengths come from FLAGS.bone_length_file through simplepyutils.load_pickle."""
+    import simplepyutils as spu
+    ji = StubJointInfo(names, edges)
+    spu.FLAGS.bone_length_dataset = None
+    spu.FLAGS.bone_length_file = 'stub'
+    spu.load_pickle = lambda f: mean_bones
+    pc.FLAGS = spu.FLAGS
     mean3, mean2 = poses3d.mean(dim=1), poses2d.mean(dim=1)
     plaus = pc.is_pose_plausible(mean3, ji)
     cons = pc.are_augmentation_results_consistent(poses3d)
@@ -238,24 +250,137 @@ def main():
     torch.min = lambda x, dim=None, **kw: tmin(x, dim=dim, **kw).values if dim is not None else tmin(x)
     torch.max = lambda x, dim=None, **kw: tmax(x, dim=dim, **kw).values if dim is not None else tmax(x)
     try:
-        inbox = pc.is_pose_consistent_with_box(mean2, boxes2)
+        inbox = pc.is_pose_consistent_with_box(mean2, boxes)
     finally:
         torch.min, torch.max = tmin, tmax
-    # NOTE torch.min/max(dim=) return (values, indices) tuples: the reference's is_pose_consistent_with_box is written for
-    # TF semantics; feed it through a thin wrapper if it raises
     mask = plaus & cons & inbox
-    keep = torch.zeros(len(boxes2), dtype=torch.bool)
+    keep = torch.zeros(len(boxes), dtype=torch.bool)
     s = 0
     for n in n_per_image:
-        idx = pc.pose_non_max_suppression(mean3[s:s + n], boxes2[s:s + n, 4], mask[s:s + n])
+        idx = pc.pose_non_max_suppression(mean3[s:s + n], boxes[s:s + n, 4], mask[s:s + n])
         keep[s + idx] = True
         s += n
-    np.savez_compressed(os.path.join(OUT, 'multiperson_filter.npz'), poses3d=poses3d.numpy(), poses2d=poses2d.numpy(),
-                        boxes=boxes2.numpy(), n_per_image=np.array(n_per_image), bones=np.array(JOINT_EDGES),
-                        mean_bones=mean_bones.numpy(), plausible_bones=plaus.numpy(), consistent=cons.numpy(), in_box=inbox.numpy(),
-                        keep=keep.numpy())
-    print('plausible', plaus.tolist(), '\nconsistent', cons.tolist(), '\nin_box', inbox.tolist(), '\nkeep', keep.tolist())
+    return plaus, cons, inbox, keep
+
+
+CROWD_MARGIN = 1e-3  # every decision at least this far from its threshold, relative to the threshold
+
+
+def crowd_group(seed, n_per_image, J, A, cases):
+    """Poses of many people (a grid of viewing directions, 3-6 m deep, so distinct people never look alike after scale
+    alignment) plus the listed special cases, each {image, kind(, of, m)}, placed at the given box index of its image.
+    -> poses3d [n,A,J,3], poses2d [n,A,J,2], boxes [n,5], bones [J-1,2], mean_bones [J-1]."""
+    g = torch.Generator().manual_seed(seed)
+    parent = [(k - 1) // 2 for k in range(J)]
+    bones = torch.tensor([[parent[k], k] for k in range(1, J)])
+    lengths = 60 + 390 * torch.rand(J - 1, generator=g)
+    lengths[J - 2] = 50.  # a short leaf bone: three times too long is still within 300 mm
+    lengths[J - 3] = 440.  # a long leaf bone: collapsing it is implausible
+    dirs = torch.nn.functional.normalize(torch.randn(J - 1, 3, generator=g), dim=-1)
+    template = torch.zeros(J, 3)
+    for k in range(1, J):
+        template[k] = template[parent[k]] + dirs[k - 1] * lengths[k - 1]
+    n_total = sum(n_per_image)
+    grid = torch.randperm(196, generator=g)[:n_total]
+    poses = []
+    for i in range(n_total):
+        gx, gy = (grid[i] % 14 - 6.5) * 0.2, (grid[i] // 14 - 6.5) * 0.2
+        z = 3000 + 3000 * torch.rand(1, generator=g)
+        root = torch.cat([gx * z, gy * z, z])
+        p = template * (0.9 + 0.2 * torch.rand(1, generator=g)) + root
+        poses.append(p[None].repeat(A, 1, 1) + 15 * torch.randn(A, J, 3, generator=g))
+    starts = np.cumsum([0] + list(n_per_image))
+    box_shift = {}
+    for c in cases:
+        i = int(starts[c['image']] + c['index'])
+        kind = c['kind']
+        p = poses[i]
+        if kind in ('dup', 'partial_dup', 'shift'):
+            src = int(starts[c['image']] + c['of'])
+            p = poses[src] + 8 * torch.randn(A, J, 3, generator=g)
+            if kind == 'partial_dup':  # m joints 700 mm away: the J//4 largest distances include them
+                sel = torch.randperm(J, generator=g)[:c['m']]
+                p[:, sel] += torch.tensor([700., 0., 0.])
+            if kind == 'shift':
+                p = p + torch.tensor([c['m'], 0., 0.])
+        elif kind == 'bone_far':
+            p[:, J - 1] += torch.tensor([0., 2500., 0.])
+        elif kind == 'bone_collapse':
+            p[:, J - 2] = p[:, parent[J - 2]]
+        elif kind == 'bone_short_long':  # 200 mm instead of 50 mm: relatively absurd, absolutely not
+            v = torch.nn.functional.normalize(p[:, J - 1] - p[:, parent[J - 1]], dim=-1)
+            p[:, J - 1] = p[:, parent[J - 1]] + 200 * v
+        elif kind == 'unstable':  # all but m joints disagree across the augmentations
+            sel = torch.randperm(J, generator=g)[c['m']:]
+            p[:, sel] += 600 * torch.randn(A, len(sel), 3, generator=g)
+        elif kind in ('offbox', 'box_partial'):
+            box_shift[i] = c['m']
+        poses[i] = p
+    poses3d = torch.stack(poses)
+    k = torch.tensor([[1200., 0, 640], [0, 1200., 360], [0, 0, 1]])
+    poses2d = torch.einsum('bank,jk->banj', poses3d / poses3d[..., 2:], k[:2])
+    boxes = []
+    for i, p2 in enumerate(poses2d.mean(dim=1)):
+        lo, hi = p2.min(dim=0).values, p2.max(dim=0).values
+        box = torch.cat([lo - 10, hi - lo + 20, 0.2 + 0.8 * torch.rand(1, generator=g)])
+        if i in box_shift:  # shift the detection by a fraction of its width
+            box[0] += box_shift[i] * box[2]
+        boxes.append(box)
+    boxes = torch.stack(boxes)
+    for c in cases:
+        if c['kind'] == 'same_score':
+            boxes[starts[c['image']] + c['index'], 4] = boxes[starts[c['image']] + c['of'], 4]
+    return poses3d, poses2d, boxes, bones, lengths
+
+
+def crowd(pc):
+    """tests/golden/multiperson_filter_crowd.npz: the filter on crowded images.  Group `crowd`: J = 24, A = 5, image 0 with
+    170 boxes and every kind of decision spread past box 128, image 1 with 9.  Group `wide`: J = 122 (J//4 = 30), A = 16,
+    two images of three boxes.  Every decision is asserted to lie CROWD_MARGIN from its threshold in fp64 (fp32 cannot
+    flip it), and the fp64 restatement (oracle/port_multiperson.py) must agree with the reference."""
+    from oracle import port_multiperson as pm
+    kinds = [('dup', 0, 0), ('partial_dup', 2, 0), ('partial_dup', 4, 0), ('partial_dup', 6, 0), ('shift', 150, 0),
+             ('shift', 220, 0), ('bone_far', 0, None), ('bone_collapse', 0, None), ('bone_short_long', 0, None),
+             ('unstable', 0, None), ('unstable', 6, None), ('unstable', 7, None), ('offbox', 3, None), ('box_partial', 0.3, None),
+             ('box_partial', 0.7, None), ('same_score', 0, 0)]
+    g = torch.Generator().manual_seed(7)
+    cases, used = [], set()
+    for rep in range(3):  # each kind three times: before, around and past box 128
+        for kind, m, of in kinds:
+            lo, hi = [(5, 100), (100, 140), (129, 170)][rep]
+            while True:
+                i = int(torch.randint(lo, hi, (1,), generator=g))
+                src = int(torch.randint(0, 170, (1,), generator=g))
+                if i not in used and src not in used and src != i:
+                    break
+            used.update({i, src})
+            cases.append(dict(image=0, index=i, kind=kind, m=m, of=src if of is not None else None))
+    cases.append(dict(image=1, index=4, kind='dup', m=0, of=1))
+    out = {}
+    groups = dict(crowd=(41, [170, 9], 24, 5, cases),
+                  wide=(43, [3, 3], 122, 16, [dict(image=0, index=1, kind='dup', of=0), dict(image=0, index=2, kind='unstable', m=31),
+                                               dict(image=1, index=1, kind='unstable', m=30), dict(image=1, index=2, kind='partial_dup', m=20, of=0)]))
+    for name, (seed, n_per_image, J, A, cs) in groups.items():
+        poses3d, poses2d, boxes, bones, mean_bones = crowd_group(seed, n_per_image, J, A, cs)
+        names = [f'j{i}' for i in range(J)]
+        plaus, cons, inbox, keep = reference_filter(pc, poses3d, poses2d, boxes, n_per_image, names, bones.tolist(), mean_bones)
+        plausible = plaus & cons & inbox
+        dec = pm.filter_decisions(poses3d, poses2d, boxes, n_per_image, bones, mean_bones)
+        assert dec['plausible'].tolist() == plausible.tolist() and dec['keep'].tolist() == keep.tolist(), name
+        worst = float(dec['margin'].min())
+        assert worst > CROWD_MARGIN, (name, worst, int(dec['margin'].argmin()))
+        print(f'{name}: {len(boxes)} boxes, plausible {int(plausible.sum())}, kept {int(keep.sum())}, kept past box 128 of image 0 '
+              f'{int(keep[128:n_per_image[0]].sum())}, smallest decision margin {worst:.3g}')
+        out.update({f'{name}_poses3d': poses3d.numpy(), f'{name}_poses2d': poses2d.numpy(), f'{name}_boxes': boxes.numpy(),
+                    f'{name}_n_per_image': np.array(n_per_image), f'{name}_bones': bones.numpy(),
+                    f'{name}_mean_bones': mean_bones.numpy(), f'{name}_plausible': plausible.numpy(), f'{name}_keep': keep.numpy()})
+    np.savez_compressed(os.path.join(OUT, 'multiperson_filter_crowd.npz'), **out)
 
 
 if __name__ == '__main__':
-    main()
+    # `python oracle/gen_golden_multiperson.py crowd` writes tests/golden/multiperson_filter_crowd.npz only
+    if sys.argv[1:] == ['crowd']:
+        _, _, _, pc_ = import_multiperson(port.PathConfig(proc_side=64))
+        crowd(pc_)
+    else:
+        main()
