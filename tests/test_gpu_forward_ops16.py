@@ -34,7 +34,8 @@ from tests.test_gpu_ops16_vs_conv2d import H, POOL_SLICES, dw_plan, expected_cla
 
 pytestmark = pytest.mark.gpu
 
-J = 8
+J = 8  # joints of the head, except where JOINTS says otherwise
+JOINTS = {'efficientnetv2-s-j122': 122}  # c4: 122 joints, 1098 head channels = 9 M tiles of 128, the last one ragged
 CHUNK = 1 << 25  # elements per crop chunk of the fp64 reference (input or output, whichever is larger)
 DW_NAMES = {_lib.DW_GENERIC: 'generic', _lib.DW_TMA: 'tma', _lib.DW_STRIP_16B: 'strip16',
             _lib.DW_STRIP_F32: 'strip32', _lib.DW_5X5_16B: '5x5', _lib.DW_5X5_POOL_16B: '5x5_pool',
@@ -43,18 +44,27 @@ DW_NAMES = {_lib.DW_GENERIC: 'generic', _lib.DW_TMA: 'tma', _lib.DW_STRIP_16B: '
 POOLS_FP32 = {_lib.DW_TMA, _lib.DW_TMA_DIL, _lib.DW_STRIP_16B, _lib.DW_STRIP_F32}
 
 # (configuration, crops): the benchmark scripts' models and batches (bench.py / f16_step.py, effnet_stride_step.py,
-# effnet_b_step.py, mobilenet_step.py, resnet_step.py)
+# effnet_b_step.py, mobilenet_step.py, resnet_step.py), and BASELINE.md's c3 (EfficientNetV2-L@384, one GPU's 32 crops
+# of the strong-scaling batch) and c4 (EfficientNetV2-S@256 with 122 joints, 64 crops)
 CONFIGS = [('efficientnetv2-l', 256), ('efficientnetv2-s-os8', 256), ('efficientnet-b0', 256), ('efficientnet-b4', 256),
-           ('mobilenetv3-large', 256), ('resnet50-s8', 128)]
+           ('mobilenetv3-large', 256), ('resnet50-s8', 128), ('efficientnetv2-l@384', 32), ('efficientnetv2-s-j122', 64)]
+# EfficientNetV2 configurations of the reference's own block grammar: configuration -> (model, crop side)
+EFFNETV2 = {'efficientnetv2-l': ('efficientnetv2-l', 256), 'efficientnetv2-l@384': ('efficientnetv2-l', 384),
+            'efficientnetv2-s-j122': ('efficientnetv2-s', 256)}
+
+
+def n_joints(config):
+    return JOINTS.get(config, J)
 
 
 def build(H, config, precision):
     """-> (pcfg, spec, state dict, engine, op table, bound(name, x, res, scale) -> (ref, tol), SE activations (fc1, fc2))."""
-    if config == 'efficientnetv2-l':
-        pcfg = port.PathConfig(proc_side=256)
-        spec = port.effnet_spec(config)
-        sd = port.make_effnet_state_dict(spec, pcfg, J, seed=0, calib_batch=1)
-        eng = H.device_model(config, pcfg, J, sd, precision=precision).engine()
+    if config in EFFNETV2:
+        name, side = EFFNETV2[config]
+        pcfg = port.PathConfig(proc_side=side)
+        spec = port.effnet_spec(name)
+        sd = port.make_effnet_state_dict(spec, pcfg, n_joints(config), seed=0, calib_batch=1)
+        eng = H.device_model(name, pcfg, n_joints(config), sd, precision=precision).engine()
         return (pcfg, spec, sd, eng, port_ops.effnet_op_table(spec),
                 lambda nm, x, res, sc: port_ops.layer_bound(sd, spec, nm, x, res, sc, precision), ('silu', 'sigmoid'))
     if config == 'efficientnetv2-s-os8':
@@ -137,11 +147,11 @@ def check_head_per_coordinate(sd, feats, pcfg, c2d, c3d, tc32, n_joints=J):
     return w2, w3
 
 
-def heads_reference(sd, feats, pcfg):
+def heads_reference(sd, feats, pcfg, n_joints=J):
     """port.heads with the head's 1x1 conv evaluated in fp64 on the device (ResNet-50 at stride 8: 2048 channels on 32x32
     maps) and the soft-argmax decode on the host, where port.heads keeps its coordinate grids."""
     logits = port.head_logits(sd, feats.double().permute(0, 3, 1, 2)).cpu()
-    logits2d, logits3d = port.split_logits(logits, J, pcfg.depth)
+    logits2d, logits3d = port.split_logits(logits, n_joints, pcfg.depth)
     coords3d = port.heatmap_to_metric(port.soft_argmax(logits3d.float(), dims=(4, 3, 1)), pcfg)
     return port.heatmap_to_image(port.soft_argmax(logits2d.float(), dims=(3, 2)), pcfg), coords3d
 
@@ -204,9 +214,10 @@ def test_forward_ops_vs_conv2d(H, config, batch, precision):
                 if dk in (_lib.DW_TMA, _lib.DW_TMA_DIL):
                     hh, ww = (-(-n // op['dil']) for n in io['out_shape'][:2])
                     assert dw_plan(hh, ww)[0] > 0, nm
+                    reached.add(('dw tma', hh))
             elif k > 0 and eng.op_is_fused_block(k - 1):
                 kind = 'fmb_kernel'  # the block output; its input is the unfused expand's output, checked one op before
-                reached.add('fmb')
+                reached |= {'fmb', ('fmb', io['out_shape'][0])}
             elif classes[nm] in ('tc_conv_kernel', 'fmb_kernel'):
                 tk = eng.op_kernel(k)
                 kind = 'tc_conv3x3s1_kernel' if tk == _lib.TC_CONV3X3S1 else 'tc_conv_kernel'
@@ -234,13 +245,16 @@ def test_forward_ops_vs_conv2d(H, config, batch, precision):
     # the backbone's features are the full prefix's, bit for bit; the fused head decodes them like the reference
     feats = eng.backbone(crops)
     assert torch.equal(feats.float(), live[_lib.BUF_FEATURES])
+    eng.profile_begin()
     c2d, c3d = eng.head_decode(feats)
+    head_prof = eng.profile_end()
     head = {'heatmap_heads.conv_final.weight': sd['heatmap_heads.conv_final.weight'].to(st).double().cuda(),
             'heatmap_heads.conv_final.bias': sd['heatmap_heads.conv_final.bias'].float().double().cuda()}
-    ref2d, ref3d = heads_reference(head, feats, pcfg)
+    nj = n_joints(config)
+    ref2d, ref3d = heads_reference(head, feats, pcfg, nj)
     e2, e3 = H.rel_err(c2d, ref2d), H.rel_err(c3d, ref3d)
     assert e2 < 2e-4 and e3 < 2e-4, (e2, e3)
-    worst['head 2D'], worst['head 3D'] = check_head_per_coordinate(head, feats, pcfg, c2d, c3d, tc32=False)
+    worst['head 2D'], worst['head 3D'] = check_head_per_coordinate(head, feats, pcfg, c2d, c3d, tc32=False, n_joints=nj)
     # eager run, graph capture, graph replay (mtb_forward keys its graphs on buffers, batch and stream)
     o = torch.empty(batch, eng.n_out, 3, device=crops.device)
     joints = []
@@ -257,6 +271,16 @@ def test_forward_ops_vs_conv2d(H, config, batch, precision):
     if config == 'efficientnetv2-l':
         assert {('dw', _lib.DW_TMA), ('dw', _lib.DW_STRIP_16B), ('tc', _lib.TC_CONV3X3S1), 'fmb', 'stem3x3s2'} <= reached, reached
         assert {c for _, c in se_proj} == {192, 224, 384, 640} and se_wide == 32, se_proj
+    elif config == 'efficientnetv2-l@384':
+        # the fused head with one crop per tile (tc_head_plan: P = 144, 256 // 144 = 1 crop), the TMA depthwise plans of
+        # the 24x24 and 12x12 maps, fmb_kernel on the 96x96 and 48x48 stages
+        assert eng.feature_side == 12 and set(head_prof) == {'tc_head_softargmax_kernel'}, set(head_prof)
+        assert {('dw tma', 24), ('dw tma', 12), ('fmb', 96), ('fmb', 48)} <= reached, reached
+    elif config == 'efficientnetv2-s-j122':
+        # nine M tiles of the fused head, the last one 74 of 128 channels
+        n_out = sd['heatmap_heads.conv_final.weight'].shape[0]
+        assert n_out == 122 * 9 and -(-n_out // 128) == 9 and n_out % 128 == 74, n_out
+        assert set(head_prof) == {'tc_head_softargmax_kernel'}, set(head_prof)
     elif config == 'efficientnetv2-s-os8':
         assert {('dw dil', _lib.DW_TMA_DIL, 2), ('dw dil', _lib.DW_TMA_DIL, 4)} <= reached, reached
     elif config.startswith('efficientnet-b'):

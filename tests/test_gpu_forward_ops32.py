@@ -27,8 +27,8 @@ import torch
 
 from metrabs_b200 import _lib
 from oracle import port, port_ops
-from tests.test_gpu_forward_ops16 import (CONFIGS, DW_NAMES, J, build, check_conv, check_head_per_coordinate, check_se_fc,
-                                          heads_reference)
+from tests.test_gpu_forward_ops16 import (CONFIGS, DW_NAMES, build, check_conv, check_head_per_coordinate, check_se_fc,
+                                          heads_reference, n_joints)
 from tests.test_gpu_ops16_vs_conv2d import H, POOL_SLICES  # noqa: F401  (H: the fixture)
 
 pytestmark = pytest.mark.gpu
@@ -77,12 +77,12 @@ def oracle_features(spec, sd, crops):
     return torch.cat(feats)
 
 
-def oracle_tail(sd, feats, pcfg, intr):
+def oracle_tail(sd, feats, pcfg, intr, nj):
     """port.heads + port.reconstruct_absolute on NHWC features: the head's 1x1 conv in fp64 on the device, the soft-argmax
     (in fp32, as port.heads) and the reconstruction on the host."""
     head = {k: sd[k].double().cuda() for k in ('heatmap_heads.conv_final.weight', 'heatmap_heads.conv_final.bias')}
     with torch.inference_mode():
-        c2d, c3d = heads_reference(head, feats, pcfg)
+        c2d, c3d = heads_reference(head, feats, pcfg, nj)
     return port.reconstruct_absolute(c2d, c3d, intr.cpu(), pcfg)
 
 
@@ -192,7 +192,8 @@ def test_forward_ops_vs_conv2d(H, config, batch, precision):
     tc32_head = 'tc32_conv_kernel' in head_prof
     head = {'heatmap_heads.conv_final.weight': sd['heatmap_heads.conv_final.weight'].float().double().cuda(),
             'heatmap_heads.conv_final.bias': sd['heatmap_heads.conv_final.bias'].float().double().cuda()}
-    worst['head 2D'], worst['head 3D'] = check_head_per_coordinate(head, feats, pcfg, c2d, c3d, tc32_head)
+    nj = n_joints(config)
+    worst['head 2D'], worst['head 3D'] = check_head_per_coordinate(head, feats, pcfg, c2d, c3d, tc32_head, nj)
     # joints: eager run, graph capture, graph replay identical
     o = torch.empty(batch, eng.n_out, 3, device=crops.device)
     joints = []
@@ -210,9 +211,9 @@ def test_forward_ops_vs_conv2d(H, config, batch, precision):
     f64 = oracle_features(spec, sd, crops)
     e_feat = float((feats.double() - f64).abs().max() / f64.abs().max())
     assert e_feat < FEATURE_BAR, f'{config} x{batch} [{precision}]: features vs the fp64 oracle {e_feat:.2e}'
-    e_head = port.relative_error(joints[0].cpu(), oracle_tail(sd, feats.double(), pcfg, intr))
+    e_head = port.relative_error(joints[0].cpu(), oracle_tail(sd, feats.double(), pcfg, intr, nj))
     assert e_head < 1e-3, f'{config} x{batch} [{precision}]: joints vs the oracle head on the device features {e_head:.2e}'
-    e_joints = port.relative_error(joints[0].cpu(), oracle_tail(sd, f64, pcfg, intr))
+    e_joints = port.relative_error(joints[0].cpu(), oracle_tail(sd, f64, pcfg, intr, nj))
     del feats, f64
     torch.cuda.empty_cache()
 

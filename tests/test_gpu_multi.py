@@ -1,6 +1,8 @@
 """GPU, >= 2 devices (skipped otherwise): the data-parallel path over NCCL - mtb_forward_sharded (local backbone + head
 decode, ONE ncclAllGather of [coords2d|coords3d_rel], full-batch reconstruction) must reproduce the UNSHARDED forward of
-the concatenated batch on every rank (SURVEY.md 8e; batch-global RMS, ptu3d.py:71-74), including ragged and empty shards."""
+the concatenated batch on every rank (SURVEY.md 8e; batch-global RMS, ptu3d.py:71-74), including ragged and empty shards.
+Every per-crop stage is batch-invariant (test_gpu_batch_invariance.py), so every rank's result equals the unsharded one
+bit for bit."""
 import os
 import sys
 
@@ -13,7 +15,12 @@ pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _worker(rank, world, port_no, precision, out_dir):
+# (model, crop side, joints, crops per rank of the equal-shard case): the small model, and EfficientNetV2-L@256 at c3's
+# 32 crops per GPU
+MODELS = {'tiny': ('efficientnetv2-tiny', 64, 8, 4), 'l': ('efficientnetv2-l', 256, 24, 32)}
+
+
+def _worker(rank, world, port_no, precision, model, out_dir):
     sys.path.insert(0, ROOT)
     os.environ['MASTER_ADDR'] = '127.0.0.1'
     os.environ['MASTER_PORT'] = str(port_no)
@@ -23,9 +30,10 @@ def _worker(rank, world, port_no, precision, out_dir):
     from metrabs_b200 import parallel
     from oracle import port
     from tests import helpers
-    pcfg = port.PathConfig(proc_side=64)
-    sd = port.make_effnet_state_dict(port.effnet_spec('efficientnetv2-tiny'), pcfg, 8, seed=0)
-    m = helpers.device_model('efficientnetv2-tiny', pcfg, 8, sd, precision=precision).to(dev)
+    name, side, nj, per_rank = MODELS[model]
+    pcfg = port.PathConfig(proc_side=side)
+    sd = port.make_effnet_state_dict(port.effnet_spec(name), pcfg, nj, seed=0, **({'calib_batch': 1} if model == 'l' else {}))
+    m = helpers.device_model(name, pcfg, nj, sd, precision=precision).to(dev)
     eng = m.engine(dev)
 
     def bcast(raw):
@@ -35,8 +43,8 @@ def _worker(rank, world, port_no, precision, out_dir):
     eng.comm_init(rank, world, bcast)
     sh = parallel.ShardedMetrabs(m, rank, world)
     res = {}
-    for n_total in (8, 5, 1):  # equal shards (library path), ragged, fewer crops than ranks
-        crops, k = port.synthetic_inputs(n_total, 64, seed=3)
+    for n_total in (world * per_rank, 5, 1):  # equal shards (library path), ragged, fewer crops than ranks
+        crops, k = port.synthetic_inputs(n_total, side, seed=3)
         crops, k = crops.to(dev), k.to(dev)
         out = sh.forward(crops, k)
         ref = eng.forward(crops, k)
@@ -46,19 +54,26 @@ def _worker(rank, world, port_no, precision, out_dir):
     dist.destroy_process_group()
 
 
-@pytest.mark.parametrize('precision', ['fp32', 'bf16'])
-def test_sharded_equals_unsharded_nccl(tmp_path, precision):
+def _run(tmp_path, precision, model, port_no):
     if not torch.cuda.is_available() or torch.cuda.device_count() < 2:
         pytest.skip('needs >= 2 CUDA devices')
     world = 2
-    port_no = 33500 + (os.getpid() % 2000) + (0 if precision == 'fp32' else 1)
-    mp.spawn(_worker, args=(world, port_no, precision, str(tmp_path)), nprocs=world, join=True)
+    mp.spawn(_worker, args=(world, port_no, precision, model, str(tmp_path)), nprocs=world, join=True)
     outs = [torch.load(tmp_path / f'r{r}.pt') for r in range(world)]
-    tol = 1e-6 if precision == 'fp32' else 2e-2
-    for n_total in (8, 5, 1):
+    _, _, nj, per_rank = MODELS[model]
+    for n_total in (world * per_rank, 5, 1):
         for r in range(world):
             out, ref = outs[r][n_total]
-            assert out.shape == (n_total, 8, 3)
-            err = float((out - ref).abs().max() / ref.abs().max())
-            assert err <= tol, (n_total, r, err)
+            assert out.shape == (n_total, nj, 3)
+            assert torch.equal(out, ref), (n_total, r, float((out - ref).abs().max()))
         assert torch.equal(outs[0][n_total][0], outs[1][n_total][0])  # every rank holds the same full result
+
+
+@pytest.mark.parametrize('precision', ['fp32', 'bf16'])
+def test_sharded_equals_unsharded_nccl(tmp_path, precision):
+    _run(tmp_path, precision, 'tiny', 33500 + (os.getpid() % 2000) + (0 if precision == 'fp32' else 1))
+
+
+def test_sharded_effnetv2_l_c3_share_nccl(tmp_path):
+    """EfficientNetV2-L@256 in bf16 at 2 x 32 crops: c3's share per GPU on the benchmark's model"""
+    _run(tmp_path, 'bf16', 'l', 33500 + (os.getpid() % 2000) + 2)
