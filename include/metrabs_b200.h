@@ -45,12 +45,14 @@ typedef enum { MTB_DTYPE_F32 = 0, MTB_DTYPE_BF16 = 1, MTB_DTYPE_F16 = 2, MTB_DTY
  * (backbones/efficientnet.py:379-433) with BatchNorm epsilon 1e-3; EFFNET_EPS1E5 is the same grammar with torchvision's
  * default epsilon 1e-5, for EfficientNet-B0..B4 (:753-960), and takes MBConv rows only (kernel 3 or 5, stride 1 or 2;
  * anything else fails with MTB_ERR_UNSUPPORTED); the RESNET* values (V1, metrabs_tf/backbones/resnet.py: ResNet-18/34 with the
- * basic block :322-388, ResNet-50/101/152 with the bottleneck :239-319) and MOBILENETV3_SMALL / _LARGE
+ * basic block :322-388, ResNet-50/101/152 with the bottleneck :239-319), the RESNET*V2 values (the pre-activation
+ * ResNet-50/101/152, ResNetUnifiedV2 :710-745 with block2_dense :391-456, output strides 8, 16 and 32) and MOBILENETV3_SMALL / _LARGE
  * (metrabs_tf/backbones/mobilenet_v3.py:348-384 / :387-428, alpha 1, not minimalistic) follow the TF-only
  * metrabs_tf/backbones/{resnet,mobilenet_v3}.py. */
 typedef enum { MTB_ARCH_EFFNET = 0, MTB_ARCH_RESNET50 = 1, MTB_ARCH_MOBILENETV3_SMALL = 2,
                MTB_ARCH_HEAD_ONLY = 3, MTB_ARCH_RESNET18 = 4, MTB_ARCH_RESNET34 = 5, MTB_ARCH_RESNET101 = 6,
-               MTB_ARCH_RESNET152 = 7, MTB_ARCH_MOBILENETV3_LARGE = 8, MTB_ARCH_EFFNET_EPS1E5 = 9 } mtb_arch;
+               MTB_ARCH_RESNET152 = 7, MTB_ARCH_MOBILENETV3_LARGE = 8, MTB_ARCH_EFFNET_EPS1E5 = 9,
+               MTB_ARCH_RESNET50V2 = 10, MTB_ARCH_RESNET101V2 = 11, MTB_ARCH_RESNET152V2 = 12 } mtb_arch;
 
 /* Arithmetic of the conv/GEMM kernels.  FP32: CUDA-core fp32 FMA everywhere (the 1e-3 parity mode).
  * BF16_TC: bf16 operands on wgmma tensor cores with fp32 accumulation in registers, bf16 activations in HBM
@@ -333,6 +335,14 @@ int mtb_debug_run_op(mtb_handle* h, int op_index, const float* in, const float* 
 int mtb_op_is_fused_block(const mtb_handle* h, int op_index);
 int mtb_debug_run_fused_block(mtb_handle* h, int op_index, const float* in, int batch, float* out, size_t out_floats,
                               void* workspace, size_t workspace_bytes, void* stream);
+/* ResNet V2 pre-activation fusion (BF16_TC and F16_TC modes): 1 when backbone op `op_index` (a block's 1x1 _3_conv, + shortcut)
+ * and the op after it (the next block's _preact_bn + ReLU, or post_bn + ReLU: a 1x1 depthwise op) run as ONE
+ * tc_conv_preact_kernel launch [tc_conv_preact_kernel] that stores both outputs, bit-identical to the two launches.
+ * mtb_debug_run_preact_pair runs that pair in isolation on caller-provided fp32 NHWC device tensors `in` [B,H,W,Cin] and
+ * `res` [B,H,W,Cout]; `out` receives the GEMM's output and `out_preact` the pre-activation, both [B,H,W,Cout] as fp32. */
+int mtb_op_is_preact_pair(const mtb_handle* h, int op_index);
+int mtb_debug_run_preact_pair(mtb_handle* h, int op_index, const float* in, const float* res, int batch, float* out, float* out_preact,
+                              size_t out_floats, void* workspace, size_t workspace_bytes, void* stream);
 /* CUDA-event profiler (bench.py's live roofline measurement): between begin and end, every kernel launch of the
  * classes selected by `class_mask` (bit i = class i) is bracketed by cudaEventRecord on the launching stream.
  * mtb_profile_end synchronises those events and returns, per class, the summed device time (ms), algorithmic

@@ -10,6 +10,7 @@ ARCH_EFFNET, ARCH_RESNET50, ARCH_MOBILENETV3_SMALL, ARCH_HEAD_ONLY = 0, 1, 2, 3
 ARCH_RESNET18, ARCH_RESNET34, ARCH_RESNET101, ARCH_RESNET152 = 4, 5, 6, 7
 ARCH_MOBILENETV3_LARGE = 8
 ARCH_EFFNET_EPS1E5 = 9  # the EFFNET grammar with BatchNorm eps 1e-5 (EfficientNet-B0..B4)
+ARCH_RESNET50V2, ARCH_RESNET101V2, ARCH_RESNET152V2 = 10, 11, 12  # the pre-activation ResNets
 # mtb_kernel (mtb_op_kernel): the kernel that runs an op
 DW_GENERIC, DW_TMA, DW_STRIP_16B, DW_STRIP_F32, DW_5X5_16B, DW_5X5_POOL_16B, DW_TMA_DIL = 0, 1, 2, 3, 4, 5, 6
 STEM_3X3S2, STEM_WIDE, STEM_GENERIC = 7, 8, 9
@@ -128,6 +129,9 @@ _SIGNATURES = {
                                    C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
     'mtb_op_kernel': (C.c_int, [C.c_void_p, C.c_int]),
     'mtb_op_is_fused_block': (C.c_int, [C.c_void_p, C.c_int]),
+    'mtb_op_is_preact_pair': (C.c_int, [C.c_void_p, C.c_int]),
+    'mtb_debug_run_preact_pair': (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                            C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
     'mtb_debug_run_fused_block': (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p,
                                             C.c_size_t, C.c_void_p]),
     'mtb_profile_begin': (C.c_int, [C.c_void_p, C.c_uint]),

@@ -1,5 +1,5 @@
-"""ResNet V1 (MeTRAbs stride/dilation switching) parameter holders for the H100 engine: ResNet-18 / 34 (basic block) and
-ResNet-50 / 101 / 152 (bottleneck).
+"""ResNet (MeTRAbs stride/dilation switching) parameter holders for the H100 engine: ResNet-18 / 34 (V1 basic block),
+ResNet-50 / 101 / 152 (V1 bottleneck) and the pre-activation ResNet-50 / 101 / 152 V2 (``FeaturesV2``).
 
 The reference has these backbones only as Keras code (metrabs_tf/backbones/resnet.py:239-319 bottleneck,
 :322-388 basic block, :601-707 stride plan and stacks, :746-788 depths); there is no PyTorch key schema for them, so this
@@ -76,3 +76,56 @@ def resnet101(**kwargs):
 def resnet152(**kwargs):
     """Use as ``Metrabs(resnet152(), joint_info)`` (keys ``backbone.<keras layer>...``)."""
     return Features(152)
+
+
+# depth -> (arch, blocks in conv2..conv5) of the pre-activation nets (metrabs_tf/backbones/resnet.py:803-831)
+DEPTHS_V2 = {50: (_lib.ARCH_RESNET50V2, [3, 4, 6, 3]), 101: (_lib.ARCH_RESNET101V2, [3, 4, 23, 3]),
+             152: (_lib.ARCH_RESNET152V2, [3, 8, 36, 3])}
+
+
+class FeaturesV2(nn.Module):
+    """ResNetUnifiedV2 (metrabs_tf/backbones/resnet.py:710-745, block2_dense :391-456) parameters under the Keras layer
+    names: ``backbone.conv1_conv.{weight,bias}`` (no stem BN), per block ``_preact_bn``, ``_0_conv.{weight,bias}`` (block1
+    of a stack only), ``_1_conv.weight`` + ``_1_bn``, ``_2_conv.weight`` + ``_2_bn``, ``_3_conv.{weight,bias}`` (no BN),
+    and ``backbone.post_bn``.  The bias of ``_0_conv`` is Keras' default for a ``Conv2DDenseSame`` that does not pass
+    ``use_bias`` (the class is from the un-vendored ``fleras``: a reading, as for V1)."""
+    stages = []
+
+    def __init__(self, depth=50):
+        super().__init__()
+        self.arch, counts = DEPTHS_V2[depth]
+        self.depth = depth
+        self.last_channel = 2048
+        self.add_module('conv1_conv', nn.Conv2d(3, 64, 7, bias=True))
+        cin = 64
+        for st, (f, n) in enumerate(zip([64, 128, 256, 512], counts)):
+            for bi in range(n):
+                name = f'conv{st + 2}_block{bi + 1}'
+                self.add_module(name + '_preact_bn', nn.BatchNorm2d(cin, eps=1e-5))
+                if bi == 0:
+                    self.add_module(name + '_0_conv', nn.Conv2d(cin, 4 * f, 1, bias=True))
+                self.add_module(name + '_1_conv', nn.Conv2d(cin, f, 1, bias=False))
+                self.add_module(name + '_1_bn', nn.BatchNorm2d(f, eps=1e-5))
+                self.add_module(name + '_2_conv', nn.Conv2d(f, f, 3, bias=False))
+                self.add_module(name + '_2_bn', nn.BatchNorm2d(f, eps=1e-5))
+                self.add_module(name + '_3_conv', nn.Conv2d(f, 4 * f, 1, bias=True))
+                cin = 4 * f
+        self.add_module('post_bn', nn.BatchNorm2d(cin, eps=1e-5))
+
+    def forward(self, x):
+        raise RuntimeError('metrabs_b200 backbones run inside Metrabs.forward (libmetrabs_b200.so)')
+
+
+def resnet50v2(**kwargs):
+    """Use as ``Metrabs(resnet50v2(), joint_info)`` (keys ``backbone.<keras layer>...``, see FeaturesV2)."""
+    return FeaturesV2(50)
+
+
+def resnet101v2(**kwargs):
+    """Use as ``Metrabs(resnet101v2(), joint_info)`` (keys ``backbone.<keras layer>...``, see FeaturesV2)."""
+    return FeaturesV2(101)
+
+
+def resnet152v2(**kwargs):
+    """Use as ``Metrabs(resnet152v2(), joint_info)`` (keys ``backbone.<keras layer>...``, see FeaturesV2)."""
+    return FeaturesV2(152)

@@ -34,12 +34,12 @@ enum OpType { OP_STEM = 0, OP_CONV = 1, OP_DW = 2, OP_POOL = 3, OP_MAXPOOL = 4 }
 // kernel classes for the CUDA-event profiler (mtb_profile_begin / mtb_profile_end)
 enum KClass { KC_STEM = 0, KC_IGEMM_SIMT = 1, KC_DWCONV = 2, KC_POOL = 3, KC_SE_FC = 4, KC_TC_GEMM = 5, KC_FMB = 6,
               KC_HEAD_FUSED = 7, KC_HEAD_CONV_SIMT = 8, KC_SOFTARGMAX = 9, KC_RECON = 10, KC_OTHER = 11, KC_SE_SCALE = 12, KC_TC32 = 13,
-              KC_COMBINE = 14, KC_COUNT = 15 };
+              KC_COMBINE = 14, KC_TC_PREACT = 15, KC_COUNT = 16 };
 const char* kKClassNames[KC_COUNT] = {"stem_conv_kernel", "conv_igemm_kernel", "dwconv_kernel", "pool_mean_kernel",
                                       "se_fc(conv_igemm_kernel)", "tc_conv_kernel", "fmb_kernel",
                                       "tc_head_softargmax_kernel", "head_conv(conv_igemm_kernel)",
                                       "softargmax_bhwn_kernel", "recon_pass1+2_kernel", "other", "se_scale_kernel", "tc32_conv_kernel",
-                                      "combine_points_kernel"};
+                                      "combine_points_kernel", "tc_conv_preact_kernel"};
 // One row per mtb_kernel value: the profiler class of its launches, whether it exists for 16-bit storage only (bf16 /
 // fp16), and whether it also writes the SE pooling slices of its output (depthwise)
 struct KernelTraits { mtb_kernel kernel; KClass cls; bool only16, pools; };
@@ -98,6 +98,8 @@ struct Op {
   TcWeights tc;             // 16-bit (bf16 / fp16) K-major copy + TMA descriptor state for the wgmma path
   Tc32Weights tc32;         // fp32 K-major copy + TMA descriptor state for the 3xTF32 wgmma path (MTB_PRECISION_TF32X3)
   FmbWeights fmb;           // 16-bit tensor-core modes: this 3x3 expand conv and the NEXT op (1x1 projection) run as one fmb_kernel launch
+  bool preact_next = false;  // 16-bit tensor-core modes: this 1x1 GEMM also writes the NEXT op's output (ResNet V2 pre-activation,
+                             // a 1x1 depthwise BN + ReLU) in one tc_conv_preact_kernel launch
   mutable TmapCache dw_maps;    // DW_TMA / DW_TMA_DIL: its input tensor maps
   double flops = 0;         // 2*MACs per crop
 };
@@ -532,6 +534,111 @@ int plan_resnet(mtb_handle* h, const int counts[4], bool basic) {
   return MTB_OK;
 }
 
+// The pre-activation ResNets (ResNetUnifiedV2, metrabs_tf/backbones/resnet.py:710-745; ResNet :160-193 with preact=True,
+// use_bias=True; block2_dense :391-456; stack2_dense :558-580; BN eps 1e-5 :52) at output stride `stride_test`, `counts`
+// blocks in conv2..conv5, preprocessing tf_preproc 2x - 1 (builder.py:111-113):
+// * stem: conv1_conv 7x7 stride 2 with bias, no BN and no ReLU; zero pad 1 + 3x3 stride-2 max pool of the signed values;
+// * block: preact = relu(_preact_bn(x)) (a 1x1 depthwise op, BN only); shortcut _0_conv(preact) (1x1 with bias, block1 of a
+//   stack), x[c::2, c::2] (a 1x1 max pool with stride 2 and begin pad -c, the strided last block of conv2..conv4) or x;
+//   _1_conv (1x1, BN, ReLU) and _2_conv (3x3 dense SAME sampled at c::s, dilated, BN, ReLU) without biases; out = shortcut
+//   + _3_conv (1x1 with bias, no BN, no activation);
+// * stride plan: the stride sits on the LAST block of conv2..conv4 (dilation dil_in of its stack, shift brs), the other
+//   blocks of those stacks have stride 1 and dil_in; conv5 uses dil_out[2] throughout;
+// * features: relu(post_bn(x)).
+// Keys: "backbone.conv1_conv.{weight,bias}", "backbone.conv<k>_block<i>_preact_bn.*", "_0_conv.{weight,bias}",
+// "_1_conv.weight", "_1_bn.*", "_2_conv.weight", "_2_bn.*", "_3_conv.{weight,bias}", "backbone.post_bn.*".
+int plan_resnet_v2(mtb_handle* h, const int counts[4]) {
+  const mtb_config& c = h->cfg;
+  if (c.stride_test != 8 && c.stride_test != 16 && c.stride_test != 32)
+    return fail(h, MTB_ERR_UNSUPPORTED, "ResNet V2: stride_test must be 8, 16 or 32 (got %d)", c.stride_test);
+  int strides[3], dil_in[3], dil_out[3];
+  bool brs[3];
+  resnet_stride_plan(c.stride_test, c.centered_stride, strides, dil_in, dil_out, brs);
+  Planner P{h, c.proc_side, c.proc_side, 3};
+  const std::string pre = "backbone.";
+  const float eps = 1e-5f;
+  // relu(BN(x)) of the tensor in `in`, as a 1x1 depthwise op with no conv weight
+  auto preact = [&](const std::string& name, int in, int out) {
+    P.conv_k(name, "", "", name, P.C, 1, 1, 0, 0, ACT_RELU, in, out, true, 1, eps);
+  };
+  {
+    Op op;
+    op.type = OP_STEM;
+    op.name = pre + "conv1_conv";
+    op.wkey = op.name + ".weight"; op.biaskey = op.name + ".bias";
+    op.Hin = op.Win = c.proc_side; op.Cin = 3; op.Cout = 64;
+    op.R = op.S = 7; op.stride = 2; op.pad_t = op.pad_l = 3; op.act = ACT_NONE;  // pre_scale / pre_shift: 2x - 1
+    op.Hout = op.Wout = (c.proc_side + 6 - 7) / 2 + 1;
+    op.in_buf = BUF_NONE; op.out_buf = 0;
+    op.flops = 2.0 * op.Hout * op.Wout * 64 * 147;
+    P.H = op.Hout; P.W = op.Wout; P.C = 64;
+    P.track(P.H, P.W, P.C);
+    h->ops.push_back(op);
+    Op mp;
+    mp.type = OP_MAXPOOL; mp.name = pre + "pool1_pool";
+    mp.Hin = P.H; mp.Win = P.W; mp.Cin = mp.Cout = 64; mp.R = mp.S = 3; mp.stride = 2; mp.pad_t = mp.pad_l = 1;
+    mp.Hout = (P.H + 2 - 3) / 2 + 1; mp.Wout = (P.W + 2 - 3) / 2 + 1;
+    mp.in_buf = 0; mp.out_buf = 1;
+    P.H = mp.Hout; P.W = mp.Wout; P.cur = 1;
+    h->ops.push_back(mp);
+  }
+  const int filters[4] = {64, 128, 256, 512};
+  // the previous block's _3_conv reads these while a fused launch writes the pre-activation: keep it out of them
+  int prev_in = BUF_NONE, prev_res = BUF_NONE;
+  for (int st = 0; st < 4; ++st) {
+    for (int bi = 0; bi < counts[st]; ++bi) {
+      const bool first = bi == 0, last_of_stack = bi == counts[st] - 1;
+      const bool strided = st < 3 && last_of_stack && strides[st] == 2;
+      const int stride = strided ? 2 : 1;
+      const int shift = (st < 3 && last_of_stack && brs[st]) ? 1 : 0;
+      const int dil = st < 3 ? dil_in[st] : dil_out[2];
+      const int f = filters[st];
+      char nm[64];
+      snprintf(nm, sizeof(nm), "conv%d_block%d", st + 2, bi + 1);
+      const std::string b = pre + nm;
+      const int x_in = P.cur;
+      const int Hin = P.H, Win = P.W, Cin = P.C;
+      const int pa = P.pick({x_in, prev_in, prev_res});
+      preact(b + "_preact_bn", x_in, pa);
+      int sc = x_in;
+      if (first) {
+        sc = P.pick({x_in, pa});
+        P.conv_k(b + "_0_conv", b + "_0_conv.weight", b + "_0_conv.bias", "", 4 * f, 1, 1, 0, 0, ACT_NONE, pa, sc, false, 1, eps);
+        P.H = Hin; P.W = Win; P.C = Cin;  // the main branch restarts from the pre-activation
+      } else if (stride > 1 || shift) {  // x[c::2, c::2]: Cropping2D(c) + MaxPooling2D(1, 2)
+        sc = P.pick({x_in, pa});
+        Op mp;
+        mp.type = OP_MAXPOOL; mp.name = b + "_shortcut_pool";
+        mp.Hin = Hin; mp.Win = Win; mp.Cin = mp.Cout = Cin; mp.stride = stride; mp.pad_t = mp.pad_l = -shift;
+        mp.Hout = Hin / stride; mp.Wout = Win / stride;
+        mp.in_buf = x_in; mp.out_buf = sc;
+        P.track(mp.Hout, mp.Wout, Cin);
+        h->ops.push_back(mp);
+      }
+      const int t1 = P.pick({pa, sc});
+      P.conv_k(b + "_1_conv", b + "_1_conv.weight", "", b + "_1_bn", f, 1, 1, 0, 0, ACT_RELU, pa, t1, false, 1, eps);
+      const int t2 = P.pick({sc, t1});
+      // _2_conv: dense SAME 3x3 sampled at shift::stride, i.e. a strided conv with begin pad dil - shift
+      Op& o2 = P.conv_k(b + "_2_conv", b + "_2_conv.weight", "", b + "_2_bn", f, 3, stride, dil - shift, 2 * dil, ACT_RELU, t1, t2,
+                        false, dil, eps);
+      o2.Hout = Hin / stride; o2.Wout = Win / stride;
+      o2.flops = 2.0 * o2.Hout * o2.Wout * f * f * 9;
+      P.H = o2.Hout; P.W = o2.Wout;
+      const int t3 = P.pick({sc, t2});
+      Op& o3 = P.conv_k(b + "_3_conv", b + "_3_conv.weight", b + "_3_conv.bias", "", 4 * f, 1, 1, 0, 0, ACT_NONE, t2, t3, false, 1, eps);
+      o3.res_buf = sc;
+      P.cur = t3;
+      prev_in = t2; prev_res = sc;
+    }
+  }
+  preact(pre + "post_bn", P.cur, BUF_FEATURES);
+  h->feat_side = P.H;
+  h->feat_c = P.C;
+  h->big_elems_per_crop = P.max_elems;
+  h->small_c = 4;
+  return MTB_OK;
+}
+
 // One row of a MobileNetV3 table: _inverted_res_block(x, expansion, filters, kernel, stride, se_ratio, activation, ...)
 // with the expanded width already rounded by _depth
 struct MbV3Row { int exp_ch, filters, k, stride; bool se; int act; bool br; };
@@ -624,6 +731,9 @@ struct ResNetArch { int arch; int counts[4]; bool basic; };
 const ResNetArch kResNets[] = {{MTB_ARCH_RESNET18, {2, 2, 2, 2}, true},    {MTB_ARCH_RESNET34, {3, 4, 6, 3}, true},
                                {MTB_ARCH_RESNET50, {3, 4, 6, 3}, false},   {MTB_ARCH_RESNET101, {3, 4, 23, 3}, false},
                                {MTB_ARCH_RESNET152, {3, 8, 36, 3}, false}};
+// block counts of the pre-activation nets (resnet.py:803-831)
+const ResNetArch kResNetsV2[] = {{MTB_ARCH_RESNET50V2, {3, 4, 6, 3}, false}, {MTB_ARCH_RESNET101V2, {3, 4, 23, 3}, false},
+                                 {MTB_ARCH_RESNET152V2, {3, 8, 36, 3}, false}};
 
 int plan(mtb_handle* h) {
   const mtb_config& c = h->cfg;
@@ -631,8 +741,14 @@ int plan(mtb_handle* h) {
   const ResNetArch* resnet = nullptr;
   for (const ResNetArch& r : kResNets)
     if (c.arch == r.arch) resnet = &r;
+  const ResNetArch* resnet_v2 = nullptr;
+  for (const ResNetArch& r : kResNetsV2)
+    if (c.arch == r.arch) resnet_v2 = &r;
   if (resnet) {
     int rc = plan_resnet(h, resnet->counts, resnet->basic);
+    if (rc) return rc;
+  } else if (resnet_v2) {
+    int rc = plan_resnet_v2(h, resnet_v2->counts);
     if (rc) return rc;
   } else switch (c.arch) {
     case MTB_ARCH_EFFNET: plan_effnet(h, 1e-3f); break;
@@ -676,8 +792,11 @@ int upload(mtb_handle* h, const void* host, size_t bytes, void** dev) {
 
 int prepare_op_weights(mtb_handle* h, Op& op) {
   if (op.type == OP_POOL || op.type == OP_MAXPOOL) return MTB_OK;
-  const HostTensor* w = find(h, op.wkey);
-  if (!w) return fail(h, MTB_ERR_MISSING_WEIGHT, "missing weight '%s'", op.wkey.c_str());
+  // a BatchNorm alone (ResNet V2 pre-activation): a 1x1 depthwise op whose conv weight is 1
+  HostTensor ones;
+  if (op.wkey.empty() && op.depthwise && op.R == 1 && op.S == 1) ones = {std::vector<float>(op.Cout, 1.f), {op.Cout, 1, 1, 1}};
+  const HostTensor* w = op.wkey.empty() ? &ones : find(h, op.wkey);
+  if (!w || w->data.empty()) return fail(h, MTB_ERR_MISSING_WEIGHT, "missing weight '%s'", op.wkey.c_str());
   const int cin_g = op.depthwise ? 1 : op.Cin;
   const int64_t expect[4] = {op.Cout, cin_g, op.R, op.S};
   bool shape_ok = w->shape.size() == 4 && std::equal(expect, expect + 4, w->shape.begin());
@@ -942,7 +1061,7 @@ void choose_kernels(mtb_handle* h) {
 }
 
 // profiler class of a backbone op: fmb_kernel for the first op of a fused FusedMBConv block
-int op_class(const Op& op) { return op.fmb.ready ? KC_FMB : kKernels[op.kernel].cls; }
+int op_class(const Op& op) { return op.fmb.ready ? KC_FMB : op.preact_next ? KC_TC_PREACT : kKernels[op.kernel].cls; }
 
 double op_weight_bytes(const Op& op) {
   if (op.type == OP_POOL || op.type == OP_MAXPOOL) return 0.0;
@@ -1114,6 +1233,28 @@ int run_fused_block(mtb_handle* h, const Op& a, const Op& b, int B, const Worksp
   return MTB_OK;
 }
 
+// one tc_conv_preact_kernel launch for a 1x1 GEMM (a) and the pre-activation op behind it (b)
+int run_preact_pair(mtb_handle* h, const Op& a, const Op& b, int B, const Workspace& ws, void* features, cudaStream_t st) {
+  ConvParams p;
+  p.in = buf_ptr(ws, a.in_buf, features);
+  p.out = buf_ptr(ws, a.out_buf, features);
+  p.res = buf_ptr(ws, a.res_buf, features);
+  p.a_scale = nullptr;
+  p.w = a.d_w; p.bias = a.d_bias;
+  p.B = B; p.Hin = a.Hin; p.Win = a.Win; p.Cin = a.Cin; p.Hout = a.Hout; p.Wout = a.Wout; p.Cout = a.Cout;
+  p.R = a.R; p.S = a.S; p.stride = a.stride; p.dil = a.dil; p.pad_t = a.pad_t; p.pad_l = a.pad_l; p.act = a.act;
+  p.res_first = 0;
+  ProfScope prof(h, KC_TC_PREACT, (a.flops + b.flops) * B, op_bytes(h, a, B) + (double)B * b.Hout * b.Wout * b.Cout * elem_size(h), st);
+  const char* e = with_storage16(h, [&](auto* tag) {
+    return tc_conv_launch<std::remove_pointer_t<decltype(tag)>>(a.tc, p, false, false, st, buf_ptr(ws, b.out_buf, features),
+                                                                TcPreact{b.d_w, b.d_bias});
+  });
+  if (!e) e = cuda_msg(cudaGetLastError());
+  if (e) return fail(h, MTB_ERR_CUDA, "fused pre-activation launch %s: %s", a.name.c_str(), e);
+  h->launches++;
+  return MTB_OK;
+}
+
 // ops [first, last): fusable pairs that lie inside the range run fused
 int run_ops_range(mtb_handle* h, size_t first, size_t last, const float* crops, int B, const Workspace& ws, void* features,
                   cudaStream_t st) {
@@ -1122,6 +1263,9 @@ int run_ops_range(mtb_handle* h, size_t first, size_t last, const float* crops, 
     int rc;
     if (h->ops[k].fmb.ready && k + 1 < last) {
       rc = run_fused_block(h, h->ops[k], h->ops[k + 1], B, ws, features, st);
+      ++k;
+    } else if (h->ops[k].preact_next && k + 1 < last) {
+      rc = run_preact_pair(h, h->ops[k], h->ops[k + 1], B, ws, features, st);
       ++k;
     } else {
       rc = run_op(h, h->ops[k], crops, B, ws, features, st);
@@ -1480,6 +1624,16 @@ int mtb_finalize_weights(mtb_handle* h) {
     if (b.res_buf != BUF_NONE && b.res_buf != a.in_buf) continue;
     if (a.Hin != a.Hout || a.Win != a.Wout || b.out_buf == a.in_buf) continue;
     fmb_prepare(a.fmb, a.tc, b.tc);
+  }
+  // ResNet V2: a block's _3_conv and the pre-activation behind it (the next block's, or post_bn): one tc_conv_preact_kernel.
+  // Its tiles store the pre-activation while later tiles still read the GEMM's input and residual, so b writes neither.
+  for (size_t i = 0; i + 1 < h->ops.size(); ++i) {
+    Op& a = h->ops[i];
+    const Op& b = h->ops[i + 1];
+    a.preact_next = a.kernel == MTB_TC_CONV && b.kernel == MTB_DW_GENERIC && b.R == 1 && b.S == 1 && b.stride == 1 &&
+                    b.act == ACT_RELU && b.Cout == a.Cout && b.in_buf == a.out_buf && b.out_buf != a.out_buf &&
+                    b.out_buf != a.in_buf && b.out_buf != a.res_buf && a.scale_buf == BUF_NONE && !a.res_first &&
+                    tc_preact_eligible(a.R, a.stride, a.Cout, a.act, a.res_buf != BUF_NONE);
   }
   {
     Op& hd = h->head;
@@ -2281,6 +2435,34 @@ int mtb_debug_run_fused_block(mtb_handle* h, int op_index, const float* in, int 
   rc = run_fused_block(h, a, b, batch, ws, nullptr, st);
   if (rc) return rc;
   copy_to_float(h, buf_ptr(ws, 2, nullptr), out, n_out, st);
+  CUDA_TRY(h, cudaGetLastError());
+  return MTB_OK;
+}
+
+int mtb_op_is_preact_pair(const mtb_handle* h, int op_index) {
+  return (h && op_index >= 0 && op_index + 1 < (int)h->ops.size() && h->ops[op_index].preact_next) ? 1 : 0;
+}
+
+int mtb_debug_run_preact_pair(mtb_handle* h, int op_index, const float* in, const float* res, int batch, float* out, float* out_preact,
+                              size_t out_floats, void* workspace, size_t workspace_bytes, void* stream) {
+  int rc = check_common(h, batch, workspace_bytes, workspace);
+  if (rc) return rc;
+  if (op_index < 0 || op_index + 1 >= (int)h->ops.size() || !in || !res || !out || !out_preact)
+    return fail(h, MTB_ERR_INVALID_ARG, "invalid debug arguments");
+  if (!h->ops[op_index].preact_next) return fail(h, MTB_ERR_UNSUPPORTED, "op %d does not run fused with the pre-activation after it", op_index);
+  DeviceGuard g(h->cfg.device);
+  cudaStream_t st = (cudaStream_t)stream;
+  Workspace ws = layout(h, batch, workspace);
+  Op a = h->ops[op_index], b = h->ops[op_index + 1];
+  const size_t n_in = (size_t)batch * a.Hin * a.Win * a.Cin, n_out = (size_t)batch * a.Hout * a.Wout * a.Cout;
+  if (n_out > out_floats) return fail(h, MTB_ERR_INVALID_ARG, "debug output buffer too small");
+  copy_from_float(h, in, buf_ptr(ws, 0, nullptr), n_in, st);
+  copy_from_float(h, res, buf_ptr(ws, 1, nullptr), n_out, st);
+  a.in_buf = 0; a.res_buf = 1; a.out_buf = 2; b.in_buf = 2; b.out_buf = 3;
+  rc = run_preact_pair(h, a, b, batch, ws, nullptr, st);
+  if (rc) return rc;
+  copy_to_float(h, buf_ptr(ws, 2, nullptr), out, n_out, st);
+  copy_to_float(h, buf_ptr(ws, 3, nullptr), out_preact, n_out, st);
   CUDA_TRY(h, cudaGetLastError());
   return MTB_OK;
 }

@@ -242,9 +242,35 @@ __device__ __forceinline__ void tma_load_tap_boxes(uint8_t* dst, int box_bytes, 
 // min(BN, 64)), then one thread stores the slabs with the TMA (2D box for mode 0, 4D 16 x 8-pixel box for mode 1).  The
 // TMA clips what lies outside the tensor: the M tail, the parts of a 16 x 8 box beyond the map, the Cout tail.  Uses the
 // named barrier 3 + c; the staging tile is rewritten only after the warpgroup's previous stores have read it.
-template <typename T, int ACT, int RES, int BN>
+//
+// PRE (ResNet V2, mode 0): the tile is also the input of the next block's pre-activation, a 1x1 depthwise op
+// z = relu(x * pre.w[c] + pre.b[c]) (its BatchNorm folded).  Once the TMA has read the stored tile out of the staging tile,
+// every thread rewrites the elements it wrote with z, computed from the stored 16-bit value exactly as dwconv_kernel
+// computes it (fmaf(x, w, b), then fmaxf(., 0), rounded to nearest even), and the leader stores the tile again through
+// tmZ.  The two outputs are bit-identical to the GEMM and dwconv_kernel launched one after the other.
+struct TcPreact {
+  const float* w;  // [Cout] folded BN scale of the absorbed op
+  const float* b;  // [Cout] folded BN shift
+};
+template <int BN>
+__device__ __forceinline__ void tc_store_staging(const uint8_t* stg, const CUtensorMap* map, const TcConvParams& p, int m_blk, int n_blk) {
+  constexpr int SW = BN < 64 ? BN : 64, RB = SW * 2;
+#pragma unroll
+  for (int sl = 0; sl < BN / SW; ++sl) {
+    const int col0 = n_blk * BN + sl * SW;
+    if (col0 >= p.Cout) break;
+    if (p.mode == 0) {
+      tma_store_2d(map, stg + sl * TC_BM * RB, col0, m_blk * TC_BM);
+    } else {
+      const int tw = m_blk % p.tiles_w, th = (m_blk / p.tiles_w) % p.tiles_h, b = m_blk / (p.tiles_w * p.tiles_h);
+      tma_store_4d(map, stg + sl * TC_BM * RB, col0, tw * TC_TILE_W, th * TC_TILE_H, b);
+    }
+  }
+  bulk_commit();
+}
+template <typename T, int ACT, int RES, int BN, bool PRE = false>
 __device__ __forceinline__ void tc_tile_epilogue(const float* acc, uint8_t* stg, const CUtensorMap* tmO, const TcConvParams& p, int m_blk,
-                                                 int n_blk, int c) {
+                                                 int n_blk, int c, const CUtensorMap* tmZ = nullptr, TcPreact pre = {}) {
   constexpr int SW = BN < 64 ? BN : 64, RB = SW * 2;  // staging slab: columns, bytes per row
   typedef typename Pair16<T>::type T2;
   const T* __restrict__ res = (const T*)p.res;
@@ -305,19 +331,32 @@ __device__ __forceinline__ void tc_tile_epilogue(const float* acc, uint8_t* stg,
   }
   fence_proxy_async();  // generic-proxy writes -> visible to the TMA (async proxy)
   wg_sync(2 + c);
-  if (leader) {
+  if (leader) tc_store_staging<BN>(stg, tmO, p, m_blk, n_blk);
+  if constexpr (PRE) {
+    if (leader) bulk_wait_read();  // the block output has left the staging tile
+    wg_sync(2 + c);
 #pragma unroll
-    for (int sl = 0; sl < BN / SW; ++sl) {
-      const int col0 = n_blk * BN + sl * SW;
-      if (col0 >= p.Cout) break;
-      if (p.mode == 0) {
-        tma_store_2d(tmO, stg + sl * TC_BM * RB, col0, m_blk * TC_BM);
-      } else {
-        const int tw = m_blk % p.tiles_w, th = (m_blk / p.tiles_w) % p.tiles_h, b = m_blk / (p.tiles_w * p.tiles_h);
-        tma_store_4d(tmO, stg + sl * TC_BM * RB, col0, tw * TC_TILE_W, th * TC_TILE_H, b);
+    for (int mh = 0; mh < 2; ++mh) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = mh * 64 + warp * 16 + (lane >> 2) + 8 * h;  // rows past M hold what the TMA clips
+        const uint32_t swz = RB == 128 ? (uint32_t)(r & 7) : (uint32_t)((r >> 1) & 3);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int cc = c0 + 8 * j;
+          if (cc >= p.Cout) break;
+          const float2 wv = __ldg(reinterpret_cast<const float2*>(pre.w + cc)), bv = __ldg(reinterpret_cast<const float2*>(pre.b + cc));
+          const int col = 8 * j + 2 * (lane & 3), cs = col % SW;
+          T2* q = reinterpret_cast<T2*>(stg + (uint32_t)(col / SW) * (TC_BM * RB) + (uint32_t)r * RB + ((((uint32_t)cs >> 3) ^ swz) << 4) +
+                                        (cs & 7) * 2);
+          const float2 x = Pair16<T>::unpack(*q);
+          *q = Pair16<T>::pack(act_t<ACT_RELU>(fmaf(x.x, wv.x, bv.x)), act_t<ACT_RELU>(fmaf(x.y, wv.y, bv.y)));
+        }
       }
     }
-    bulk_commit();
+    fence_proxy_async();
+    wg_sync(2 + c);
+    if (leader) tc_store_staging<BN>(stg, tmZ, p, m_blk, n_blk);
   }
 }
 
@@ -428,10 +467,11 @@ __device__ __forceinline__ void se_scale_a_tile(uint32_t a, uint64_t* full, uint
 // arrive per warp); the consumers wait on ready[s] instead of full[s].  The parities stay in phase: full[s] completes phase
 // k + 1 only after the producer saw empty[s] complete phase k, which needs the consumers to have taken ready[s] phase k,
 // which needs every transform warp to have finished phase k; so no barrier runs more than one phase ahead of its waiters.
-template <typename T, int ACT, int RES, int BN, bool SE = false>
-__global__ void __launch_bounds__(TCP_THREADS, 1)
-tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
-               const TcConvParams p, const float* __restrict__ a_scale) {
+//
+// PRE: the epilogue also writes the next op's pre-activation through tmZ (tc_tile_epilogue); tc_conv_preact_kernel.
+template <typename T, int ACT, int RES, int BN, bool SE, bool PRE>
+__device__ __forceinline__ void tc_conv_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, const CUtensorMap* tmZ,
+                                             const TcConvParams& p, const float* __restrict__ a_scale, TcPreact pre) {
   using Ring = TcRing<BN>;
   constexpr int STAGES = Ring::stages;
   extern __shared__ uint8_t tc_smem_raw[];
@@ -529,9 +569,25 @@ tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[prev]);
     if (t + (int)gridDim.x < tiles) named_bar_arrive(2 - c);  // the other consumer may start the next tile
-    tc_tile_epilogue<T, ACT, RES, BN>(acc, smem + Ring::out_off + c * Ring::out_bytes, &tmO, p, m_blk, n_blk, c);
+    tc_tile_epilogue<T, ACT, RES, BN, PRE>(acc, smem + Ring::out_off + c * Ring::out_bytes, &tmO, p, m_blk, n_blk, c, tmZ, pre);
   }
   if ((threadIdx.x & 127) == 0) bulk_wait();
+}
+
+template <typename T, int ACT, int RES, int BN, bool SE = false>
+__global__ void __launch_bounds__(TCP_THREADS, 1)
+tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
+               const TcConvParams p, const float* __restrict__ a_scale) {
+  tc_conv_body<T, ACT, RES, BN, SE, false>(tmA, tmB, tmO, nullptr, p, a_scale, TcPreact{});
+}
+
+// tc_conv_kernel whose epilogue also stores the next op's pre-activation (ResNet V2: a block's _3_conv and the next block's
+// _preact_bn + _preact_relu, or the last block's and post_bn + post_relu) through tmZ
+template <typename T, int ACT, int RES, int BN>
+__global__ void __launch_bounds__(TCP_THREADS, 1)
+tc_conv_preact_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
+                      const __grid_constant__ CUtensorMap tmZ, const TcConvParams p, const TcPreact pre) {
+  tc_conv_body<T, ACT, RES, BN, false, true>(tmA, tmB, tmO, &tmZ, p, nullptr, pre);
 }
 
 // ------------------------------------------------------------------- 3x3 stride-1 conv with Cin, Cout <= 64
@@ -733,10 +789,10 @@ inline const char* make_tmap_nhwc(CUtensorMap* m, const void* ptr, uint64_t B, u
 // copied Op that runs on other buffers encodes its own.  Encoding on every launch would sit on the host's launch path; a
 // handle alternates between a few (workspace, batch) pairs, and past kEntries the oldest entry is replaced.
 struct TmapCache {
-  static constexpr int kEntries = 16, kKeyWords = 14;
+  static constexpr int kEntries = 16, kKeyWords = 15;
   struct Entry {
     uint64_t key[kKeyWords];
-    CUtensorMap map[3];
+    CUtensorMap map[4];
   };
   std::vector<Entry> entries;
   size_t replaced = 0;
@@ -826,6 +882,11 @@ inline const char* tc_prepare_weights(TcWeights& w, const float* wk, const float
 
 // N-tile width: the narrowest wgmma N in {32, 64, 128} that covers Cout, else 128 (Cout > 128 runs several N tiles)
 inline int tc_pick_bn(int cout) { return cout <= 32 ? 32 : cout <= 64 ? 64 : 128; }
+// The GEMMs tc_conv_preact_kernel runs: 1x1 stride 1, no activation, a residual added, one or more 128-wide N tiles
+// (every ResNet V2 _3_conv: Cout 256 to 2048)
+inline bool tc_preact_eligible(int R, int stride, int cout, int act, bool res) {
+  return R == 1 && stride == 1 && act == ACT_NONE && res && tc_pick_bn(cout) == 128 && cout % 8 == 0;
+}
 // Where a 1x1 projection's squeeze-excitation scale is applied: inside tc_conv_kernel (SE instances) when the GEMM has at
 // most two N tiles (Cout <= 256), else by se_scale_kernel in place ahead of it.  The GEMM scales its A tile once per N tile,
 // in warps whose throughput bounds the projection: at 2 N tiles that costs less than the separate pass's read and write of
@@ -833,9 +894,11 @@ inline int tc_pick_bn(int cout) { return cout <= 32 ? 32 : cout <= 64 ? 64 : 128
 inline bool tc_se_in_gemm(int cout) { return cout <= 256; }
 
 // T: the storage type the weights were prepared in (tc_prepare_weights<T>).  s1: run tc_conv3x3s1_kernel, for a shape
-// that tc3x3s1_eligible takes; else tc_conv_kernel.
+// that tc3x3s1_eligible takes; else tc_conv_kernel.  z (tc_preact_eligible shapes): run tc_conv_preact_kernel, which also
+// stores relu(out * pre.w + pre.b) to z.
 template <typename T>
-inline const char* tc_conv_launch(const TcWeights& w, const ConvParams& p, bool res_first, bool s1, cudaStream_t st) {
+inline const char* tc_conv_launch(const TcWeights& w, const ConvParams& p, bool res_first, bool s1, cudaStream_t st, void* z = nullptr,
+                                  TcPreact pre = {}) {
   TcConvParams q;
   q.res = p.res; q.bias = w.d_bias; q.out = p.out;
   q.mode = (p.R == 1 && p.stride == 1) ? 0 : 1;
@@ -849,6 +912,8 @@ inline const char* tc_conv_launch(const TcWeights& w, const ConvParams& p, bool 
   q.M = p.B * p.Hout * p.Wout;
   if (p.a_scale && (q.mode != 0 || !tc_se_in_gemm(p.Cout)))
     return "squeeze-excitation scale outside the 1x1 projections tc_conv_kernel scales (tc_se_in_gemm)";
+  if (z && (q.mode != 0 || s1 || p.a_scale || tc_pick_bn(p.Cout) != 128))
+    return "pre-activation output outside the 1x1 GEMMs tc_conv_preact_kernel runs (tc_preact_eligible)";
   // tc_conv3x3s1_kernel: bn is its K per tap and N tile
   const int bn = s1 ? tc3x3s1_width(p.Cin, p.Cout) : tc_pick_bn(p.Cout);
   q.m_tiles = q.mode == 0 ? (q.M + TC_BM - 1) / TC_BM : p.B * q.tiles_w * q.tiles_h;
@@ -870,11 +935,19 @@ inline const char* tc_conv_launch(const TcWeights& w, const ConvParams& p, bool 
     if (!r)
       r = q.mode == 0 ? make_tmap_2d<T>(&c[2], p.out, q.M, p.Cout, TC_BM, slab, out_sw)
                       : make_tmap_nhwc<T>(&c[2], p.out, p.B, p.Hout, p.Wout, p.Cout, slab, TC_TILE_W, TC_TILE_H, 1, 1, out_sw);
+    if (!r && z) r = make_tmap_2d<T>(&c[3], z, q.M, p.Cout, TC_BM, slab, out_sw);
     return r;
-  }, p.in, p.out, w.d_w, p.B, p.Hin, p.Win, p.Cin, p.Hout, p.Wout, p.Cout, w.taps, p.stride, bn, s1);
+  }, p.in, p.out, w.d_w, p.B, p.Hin, p.Win, p.Cin, p.Hout, p.Wout, p.Cout, w.taps, p.stride, bn, s1, z);
   if (e) return e;
   const dim3 grid(std::min(q.m_tiles * q.n_tiles, num_sms()));  // persistent: one CTA per SM
   const int res_mode = p.res ? (res_first ? 2 : 1) : 0;
+  if (z)  // ResNet V2 _3_conv: no activation, the shortcut added, Cout >= 256
+    return with_const<ACT_NONE>(p.act, "unsupported activation in tc_conv_preact_kernel", [&](auto act) {
+      return with_const<1>(res_mode, "tc_conv_preact_kernel adds a residual after the (identity) activation", [&](auto res) {
+        return launch_smem(tc_conv_preact_kernel<T, act, res, 128>, grid, dim3(TCP_THREADS), TcRing<128>::smem_bytes, st, m[0], m[1], m[2],
+                           m[3], q, pre);
+      });
+    });
   if (s1)
     return with_const<ACT_SILU, ACT_RELU>(p.act, "unsupported activation in tc_conv3x3s1_kernel", [&](auto act) {
       return with_const<0, 1, 2>(res_mode, "unsupported residual mode", [&](auto res) {

@@ -362,6 +362,23 @@ class Engine:
                                               ws.numel(), _stream_ptr(self.device)), self._h)
         return out
 
+    def op_is_preact_pair(self, op):
+        """True when backbone op `op` (a ResNet V2 _3_conv) and op + 1 (the pre-activation behind it) run as one
+        tc_conv_preact_kernel launch."""
+        return bool(lib().mtb_op_is_preact_pair(self._h, op))
+
+    def debug_run_preact_pair(self, op, x, res):
+        """The fused pair starting at op `op` in isolation: x [B,H,W,Cin], res [B,H,W,Cout] fp32 -> (op output,
+        pre-activation), both [B,H,W,Cout] fp32."""
+        io = self.op_io(op)
+        b = x.shape[0]
+        out, z = (torch.empty((b,) + io['out_shape'], dtype=torch.float32, device=self.device) for _ in range(2))
+        ws = self.workspace(b)
+        x, res = x.float().contiguous(), res.float().contiguous()
+        check(lib().mtb_debug_run_preact_pair(self._h, op, x.data_ptr(), res.data_ptr(), b, out.data_ptr(), z.data_ptr(), out.numel(),
+                                              ws.data_ptr(), ws.numel(), _stream_ptr(self.device)), self._h)
+        return out, z
+
     def profile_begin(self, classes=None):
         """Brackets every launch of the selected kernel classes (None = all) with CUDA events on the launch stream."""
         n = lib().mtb_num_kernel_classes()
