@@ -2,7 +2,8 @@
 
 Mirrors the constructor surface of /root/reference/metrabs_pytorch/backbones/efficientnet.py
 (``efficientnet_v2_{s,m,l}()`` and ``efficientnet_b0()`` .. ``efficientnet_b7()`` returning an object whose ``.features``
-is used, and ``PreprocLayer``; model
+is used, plus ``efficientnet_v2_xl()`` and ``efficientnet_v2_b0()`` .. ``_b3()`` for the TF reference's
+``efficientnetv2-xl`` / ``-b0`` .. ``-b3`` tables, and ``PreprocLayer``; model
 assembly recipe scripts/demo_image.py:59-74).  The modules built here only HOLD parameters under the reference's
 ``state_dict`` key schema (``<stage>.<block>.block.<i>.{0.weight,1.weight,1.bias,1.running_mean,...}``); the
 arithmetic runs in libmetrabs_b200.so (stem / FusedMBConv / MBConv / SE kernels), which receives the block table
@@ -28,7 +29,32 @@ _TABLES = {
            ('mb', 6, 3, 1, 384, 640, 7)], 1280),
     'tiny': ([('fused', 1, 3, 1, 8, 8, 1), ('fused', 4, 3, 2, 8, 16, 2), ('fused', 4, 3, 2, 16, 24, 1),
               ('mb', 4, 3, 2, 24, 32, 2), ('mb', 6, 3, 1, 32, 40, 1), ('mb', 6, 3, 2, 40, 48, 2, True)], 64),
+    # the TF reference's v2_xl_block (metrabs_tf effnetv2_configs.py:240-248), width and depth 1.0
+    'xl': ([('fused', 1, 3, 1, 32, 32, 4), ('fused', 4, 3, 2, 32, 64, 8), ('fused', 4, 3, 2, 64, 96, 8),
+            ('mb', 4, 3, 2, 96, 192, 16), ('mb', 6, 3, 1, 192, 256, 24), ('mb', 6, 3, 2, 256, 512, 32, True),
+            ('mb', 6, 3, 1, 512, 640, 8)], 1280),
 }
+
+# The TF reference's v2_base_block (effnetv2_configs.py:145-152), scaled per EfficientNetV2-B variant by (width, depth)
+# (:266-281) with TF's rules, not torchvision's: channels round_filters, layers round_repeats, head round_filters(1280)
+_V2_BASE = [('fused', 1, 3, 1, 32, 16, 1), ('fused', 4, 3, 2, 16, 32, 2), ('fused', 4, 3, 2, 32, 48, 2),
+            ('mb', 4, 3, 2, 48, 96, 3), ('mb', 6, 3, 1, 96, 112, 5), ('mb', 6, 3, 2, 112, 192, 8, True)]
+_V2_SCALED = {'v2-b0': (1.0, 1.0), 'v2-b1': (1.0, 1.1), 'v2-b2': (1.1, 1.2), 'v2-b3': (1.2, 1.4)}
+
+
+def round_filters(filters, width):
+    """effnetv2_model.py:76-87 with depth_divisor 8: the nearest multiple of 8, at least 8 (no 0.9 rule)."""
+    return max(8, int(filters * width + 4) // 8 * 8)
+
+
+def round_repeats(repeats, depth):
+    """effnetv2_model.py:90-94."""
+    return int(math.ceil(depth * repeats))
+
+
+for _v, (_w, _d) in _V2_SCALED.items():
+    _TABLES[_v] = ([r[:4] + (round_filters(r[4], _w), round_filters(r[5], _w), round_repeats(r[6], _d)) + r[7:]
+                    for r in _V2_BASE], round_filters(1280, _w))
 
 
 # EfficientNet-B base table (efficientnet.py:388-396): (expand, kernel, stride, cin, cout, layers, bottomright on the last
@@ -89,7 +115,8 @@ def dilate_stages(stages, output_stride, centered_stride):
 
 
 def stage_table(size, centered_stride=None, output_stride=32):
-    """-> (stages, last_channel) of EfficientNetV2-``size`` at ``output_stride`` 32, or 16 / 8 for 's', 'l' and 'tiny'."""
+    """-> (stages, last_channel) of EfficientNetV2-``size`` ('s', 'm', 'l', 'xl', 'v2-b0'..'v2-b3', 'tiny') at
+    ``output_stride`` 32, or 16 / 8 for 's', 'l' and 'tiny'."""
     if centered_stride is None:
         centered_stride = get_config().centered_stride
     if output_stride not in _OUTPUT_STRIDES:
@@ -165,8 +192,8 @@ class Features(nn.Module):
 
 
 class EfficientNet(nn.Module):
-    """``size``: a V2 table ('s', 'm', 'l', 'tiny') or a B variant ('b0'..'b7').  ``output_stride`` 16 or 8 builds the
-    dilated V2-S / V2-L (and 'tiny') tables; the model's ``Config.stride_test`` must then equal it."""
+    """``size``: a V2 table ('s', 'm', 'l', 'xl', 'v2-b0'..'v2-b3', 'tiny') or a B variant ('b0'..'b7').  ``output_stride``
+    16 or 8 builds the dilated V2-S / V2-L (and 'tiny') tables; the model's ``Config.stride_test`` must then equal it."""
 
     def __init__(self, size, output_stride=32):
         super().__init__()
@@ -197,6 +224,26 @@ def efficientnet_v2_m(**kwargs):
 
 def efficientnet_v2_l(output_stride=32, **kwargs):
     return EfficientNet('l', output_stride)
+
+
+def efficientnet_v2_xl(**kwargs):
+    return EfficientNet('xl')
+
+
+def efficientnet_v2_b0(**kwargs):
+    return EfficientNet('v2-b0')
+
+
+def efficientnet_v2_b1(**kwargs):
+    return EfficientNet('v2-b1')
+
+
+def efficientnet_v2_b2(**kwargs):
+    return EfficientNet('v2-b2')
+
+
+def efficientnet_v2_b3(**kwargs):
+    return EfficientNet('v2-b3')
 
 
 def efficientnet_v2_tiny(output_stride=32, **kwargs):

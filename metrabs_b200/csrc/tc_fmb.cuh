@@ -31,8 +31,8 @@ constexpr int FMB_W_BYTES = FMB_NC * TC_BK * 2;                     // ring stag
 constexpr int FMB_A2_BYTES = TC_BM * FMB_NC * 2;  // two 16 KB swizzle tiles (expanded channels 0-63, 64-127 of the chunk)
 
 // Shared memory per BN2 (= tc_pick_bn(Cout), Cout = Cin): [3 x kchunks boxes | ring | A2 | barriers].  Cin <= 64 is one
-// 64-channel k-chunk (BN2 <= 64): 60 KB of boxes + 8 x 16 KB ring + 32 KB = 221 KB; Cin 80 / 96 is two (BN2 = 128): 120 KB of
-// boxes + 4 x 16 KB + 32 KB = 216 KB.
+// 64-channel k-chunk (BN2 <= 64): 60 KB of boxes + 8 x 16 KB ring + 32 KB = 221 KB; Cin 72 to 96 is two (BN2 = 128): 120 KB
+// of boxes + 4 x 16 KB + 32 KB = 216 KB.
 template <int BN2>
 struct FmbSmem {
   static constexpr int kchunks = BN2 == 128 ? 2 : 1;
@@ -224,9 +224,22 @@ struct FmbWeights {
   mutable TmapCache maps;         // (block input in 16 x 10-pixel boxes for tma_load_tap_boxes, W1, W2)
 };
 
-// shapes the fused kernel covers: 3x3 stride-1 expand (SiLU) + 1x1 projection, Cin = Cout (identity-shaped block)
+// shapes the fused kernel covers: 3x3 stride-1 expand (SiLU) + 1x1 projection, Cin = Cout (identity-shaped block).
+// Cin = Cout a multiple of 8 but not of 16 (24, 40, 56, 72, 88; EfficientNetV2-B2 / -B3 run 40 and 56) takes the same path as
+// the multiples of 16, with nothing left over per 16-wide k step that is not already zeros:
+//  - every row stride is a multiple of 16 bytes, as the TMA requires: input pixels 2 Cin (80, 112 B), W1 rows 18 Cin, W2 rows
+//    2 Cexp = 8 Cin;
+//  - the boxes' channels Cin..63 of a 64-channel k-chunk are TMA zero fill, and they meet the columns tap * Cin + Cin.. of the
+//    tap's W1 k-block (the next tap's first columns, or zero fill past 9 Cin): the products are zeros, the same ones
+//    tc_conv_kernel multiplies on its own 3x3 launch, whose k-blocks start at the same tap * Cin + kc * 64;
+//  - Cexp = 4 Cin is a multiple of 32, so a partial last expand chunk (Cexp 160, 224) ends on a 16-wide k step of GEMM-2:
+//    A2 holds zeros from Cexp on and the W2 columns past Cexp are zero fill, so GEMM-2 adds zero products after the
+//    projection's own k-blocks (as at Cexp 192), and every bias1 pair col, col + 1 lies below Cexp or both past it;
+//  - BN2 = tc_pick_bn(Cout) = 64 at Cout 40, 56 (32 at 24, 128 at 72, 88), with one k-chunk exactly when Cin <= 64; W2 rows
+//    Cout..BN2-1 are zero fill, and epilogue-2 stops at the first column pair >= Cout, each pair (bias, residual, output)
+//    4-byte aligned because Cout and the pair's column are even.
 inline bool fmb_shape_ok(int cin, int cexp, int cout) {
-  return cin % 16 == 0 && cin >= 16 && cin <= 96 && cout == cin && cexp % 16 == 0 && cexp >= 32 && cexp <= 512;
+  return cin % 8 == 0 && cin >= 16 && cin <= 96 && cout == cin && cexp % 16 == 0 && cexp >= 32 && cexp <= 512;
 }
 
 inline void fmb_prepare(FmbWeights& f, const TcWeights& w1, const TcWeights& w2) {
