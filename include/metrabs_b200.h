@@ -46,13 +46,18 @@ typedef enum { MTB_DTYPE_F32 = 0, MTB_DTYPE_BF16 = 1, MTB_DTYPE_F16 = 2, MTB_DTY
  * default epsilon 1e-5, for EfficientNet-B0..B4 (:753-960), and takes MBConv rows only (kernel 3 or 5, stride 1 or 2;
  * anything else fails with MTB_ERR_UNSUPPORTED); the RESNET* values (V1, metrabs_tf/backbones/resnet.py: ResNet-18/34 with the
  * basic block :322-388, ResNet-50/101/152 with the bottleneck :239-319), the RESNET*V2 values (the pre-activation
- * ResNet-50/101/152, ResNetUnifiedV2 :710-745 with block2_dense :391-456, output strides 8, 16 and 32) and MOBILENETV3_SMALL / _LARGE
- * (metrabs_tf/backbones/mobilenet_v3.py:348-384 / :387-428, alpha 1, not minimalistic) follow the TF-only
+ * ResNet-50/101/152, ResNetUnifiedV2 :710-745 with block2_dense :391-456, output strides 8, 16 and 32), the RESNET*V1_5 values
+ * (ResNetUnified(v1_5=True) :621-666: the V1 bottleneck nets with block 1's stride on the 3x3 _2_conv, dilated by dil_in of
+ * its stack, and torch_preproc (x - mean) / std, builder.py:99-103; output strides 8, 16 and 32) and MOBILENETV3_SMALL /
+ * _LARGE (metrabs_tf/backbones/mobilenet_v3.py:348-384 / :387-428, alpha 1; the _MINI values are the minimalistic=True
+ * form, :250-257: 3x3 depthwise kernels, ReLU everywhere, no squeeze-excitation) follow the TF-only
  * metrabs_tf/backbones/{resnet,mobilenet_v3}.py. */
 typedef enum { MTB_ARCH_EFFNET = 0, MTB_ARCH_RESNET50 = 1, MTB_ARCH_MOBILENETV3_SMALL = 2,
                MTB_ARCH_HEAD_ONLY = 3, MTB_ARCH_RESNET18 = 4, MTB_ARCH_RESNET34 = 5, MTB_ARCH_RESNET101 = 6,
                MTB_ARCH_RESNET152 = 7, MTB_ARCH_MOBILENETV3_LARGE = 8, MTB_ARCH_EFFNET_EPS1E5 = 9,
-               MTB_ARCH_RESNET50V2 = 10, MTB_ARCH_RESNET101V2 = 11, MTB_ARCH_RESNET152V2 = 12 } mtb_arch;
+               MTB_ARCH_RESNET50V2 = 10, MTB_ARCH_RESNET101V2 = 11, MTB_ARCH_RESNET152V2 = 12,
+               MTB_ARCH_RESNET50V1_5 = 13, MTB_ARCH_RESNET101V1_5 = 14, MTB_ARCH_RESNET152V1_5 = 15,
+               MTB_ARCH_MOBILENETV3_SMALL_MINI = 16, MTB_ARCH_MOBILENETV3_LARGE_MINI = 17 } mtb_arch;
 
 /* Arithmetic of the conv/GEMM kernels.  FP32: CUDA-core fp32 FMA everywhere (the 1e-3 parity mode).
  * BF16_TC: bf16 operands on wgmma tensor cores with fp32 accumulation in registers, bf16 activations in HBM

@@ -11,6 +11,8 @@ ARCH_RESNET18, ARCH_RESNET34, ARCH_RESNET101, ARCH_RESNET152 = 4, 5, 6, 7
 ARCH_MOBILENETV3_LARGE = 8
 ARCH_EFFNET_EPS1E5 = 9  # the EFFNET grammar with BatchNorm eps 1e-5 (EfficientNet-B0..B4)
 ARCH_RESNET50V2, ARCH_RESNET101V2, ARCH_RESNET152V2 = 10, 11, 12  # the pre-activation ResNets
+ARCH_RESNET50V1_5, ARCH_RESNET101V1_5, ARCH_RESNET152V1_5 = 13, 14, 15  # stride on the 3x3, torch_preproc
+ARCH_MOBILENETV3_SMALL_MINI, ARCH_MOBILENETV3_LARGE_MINI = 16, 17  # minimalistic=True
 # mtb_kernel (mtb_op_kernel): the kernel that runs an op
 DW_GENERIC, DW_TMA, DW_STRIP_16B, DW_STRIP_F32, DW_5X5_16B, DW_5X5_POOL_16B, DW_TMA_DIL = 0, 1, 2, 3, 4, 5, 6
 STEM_3X3S2, STEM_WIDE, STEM_GENERIC = 7, 8, 9

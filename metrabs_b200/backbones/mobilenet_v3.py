@@ -4,7 +4,9 @@ Keras-only in the reference (/root/reference/metrabs_tf/backbones/mobilenet_v3.p
 defined by this build from the Keras layer names with '/' -> '.': ``backbone.Conv.weight``,
 ``backbone.Conv.BatchNorm.*``, ``backbone.expanded_conv_<i>.{expand,depthwise,project}.weight`` (+ ``.BatchNorm.*``),
 ``backbone.expanded_conv_<i>.squeeze_excite.{Conv,Conv_1}.{weight,bias}``, ``backbone.Conv_1.*``, ``backbone.Conv_2.*``.
-Block 0 (``expanded_conv``) has no expand conv.  Alpha 1, not minimalistic (the variants the released models use)."""
+Block 0 (``expanded_conv``) has no expand conv.  Alpha 1.  ``minimalistic=True`` (Keras' keyword, the reference's
+``mobilenetV3{Small,Large}mini``, :250-257) gives every block a 3x3 depthwise kernel and ReLU, and no squeeze-excitation
+(no ``squeeze_excite`` keys); the stem, ``Conv_1`` and ``Conv_2`` use ReLU too."""
 from torch import nn
 
 from metrabs_b200 import _lib
@@ -18,6 +20,7 @@ _ROWS_LARGE = [  # MobileNetV3-Large (:403-428)
     (672, 112, 3, True), (672, 160, 5, True), (960, 160, 5, True), (960, 160, 5, True)]
 # variant -> (arch, rows, last point channels)
 VARIANTS = {'small': (_lib.ARCH_MOBILENETV3_SMALL, _ROWS, 1024), 'large': (_lib.ARCH_MOBILENETV3_LARGE, _ROWS_LARGE, 1280)}
+ARCH_MINI = {'small': _lib.ARCH_MOBILENETV3_SMALL_MINI, 'large': _lib.ARCH_MOBILENETV3_LARGE_MINI}
 
 
 def _depth(v, divisor=8):
@@ -37,10 +40,14 @@ def _conv(cin, cout, k, groups=1, bn=True, bias=False):
 class Features(nn.Module):
     stages = []
 
-    def __init__(self, variant='small'):
+    def __init__(self, variant='small', minimalistic=False):
         super().__init__()
         self.arch, rows, self.last_channel = VARIANTS[variant]
+        if minimalistic:
+            self.arch = ARCH_MINI[variant]
+            rows = [(cexp, filters, 3, False) for cexp, filters, _k, _se in rows]
         self.variant = variant
+        self.minimalistic = minimalistic
         self.add_module('Conv', _conv(3, 16, 3))
         cin = 16
         for i, (cexp, filters, k, se) in enumerate(rows):
@@ -63,11 +70,12 @@ class Features(nn.Module):
         raise RuntimeError('metrabs_b200 backbones run inside Metrabs.forward (libmetrabs_b200.so)')
 
 
-def mobilenet_v3_small(**kwargs):
-    """Use as ``Metrabs(mobilenet_v3_small(), joint_info)``."""
-    return Features('small')
+def mobilenet_v3_small(minimalistic=False, **kwargs):
+    """Use as ``Metrabs(mobilenet_v3_small(), joint_info)``; ``minimalistic=True`` for ``mobilenetV3Smallmini``."""
+    return Features('small', minimalistic)
 
 
-def mobilenet_v3_large(**kwargs):
-    """Use as ``Metrabs(mobilenet_v3_large(), joint_info)`` (the backbone of metrabs_mob3l_y4 / _y4t)."""
-    return Features('large')
+def mobilenet_v3_large(minimalistic=False, **kwargs):
+    """Use as ``Metrabs(mobilenet_v3_large(), joint_info)`` (the backbone of metrabs_mob3l_y4 / _y4t);
+    ``minimalistic=True`` for ``mobilenetV3Largemini``."""
+    return Features('large', minimalistic)

@@ -1,5 +1,6 @@
 """ResNet (MeTRAbs stride/dilation switching) parameter holders for the H100 engine: ResNet-18 / 34 (V1 basic block),
-ResNet-50 / 101 / 152 (V1 bottleneck) and the pre-activation ResNet-50 / 101 / 152 V2 (``FeaturesV2``).
+ResNet-50 / 101 / 152 (V1 bottleneck), their V1.5 forms (``resnet50v1_5`` ...: the same parameters, block 1's stride on
+the 3x3 conv, torch_preproc) and the pre-activation ResNet-50 / 101 / 152 V2 (``FeaturesV2``).
 
 The reference has these backbones only as Keras code (metrabs_tf/backbones/resnet.py:239-319 bottleneck,
 :322-388 basic block, :601-707 stride plan and stacks, :746-788 depths); there is no PyTorch key schema for them, so this
@@ -17,12 +18,18 @@ DEPTHS = {18: (_lib.ARCH_RESNET18, [2, 2, 2, 2], True), 34: (_lib.ARCH_RESNET34,
           152: (_lib.ARCH_RESNET152, [3, 8, 36, 3], False)}
 
 
+# depth -> arch of the V1.5 bottleneck nets (ResNetUnified(v1_5=True), metrabs_tf/backbones/resnet.py:621-666, :791-800)
+DEPTHS_V1_5 = {50: _lib.ARCH_RESNET50V1_5, 101: _lib.ARCH_RESNET101V1_5, 152: _lib.ARCH_RESNET152V1_5}
+
+
 class Features(nn.Module):
     stages = []
 
-    def __init__(self, depth=50):
+    def __init__(self, depth=50, v1_5=False):
         super().__init__()
         self.arch, counts, basic = DEPTHS[depth]
+        if v1_5:  # the same layers and keys as V1; only the plan (stride on _2_conv) and the preprocessing differ
+            self.arch = DEPTHS_V1_5[depth]
         self.depth = depth
         bias = not basic
         self.last_channel = 512 if basic else 2048
@@ -76,6 +83,21 @@ def resnet101(**kwargs):
 def resnet152(**kwargs):
     """Use as ``Metrabs(resnet152(), joint_info)`` (keys ``backbone.<keras layer>...``)."""
     return Features(152)
+
+
+def resnet50v1_5(**kwargs):
+    """Use as ``Metrabs(resnet50v1_5(), joint_info)`` (the keys of ``resnet50()``)."""
+    return Features(50, v1_5=True)
+
+
+def resnet101v1_5(**kwargs):
+    """Use as ``Metrabs(resnet101v1_5(), joint_info)`` (the keys of ``resnet101()``)."""
+    return Features(101, v1_5=True)
+
+
+def resnet152v1_5(**kwargs):
+    """Use as ``Metrabs(resnet152v1_5(), joint_info)`` (the keys of ``resnet152()``)."""
+    return Features(152, v1_5=True)
 
 
 # depth -> (arch, blocks in conv2..conv5) of the pre-activation nets (metrabs_tf/backbones/resnet.py:803-831)

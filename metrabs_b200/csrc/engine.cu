@@ -414,9 +414,12 @@ void resnet_stride_plan(int output_stride, bool centered, int strides[3], int di
 // * bottleneck (ResNet-50/101/152, ResNetUnified :621-666): block1_dense :239-319, every conv has a bias (:270);
 // * basic (ResNet-18/34, ResNetUnifiedBasic :669-707): block1_basic_dense :322-388, no conv has a bias (stem included,
 //   :704-707), conv2_block1 has an identity shortcut (conv1_shortcut=False, :689-692).
+// * V1.5 (bottleneck only, ResNetUnified(v1_5=True)): _1_conv is a plain 1x1 at stride 1 (:282-283); the stack's stride and
+//   the bottom-right shift move to the 3x3 _2_conv (:295-303), which takes dil_in of its stack in block1 (striding_infos_in,
+//   :629-634) and dil_out in the other blocks; preprocessing torch_preproc (builder.py:99-103).
 // Key schema: Keras layer names, "backbone.<layer>.{weight,bias}" / "backbone.<layer>.{weight,bias,running_mean,running_var}"
-// in torch layout.
-int plan_resnet(mtb_handle* h, const int counts[4], bool basic) {
+// in torch layout (the same for V1 and V1.5).
+int plan_resnet(mtb_handle* h, const int counts[4], bool basic, bool v1_5) {
   const mtb_config& c = h->cfg;
   auto valid_stride = [](int s) { return s == 8 || s == 16 || s == 32; };
   if (!valid_stride(c.stride_test))
@@ -449,8 +452,15 @@ int plan_resnet(mtb_handle* h, const int counts[4], bool basic) {
     op.Hin = op.Win = c.proc_side; op.Cin = 3; op.Cout = 64;
     op.R = op.S = 7; op.stride = 2; op.pad_t = op.pad_l = 3; op.act = ACT_RELU;
     op.Hout = op.Wout = (c.proc_side + 6 - 7) / 2 + 1;
-    const float mean[3] = {103.939f, 116.779f, 123.68f};  // caffe_preproc (builder.py:106-108): 255*x - mean, no channel swap
-    for (int i = 0; i < 3; ++i) { op.pre_scale[i] = 255.f; op.pre_shift[i] = -mean[i]; }
+    if (v1_5) {
+      // torch_preproc (builder.py:99-103): (x - mean) / std, applied as x * (1/std) + (-mean/std) with both constants
+      // rounded once to fp32
+      const float mean[3] = {0.485f, 0.456f, 0.406f}, stdev[3] = {0.229f, 0.224f, 0.225f};
+      for (int i = 0; i < 3; ++i) { op.pre_scale[i] = 1.f / stdev[i]; op.pre_shift[i] = -mean[i] / stdev[i]; }
+    } else {
+      const float mean[3] = {103.939f, 116.779f, 123.68f};  // caffe_preproc (builder.py:106-108): 255*x - mean, no channel swap
+      for (int i = 0; i < 3; ++i) { op.pre_scale[i] = 255.f; op.pre_shift[i] = -mean[i]; }
+    }
     op.in_buf = BUF_NONE; op.out_buf = 0;
     op.flops = 2.0 * op.Hout * op.Wout * 64 * 147;
     P.H = op.Hout; P.W = op.Wout; P.C = 64; P.cur = 0;
@@ -508,17 +518,26 @@ int plan_resnet(mtb_handle* h, const int counts[4], bool basic) {
         P.cur = t2;
         continue;
       }
-      P.conv_k(b + "_1_conv", b + "_1_conv.weight", bias(1), b + "_1_bn", f, 1, stride, -shift, 0, ACT_RELU, x_in, t1, false, 1,
-               eps);
-      {
+      int t2 = P.pick({x_in, sc, t1});
+      if (v1_5) {
+        P.conv_k(b + "_1_conv", b + "_1_conv.weight", bias(1), b + "_1_bn", f, 1, 1, 0, 0, ACT_RELU, x_in, t1, false, 1, eps);
+        // _2_conv: dense SAME 3x3 sampled at shift::stride, i.e. a strided conv with begin pad dil - shift
+        const int dil2 = (st > 0 && first) ? dil_in[st - 1] : dil;
+        Op& o = P.conv_k(b + "_2_conv", b + "_2_conv.weight", bias(2), b + "_2_bn", f, 3, stride, dil2 - shift, 2 * dil2, ACT_RELU,
+                         t1, t2, false, dil2, eps);
+        o.Hout = Hin / stride; o.Wout = Win / stride;
+        o.flops = 2.0 * o.Hout * o.Wout * f * f * 9;
+        P.H = o.Hout; P.W = o.Wout;
+      } else {
+        P.conv_k(b + "_1_conv", b + "_1_conv.weight", bias(1), b + "_1_bn", f, 1, stride, -shift, 0, ACT_RELU, x_in, t1, false, 1,
+                 eps);
         Op& o = h->ops.back();
         o.Hout = Hin / stride; o.Wout = Win / stride;
         o.flops = 2.0 * o.Hout * o.Wout * o.Cout * Cin;
         P.H = o.Hout; P.W = o.Wout;
+        P.conv_k(b + "_2_conv", b + "_2_conv.weight", bias(2), b + "_2_bn", f, 3, 1, dil, 2 * dil, ACT_RELU, t1, t2, false, dil,
+                 eps);
       }
-      int t2 = P.pick({x_in, sc, t1});
-      P.conv_k(b + "_2_conv", b + "_2_conv.weight", bias(2), b + "_2_bn", f, 3, 1, dil, 2 * dil, ACT_RELU, t1, t2, false, dil,
-               eps);
       int t3 = P.pick({sc, t2});
       Op& o3 = P.conv_k(b + "_3_conv", b + "_3_conv.weight", bias(3), b + "_3_bn", 4 * f, 1, 1, 0, 0, ACT_RELU, t2,
                         last ? BUF_FEATURES : t3, false, 1, eps);
@@ -660,11 +679,30 @@ const MbV3Row kMobileNetV3Large[] = {
     {480, 112, 3, 1, true, ACT_HSWISH, false},  {672, 112, 3, 1, true, ACT_HSWISH, false},
     {672, 160, 5, 2, true, ACT_HSWISH, true},   {960, 160, 5, 1, true, ACT_HSWISH, false},
     {960, 160, 5, 1, true, ACT_HSWISH, false}};
+// the minimalistic forms (minimalistic=True, :250-257): the same expanded widths, strides and bottom-right rows with every
+// kernel 3, every activation ReLU and no squeeze-excitation
+const MbV3Row kMobileNetV3SmallMini[] = {
+    {16, 16, 3, 2, false, ACT_RELU, false},   {72, 24, 3, 2, false, ACT_RELU, false},
+    {88, 24, 3, 1, false, ACT_RELU, false},   {96, 40, 3, 2, false, ACT_RELU, false},
+    {240, 40, 3, 1, false, ACT_RELU, false},  {240, 40, 3, 1, false, ACT_RELU, false},
+    {120, 48, 3, 1, false, ACT_RELU, false},  {144, 48, 3, 1, false, ACT_RELU, false},
+    {288, 96, 3, 2, false, ACT_RELU, true},   {576, 96, 3, 1, false, ACT_RELU, false},
+    {576, 96, 3, 1, false, ACT_RELU, false}};
+const MbV3Row kMobileNetV3LargeMini[] = {
+    {16, 16, 3, 1, false, ACT_RELU, false},   {64, 24, 3, 2, false, ACT_RELU, false},
+    {72, 24, 3, 1, false, ACT_RELU, false},   {72, 40, 3, 2, false, ACT_RELU, false},
+    {120, 40, 3, 1, false, ACT_RELU, false},  {120, 40, 3, 1, false, ACT_RELU, false},
+    {240, 80, 3, 2, false, ACT_RELU, false},  {200, 80, 3, 1, false, ACT_RELU, false},
+    {184, 80, 3, 1, false, ACT_RELU, false},  {184, 80, 3, 1, false, ACT_RELU, false},
+    {480, 112, 3, 1, false, ACT_RELU, false}, {672, 112, 3, 1, false, ACT_RELU, false},
+    {672, 160, 3, 2, false, ACT_RELU, true},  {960, 160, 3, 1, false, ACT_RELU, false},
+    {960, 160, 3, 1, false, ACT_RELU, false}};
 
 // MobileNetV3 (metrabs_tf/backbones/mobilenet_v3.py:490-553 block, :465-487 SE, :258-296 stem and Conv_1 / Conv_2,
 // :556-575 correct_pad; preprocessing 255*x then Rescaling(1/127.5, -1) = 2x-1, builder.py:116-117), `n_rows` rows of
-// `rows` and a last point conv (Conv_2) of `last_point_ch` channels: 1024 for Small, 1280 for Large.
-int plan_mobilenetv3(mtb_handle* h, const MbV3Row* rows, int n_rows, int last_point_ch) {
+// `rows` and a last point conv (Conv_2) of `last_point_ch` channels: 1024 for Small, 1280 for Large.  `act` is the
+// activation of the stem, Conv_1 and Conv_2: hard-swish, or ReLU in the minimalistic form.
+int plan_mobilenetv3(mtb_handle* h, const MbV3Row* rows, int n_rows, int last_point_ch, int act) {
   const mtb_config& c = h->cfg;
   Planner P{h, c.proc_side, c.proc_side, 3};
   const std::string pre = "backbone.";
@@ -674,7 +712,7 @@ int plan_mobilenetv3(mtb_handle* h, const MbV3Row* rows, int n_rows, int last_po
     op.name = pre + "Conv";
     op.wkey = op.name + ".weight"; op.bnkey = op.name + ".BatchNorm";
     op.Hin = op.Win = c.proc_side; op.Cin = 3; op.Cout = 16;
-    op.R = op.S = 3; op.stride = 2; op.act = ACT_HSWISH;
+    op.R = op.S = 3; op.stride = 2; op.act = act;
     op.Hout = op.Wout = (c.proc_side + 1) / 2;
     // TF 'same' with stride 2: pad_total = max((out-1)*2 + 3 - in, 0), begin = pad_total / 2  (even input: (0,1))
     const int pad_total = std::max((op.Hout - 1) * 2 + 3 - c.proc_side, 0);
@@ -715,9 +753,8 @@ int plan_mobilenetv3(mtb_handle* h, const MbV3Row* rows, int n_rows, int last_po
   }
   {
     int t1 = P.pick({P.cur});
-    P.conv_k(pre + "Conv_1", pre + "Conv_1.weight", "", pre + "Conv_1.BatchNorm", depth8(P.C * 6), 1, 1, 0, 0, ACT_HSWISH, P.cur, t1);
-    P.conv_k(pre + "Conv_2", pre + "Conv_2.weight", pre + "Conv_2.bias", "", last_point_ch, 1, 1, 0, 0, ACT_HSWISH, t1,
-             BUF_FEATURES);
+    P.conv_k(pre + "Conv_1", pre + "Conv_1.weight", "", pre + "Conv_1.BatchNorm", depth8(P.C * 6), 1, 1, 0, 0, act, P.cur, t1);
+    P.conv_k(pre + "Conv_2", pre + "Conv_2.weight", pre + "Conv_2.bias", "", last_point_ch, 1, 1, 0, 0, act, t1, BUF_FEATURES);
   }
   h->feat_side = P.H;
   h->feat_c = P.C;
@@ -726,11 +763,14 @@ int plan_mobilenetv3(mtb_handle* h, const MbV3Row* rows, int n_rows, int last_po
   return MTB_OK;
 }
 
-// block counts of conv2..conv5 (resnet.py:746-788)
-struct ResNetArch { int arch; int counts[4]; bool basic; };
+// block counts of conv2..conv5 (resnet.py:746-788, V1.5 :791-800)
+struct ResNetArch { int arch; int counts[4]; bool basic; bool v1_5 = false; };
 const ResNetArch kResNets[] = {{MTB_ARCH_RESNET18, {2, 2, 2, 2}, true},    {MTB_ARCH_RESNET34, {3, 4, 6, 3}, true},
                                {MTB_ARCH_RESNET50, {3, 4, 6, 3}, false},   {MTB_ARCH_RESNET101, {3, 4, 23, 3}, false},
-                               {MTB_ARCH_RESNET152, {3, 8, 36, 3}, false}};
+                               {MTB_ARCH_RESNET152, {3, 8, 36, 3}, false},
+                               {MTB_ARCH_RESNET50V1_5, {3, 4, 6, 3}, false, true},
+                               {MTB_ARCH_RESNET101V1_5, {3, 4, 23, 3}, false, true},
+                               {MTB_ARCH_RESNET152V1_5, {3, 8, 36, 3}, false, true}};
 // block counts of the pre-activation nets (resnet.py:803-831)
 const ResNetArch kResNetsV2[] = {{MTB_ARCH_RESNET50V2, {3, 4, 6, 3}, false}, {MTB_ARCH_RESNET101V2, {3, 4, 23, 3}, false},
                                  {MTB_ARCH_RESNET152V2, {3, 8, 36, 3}, false}};
@@ -745,7 +785,7 @@ int plan(mtb_handle* h) {
   for (const ResNetArch& r : kResNetsV2)
     if (c.arch == r.arch) resnet_v2 = &r;
   if (resnet) {
-    int rc = plan_resnet(h, resnet->counts, resnet->basic);
+    int rc = plan_resnet(h, resnet->counts, resnet->basic, resnet->v1_5);
     if (rc) return rc;
   } else if (resnet_v2) {
     int rc = plan_resnet_v2(h, resnet_v2->counts);
@@ -753,8 +793,10 @@ int plan(mtb_handle* h) {
   } else switch (c.arch) {
     case MTB_ARCH_EFFNET: plan_effnet(h, 1e-3f); break;
     case MTB_ARCH_EFFNET_EPS1E5: plan_effnet(h, 1e-5f); break;
-    case MTB_ARCH_MOBILENETV3_SMALL: { int rc = plan_mobilenetv3(h, kMobileNetV3Small, (int)std::size(kMobileNetV3Small), 1024); if (rc) return rc; break; }
-    case MTB_ARCH_MOBILENETV3_LARGE: { int rc = plan_mobilenetv3(h, kMobileNetV3Large, (int)std::size(kMobileNetV3Large), 1280); if (rc) return rc; break; }
+    case MTB_ARCH_MOBILENETV3_SMALL: { int rc = plan_mobilenetv3(h, kMobileNetV3Small, (int)std::size(kMobileNetV3Small), 1024, ACT_HSWISH); if (rc) return rc; break; }
+    case MTB_ARCH_MOBILENETV3_LARGE: { int rc = plan_mobilenetv3(h, kMobileNetV3Large, (int)std::size(kMobileNetV3Large), 1280, ACT_HSWISH); if (rc) return rc; break; }
+    case MTB_ARCH_MOBILENETV3_SMALL_MINI: { int rc = plan_mobilenetv3(h, kMobileNetV3SmallMini, (int)std::size(kMobileNetV3SmallMini), 1024, ACT_RELU); if (rc) return rc; break; }
+    case MTB_ARCH_MOBILENETV3_LARGE_MINI: { int rc = plan_mobilenetv3(h, kMobileNetV3LargeMini, (int)std::size(kMobileNetV3LargeMini), 1280, ACT_RELU); if (rc) return rc; break; }
     case MTB_ARCH_HEAD_ONLY:
       h->feat_side = c.proc_side / c.stride_test;
       h->feat_c = c.feature_channels;
