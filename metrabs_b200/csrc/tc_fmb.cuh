@@ -182,34 +182,82 @@ fmb_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
           wgmma_16b<T, BN2>(acc2, gmma_desc<128>(a2 + sub * (TC_BM * 128) + wg * 64 * 128 + ko), gmma_desc<128>(b + ko), (uint32_t)(c | k));
         }
         wgmma_commit();
-        wgmma_wait<0>();  // A2 is rewritten by the next chunk's epilogue-1
-        wgmma_fence_regs<BN2 / 2>(acc2);
-        __syncwarp();
-        if (lane == 0) {
-          mbar_arrive(&empty[s0]);
-          mbar_arrive(&empty[s1]);
+        if (BN2 == 128 || c + 1 < p.nch) {  // BN2 <= 64: the last chunk's MMAs are waited for under epilogue-2's loads
+          wgmma_wait<0>();  // A2 is rewritten by the next chunk's epilogue-1
+          wgmma_fence_regs<BN2 / 2>(acc2);
+          __syncwarp();
+          if (lane == 0) {
+            mbar_arrive(&empty[s0]);
+            mbar_arrive(&empty[s1]);
+          }
         }
         it += 2;
       }
     }
     // ---- epilogue-2: + bias, + residual x, 16-bit store ----
     const int c0 = 2 * (lane & 3);
+    if constexpr (BN2 <= 64) {
+      // All of the thread's bias and residual pairs are loaded in one batch while the last chunk's GEMM-2 runs: issued one
+      // by one between the stores, which might alias them, each waited out its L2 latency with the MMAs of both
+      // warpgroups idle.  At BN2 = 128 (Cout 72 to 96) the batch spills next to the accumulators, so that width keeps the
+      // loads at their use.
+      float2 bv[BN2 / 8];
+      T2 rv[2][BN2 / 8];
+      size_t off[2];
+      bool row_ok[2];
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      size_t off;
-      if (!tile_row_offset(1, t, r0 + 8 * h, g.M, g.Cout, g.tiles_w, g.tiles_h, g.Hout, g.Wout, off)) continue;
+      for (int j = 0; j < BN2 / 8; ++j)
+        if (c0 + 8 * j < g.Cout) bv[j] = __ldg(reinterpret_cast<const float2*>(g.bias + c0 + 8 * j));
 #pragma unroll
-      for (int j = 0; j < BN2 / 8; ++j) {
-        const int cidx = c0 + 8 * j;
-        if (cidx >= g.Cout) break;
-        const float2 bv = __ldg(reinterpret_cast<const float2*>(g.bias + cidx));
-        float o0 = acc2[4 * j + 2 * h] + bv.x, o1 = acc2[4 * j + 2 * h + 1] + bv.y;
-        if (p.has_res) {
-          const float2 rv = Pair16<T>::unpack(*reinterpret_cast<const T2*>(res + off + cidx));
-          o0 += rv.x;
-          o1 += rv.y;
+      for (int h = 0; h < 2; ++h) {
+        row_ok[h] = tile_row_offset(1, t, r0 + 8 * h, g.M, g.Cout, g.tiles_w, g.tiles_h, g.Hout, g.Wout, off[h]);
+        if (p.has_res && row_ok[h]) {
+#pragma unroll
+          for (int j = 0; j < BN2 / 8; ++j)
+            if (c0 + 8 * j < g.Cout) rv[h][j] = *reinterpret_cast<const T2*>(res + off[h] + c0 + 8 * j);
         }
-        *reinterpret_cast<T2*>(out + off + cidx) = Pair16<T>::pack(o0, o1);
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs<BN2 / 2>(acc2);
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(&empty[(it - 2) % STAGES]);
+        mbar_arrive(&empty[(it - 1) % STAGES]);
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (!row_ok[h]) continue;
+#pragma unroll
+        for (int j = 0; j < BN2 / 8; ++j) {
+          const int cidx = c0 + 8 * j;
+          if (cidx >= g.Cout) break;
+          float o0 = acc2[4 * j + 2 * h] + bv[j].x, o1 = acc2[4 * j + 2 * h + 1] + bv[j].y;
+          if (p.has_res) {
+            const float2 f = Pair16<T>::unpack(rv[h][j]);
+            o0 += f.x;
+            o1 += f.y;
+          }
+          *reinterpret_cast<T2*>(out + off[h] + cidx) = Pair16<T>::pack(o0, o1);
+        }
+      }
+    } else {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        size_t off;
+        if (!tile_row_offset(1, t, r0 + 8 * h, g.M, g.Cout, g.tiles_w, g.tiles_h, g.Hout, g.Wout, off)) continue;
+#pragma unroll
+        for (int j = 0; j < BN2 / 8; ++j) {
+          const int cidx = c0 + 8 * j;
+          if (cidx >= g.Cout) break;
+          const float2 bv = __ldg(reinterpret_cast<const float2*>(g.bias + cidx));
+          float o0 = acc2[4 * j + 2 * h] + bv.x, o1 = acc2[4 * j + 2 * h + 1] + bv.y;
+          if (p.has_res) {
+            const float2 rv = Pair16<T>::unpack(*reinterpret_cast<const T2*>(res + off + cidx));
+            o0 += rv.x;
+            o1 += rv.y;
+          }
+          *reinterpret_cast<T2*>(out + off + cidx) = Pair16<T>::pack(o0, o1);
+        }
       }
     }
   }

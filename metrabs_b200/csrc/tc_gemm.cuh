@@ -75,6 +75,14 @@ __device__ __forceinline__ uint4 ld_shared_u4(uint32_t addr) {
 __device__ __forceinline__ void st_shared_u4(uint32_t addr, const uint4& v) {
   asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
+// 4-byte shared-memory store and load with no "memory" clobber: global loads may be scheduled across them (a .shared access
+// cannot alias global memory), while volatile keeps them in order with the fences and barriers, which do clobber memory
+__device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v)); }
+__device__ __forceinline__ uint32_t ld_shared_b32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 // named barrier of one consumer warpgroup (ids 1, 2; id 0 is __syncthreads)
 __device__ __forceinline__ void wg_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
@@ -252,6 +260,19 @@ struct TcPreact {
   const float* w;  // [Cout] folded BN scale of the absorbed op
   const float* b;  // [Cout] folded BN shift
 };
+// a 16-bit pair as the 32 bits st_shared_b32 stores, and back
+template <typename T>
+__device__ __forceinline__ uint32_t pair16_bits(typename Pair16<T>::type v) {
+  uint32_t u;
+  memcpy(&u, &v, 4);
+  return u;
+}
+template <typename T>
+__device__ __forceinline__ typename Pair16<T>::type pair16_from_bits(uint32_t u) {
+  typename Pair16<T>::type v;
+  memcpy(&v, &u, 4);
+  return v;
+}
 template <int BN>
 __device__ __forceinline__ void tc_store_staging(const uint8_t* stg, const CUtensorMap* map, const TcConvParams& p, int m_blk, int n_blk) {
   constexpr int SW = BN < 64 ? BN : 64, RB = SW * 2;
@@ -280,52 +301,60 @@ __device__ __forceinline__ void tc_tile_epilogue(const float* acc, uint8_t* stg,
   if (leader) bulk_wait_read();  // the previous tile's stores have read the staging tile
   wg_sync(2 + c);                // named barriers 3, 4 (1 and 2 order tc_conv_kernel's main loops)
   const int c0 = n_blk * BN + 2 * (lane & 3);
+  const uint32_t stg_s = smem_u32(stg);
+  // Column blocks of JB 8-column groups outside, the thread's four rows inside: the block's bias pairs are loaded once per
+  // tile, in one batch ahead of its arithmetic, and each row's residual pairs in one batch too.  The staging writes are
+  // .shared stores, which no global load has to wait behind: with generic stores to `stg`, which might have aliased global
+  // memory, every load stayed behind the previous column's store and each column pair ran as one dependent chain.  Blocks
+  // are up to 8 groups wide.  At BN = 128 with a residual, the bias batch does not fit next to the 128 accumulators and the
+  // residual batch within the 168 registers of __launch_bounds__, and narrower blocks, whose residual batches are smaller,
+  // made the ResNet projections slower; so there the bias pairs are loaded at their use, free of the stores.
+  constexpr int JB = BN / 8 < 8 ? BN / 8 : 8;
+  constexpr bool BIAS_BATCH = RES == 0 || BN < 128;
 #pragma unroll
-  for (int mh = 0; mh < 2; ++mh) {
-    const float* accm = acc + mh * (BN / 2);
+  for (int j0 = 0; j0 < BN / 8; j0 += JB) {
+    float2 bv[BIAS_BATCH ? JB : 1];
+    if constexpr (BIAS_BATCH) {
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
+      for (int jj = 0; jj < JB; ++jj)
+        if (c0 + 8 * (j0 + jj) < p.Cout) bv[jj] = __ldg(reinterpret_cast<const float2*>(p.bias + c0 + 8 * (j0 + jj)));
+    }
+#pragma unroll
+    for (int g = 0; g < 4; ++g) {  // rows 64 mh + 16 warp + lane / 4 + 8 h, g = 2 mh + h
+      const int mh = g >> 1, h = g & 1;
+      const float* accm = acc + mh * (BN / 2);
       const int r = mh * 64 + warp * 16 + (lane >> 2) + 8 * h;
-      size_t off = 0;
+      T2 rv2[RES != 0 ? JB : 1];
       if constexpr (RES != 0) {
+        size_t off = 0;
         if (!tile_row_offset(p.mode, m_blk, r, p.M, p.Cout, p.tiles_w, p.tiles_h, p.Hout, p.Wout, off)) continue;
+#pragma unroll
+        for (int jj = 0; jj < JB; ++jj)
+          if (c0 + 8 * (j0 + jj) < p.Cout) rv2[jj] = *reinterpret_cast<const T2*>(res + off + c0 + 8 * (j0 + jj));
       }
       const uint32_t swz = RB == 128 ? (uint32_t)(r & 7) : (uint32_t)((r >> 1) & 3);
-      // The residual pairs of up to 64 columns are loaded ahead of their arithmetic: loaded inside the column loop, behind
-      // the previous column's staging store, each load waited out its full latency before the next one was issued.  A whole
-      // row at BN = 128 would not fit next to the accumulators in the 168 registers of __launch_bounds__.
-      constexpr int JB = BN / 8 < 8 ? BN / 8 : 8;
 #pragma unroll
-      for (int j0 = 0; j0 < BN / 8; j0 += JB) {
-        T2 rv2[RES != 0 ? JB : 1];
+      for (int jj = 0; jj < JB; ++jj) {
+        const int j = j0 + jj, cc = c0 + 8 * j;
+        if (cc >= p.Cout) break;  // Cout % 8 == 0: column cc + 1 is valid with cc
+        const float2 b = BIAS_BATCH ? bv[BIAS_BATCH ? jj : 0] : __ldg(reinterpret_cast<const float2*>(p.bias + cc));
+        float o0 = accm[4 * j + 2 * h] + b.x, o1 = accm[4 * j + 2 * h + 1] + b.y;
         if constexpr (RES != 0) {
-#pragma unroll
-          for (int jj = 0; jj < JB; ++jj)
-            if (c0 + 8 * (j0 + jj) < p.Cout) rv2[jj] = *reinterpret_cast<const T2*>(res + off + c0 + 8 * (j0 + jj));
-        }
-#pragma unroll
-        for (int j = j0; j < j0 + JB; ++j) {
-          const int cc = c0 + 8 * j;
-          if (cc >= p.Cout) break;  // Cout % 8 == 0: column cc + 1 is valid with cc
-          const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + cc));
-          float o0 = accm[4 * j + 2 * h] + bv.x, o1 = accm[4 * j + 2 * h + 1] + bv.y;
-          if constexpr (RES != 0) {
-            const float2 rv = Pair16<T>::unpack(rv2[j - j0]);
-            if constexpr (RES == 2) {
-              o0 = tc_act<ACT, T>(o0 + rv.x);
-              o1 = tc_act<ACT, T>(o1 + rv.y);
-            } else {
-              o0 = tc_act<ACT, T>(o0) + rv.x;
-              o1 = tc_act<ACT, T>(o1) + rv.y;
-            }
+          const float2 rv = Pair16<T>::unpack(rv2[jj]);
+          if constexpr (RES == 2) {
+            o0 = tc_act<ACT, T>(o0 + rv.x);
+            o1 = tc_act<ACT, T>(o1 + rv.y);
           } else {
-            o0 = tc_act<ACT, T>(o0);
-            o1 = tc_act<ACT, T>(o1);
+            o0 = tc_act<ACT, T>(o0) + rv.x;
+            o1 = tc_act<ACT, T>(o1) + rv.y;
           }
-          const int col = 8 * j + 2 * (lane & 3), cs = col % SW;  // column within the tile, within its slab
-          const uint32_t o = (uint32_t)(col / SW) * (TC_BM * RB) + (uint32_t)r * RB + ((((uint32_t)cs >> 3) ^ swz) << 4) + (cs & 7) * 2;
-          *reinterpret_cast<T2*>(stg + o) = Pair16<T>::pack(o0, o1);
+        } else {
+          o0 = tc_act<ACT, T>(o0);
+          o1 = tc_act<ACT, T>(o1);
         }
+        const int col = 8 * j + 2 * (lane & 3), cs = col % SW;  // column within the tile, within its slab
+        const uint32_t o = (uint32_t)(col / SW) * (TC_BM * RB) + (uint32_t)r * RB + ((((uint32_t)cs >> 3) ^ swz) << 4) + (cs & 7) * 2;
+        st_shared_b32(stg_s + o, pair16_bits<T>(Pair16<T>::pack(o0, o1)));
       }
     }
   }
@@ -335,22 +364,32 @@ __device__ __forceinline__ void tc_tile_epilogue(const float* acc, uint8_t* stg,
   if constexpr (PRE) {
     if (leader) bulk_wait_read();  // the block output has left the staging tile
     wg_sync(2 + c);
+    // Column blocks outside, the four rows inside, as above: each pre.w / pre.b pair is loaded once per tile, not once per
+    // row.  The blocks are one 8-column group wide: wider batches spill at BN = 128.
+    constexpr int JP = 1;
+    for (int j0 = 0; j0 < BN / 8; j0 += JP) {
+      float2 wv[JP], bv[JP];
 #pragma unroll
-    for (int mh = 0; mh < 2; ++mh) {
+      for (int jj = 0; jj < JP; ++jj) {
+        const int cc = c0 + 8 * (j0 + jj);
+        if (cc < p.Cout) {
+          wv[jj] = __ldg(reinterpret_cast<const float2*>(pre.w + cc));
+          bv[jj] = __ldg(reinterpret_cast<const float2*>(pre.b + cc));
+        }
+      }
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int r = mh * 64 + warp * 16 + (lane >> 2) + 8 * h;  // rows past M hold what the TMA clips
+      for (int g = 0; g < 4; ++g) {
+        const int r = (g >> 1) * 64 + warp * 16 + (lane >> 2) + 8 * (g & 1);  // rows past M hold what the TMA clips
         const uint32_t swz = RB == 128 ? (uint32_t)(r & 7) : (uint32_t)((r >> 1) & 3);
 #pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          const int cc = c0 + 8 * j;
-          if (cc >= p.Cout) break;
-          const float2 wv = __ldg(reinterpret_cast<const float2*>(pre.w + cc)), bv = __ldg(reinterpret_cast<const float2*>(pre.b + cc));
+        for (int jj = 0; jj < JP; ++jj) {
+          const int j = j0 + jj;
+          if (c0 + 8 * j >= p.Cout) break;
           const int col = 8 * j + 2 * (lane & 3), cs = col % SW;
-          T2* q = reinterpret_cast<T2*>(stg + (uint32_t)(col / SW) * (TC_BM * RB) + (uint32_t)r * RB + ((((uint32_t)cs >> 3) ^ swz) << 4) +
-                                        (cs & 7) * 2);
-          const float2 x = Pair16<T>::unpack(*q);
-          *q = Pair16<T>::pack(act_t<ACT_RELU>(fmaf(x.x, wv.x, bv.x)), act_t<ACT_RELU>(fmaf(x.y, wv.y, bv.y)));
+          const uint32_t q = stg_s + (uint32_t)(col / SW) * (TC_BM * RB) + (uint32_t)r * RB + ((((uint32_t)cs >> 3) ^ swz) << 4) + (cs & 7) * 2;
+          const float2 x = Pair16<T>::unpack(pair16_from_bits<T>(ld_shared_b32(q)));
+          st_shared_b32(q, pair16_bits<T>(Pair16<T>::pack(act_t<ACT_RELU>(fmaf(x.x, wv[jj].x, bv[jj].x)),
+                                                          act_t<ACT_RELU>(fmaf(x.y, wv[jj].y, bv[jj].y)))));
         }
       }
     }

@@ -216,19 +216,36 @@ tc32_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 
   // ===== epilogue: thread rows r0 = 64 wg + 16 (warp & 3) + lane / 4 and r0 + 8, columns 8 j + 2 (lane % 4) + {0, 1} =====
   const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  // The bias pairs and both rows' residual pairs are loaded in one batch before the first store: loaded between the stores,
+  // which might alias them, each load waited out its latency before the next one was issued.
   const int c0 = n_blk * BN + 2 * (lane & 3);
+  float2 bv[BN / 8], rv2[RES != 0 ? 2 : 1][BN / 8];
+  size_t off[2];
+  bool row_ok[2];
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j)
+    if (c0 + 8 * j < p.Cout) bv[j] = __ldg(reinterpret_cast<const float2*>(p.bias + c0 + 8 * j));
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    size_t off;
-    if (!tile_row_offset(p.mode, m_blk, r0 + 8 * h, p.M, p.Cout, p.tiles_w, p.tiles_h, p.Hout, p.Wout, off)) continue;
+    row_ok[h] = tile_row_offset(p.mode, m_blk, r0 + 8 * h, p.M, p.Cout, p.tiles_w, p.tiles_h, p.Hout, p.Wout, off[h]);
+    if constexpr (RES != 0) {
+      if (row_ok[h]) {
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j)
+          if (c0 + 8 * j < p.Cout) rv2[h][j] = *reinterpret_cast<const float2*>(p.res + off[h] + c0 + 8 * j);
+      }
+    }
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    if (!row_ok[h]) continue;
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j) {
       const int c = c0 + 8 * j;
       if (c >= p.Cout) break;  // Cout % 4 == 0: column c + 1 is valid with c
-      const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + c));
-      float o0 = acc[4 * j + 2 * h] + bv.x, o1 = acc[4 * j + 2 * h + 1] + bv.y;
+      float o0 = acc[4 * j + 2 * h] + bv[j].x, o1 = acc[4 * j + 2 * h + 1] + bv[j].y;
       if constexpr (RES != 0) {
-        const float2 rv = *reinterpret_cast<const float2*>(p.res + off + c);
+        const float2 rv = rv2[h][j];
         if constexpr (RES == 2) {
           o0 = t32_act<ACT>(o0 + rv.x);
           o1 = t32_act<ACT>(o1 + rv.y);
@@ -240,7 +257,7 @@ tc32_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         o0 = t32_act<ACT>(o0);
         o1 = t32_act<ACT>(o1);
       }
-      *reinterpret_cast<float2*>(p.out + off + c) = make_float2(o0, o1);
+      *reinterpret_cast<float2*>(p.out + off[h] + c) = make_float2(o0, o1);
     }
   }
 }
