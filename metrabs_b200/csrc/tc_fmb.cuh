@@ -11,7 +11,8 @@
 // and after the last chunk epilogue-2: acc2 -> + bias -> + residual x -> 16-bit store.  Each consumer warpgroup owns 64 rows
 // of the tile in both GEMMs, so the A2 hand-over needs only a warpgroup barrier.  The MMA sequence of every output element
 // (tap-major K of GEMM-1, chunk-major K of GEMM-2, K = 16 per wgmma) and every rounding are those of the two-launch path
-// (tc_conv_kernel twice, with the same activation form per element type), so the fused block reproduces it.
+// (tc_conv_kernel twice, with the same activation form per element type), less the GEMM-1 steps that would only add exact
+// zeros, so the fused block reproduces it.
 //
 // Persistent: one CTA per SM walks tiles t = blockIdx.x, blockIdx.x + gridDim.x, ...  The input of a tile is read once, as
 // three column-shifted 16 x 10-pixel boxes per 64-channel k-chunk (tma_load_tap_boxes), kept resident across the tile's
@@ -48,6 +49,15 @@ struct FmbParams {
   const float* bias1;       // [Cexp]
   int Cexp, nch, has_res;
 };
+
+// one committed group of GEMM-1: the first NK k16 steps of k-block kb (A tile at shared address a, W1 block at b)
+template <typename T, int NK>
+__device__ __forceinline__ void fmb_gemm1_kblock(float* acc1, uint32_t a, uint32_t b, int kb) {
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < NK; ++k) wgmma_16b<T, FMB_NC>(acc1, gmma_desc<128>(a + 32 * k), gmma_desc<128>(b + 32 * k), (uint32_t)(kb | k));
+  wgmma_commit();
+}
 
 template <typename T, int BN2>
 __global__ void __launch_bounds__(TC_THREADS, 1)
@@ -112,6 +122,11 @@ fmb_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
   typedef typename Pair16<T>::type T2;
   const T* __restrict__ res = (const T*)g.res;
   T* __restrict__ out = (T*)g.out;
+  // k16 steps of the last k-chunk that hold input channels: KL_HI at Cin 24-32, 56-64 and 88-96 (BN2 = 32, 64, 128), one
+  // fewer at Cin 16, 40-48 and 72-80.  The steps after them would multiply TMA zero fill only and add exact zeros, so they
+  // are not issued (as tc_conv3x3s1_kernel issues K = CK per tap).
+  constexpr int KL_HI = BN2 == 64 ? 4 : 2;
+  const bool kl_hi = g.Cin - TC_BK * (KCH - 1) > 16 * (KL_HI - 1);
   int it = 0, n = 0;
   for (int t = blockIdx.x; t < g.m_tiles; t += gridDim.x, ++n) {
     float acc2[BN2 / 2];
@@ -124,52 +139,72 @@ fmb_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
 #pragma unroll
       for (int i = 0; i < FMB_NC / 2; ++i) acc1[i] = 0.f;
       int prev = -1;
-      for (int kb = 0; kb < NUM_KB; ++kb, ++it) {
-        const int s = it % STAGES;
-        mbar_wait(&full[s], (it / STAGES) & 1);
-        const int tap = kb / KCH, kc = kb - tap * KCH, r = tap / 3, sx = tap - 3 * r;
-        const uint32_t a = boxes + (uint32_t)(3 * kc + sx) * FMB_BOX_BYTES + (uint32_t)r * (TC_TILE_W * 128);
-        const uint32_t b = ring + s * FMB_W_BYTES;
-        wgmma_fence();
+      for (int tap = 0; tap < 9; ++tap) {
+        const int r = tap / 3, sx = tap - 3 * r;
 #pragma unroll
-        for (int k = 0; k < TC_BK / 16; ++k)
-          wgmma_16b<T, FMB_NC>(acc1, gmma_desc<128>(a + 32 * k), gmma_desc<128>(b + 32 * k), (uint32_t)(kb | k));
-        wgmma_commit();
-        wgmma_wait<1>();
-        if (prev >= 0) {
+        for (int kc = 0; kc < KCH; ++kc, ++it) {
+          const int kb = tap * KCH + kc, s = it % STAGES;
+          mbar_wait(&full[s], (it / STAGES) & 1);
+          const uint32_t a = boxes + (uint32_t)(3 * kc + sx) * FMB_BOX_BYTES + (uint32_t)r * (TC_TILE_W * 128);
+          const uint32_t b = ring + s * FMB_W_BYTES;
+          if (kc + 1 < KCH) fmb_gemm1_kblock<T, TC_BK / 16>(acc1, a, b, kb);
+          else if (kl_hi) fmb_gemm1_kblock<T, KL_HI>(acc1, a, b, kb);  // one uniform branch, in the last k-chunk only
+          else fmb_gemm1_kblock<T, KL_HI - 1>(acc1, a, b, kb);
+          wgmma_wait<1>();
           __syncwarp();
-          if (lane == 0) mbar_arrive(&empty[prev]);
+          if (prev >= 0) {
+            if (lane == 0) mbar_arrive(&empty[prev]);
+          } else if (c > 0 && lane == 0) {  // the previous chunk's GEMM-2 has retired: release its two W2 stages
+            mbar_arrive(&empty[(it - 2) % STAGES]);
+            mbar_arrive(&empty[(it - 1) % STAGES]);
+          }
+          prev = s;
         }
-        prev = s;
-      }
-      wgmma_wait<0>();
-      wgmma_fence_regs<FMB_NC / 2>(acc1);
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(&empty[prev]);
-        if (c == p.nch - 1) mbar_arrive(box_empty);  // the tile's last read of its input boxes
       }
       // ---- epilogue-1: + bias, SiLU, 16-bit -> A2 (this warpgroup's rows; 16-byte chunk j of row r at j ^ (r & 7)) ----
+      // Column blocks of JB1 groups, the first block's bias pairs loaded while the last k-block's MMAs run.  A2 is written
+      // with .shared stores: a generic store might alias global memory, and no load could be issued ahead of it.  At
+      // BN2 = 128 both accumulators hold 128 of the 168 registers, and a first block of 4 or more groups spills.
+      constexpr int JB1 = BN2 == 128 ? 2 : FMB_NC / 8;
 #pragma unroll
-      for (int j = 0; j < FMB_NC / 8; ++j) {
-        const int cc = 8 * j + 2 * (lane & 3);  // column within the chunk
-        const int col = c * FMB_NC + cc;
-        float2 bv = make_float2(0.f, 0.f);
-        if (col < p.Cexp) bv = __ldg(reinterpret_cast<const float2*>(p.bias1 + col));  // Cexp % 16 == 0: col + 1 valid with col
-        const uint32_t sub = (uint32_t)(cc >> 6) * (TC_BM * 128), kc = (uint32_t)(cc & 63);
+      for (int j0 = 0; j0 < FMB_NC / 8; j0 += JB1) {
+        float2 bv[JB1];
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int r = r0 + 8 * h;
-          T2 v = Pair16<T>::pack(0.f, 0.f);
-          if (col < p.Cexp)
-            v = Pair16<T>::pack(tc_act<ACT_SILU, T>(acc1[4 * j + 2 * h] + bv.x), tc_act<ACT_SILU, T>(acc1[4 * j + 2 * h + 1] + bv.y));
-          const uint32_t off = sub + (uint32_t)r * 128 + ((((kc >> 3) ^ (uint32_t)(r & 7))) << 4) + (kc & 7) * 2;
-          *reinterpret_cast<T2*>(smem + L::a2_off + off) = v;
+        for (int jj = 0; jj < JB1; ++jj) {  // Cexp % 16 == 0: col + 1 is valid with col
+          const int col = c * FMB_NC + 8 * (j0 + jj) + 2 * (lane & 3);
+          bv[jj] = col < p.Cexp ? __ldg(reinterpret_cast<const float2*>(p.bias1 + col)) : make_float2(0.f, 0.f);
+        }
+        if (j0 == 0) {
+          wgmma_wait<0>();
+          wgmma_fence_regs<FMB_NC / 2>(acc1);
+          __syncwarp();
+          if (lane == 0) {
+            mbar_arrive(&empty[prev]);
+            if (c == p.nch - 1) mbar_arrive(box_empty);  // the tile's last read of its input boxes
+          }
+        }
+#pragma unroll
+        for (int jj = 0; jj < JB1; ++jj) {
+          const int j = j0 + jj, cc = 8 * j + 2 * (lane & 3);  // column within the chunk
+          const bool live = c * FMB_NC + cc < p.Cexp;
+          const uint32_t sub = (uint32_t)(cc >> 6) * (TC_BM * 128), kc = (uint32_t)(cc & 63);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int r = r0 + 8 * h;
+            const uint32_t v = pair16_bits<T>(
+                Pair16<T>::pack(tc_act<ACT_SILU, T>(acc1[4 * j + 2 * h] + bv[jj].x), tc_act<ACT_SILU, T>(acc1[4 * j + 2 * h + 1] + bv[jj].y)));
+            const uint32_t off = sub + (uint32_t)r * 128 + ((((kc >> 3) ^ (uint32_t)(r & 7))) << 4) + (kc & 7) * 2;
+            // zeros past Cexp by a select: a branch per column pair kept ptxas from overlapping the columns' SiLU chains
+            st_shared_b32(a2 + off, live ? v : 0u);
+          }
         }
       }
       fence_proxy_async();  // generic-proxy writes -> visible to the tensor core (async proxy)
       wg_sync(wg);
       // ---- GEMM-2: acc2 += A2 x W2[:, chunk]^T, the two 64-channel halves of the W2 slice in consecutive stages ----
+      // Not waited for here: the next chunk's first GEMM-1 k-block is issued behind it, and its wgmma.wait_group 1 retires
+      // this group (groups retire in order) before the stages are released and before epilogue-1 rewrites A2.  The last
+      // chunk's group is waited for under epilogue-2's first loads.
       {
         const int s0 = it % STAGES, s1 = (it + 1) % STAGES;
         mbar_wait(&full[s0], (it / STAGES) & 1);
@@ -182,82 +217,51 @@ fmb_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
           wgmma_16b<T, BN2>(acc2, gmma_desc<128>(a2 + sub * (TC_BM * 128) + wg * 64 * 128 + ko), gmma_desc<128>(b + ko), (uint32_t)(c | k));
         }
         wgmma_commit();
-        if (BN2 == 128 || c + 1 < p.nch) {  // BN2 <= 64: the last chunk's MMAs are waited for under epilogue-2's loads
-          wgmma_wait<0>();  // A2 is rewritten by the next chunk's epilogue-1
-          wgmma_fence_regs<BN2 / 2>(acc2);
-          __syncwarp();
-          if (lane == 0) {
-            mbar_arrive(&empty[s0]);
-            mbar_arrive(&empty[s1]);
-          }
-        }
         it += 2;
       }
     }
     // ---- epilogue-2: + bias, + residual x, 16-bit store ----
+    // All of the thread's bias and residual pairs are loaded in one batch while the last chunk's GEMM-2 runs: issued one by
+    // one between the stores, which might alias them, each waited out its L2 latency with the MMAs of both warpgroups idle.
+    // Every batch element is set on every path: an element left unset where its load is skipped stays live around the
+    // whole tile loop, next to both accumulators, and at BN2 = 128 that spilled.
     const int c0 = 2 * (lane & 3);
-    if constexpr (BN2 <= 64) {
-      // All of the thread's bias and residual pairs are loaded in one batch while the last chunk's GEMM-2 runs: issued one
-      // by one between the stores, which might alias them, each waited out its L2 latency with the MMAs of both
-      // warpgroups idle.  At BN2 = 128 (Cout 72 to 96) the batch spills next to the accumulators, so that width keeps the
-      // loads at their use.
-      float2 bv[BN2 / 8];
-      T2 rv[2][BN2 / 8];
-      size_t off[2];
-      bool row_ok[2];
+    float2 bv[BN2 / 8];
+    T2 rv[2][BN2 / 8];
+    size_t off[2];
+    bool row_ok[2];
 #pragma unroll
-      for (int j = 0; j < BN2 / 8; ++j)
-        if (c0 + 8 * j < g.Cout) bv[j] = __ldg(reinterpret_cast<const float2*>(g.bias + c0 + 8 * j));
+    for (int h = 0; h < 2; ++h)
+      row_ok[h] = tile_row_offset(1, t, r0 + 8 * h, g.M, g.Cout, g.tiles_w, g.tiles_h, g.Hout, g.Wout, off[h]);
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        row_ok[h] = tile_row_offset(1, t, r0 + 8 * h, g.M, g.Cout, g.tiles_w, g.tiles_h, g.Hout, g.Wout, off[h]);
-        if (p.has_res && row_ok[h]) {
+    for (int j = 0; j < BN2 / 8; ++j) {
+      const int cidx = c0 + 8 * j;
+      bv[j] = cidx < g.Cout ? __ldg(reinterpret_cast<const float2*>(g.bias + cidx)) : make_float2(0.f, 0.f);
 #pragma unroll
-          for (int j = 0; j < BN2 / 8; ++j)
-            if (c0 + 8 * j < g.Cout) rv[h][j] = *reinterpret_cast<const T2*>(res + off[h] + c0 + 8 * j);
+      for (int h = 0; h < 2; ++h)
+        rv[h][j] = p.has_res && row_ok[h] && cidx < g.Cout ? *reinterpret_cast<const T2*>(res + off[h] + cidx) : Pair16<T>::pack(0.f, 0.f);
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs<BN2 / 2>(acc2);
+    __syncwarp();
+    if (lane == 0) {
+      mbar_arrive(&empty[(it - 2) % STAGES]);
+      mbar_arrive(&empty[(it - 1) % STAGES]);
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (!row_ok[h]) continue;
+#pragma unroll
+      for (int j = 0; j < BN2 / 8; ++j) {
+        const int cidx = c0 + 8 * j;
+        if (cidx >= g.Cout) break;
+        float o0 = acc2[4 * j + 2 * h] + bv[j].x, o1 = acc2[4 * j + 2 * h + 1] + bv[j].y;
+        if (p.has_res) {
+          const float2 f = Pair16<T>::unpack(rv[h][j]);
+          o0 += f.x;
+          o1 += f.y;
         }
-      }
-      wgmma_wait<0>();
-      wgmma_fence_regs<BN2 / 2>(acc2);
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(&empty[(it - 2) % STAGES]);
-        mbar_arrive(&empty[(it - 1) % STAGES]);
-      }
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        if (!row_ok[h]) continue;
-#pragma unroll
-        for (int j = 0; j < BN2 / 8; ++j) {
-          const int cidx = c0 + 8 * j;
-          if (cidx >= g.Cout) break;
-          float o0 = acc2[4 * j + 2 * h] + bv[j].x, o1 = acc2[4 * j + 2 * h + 1] + bv[j].y;
-          if (p.has_res) {
-            const float2 f = Pair16<T>::unpack(rv[h][j]);
-            o0 += f.x;
-            o1 += f.y;
-          }
-          *reinterpret_cast<T2*>(out + off[h] + cidx) = Pair16<T>::pack(o0, o1);
-        }
-      }
-    } else {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        size_t off;
-        if (!tile_row_offset(1, t, r0 + 8 * h, g.M, g.Cout, g.tiles_w, g.tiles_h, g.Hout, g.Wout, off)) continue;
-#pragma unroll
-        for (int j = 0; j < BN2 / 8; ++j) {
-          const int cidx = c0 + 8 * j;
-          if (cidx >= g.Cout) break;
-          const float2 bv = __ldg(reinterpret_cast<const float2*>(g.bias + cidx));
-          float o0 = acc2[4 * j + 2 * h] + bv.x, o1 = acc2[4 * j + 2 * h + 1] + bv.y;
-          if (p.has_res) {
-            const float2 rv = Pair16<T>::unpack(*reinterpret_cast<const T2*>(res + off + cidx));
-            o0 += rv.x;
-            o1 += rv.y;
-          }
-          *reinterpret_cast<T2*>(out + off + cidx) = Pair16<T>::pack(o0, o1);
-        }
+        *reinterpret_cast<T2*>(out + off[h] + cidx) = Pair16<T>::pack(o0, o1);
       }
     }
   }
