@@ -157,6 +157,37 @@ int mtb_output_joints(const mtb_handle* h);
 int mtb_linear_combine_points(const float* points, int batch, int n_in, const float* weights, int n_out, float* out,
                               void* stream);
 
+/* Model classes of metrabs_tf/main.py:172-185 (--model-class, metrabs_tf/init.py:218).  METRABS (the default) is the path
+ * above.  METRO (metrabs_tf/models/metro.py:13-45) and MODEL_25D (metrabs_tf/models/twofive.py:14-57) share a head without
+ * the 2D block: conv_final has D*J channels (key "heatmap_head.conv_final.*", weight [D*J,C,1,1]), channel d*J + j, soft-argmax
+ * jointly over (W, H, D) with tf.linspace (a one-long axis decodes to 0, not 0.5).  METRO outputs heatmap_to_metric of it:
+ * root-relative joints in mm, crop-box frame; it takes no intrinsics.  MODEL_25D decodes heatmap_to_25d (x, y in crop pixels,
+ * z in mm) and reconstructs absolute camera-space joints with reconstruct_absolute_by_bone_lengths (metrabs_tf/tfu3d.py:
+ * 219-269): a 10-step Levenberg-Marquardt fit of each crop's depth to the ideal bone lengths, whose accept decision is taken
+ * on the objective of the whole batch, so a crop's absolute joints depend on the batch it runs in (its decoded coords25d do
+ * not). */
+typedef enum { MTB_MODEL_METRABS = 0, MTB_MODEL_METRO = 1, MTB_MODEL_25D = 2 } mtb_model_class;
+/* Sets the handle's model class; must be called before mtb_finalize_weights.  MODEL_25D takes `edges` [n_bones][2] (joint
+ * indices in [0, cfg.n_joints)) and `bone_lengths` [n_bones] (mm, finite and positive), HOST arrays that are copied; the other
+ * classes ignore them.  mean_relative != 0: depths relative to the mean joint (the reference default, init.py:228), else to the
+ * last joint.  On a METRO or MODEL_25D handle:
+ *   - mtb_head_decode writes the decoded [B,J,3] (Metro: mm; 2.5D: x px, y px, z mm) into coords3d_rel and its x, y into
+ *     coords2d when coords2d is non-null;
+ *   - mtb_forward, mtb_forward_host*, and mtb_forward_sharded run the whole class (METRO ignores intrinsics, which may be null);
+ *     MODEL_25D's sharded forward all-gathers coords25d (3 floats per joint) and solves the full batch on every rank;
+ *   - mtb_reconstruct_absolute fails with MTB_ERR_UNSUPPORTED.
+ * MTB_ERR_INVALID_ARG for an unknown class, a bone index out of range, a bad length, n_bones outside [1, 4096] (MODEL_25D), a
+ * METRO / MODEL_25D class with cfg.legacy_centered_stride_bug (the TF decode has no such term), a finalized or head-only
+ * handle, or one with a latent recombination (mtb_set_latent_recombination in turn refuses a METRO / MODEL_25D handle). */
+int mtb_set_model_class(mtb_handle* h, int model_class, const int32_t* edges, const float* bone_lengths, int n_bones,
+                        int mean_relative);
+/* The MODEL_25D absolute step on its own: coords25d [batch,J,3] (as mtb_head_decode writes them) + intrinsics [batch,3,3] ->
+ * coords3d_abs [batch,J,3], one bone_solve_kernel launch, no host synchronisation.  Bit-identical from run to run.
+ * scratch >= mtb_bone_lengths_scratch_bytes(h, batch) bytes (0 for a handle of another class). */
+size_t mtb_bone_lengths_scratch_bytes(const mtb_handle* h, int batch);
+int mtb_reconstruct_by_bone_lengths(mtb_handle* h, const float* coords25d, const float* intrinsics, int batch, float* coords3d_abs,
+                                    void* scratch, void* stream);
+
 size_t mtb_workspace_bytes(const mtb_handle* h, int batch);
 /* Elements per crop of the feature map [H*W*C] and its spatial side, after finalize. */
 int mtb_feature_shape(const mtb_handle* h, int* hw_side, int* channels);

@@ -25,6 +25,7 @@ BUF_FEATURES, BUF_NONE = -2, -1  # mtb_debug_op_buffers; 0-3 the large buffers, 
 PRECISION_FP32, PRECISION_BF16_TC, PRECISION_BF16_SIMT, PRECISION_TF32X3, PRECISION_F16_TC, PRECISION_F16_SIMT = 0, 1, 2, 3, 4, 5
 DTYPE_F32, DTYPE_BF16, DTYPE_F16, DTYPE_I64 = 0, 1, 2, 3
 LAYOUT_BDJHW, LAYOUT_BHWN = 0, 1
+MODEL_METRABS, MODEL_METRO, MODEL_25D = 0, 1, 2  # mtb_model_class (mtb_set_model_class)
 
 LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'libmetrabs_b200.so')
 
@@ -90,6 +91,10 @@ _SIGNATURES = {
     'mtb_set_latent_recombination': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
     'mtb_output_joints': (C.c_int, [C.c_void_p]),
     'mtb_linear_combine_points': (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    'mtb_set_model_class': (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
+    'mtb_bone_lengths_scratch_bytes': (C.c_size_t, [C.c_void_p, C.c_int]),
+    'mtb_reconstruct_by_bone_lengths': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                                  C.c_void_p]),
     'mtb_workspace_bytes': (C.c_size_t, [C.c_void_p, C.c_int]),
     'mtb_feature_shape': (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     'mtb_backbone_forward': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t,

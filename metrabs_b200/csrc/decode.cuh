@@ -38,6 +38,10 @@ __device__ __forceinline__ SoftState soft_shfl_xor(const SoftState& a, int o) {
 __device__ __forceinline__ float soft_coord(float weighted_index_sum, float s, int n) {
   return n > 1 ? weighted_index_sum / s / (float)(n - 1) : 0.5f;
 }
+// the same expectation with tf.linspace(0, 1, n), which is [0] for n == 1 (tfu.py:230): the TF-only Metro and Model25D heads
+__device__ __forceinline__ float soft_coord_tf(float weighted_index_sum, float s, int n) {
+  return n > 1 ? weighted_index_sum / s / (float)(n - 1) : 0.f;
+}
 
 // ----------------------------------------------------------------------------------------------------------
 // Standalone soft-argmax over the REFERENCE layout: logits [B,D,J,H,W] (D >= 1) -> out [B,J,3] = (x,y,z), or,
@@ -228,20 +232,23 @@ __global__ void __launch_bounds__(256) softargmax_bdjhw_kernel(const T* __restri
 // One CTA per crop; thread (cx, py): channel lane cx, pixel slice py; per-channel states merged in smem, then
 // the D depth slices of each joint are merged.  Outputs are the [0,1] heatmap coordinates; `scale` applies
 // heatmap_to_image / heatmap_to_metric (models/util.py) when non-null.
+// HEAD3D: the head of the TF-only Metro / Model25D classes (metrabs_tf/models/metro.py:34-44, twofive.py:46-56): no 2D
+// block, N = D*J with channel n = d*J + j, tf.linspace's n == 1 rule, and the 3D scale (met_*) applied to x and y; out2d,
+// when non-null, receives the same x and y.
 // ----------------------------------------------------------------------------------------------------------
 struct DecodeScale {
   float img_mul, img_add;  // coords2d px = c * img_mul + img_add          (heatmap_to_image)
-  float met_mul, met_add;  // xy_mm = (c * img_mul + img_add) * box/S  =>  c * met_mul + met_add
+  float met_mul, met_add;  // xy_mm = (c * img_mul + img_add) * box/S  =>  c * met_mul + met_add (Model25D: = img_*)
   float z_mul;             // z_mm = c * box_size_mm
   int apply;
 };
 
-template <typename T>
+template <typename T, bool HEAD3D = false>
 __global__ void __launch_bounds__(512) softargmax_bhwn_kernel(const T* __restrict__ logits, float* __restrict__ out2d,
                                                               float* __restrict__ out3d, int J, int D, int H, int W,
                                                               int ld, DecodeScale sc) {
   extern __shared__ float sm[];  // [N][4] per-channel (m, s, sx, sy) + [PY][128][4] merge scratch
-  const int N = J * (1 + D);
+  const int N = HEAD3D ? J * D : J * (1 + D);
   const int P = H * W;
   const int b = blockIdx.x;
   const int cx = threadIdx.x & 127, py = threadIdx.x >> 7;  // 128 x 4
@@ -284,6 +291,27 @@ __global__ void __launch_bounds__(512) softargmax_bhwn_kernel(const T* __restric
     __syncthreads();
   }
   for (int j = threadIdx.x; j < J; j += blockDim.x) {
+    if constexpr (HEAD3D) {
+      SoftState a;
+      soft_init(a);
+      for (int d = 0; d < D; ++d) {
+        float4 c = chan[d * J + j];
+        SoftState bb;
+        bb.m = c.x; bb.s = c.y; bb.sx = c.z; bb.sy = c.w; bb.sz = c.y * (float)d;
+        soft_merge(a, bb);
+      }
+      const float x = fmaf(soft_coord_tf(a.sx, a.s, W), sc.met_mul, sc.met_add);
+      const float y = fmaf(soft_coord_tf(a.sy, a.s, H), sc.met_mul, sc.met_add);
+      const float z = soft_coord_tf(a.sz, a.s, D) * sc.z_mul;
+      out3d[((size_t)b * J + j) * 3 + 0] = x;
+      out3d[((size_t)b * J + j) * 3 + 1] = y;
+      out3d[((size_t)b * J + j) * 3 + 2] = z;
+      if (out2d) {
+        out2d[((size_t)b * J + j) * 2 + 0] = x;
+        out2d[((size_t)b * J + j) * 2 + 1] = y;
+      }
+      continue;
+    }
     if (out2d) {
       float4 c = chan[j];
       float x = soft_coord(c.z, c.y, W), y = soft_coord(c.w, c.y, H);
@@ -467,6 +495,166 @@ __global__ void __launch_bounds__(128) recon_pass2_kernel(ReconParams p) {
     p.out[o * 3 + 0] = infov ? a2x : a3x;
     p.out[o * 3 + 1] = infov ? a2y : a3y;
     p.out[o * 3 + 2] = infov ? a2z : a3z;
+  }
+}
+
+// ----------------------------------------------------------------------------------------------------------
+// reconstruct_absolute_by_bone_lengths (metrabs_tf/tfu3d.py:219-269), the absolute step of Model25D: coords25d [B,J,3] =
+// (x px, y px, z mm) -> camera-space joints [B,J,3].  Per crop b, with n2d = ([x, y, 1] K^-1^T)[:2], z_rel = z - mean_j z
+// (or z - z[J-1]), x_j = [n2d_j, 1] and per bone e = (i, j):  a = x_i - x_j, bv = x_i z_rel_i - x_j z_rel_j, c = |a|^2,
+// d = 2 a.bv, e = |bv|^2, w = (in_fov_i && in_fov_j) + 1e-8, the residual r_e(z) = (sqrt(z^2 c + z d + e) - L_e) w.
+// tensorflow_graphics' Levenberg-Marquardt minimises sum_b sum_e r^2 over the z of the WHOLE batch from 1500 / projected
+// size: its Jacobian [B*E, B] is block-diagonal, so each step is per crop z -= sum_e J r / (sum_e J^2 + lam), and the step
+// is taken for every crop iff the batch objective decreases, else lam *= 10 (lam starts at 1e-20; 10 iterations).  The
+// accept decision couples the crops, so one CTA runs the whole solve: a warp per crop (crops strided over the warps), the
+// per-crop sums as fixed warp butterflies, the batch sums over crops in ascending order per thread and then over threads in
+// a fixed tree.  No atomics: the result is bit-identical from run to run.
+// ----------------------------------------------------------------------------------------------------------
+struct BoneSolveParams {
+  const float* c25;   // [B,J,3]
+  const float* K;     // [B,3,3]
+  const int2* edges;  // [E] joint pairs
+  const float* len;   // [E] ideal bone lengths, mm
+  float* out;         // [B,J,3]
+  float4* coef;       // [B][E] scratch: (c, d, e, w) per bone
+  float* z;           // [B] scratch: the accepted z_ref
+  float* z_new;       // [B] scratch: the candidate of this iteration
+  float* obj;         // [B] scratch: per-crop objective of the candidate (before the loop: of the initial guess)
+  int B, J, E;
+  float fov_lower, fov_upper;
+  int mean_relative;
+};
+constexpr int BONE_THREADS = 512;
+constexpr int BONE_ITERS = 10;
+
+// K^-1 and the centre of z (mean over the joints, or the last joint) of crop b; identical in every lane of the warp
+__device__ __forceinline__ void bone_crop_setup(const BoneSolveParams& p, int b, int lane, float* kinv, float& zc) {
+  inv3x3(p.K + (size_t)b * 9, kinv);
+  const float* c = p.c25 + (size_t)b * p.J * 3;
+  if (p.mean_relative) {
+    float s = 0.f;
+    for (int j = lane; j < p.J; j += 32) s += c[j * 3 + 2];
+    zc = warp_sum(s) / (float)p.J;
+  } else {
+    zc = c[(p.J - 1) * 3 + 2];
+  }
+}
+
+__device__ __forceinline__ float bone_residual(float4 q, float L, float z) {
+  return (sqrtf(z * z * q.x + z * q.y + q.z) - L) * q.w;
+}
+
+// sum of v[0..n) in ascending order per thread, then a fixed tree over the CTA (every thread gets the total)
+__device__ __forceinline__ float bone_block_sum(const float* v, int n, float* red) {
+  float s = 0.f;
+  for (int i = threadIdx.x; i < n; i += BONE_THREADS) s += v[i];
+  s = warp_sum(s);
+  __syncthreads();  // red[] is reused by consecutive calls
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+  __syncthreads();
+  float t = 0.f;
+  for (int w = 0; w < BONE_THREADS / 32; ++w) t += red[w];
+  return t;
+}
+
+__global__ void __launch_bounds__(BONE_THREADS) bone_solve_kernel(BoneSolveParams p) {
+  __shared__ float red[BONE_THREADS / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  constexpr int n_warps = BONE_THREADS / 32;
+  // pass 1: bone coefficients, initial guess and its objective
+  for (int b = warp; b < p.B; b += n_warps) {
+    float kinv[9], zc;
+    bone_crop_setup(p, b, lane, kinv, zc);
+    const float* c = p.c25 + (size_t)b * p.J * 3;
+    float lox = INFINITY, hix = -INFINITY, loy = INFINITY, hiy = -INFINITY;
+    for (int j = lane; j < p.J; j += 32) {
+      const float x = c[j * 3], y = c[j * 3 + 1];
+      const float nx = x * kinv[0] + y * kinv[1] + kinv[2], ny = x * kinv[3] + y * kinv[4] + kinv[5];
+      lox = fminf(lox, nx); hix = fmaxf(hix, nx);
+      loy = fminf(loy, ny); hiy = fmaxf(hiy, ny);
+    }
+    lox = -warp_max(-lox); loy = -warp_max(-loy);
+    hix = warp_max(hix); hiy = warp_max(hiy);
+    const float guess = 1500.f / fmaxf(hix - lox, hiy - loy);
+    float r2 = 0.f;
+    for (int e = lane; e < p.E; e += 32) {
+      const int2 ij = p.edges[e];
+      float n[2][2], zr[2];
+      bool fov[2];
+      for (int k = 0; k < 2; ++k) {
+        const float* q = c + (k == 0 ? ij.x : ij.y) * 3;
+        n[k][0] = q[0] * kinv[0] + q[1] * kinv[1] + kinv[2];
+        n[k][1] = q[0] * kinv[3] + q[1] * kinv[4] + kinv[5];
+        zr[k] = q[2] - zc;
+        fov[k] = q[0] >= p.fov_lower && q[0] <= p.fov_upper && q[1] >= p.fov_lower && q[1] <= p.fov_upper;
+      }
+      const float ax = n[0][0] - n[1][0], ay = n[0][1] - n[1][1];  // the homogeneous components cancel
+      const float bx = n[0][0] * zr[0] - n[1][0] * zr[1], by = n[0][1] * zr[0] - n[1][1] * zr[1], bz = zr[0] - zr[1];
+      const float4 q = make_float4(ax * ax + ay * ay, 2.f * (ax * bx + ay * by), bx * bx + by * by + bz * bz,
+                                   (fov[0] && fov[1] ? 1.f : 0.f) + 1e-8f);
+      p.coef[(size_t)b * p.E + e] = q;
+      const float r = bone_residual(q, p.len[e], guess);
+      r2 += r * r;
+    }
+    r2 = warp_sum(r2);
+    if (lane == 0) {
+      p.z[b] = guess;
+      p.obj[b] = r2;
+    }
+  }
+  __syncthreads();
+  float total = bone_block_sum(p.obj, p.B, red);
+  float lam = 1e-20f;
+  for (int it = 0; it < BONE_ITERS; ++it) {
+    for (int b = warp; b < p.B; b += n_warps) {
+      const float z = p.z[b];
+      const float4* q = p.coef + (size_t)b * p.E;
+      float jr = 0.f, jj = 0.f;
+      for (int e = lane; e < p.E; e += 32) {
+        const float4 c = q[e];
+        const float s = sqrtf(z * z * c.x + z * c.y + c.z);
+        const float r = (s - p.len[e]) * c.w;
+        const float jac = c.w * (2.f * z * c.x + c.y) / (2.f * s);
+        jr += jac * r;
+        jj += jac * jac;
+      }
+      const float zn = z - warp_sum(jr) / (warp_sum(jj) + lam);
+      float r2 = 0.f;
+      for (int e = lane; e < p.E; e += 32) {
+        const float r = bone_residual(q[e], p.len[e], zn);
+        r2 += r * r;
+      }
+      r2 = warp_sum(r2);
+      if (lane == 0) {
+        p.z_new[b] = zn;
+        p.obj[b] = r2;
+      }
+    }
+    __syncthreads();
+    const float total_new = bone_block_sum(p.obj, p.B, red);
+    if (total_new < total) {  // the same decision in every thread
+      total = total_new;
+      for (int b = threadIdx.x; b < p.B; b += BONE_THREADS) p.z[b] = p.z_new[b];
+    } else {
+      lam *= 10.f;
+    }
+    __syncthreads();
+  }
+  // back_project (tfu3d.py:200-201): [n2d, 1] * (z_rel + z_ref)
+  for (int b = warp; b < p.B; b += n_warps) {
+    float kinv[9], zc;
+    bone_crop_setup(p, b, lane, kinv, zc);
+    const float zref = p.z[b];
+    const float* c = p.c25 + (size_t)b * p.J * 3;
+    float* o = p.out + (size_t)b * p.J * 3;
+    for (int j = lane; j < p.J; j += 32) {
+      const float x = c[j * 3], y = c[j * 3 + 1];
+      const float nx = x * kinv[0] + y * kinv[1] + kinv[2], ny = x * kinv[3] + y * kinv[4] + kinv[5];
+      const float zz = (c[j * 3 + 2] - zc) + zref;
+      o[j * 3 + 0] = nx * zz;
+      o[j * 3 + 1] = ny * zz;
+      o[j * 3 + 2] = zz;
+    }
   }
 }
 

@@ -34,12 +34,12 @@ enum OpType { OP_STEM = 0, OP_CONV = 1, OP_DW = 2, OP_POOL = 3, OP_MAXPOOL = 4 }
 // kernel classes for the CUDA-event profiler (mtb_profile_begin / mtb_profile_end)
 enum KClass { KC_STEM = 0, KC_IGEMM_SIMT = 1, KC_DWCONV = 2, KC_POOL = 3, KC_SE_FC = 4, KC_TC_GEMM = 5, KC_FMB = 6,
               KC_HEAD_FUSED = 7, KC_HEAD_CONV_SIMT = 8, KC_SOFTARGMAX = 9, KC_RECON = 10, KC_OTHER = 11, KC_SE_SCALE = 12, KC_TC32 = 13,
-              KC_COMBINE = 14, KC_TC_PREACT = 15, KC_COUNT = 16 };
+              KC_COMBINE = 14, KC_TC_PREACT = 15, KC_BONE_SOLVE = 16, KC_COUNT = 17 };
 const char* kKClassNames[KC_COUNT] = {"stem_conv_kernel", "conv_igemm_kernel", "dwconv_kernel", "pool_mean_kernel",
                                       "se_fc(conv_igemm_kernel)", "tc_conv_kernel", "fmb_kernel",
                                       "tc_head_softargmax_kernel", "head_conv(conv_igemm_kernel)",
                                       "softargmax_bhwn_kernel", "recon_pass1+2_kernel", "other", "se_scale_kernel", "tc32_conv_kernel",
-                                      "combine_points_kernel", "tc_conv_preact_kernel"};
+                                      "combine_points_kernel", "tc_conv_preact_kernel", "bone_solve_kernel"};
 // One row per mtb_kernel value: the profiler class of its launches, whether it exists for 16-bit storage only (bf16 /
 // fp16), and whether it also writes the SE pooling slices of its output (depthwise)
 struct KernelTraits { mtb_kernel kernel; KClass cls; bool only16, pools; };
@@ -116,6 +116,14 @@ struct mtb_handle {
   int n_latents = 0, n_out = 0;
   std::vector<float> recomb;
   float* d_recomb = nullptr;  // device copy in the weight arena (uploaded by mtb_finalize_weights)
+  // model class (mtb_set_model_class): MeTRAbs, Metro (root-relative metric output) or Model25D (2.5D head + bone-length
+  // depth solve over bone_edges / bone_len); the device copies live in the weight arena
+  int model_class = MTB_MODEL_METRABS;
+  std::vector<int32_t> bone_edges;  // [n_bones][2]
+  std::vector<float> bone_len;      // [n_bones] mm
+  int mean_relative = 1;
+  int2* d_edges = nullptr;
+  float* d_len = nullptr;
   bool finalized = false;
   mutable std::string err;
   std::vector<void*> dev_allocs;
@@ -223,10 +231,14 @@ auto with_storage16(const mtb_handle* h, F&& f) {
 // points the head decodes and the reconstruction solves for: the latents of a latent-point model, cfg.n_joints otherwise
 inline int head_points(const mtb_handle* h) { return h->n_latents > 0 ? h->n_latents : h->cfg.n_joints; }
 inline int output_joints(const mtb_handle* h) { return h->n_latents > 0 ? h->n_out : h->cfg.n_joints; }
-// head channel count (1 + D per point) padded to a multiple of 4 with zero weights (J=122: 1098 -> 1100), and its FLOPs
+// the TF-only Metro / Model25D head: D*J channels (channel d*J + j), no 2D block
+inline bool head3d(const mtb_handle* h) { return h->model_class != MTB_MODEL_METRABS; }
+// head channels before padding: 1 + D per point (MeTRAbs), D per point (Metro / Model25D)
+inline int head_channels(const mtb_handle* h) { return head_points(h) * (h->cfg.depth + (head3d(h) ? 0 : 1)); }
+// head channel count padded to a multiple of 4 with zero weights (J=122: 1098 -> 1100), and its FLOPs
 inline void size_head(mtb_handle* h) {
   Op& hd = h->head;
-  hd.Cout = (head_points(h) * (1 + h->cfg.depth) + 3) / 4 * 4;
+  hd.Cout = (head_channels(h) + 3) / 4 * 4;
   hd.flops = 2.0 * hd.Hout * hd.Wout * hd.Cin * hd.Cout;
 }
 
@@ -909,8 +921,26 @@ int prepare_op_weights(mtb_handle* h, Op& op) {
 struct Workspace {
   char* base;
   size_t big_stride, small_stride;
-  size_t off_small, off_features, off_logits, off_c2d, off_c3d, off_n2d, off_partial, off_latents, total;
+  size_t off_small, off_features, off_logits, off_c2d, off_c3d, off_n2d, off_partial, off_latents, off_bones, total;
 };
+
+// scratch of bone_solve_kernel for B crops: per-bone coefficients [B][E] float4, then z, z_new and the objective [B]
+struct BoneScratch {
+  float4* coef;
+  float *z, *z_new, *obj;
+};
+size_t bone_scratch_bytes(const mtb_handle* h, int B) {
+  return align_up((size_t)B * h->bone_len.size() * 16, 256) + 3 * align_up((size_t)B * 4, 256);
+}
+BoneScratch bone_scratch(const mtb_handle* h, int B, void* base) {
+  char* p = (char*)base;
+  BoneScratch s;
+  s.coef = (float4*)p; p += align_up((size_t)B * h->bone_len.size() * 16, 256);
+  s.z = (float*)p;     p += align_up((size_t)B * 4, 256);
+  s.z_new = (float*)p; p += align_up((size_t)B * 4, 256);
+  s.obj = (float*)p;
+  return s;
+}
 
 Workspace layout(const mtb_handle* h, int B, void* base) {
   Workspace w;
@@ -923,7 +953,7 @@ Workspace layout(const mtb_handle* h, int B, void* base) {
   const size_t P = (size_t)h->feat_side * h->feat_side;
   w.off_features = o; o += align_up(P * h->feat_c * B * es, 1024);
   const size_t J = (size_t)head_points(h);
-  const int N = (int)((J * (1 + h->cfg.depth) + 3) / 4 * 4);
+  const int N = (head_channels(h) + 3) / 4 * 4;
   w.off_logits = o; o += align_up(std::max<size_t>(P, 4) * N * B * 4, 1024);  // also the fused head's state scratch
   w.off_c2d = o; o += align_up((size_t)B * J * 2 * 4, 1024);
   w.off_c3d = o; o += align_up((size_t)B * J * 3 * 4, 1024);
@@ -931,6 +961,8 @@ Workspace layout(const mtb_handle* h, int B, void* base) {
   w.off_partial = o; o += align_up((size_t)B * 2 * 8, 1024);
   w.off_latents = o;  // latent-point model: absolute latents [B,L,3] between the reconstruction and the recombination
   if (h->n_latents > 0) o += align_up((size_t)B * J * 3 * 4, 1024);
+  w.off_bones = o;  // Model25D: the bone-length solve's scratch
+  if (h->model_class == MTB_MODEL_25D) o += align_up(bone_scratch_bytes(h, B), 1024);
   w.total = o;
   return w;
 }
@@ -1349,11 +1381,23 @@ DecodeScale make_scale(const mtb_config& c) {
   return s;
 }
 
-template <typename T>
+template <typename T, bool HEAD3D = false>
 const char* launch_softargmax_bhwn(const void* logits, float* out2d, float* out3d, int B, int J, int D, int H, int W,
                                    int ld, DecodeScale sc, cudaStream_t st) {
-  const int smem = (J * (1 + D) + 4 * 128) * (int)sizeof(float4);
-  return launch_smem(softargmax_bhwn_kernel<T>, dim3(B), dim3(512), smem, st, (const T*)logits, out2d, out3d, J, D, H, W, ld, sc);
+  const int smem = (J * (HEAD3D ? D : 1 + D) + 4 * 128) * (int)sizeof(float4);
+  return launch_smem(softargmax_bhwn_kernel<T, HEAD3D>, dim3(B), dim3(512), smem, st, (const T*)logits, out2d, out3d, J, D, H, W,
+                     ld, sc);
+}
+
+// the decode scale of the handle's head: heatmap_to_image / heatmap_to_metric for MeTRAbs and Metro, heatmap_to_25d
+// (metrabs_tf/models/util.py:21-23: image pixels for x and y, mm for z) for Model25D
+DecodeScale head_scale(const mtb_handle* h) {
+  DecodeScale s = make_scale(h->cfg);
+  if (h->model_class == MTB_MODEL_25D) {
+    s.met_mul = s.img_mul;
+    s.met_add = s.img_add;
+  }
+  return s;
 }
 
 int head_decode_impl(mtb_handle* h, const void* features, int B, float* c2d, float* c3d, const Workspace& ws,
@@ -1369,7 +1413,7 @@ int head_decode_impl(mtb_handle* h, const void* features, int B, float* c2d, flo
     ProfScope prof(h, KC_HEAD_FUSED, op.flops * B, feat_bytes + (double)op.Cin * op.Cout * 2 + out_bytes, st);
     const char* e = with_storage16(h, [&](auto* tag) {
       return tc_head_launch<std::remove_pointer_t<decltype(tag)>>(op.tc, features, B, h->feat_side, h->feat_side, J, c.depth,
-                                                                  make_scale(c), c2d, c3d, ws.base + ws.off_logits, st);
+                                                                  head3d(h), head_scale(h), c2d, c3d, ws.base + ws.off_logits, st);
     });
     if (e) return fail(h, MTB_ERR_CUDA, "fused head: %s", e);
     h->launches += 2;
@@ -1390,7 +1434,8 @@ int head_decode_impl(mtb_handle* h, const void* features, int B, float* c2d, flo
     if (e) return fail(h, MTB_ERR_CUDA, "head conv: %s", e);
   }
   ProfScope prof(h, KC_SOFTARGMAX, 0.0, logit_bytes + out_bytes, st);
-  const char* se = launch_softargmax_bhwn<float>(p.out, c2d, c3d, B, J, c.depth, op.Hin, op.Win, op.Cout, make_scale(c), st);
+  const char* se = head3d(h) ? launch_softargmax_bhwn<float, true>(p.out, c2d, c3d, B, J, c.depth, op.Hin, op.Win, op.Cout, head_scale(h), st)
+                             : launch_softargmax_bhwn<float>(p.out, c2d, c3d, B, J, c.depth, op.Hin, op.Win, op.Cout, make_scale(c), st);
   if (se) return fail(h, MTB_ERR_CUDA, "softargmax: %s", se);
   h->launches += 2;
   return MTB_OK;
@@ -1413,6 +1458,28 @@ int recon_impl(mtb_handle* h, const float* c2d, const float* c3d, const float* K
   h->launches += 2;
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(h, MTB_ERR_CUDA, "reconstruct: %s", cudaGetErrorString(e));
+  return MTB_OK;
+}
+
+// Model25D: coords25d [B,J,3] -> absolute joints [B,J,3] (bone_solve_kernel, one CTA over the whole batch)
+int bone_solve_impl(mtb_handle* h, const float* c25, const float* K, int B, float* out, void* scratch, cudaStream_t st) {
+  const mtb_config& c = h->cfg;
+  const BoneScratch sc = bone_scratch(h, B, scratch);
+  BoneSolveParams p;
+  p.c25 = c25; p.K = K; p.edges = h->d_edges; p.len = h->d_len; p.out = out;
+  p.coef = sc.coef; p.z = sc.z; p.z_new = sc.z_new; p.obj = sc.obj;
+  p.B = B; p.J = c.n_joints; p.E = (int)h->bone_len.size();
+  const float offset = c.centered_stride ? 0.f : -(float)c.stride_train / 2.f;  // is_within_fov (tfu3d.py:210-216)
+  p.fov_lower = (float)c.stride_train * 0.75f + offset;
+  p.fov_upper = (float)c.proc_side - (float)c.stride_train * 0.75f + offset;
+  p.mean_relative = h->mean_relative;
+  // per iteration: 2 residual passes + the Jacobian over every bone (about 30 flops per bone)
+  ProfScope prof(h, KC_BONE_SOLVE, (double)B * p.E * 30.0 * (BONE_ITERS + 1),
+                 (double)B * p.J * 6 * 4 + (double)B * 36 + (double)B * p.E * 16 * (2 * BONE_ITERS + 1), st);
+  launch_k(bone_solve_kernel, dim3(1), dim3(BONE_THREADS), 0, st, p);
+  h->launches += 1;
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(h, MTB_ERR_CUDA, "bone-length solve: %s", cudaGetErrorString(e));
   return MTB_OK;
 }
 
@@ -1682,10 +1749,11 @@ int mtb_finalize_weights(mtb_handle* h) {
     const HostTensor* w = find(h, hd.wkey);
     if (!w) return fail(h, MTB_ERR_MISSING_WEIGHT, "missing weight '%s'", hd.wkey.c_str());
     const int n_raw = h->cfg.n_joints, D = h->cfg.depth;
-    if (w->shape.size() != 4 || w->shape[0] != n_raw * (1 + D) || w->shape[1] != hd.Cin)
-      return fail(h, MTB_ERR_INVALID_ARG, "'%s' must be [%d,%d,1,1]", hd.wkey.c_str(), n_raw * (1 + D), hd.Cin);
+    const int n_ch = n_raw * (head3d(h) ? D : 1 + D);  // the checkpoint's channels (all raw points)
+    if (w->shape.size() != 4 || w->shape[0] != n_ch || w->shape[1] != hd.Cin)
+      return fail(h, MTB_ERR_INVALID_ARG, "'%s' must be [%d,%d,1,1]", hd.wkey.c_str(), n_ch, hd.Cin);
     const HostTensor* hb = find(h, hd.biaskey);
-    if (!hb || (int)hb->data.size() != n_raw * (1 + D))
+    if (!hb || (int)hb->data.size() != n_ch)
       return fail(h, MTB_ERR_MISSING_WEIGHT, "missing weight '%s'", hd.biaskey.c_str());
     const int P = head_points(h);
     if (P < n_raw) {
@@ -1709,7 +1777,7 @@ int mtb_finalize_weights(mtb_handle* h) {
       w = find(h, hd.wkey);
       hb = find(h, hd.biaskey);
     }
-    const int n_real = P * (1 + D);
+    const int n_real = head_channels(h);
     if (n_real != hd.Cout) {  // zero-pad the output channels
       HostTensor wp = *w, bp = *hb;
       wp.data.resize((size_t)hd.Cout * hd.Cin, 0.f);
@@ -1740,6 +1808,13 @@ int mtb_finalize_weights(mtb_handle* h) {
     int rc = upload(h, h->recomb.data(), h->recomb.size() * sizeof(float), (void**)&h->d_recomb);
     if (rc) return rc;
   }
+  h->d_edges = nullptr;
+  h->d_len = nullptr;
+  if (h->model_class == MTB_MODEL_25D) {
+    int rc = upload(h, h->bone_edges.data(), h->bone_edges.size() * sizeof(int32_t), (void**)&h->d_edges);
+    if (!rc) rc = upload(h, h->bone_len.data(), h->bone_len.size() * sizeof(float), (void**)&h->d_len);
+    if (rc) return rc;
+  }
   h->raw.clear();
   h->finalized = true;
   return MTB_OK;
@@ -1751,6 +1826,8 @@ int mtb_set_latent_recombination(mtb_handle* h, const float* weights, int n_late
   if (h->finalized)
     return fail(h, MTB_ERR_INVALID_ARG, "the latent recombination must be set before mtb_finalize_weights (load the weights again first)");
   if (h->cfg.arch == MTB_ARCH_HEAD_ONLY) return fail(h, MTB_ERR_INVALID_ARG, "a head-only handle has no forward to recombine");
+  if (h->model_class != MTB_MODEL_METRABS)
+    return fail(h, MTB_ERR_INVALID_ARG, "latent points are a MeTRAbs feature: this handle is a Metro or Model25D model");
   if (n_latents < 1 || n_latents > h->cfg.n_joints)
     return fail(h, MTB_ERR_INVALID_ARG, "n_latents must be in [1, %d] (the head's points), got %d", h->cfg.n_joints, n_latents);
   if (n_out < 1 || n_out > kMaxCombinePoints)
@@ -1761,6 +1838,48 @@ int mtb_set_latent_recombination(mtb_handle* h, const float* weights, int n_late
   h->recomb.assign(weights, weights + n);
   h->n_latents = n_latents;
   h->n_out = n_out;
+  size_head(h);
+  return MTB_OK;
+}
+
+int mtb_set_model_class(mtb_handle* h, int model_class, const int32_t* edges, const float* bone_lengths, int n_bones,
+                        int mean_relative) {
+  if (!h) return fail(nullptr, MTB_ERR_INVALID_ARG, "null handle");
+  if (h->finalized)
+    return fail(h, MTB_ERR_INVALID_ARG, "the model class must be set before mtb_finalize_weights (load the weights again first)");
+  if (h->cfg.arch == MTB_ARCH_HEAD_ONLY) return fail(h, MTB_ERR_INVALID_ARG, "a head-only handle has no model class");
+  if (model_class != MTB_MODEL_METRABS && model_class != MTB_MODEL_METRO && model_class != MTB_MODEL_25D)
+    return fail(h, MTB_ERR_INVALID_ARG, "unknown model class %d", model_class);
+  if (h->n_latents > 0)
+    return fail(h, MTB_ERR_INVALID_ARG, "this handle has a latent recombination, which only MeTRAbs models have");
+  if (model_class != MTB_MODEL_METRABS && h->cfg.legacy_centered_stride_bug)
+    return fail(h, MTB_ERR_INVALID_ARG, "legacy_centered_stride_bug does not exist in the TF heatmap_to_image that Metro and "
+                "Model25D decode with (metrabs_tf/models/util.py:8-18)");
+  std::vector<int32_t> e;
+  std::vector<float> len;
+  if (model_class == MTB_MODEL_25D) {
+    if (!edges || !bone_lengths) return fail(h, MTB_ERR_INVALID_ARG, "a Model25D needs its bone edges and lengths");
+    if (n_bones < 1 || n_bones > kMaxCombinePoints)
+      return fail(h, MTB_ERR_INVALID_ARG, "n_bones must be in [1, %d], got %d", kMaxCombinePoints, n_bones);
+    for (int i = 0; i < n_bones; ++i) {
+      for (int k = 0; k < 2; ++k)
+        if (edges[2 * i + k] < 0 || edges[2 * i + k] >= h->cfg.n_joints)
+          return fail(h, MTB_ERR_INVALID_ARG, "bone %d: joint index %d outside [0, %d)", i, edges[2 * i + k], h->cfg.n_joints);
+      if (!std::isfinite(bone_lengths[i]) || !(bone_lengths[i] > 0.f))
+        return fail(h, MTB_ERR_INVALID_ARG, "bone %d: length %g is not finite and positive", i, (double)bone_lengths[i]);
+    }
+    e.assign(edges, edges + 2 * (size_t)n_bones);
+    len.assign(bone_lengths, bone_lengths + n_bones);
+  }
+  h->model_class = model_class;
+  h->bone_edges = std::move(e);
+  h->bone_len = std::move(len);
+  h->mean_relative = mean_relative ? 1 : 0;
+  // the TF heads' key schema: metrabs_tf/models/{metro,twofive}.py name the head `heatmap_head`
+  Op& hd = h->head;
+  hd.name = head3d(h) ? "heatmap_head.conv_final" : "heatmap_heads.conv_final";
+  hd.wkey = hd.name + ".weight";
+  hd.biaskey = hd.name + ".bias";
   size_head(h);
   return MTB_OK;
 }
@@ -1805,7 +1924,7 @@ int mtb_head_decode(mtb_handle* h, const void* features, int batch, float* coord
                     void* workspace, size_t workspace_bytes, void* stream) {
   int rc = check_common(h, batch, workspace_bytes, workspace);
   if (rc) return rc;
-  if (!features || !coords2d || !coords3d_rel) return fail(h, MTB_ERR_INVALID_ARG, "null argument");
+  if (!features || !coords3d_rel || (!coords2d && !head3d(h))) return fail(h, MTB_ERR_INVALID_ARG, "null argument");
   DeviceGuard g(h->cfg.device);
   h->launches = 0;
   Workspace ws = layout(h, batch, workspace);
@@ -1872,11 +1991,31 @@ int mtb_reconstruct_absolute(mtb_handle* h, const float* coords2d, const float* 
   if (!coords2d || !coords3d_rel || !intrinsics || !coords3d_abs || !scratch || batch <= 0)
     return fail(h, MTB_ERR_INVALID_ARG, "null/invalid argument");
   if (head_points(h) > 4096) return fail(h, MTB_ERR_UNSUPPORTED, "more than 4096 joints");
+  if (head3d(h))
+    return fail(h, MTB_ERR_UNSUPPORTED, "a Metro or Model25D handle has no MeTRAbs reconstruction (Model25D: "
+                "mtb_reconstruct_by_bone_lengths)");
   DeviceGuard g(h->cfg.device);
   h->launches = 0;
   double* partial = (double*)scratch;
   float* n2d = (float*)((char*)scratch + align_up((size_t)batch * 2 * 8, 256));
   return recon_impl(h, coords2d, coords3d_rel, intrinsics, batch, coords3d_abs, n2d, partial, (cudaStream_t)stream);
+}
+
+size_t mtb_bone_lengths_scratch_bytes(const mtb_handle* h, int batch) {
+  if (!h || batch <= 0 || h->model_class != MTB_MODEL_25D) return 0;
+  return bone_scratch_bytes(h, batch);
+}
+
+int mtb_reconstruct_by_bone_lengths(mtb_handle* h, const float* coords25d, const float* intrinsics, int batch, float* coords3d_abs,
+                                    void* scratch, void* stream) {
+  if (!h) return fail(nullptr, MTB_ERR_INVALID_ARG, "null handle");
+  if (h->model_class != MTB_MODEL_25D) return fail(h, MTB_ERR_INVALID_ARG, "not a Model25D handle (mtb_set_model_class)");
+  if (!h->finalized) return fail(h, MTB_ERR_NOT_FINALIZED, "mtb_finalize_weights has not been called");
+  if (!coords25d || !intrinsics || !coords3d_abs || !scratch || batch <= 0)
+    return fail(h, MTB_ERR_INVALID_ARG, "null/invalid argument");
+  DeviceGuard g(h->cfg.device);
+  h->launches = 0;
+  return bone_solve_impl(h, coords25d, intrinsics, batch, coords3d_abs, scratch, (cudaStream_t)stream);
 }
 
 // the forward proper: every launch of one step on `st` (no allocation, no synchronisation: capturable)
@@ -1889,8 +2028,10 @@ static int forward_body(mtb_handle* h, const float* crops, const float* intrinsi
   if (rc) return rc;
   float* c2d = (float*)(ws.base + ws.off_c2d);
   float* c3d = (float*)(ws.base + ws.off_c3d);
-  rc = head_decode_impl(h, features, batch, c2d, c3d, ws, st);
+  if (h->model_class == MTB_MODEL_METRO) return head_decode_impl(h, features, batch, nullptr, coords3d_abs, ws, st);
+  rc = head_decode_impl(h, features, batch, head3d(h) ? nullptr : c2d, c3d, ws, st);
   if (rc) return rc;
+  if (h->model_class == MTB_MODEL_25D) return bone_solve_impl(h, c3d, intrinsics, batch, coords3d_abs, ws.base + ws.off_bones, st);
   return recon_and_combine(h, c2d, c3d, intrinsics, batch, coords3d_abs, (float*)(ws.base + ws.off_n2d),
                            (double*)(ws.base + ws.off_partial), (float*)(ws.base + ws.off_latents), st);
 }
@@ -1915,7 +2056,8 @@ int mtb_forward(mtb_handle* h, const float* crops, const float* intrinsics, int 
                 void* workspace, size_t workspace_bytes, void* stream) {
   int rc = check_common(h, batch, workspace_bytes, workspace);
   if (rc) return rc;
-  if (!crops || !intrinsics || !coords3d_abs) return fail(h, MTB_ERR_INVALID_ARG, "null argument");
+  if (!crops || (!intrinsics && h->model_class != MTB_MODEL_METRO) || !coords3d_abs)
+    return fail(h, MTB_ERR_INVALID_ARG, "null argument");
   if (h->ops.empty()) return fail(h, MTB_ERR_UNSUPPORTED, "this handle has no backbone (head-only)");
   DeviceGuard g(h->cfg.device);
   cudaStream_t st = (cudaStream_t)stream;
@@ -1988,7 +2130,8 @@ int mtb_forward_host(mtb_handle* h, const float* host_crops, const float* host_i
                      float* host_coords3d_abs, void* stream) {
   if (!h) return fail(nullptr, MTB_ERR_INVALID_ARG, "null handle");
   if (!h->finalized) return fail(h, MTB_ERR_NOT_FINALIZED, "mtb_finalize_weights has not been called");
-  if (!host_crops || !host_intrinsics || !host_coords3d_abs || batch <= 0) return fail(h, MTB_ERR_INVALID_ARG, "null/invalid argument");
+  if (!host_crops || (!host_intrinsics && h->model_class != MTB_MODEL_METRO) || !host_coords3d_abs || batch <= 0)
+    return fail(h, MTB_ERR_INVALID_ARG, "null/invalid argument");
   DeviceGuard g(h->cfg.device);
   cudaStream_t st = (cudaStream_t)stream;
   const size_t S = h->cfg.proc_side;
@@ -2012,7 +2155,7 @@ int mtb_forward_host(mtb_handle* h, const float* host_crops, const float* host_i
   float* d_out = (float*)(base + crops_b + k_b);
   void* d_ws = base + crops_b + k_b + out_b;
   CUDA_TRY(h, cudaMemcpyAsync(d_crops, host_crops, (size_t)batch * 3 * S * S * 4, cudaMemcpyHostToDevice, st));
-  CUDA_TRY(h, cudaMemcpyAsync(d_k, host_intrinsics, (size_t)batch * 9 * 4, cudaMemcpyHostToDevice, st));
+  if (host_intrinsics) CUDA_TRY(h, cudaMemcpyAsync(d_k, host_intrinsics, (size_t)batch * 9 * 4, cudaMemcpyHostToDevice, st));
   int rc = mtb_forward(h, d_crops, d_k, batch, d_out, d_ws, ws_b, stream);
   if (rc) return rc;
   CUDA_TRY(h, cudaMemcpyAsync(host_coords3d_abs, d_out, (size_t)batch * output_joints(h) * 3 * 4, cudaMemcpyDeviceToHost, st));
@@ -2024,7 +2167,8 @@ int mtb_forward_host_submit(mtb_handle* h, const float* host_crops, const float*
                             float* host_coords3d_abs, int slot, void* stream) {
   if (!h) return fail(nullptr, MTB_ERR_INVALID_ARG, "null handle");
   if (!h->finalized) return fail(h, MTB_ERR_NOT_FINALIZED, "mtb_finalize_weights has not been called");
-  if (!host_crops || !host_intrinsics || !host_coords3d_abs || batch <= 0 || slot < 0 || slot > 1)
+  if (!host_crops || (!host_intrinsics && h->model_class != MTB_MODEL_METRO) || !host_coords3d_abs || batch <= 0 || slot < 0 ||
+      slot > 1)
     return fail(h, MTB_ERR_INVALID_ARG, "null/invalid argument");
   DeviceGuard g(h->cfg.device);
   cudaStream_t st = (cudaStream_t)stream;
@@ -2061,7 +2205,8 @@ int mtb_forward_host_submit(mtb_handle* h, const float* host_crops, const float*
   // copy stream: this slot's staging is free once its previous forward + read-back have completed
   if (sl.used) CUDA_TRY(h, cudaStreamWaitEvent(h->copy_stream, sl.done, 0));
   CUDA_TRY(h, cudaMemcpyAsync(d_crops, host_crops, (size_t)batch * 3 * S * S * 4, cudaMemcpyHostToDevice, h->copy_stream));
-  CUDA_TRY(h, cudaMemcpyAsync(d_k, host_intrinsics, (size_t)batch * 9 * 4, cudaMemcpyHostToDevice, h->copy_stream));
+  if (host_intrinsics)
+    CUDA_TRY(h, cudaMemcpyAsync(d_k, host_intrinsics, (size_t)batch * 9 * 4, cudaMemcpyHostToDevice, h->copy_stream));
   CUDA_TRY(h, cudaEventRecord(sl.h2d_done, h->copy_stream));
   // compute stream: forward of this step behind its own copy (and behind the previous step's forward: one workspace)
   CUDA_TRY(h, cudaStreamWaitEvent(st, sl.h2d_done, 0));
@@ -2244,6 +2389,8 @@ int mtb_filter_poses(const mtb_filter_args* a, void* stream) {
 size_t mtb_sharded_scratch_bytes(const mtb_handle* h, int batch_local) {
   if (!h || batch_local <= 0 || h->nccl_world <= 0) return 0;
   const size_t J = (size_t)head_points(h), bl = (size_t)batch_local, bt = bl * (size_t)h->nccl_world;
+  if (head3d(h))  // the gathered coords25d [bt,J,3] and the solve's scratch (a Metro handle gathers into the output)
+    return align_up(bt * J * 3 * 4, 256) + (h->model_class == MTB_MODEL_25D ? bone_scratch_bytes(h, (int)bt) : 0);
   return align_up(bl * J * 5 * 4, 256) + align_up(bt * J * 5 * 4, 256) + align_up(bt * J * 2 * 4, 256) + align_up(bt * J * 3 * 4, 256) +
          align_up(bt * J * 2 * 4, 256) + align_up(bt * 2 * 8, 256) + (h->n_latents > 0 ? align_up(bt * J * 3 * 4, 256) : 0);
 }
@@ -2252,7 +2399,9 @@ int mtb_forward_sharded(mtb_handle* h, const float* crops_local, int batch_local
                         void* scratch, void* workspace, size_t workspace_bytes, void* stream) {
   int rc = check_common(h, batch_local, workspace_bytes, workspace);
   if (rc) return rc;
-  if (!crops_local || !intrinsics_all || !coords3d_abs_all || !scratch) return fail(h, MTB_ERR_INVALID_ARG, "null argument");
+  if (!crops_local || (!intrinsics_all && h->model_class != MTB_MODEL_METRO) || !coords3d_abs_all ||
+      (!scratch && h->model_class != MTB_MODEL_METRO))
+    return fail(h, MTB_ERR_INVALID_ARG, "null argument");
   if (!h->nccl_comm) return fail(h, MTB_ERR_NCCL, "mtb_comm_init has not been called");
   if (h->ops.empty()) return fail(h, MTB_ERR_UNSUPPORTED, "this handle has no backbone (head-only)");
   DeviceGuard g(h->cfg.device);
@@ -2273,6 +2422,18 @@ int mtb_forward_sharded(mtb_handle* h, const float* crops_local, int batch_local
   if (rc) return rc;
   float* c2d = (float*)(ws.base + ws.off_c2d);
   float* c3d = (float*)(ws.base + ws.off_c3d);
+  if (head3d(h)) {
+    // Metro: the decoded joints are the output, gathered in rank order.  Model25D: ONE all-gather of coords25d (3 floats per
+    // joint), then the batch-coupled bone-length solve on the full batch on every rank, as the unsharded forward runs it.
+    float* all = h->model_class == MTB_MODEL_METRO ? coords3d_abs_all : (float*)scratch;
+    rc = head_decode_impl(h, features, batch_local, nullptr, c3d, ws, st);
+    if (rc) return rc;
+    rc = mtb_allgather_joints(h, c3d, (int)(bl * J * 3), all, stream);
+    if (rc) return rc;
+    h->launches += 1;
+    if (h->model_class == MTB_MODEL_METRO) return MTB_OK;
+    return bone_solve_impl(h, all, intrinsics_all, (int)bt, coords3d_abs_all, (char*)scratch + align_up(bt * J * 3 * 4, 256), st);
+  }
   rc = head_decode_impl(h, features, batch_local, c2d, c3d, ws, st);
   if (rc) return rc;
   const int64_t before = h->launches;

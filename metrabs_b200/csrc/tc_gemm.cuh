@@ -1204,14 +1204,38 @@ tc_head_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
   }
 }
 
-// merges the per-channel states of one crop into coords2d [J,2] (px) and coords3d_rel [J,3] (mm)
+// merges the per-channel states of one crop into coords2d [J,2] (px) and coords3d_rel [J,3] (mm).  HEAD3D: the Metro /
+// Model25D head (channel d*J + j, no 2D block): merges the D slices as softargmax_bhwn_kernel<T, true> does and writes its
+// x and y to out2d too when out2d is non-null.
+template <bool HEAD3D = false>
 __global__ void __launch_bounds__(128) head_finalize_kernel(const float4* __restrict__ states, float* __restrict__ out2d,
                                                             float* __restrict__ out3d, int J, int D, int H, int W,
                                                             DecodeScale sc) {
   const int b = blockIdx.x;
-  const int n_out = J * (1 + D);
+  const int n_out = HEAD3D ? J * D : J * (1 + D);
   for (int j = threadIdx.x; j < J; j += blockDim.x) {
     const float4* st = states + (size_t)b * n_out;
+    if constexpr (HEAD3D) {
+      SoftState a;
+      soft_init(a);
+      for (int d = 0; d < D; ++d) {
+        float4 c = st[d * J + j];
+        SoftState bb;
+        bb.m = c.x; bb.s = c.y; bb.sx = c.z; bb.sy = c.w; bb.sz = c.y * (float)d;
+        soft_merge(a, bb);
+      }
+      const float x = fmaf(soft_coord_tf(a.sx, a.s, W), sc.met_mul, sc.met_add);
+      const float y = fmaf(soft_coord_tf(a.sy, a.s, H), sc.met_mul, sc.met_add);
+      const float z = soft_coord_tf(a.sz, a.s, D) * sc.z_mul;
+      out3d[((size_t)b * J + j) * 3 + 0] = x;
+      out3d[((size_t)b * J + j) * 3 + 1] = y;
+      out3d[((size_t)b * J + j) * 3 + 2] = z;
+      if (out2d) {
+        out2d[((size_t)b * J + j) * 2 + 0] = x;
+        out2d[((size_t)b * J + j) * 2 + 1] = y;
+      }
+      continue;
+    }
     {
       float4 c = st[j];
       float x = soft_coord(c.z, c.y, W), y = soft_coord(c.w, c.y, H);
@@ -1272,8 +1296,8 @@ inline bool tc_head_plan(int P, int* bnp, int* cpt, int* npt) {
 }
 
 template <typename T>
-inline const char* tc_head_launch(const TcWeights& w, const void* features, int B, int H, int W, int J, int D, DecodeScale sc,
-                                  float* c2d, float* c3d, void* scratch, cudaStream_t st) {
+inline const char* tc_head_launch(const TcWeights& w, const void* features, int B, int H, int W, int J, int D, bool head3d,
+                                  DecodeScale sc, float* c2d, float* c3d, void* scratch, cudaStream_t st) {
   TcHeadParams q;
   q.states = (float4*)scratch;
   q.bias = w.d_bias;
@@ -1289,7 +1313,8 @@ inline const char* tc_head_launch(const TcWeights& w, const void* features, int 
   }, w.d_w, features, B, H, W, q.C, q.n_out);
   if (!e) e = launch_smem(tc_head_kernel<T>, dim3(n_groups * q.m_tiles), dim3(TC_THREADS), TCH_SMEM_BYTES, st, m[0], m[1], q);
   if (e) return e;
-  launch_k(head_finalize_kernel, dim3(B), dim3(128), 0, st, q.states, c2d, c3d, J, D, H, W, sc);
+  if (head3d) launch_k(head_finalize_kernel<true>, dim3(B), dim3(128), 0, st, q.states, c2d, c3d, J, D, H, W, sc);
+  else launch_k(head_finalize_kernel<false>, dim3(B), dim3(128), 0, st, q.states, c2d, c3d, J, D, H, W, sc);
   const cudaError_t ce = cudaGetLastError();
   return ce == cudaSuccess ? nullptr : cudaGetErrorString(ce);
 }

@@ -72,6 +72,9 @@ class Engine:
         self.feature_side, self.feature_channels = hw.value, ch.value
         self.n_joints, self.depth = mtb_config.n_joints, mtb_config.depth
         self._recombination = None  # (host fp32 [L, n_out] weights, device copy) of a latent-point model
+        self.model_class = _lib.MODEL_METRABS
+        self._bones = None  # (host int32 [E, 2] edges, host fp32 [E] lengths, mean_relative) of a Model25D
+        self._bone_scratch = None
         self.feature_dtype = {_lib.PRECISION_FP32: torch.float32, _lib.PRECISION_TF32X3: torch.float32,
                               _lib.PRECISION_BF16_TC: torch.bfloat16, _lib.PRECISION_BF16_SIMT: torch.bfloat16,
                               _lib.PRECISION_F16_TC: torch.float16, _lib.PRECISION_F16_SIMT: torch.float16}[mtb_config.precision]
@@ -98,6 +101,20 @@ class Engine:
         if w.ndim != 2:
             raise ValueError(f'recombination weights must be [n_latents, n_out], got shape {tuple(w.shape)}')
         self._recombination = (w, w.to(self.device))
+
+    def set_model_class(self, model_class, edges=None, bone_lengths=None, mean_relative=True):
+        """Makes this a Metro (_lib.MODEL_METRO) or Model25D (_lib.MODEL_25D) handle: a D*J-channel head without the 2D block
+        and, for Model25D, the bone-length depth solve over ``edges`` [E, 2] with ``bone_lengths`` [E] mm.  Takes effect at
+        the next load_state_dict (mtb_set_model_class precedes every mtb_finalize_weights)."""
+        if model_class == _lib.MODEL_25D:
+            e = torch.as_tensor(np.asarray(edges), dtype=torch.int32).reshape(-1, 2).contiguous()
+            bl = torch.as_tensor(np.asarray(bone_lengths), dtype=torch.float32).reshape(-1).contiguous()
+            if e.shape[0] != bl.shape[0]:
+                raise ValueError(f'{e.shape[0]} bone edges but {bl.shape[0]} bone lengths')
+            self._bones = (e, bl, bool(mean_relative))
+        else:
+            self._bones = None
+        self.model_class = model_class
 
     @property
     def n_points(self):
@@ -128,6 +145,11 @@ class Engine:
         if self._recombination is not None:
             w = self._recombination[0]
             check(lib().mtb_set_latent_recombination(self._h, C.c_void_p(w.data_ptr()), w.shape[0], w.shape[1]), self._h)
+        if self.model_class != _lib.MODEL_METRABS:
+            e, bl, mean_rel = self._bones if self._bones is not None else (None, None, True)
+            check(lib().mtb_set_model_class(self._h, self.model_class, C.c_void_p(e.data_ptr()) if e is not None else None,
+                                            C.c_void_p(bl.data_ptr()) if bl is not None else None,
+                                            0 if bl is None else bl.shape[0], int(mean_rel)), self._h)
         check(lib().mtb_finalize_weights(self._h), self._h)
 
     # ---- buffers --------------------------------------------------------------------------------------
@@ -182,15 +204,35 @@ class Engine:
                                              self._scratch.data_ptr(), _stream_ptr(self.device)), self._h)
         return out
 
+    def reconstruct_by_bone_lengths(self, coords25d, intrinsics):
+        """Model25D's absolute step (mtb_reconstruct_by_bone_lengths): coords25d [B,J,3] (x px, y px, z mm) + intrinsics
+        [B,3,3] -> camera-space joints [B,J,3].  The solve is coupled across the batch, as in the reference."""
+        b = coords25d.shape[0]
+        c = self._check_in(coords25d, (b, self.n_points, 3))
+        k = self._check_in(intrinsics, (b, 3, 3))
+        out = torch.empty(b, self.n_points, 3, dtype=torch.float32, device=self.device)
+        need = lib().mtb_bone_lengths_scratch_bytes(self._h, b)
+        if self._bone_scratch is None or self._bone_scratch.numel() < need:
+            self._bone_scratch = torch.empty(max(need, 1), dtype=torch.uint8, device=self.device)
+        check(lib().mtb_reconstruct_by_bone_lengths(self._h, c.data_ptr(), k.data_ptr(), b, out.data_ptr(),
+                                                    self._bone_scratch.data_ptr(), _stream_ptr(self.device)), self._h)
+        return out
+
+    def _intrinsics_in(self, intrinsics, b):
+        """Device intrinsics [b,3,3], or None for a Metro handle, whose forward takes none."""
+        if intrinsics is None and self.model_class == _lib.MODEL_METRO:
+            return None
+        return self._check_in(intrinsics, (b, 3, 3))
+
     def forward(self, crops, intrinsics, out=None):
         b, s = crops.shape[0], self.cfg.proc_side
         crops = self._check_in(crops, (b, 3, s, s))
-        k = self._check_in(intrinsics, (b, 3, 3))
+        k = self._intrinsics_in(intrinsics, b)
         if out is None:
             out = torch.empty(b, self.n_out, 3, dtype=torch.float32, device=self.device)
         ws = self.workspace(b)
-        check(lib().mtb_forward(self._h, crops.data_ptr(), k.data_ptr(), b, out.data_ptr(), ws.data_ptr(), ws.numel(),
-                                _stream_ptr(self.device)), self._h)
+        check(lib().mtb_forward(self._h, crops.data_ptr(), k.data_ptr() if k is not None else None, b, out.data_ptr(),
+                                ws.data_ptr(), ws.numel(), _stream_ptr(self.device)), self._h)
         return out
 
     def capture_forward(self, crops, intrinsics, out):
@@ -200,7 +242,7 @@ class Engine:
         Run at least one plain ``forward`` on the same buffers first (tensor maps, kernel attributes, workspace)."""
         b, s = crops.shape[0], self.cfg.proc_side
         crops = self._check_in(crops, (b, 3, s, s))
-        k = self._check_in(intrinsics, (b, 3, 3))
+        k = self._intrinsics_in(intrinsics, b)
         ws = self.workspace(b)
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
@@ -213,13 +255,15 @@ class Engine:
     def forward_host(self, crops_host, intrinsics_host, out_host=None):
         """End-to-end call on HOST tensors (pinned for full-speed copies): H2D + forward + D2H + stream sync."""
         b = crops_host.shape[0]
-        if crops_host.is_cuda or intrinsics_host.is_cuda:
+        if crops_host.is_cuda or (intrinsics_host is not None and intrinsics_host.is_cuda):
             raise ValueError('forward_host takes host tensors')
         crops_host = crops_host.contiguous().float()
-        intrinsics_host = intrinsics_host.contiguous().float()
+        if intrinsics_host is not None:
+            intrinsics_host = intrinsics_host.contiguous().float()
         if out_host is None:
             out_host = torch.empty(b, self.n_out, 3, dtype=torch.float32).pin_memory()
-        check(lib().mtb_forward_host(self._h, crops_host.data_ptr(), intrinsics_host.data_ptr(), b,
+        check(lib().mtb_forward_host(self._h, crops_host.data_ptr(),
+                                     intrinsics_host.data_ptr() if intrinsics_host is not None else None, b,
                                      out_host.data_ptr(), _stream_ptr(self.device)), self._h)
         return out_host
 
@@ -254,14 +298,14 @@ class Engine:
         Buffers (scratch, workspace, and `out` when given) are reused across calls."""
         b, s = crops_local.shape[0], self.cfg.proc_side
         crops_local = self._check_in(crops_local, (b, 3, s, s))
-        k = self._check_in(intrinsics_all, (self.world_size * b, 3, 3))
+        k = self._intrinsics_in(intrinsics_all, self.world_size * b)
         if out is None:
             out = torch.empty(self.world_size * b, self.n_out, 3, dtype=torch.float32, device=self.device)
         need = lib().mtb_sharded_scratch_bytes(self._h, b)
         if getattr(self, '_sh_scratch', None) is None or self._sh_scratch.numel() < need:
             self._sh_scratch = torch.empty(need, dtype=torch.uint8, device=self.device)
         ws = self.workspace(b)
-        check(lib().mtb_forward_sharded(self._h, crops_local.data_ptr(), b, k.data_ptr(), out.data_ptr(),
+        check(lib().mtb_forward_sharded(self._h, crops_local.data_ptr(), b, k.data_ptr() if k is not None else None, out.data_ptr(),
                                         self._sh_scratch.data_ptr(), ws.data_ptr(), ws.numel(), _stream_ptr(self.device)), self._h)
         return out
 

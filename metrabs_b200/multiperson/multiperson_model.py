@@ -77,6 +77,9 @@ class Pose3dEstimator(torch.nn.Module):
     def __init__(self, crop_model, skeleton_infos, joint_transform_matrix, detector=None, joint_info=None,
                  mean_bone_lengths=None):
         super().__init__()
+        if getattr(crop_model, 'has_absolute_output', True) is False:
+            raise ValueError(f'{type(crop_model).__name__} has no absolute output: its joints are relative to the crop box, '
+                             'and the estimator needs camera-space joints (use Metrabs or Model25D)')
         self.crop_model = crop_model
         self.joint_names = self.crop_model.joint_names
         self.joint_edges = self.crop_model.joint_edges

@@ -6,8 +6,12 @@ exchange is ONE all-gather per forward.  Because ``reconstruct_ref_fullpersp`` n
 scalars (ptu3d.py:71-74), the gathered tensor is ``[coords2d | coords3d_rel]`` (5 floats per joint) and every rank
 runs the (tiny) absolute reconstruction on the full batch: the sharded result is then identical to the unsharded
 reference, not merely within tolerance.  Chunk order = rank order, so the gather is a plain concatenation.  A
-latent-point model gathers and reconstructs its latents and maps them to joints after the reconstruction."""
+latent-point model gathers and reconstructs its latents and maps them to joints after the reconstruction.  A Metro model
+gathers its decoded joints, which are its output; a Model25D gathers its coords25d [b,J,3] and every rank runs the
+batch-coupled bone-length solve on the full batch."""
 import torch
+
+from metrabs_b200 import _lib
 
 
 def shard_range(n, world_size, rank):
@@ -64,6 +68,14 @@ class ShardedMetrabs:
         if min(sizes) == max(sizes) and sizes[0] > 0 and hasattr(eng, 'forward_sharded'):
             # equal shards: the whole step in one library call on preallocated buffers (mtb_forward_sharded)
             return eng.forward_sharded(local, intrinsics)
+        model_class = getattr(eng, 'model_class', _lib.MODEL_METRABS)
+        if model_class != _lib.MODEL_METRABS:
+            # Metro: the decoded joints are the output; Model25D: gather coords25d, then the batch-coupled bone-length
+            # solve on the full batch
+            c25 = (eng.head_decode(eng.backbone(local))[1] if local.shape[0] else
+                   torch.zeros((0, eng.n_joints, 3), dtype=torch.float32, device=crops.device))
+            gathered = gather_decoded(c25, n_total, self.world, lambda t: eng.allgather(t).clone())
+            return gathered if model_class == _lib.MODEL_METRO else eng.reconstruct_by_bone_lengths(gathered, intrinsics)
         if local.shape[0] == 0:
             # fewer crops than ranks (e.g. 3 person-crops on 8 GPUs): this rank has nothing to compute but must still
             # take part in the collective

@@ -21,6 +21,8 @@ class Config:
     transform_coords: bool = False
     predict_all_and_latents: bool = False
     regularize_to_manifold: bool = False
+    # Model25D: bone-length depths relative to the mean joint (the reference default, metrabs_tf/init.py:228), else to the last
+    mean_relative: bool = True
     # build-specific: arithmetic of the conv kernels: 'fp32' and 'tf32x3' (parity modes), 'bf16' (tensor-core throughput
     # mode), 'fp16' (tensor cores, the reference's fp16-autocast arithmetic); 'bf16_simt' / 'fp16_simt' are their CUDA-core
     # verification twins
