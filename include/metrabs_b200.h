@@ -284,7 +284,9 @@ int mtb_crop_setup(const mtb_crop_setup_args* args, void* stream);
 
 /* warp_images_with_pyramid + the gamma of _get_crops (warping.py:6-52, multiperson_model.py:295-319): every crop of the
  * batch in ONE launch, written as the fp32 NCHW [num_aug*n_boxes,3,res,res] tensor mtb_forward reads.  antialias_factor
- * 1, 2 or 4 (rendered by supersampling = the reference's larger render followed by avg_pool2d). */
+ * 1, 2 or 4 (rendered by supersampling = the reference's larger render followed by avg_pool2d) or 5..16 (the larger
+ * render shrunk by the antialiased bilinear resize, per output tile in on-chip memory); mtb_crop_setup takes the same
+ * factors.  Others, 3 included, return MTB_ERR_UNSUPPORTED. */
 typedef struct {
   const uint8_t* images;         /* [n_images,3,H,W] u8 */
   const float* level1;           /* from mtb_image_pyramid */

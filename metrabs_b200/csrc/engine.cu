@@ -2292,6 +2292,15 @@ int mtb_image_pyramid(const uint8_t* images, int n_images, int height, int width
   return MTB_OK;
 }
 
+// The reference's antialias factors: 2 and 4 average-pool the larger render, factors above 4 shrink it with the
+// antialiased bilinear resize.  3 has no shrink there (its reshape fails), and past AA_MAX_F the tile footprint no longer
+// fits warp_crops_aa_kernel's shared memory.
+static bool antialias_supported(int f) { return f == 1 || f == 2 || f == 4 || (f >= 5 && f <= AA_MAX_F); }
+static int antialias_refusal(int f) {
+  return fail(nullptr, MTB_ERR_UNSUPPORTED, "antialias_factor must be 1, 2, 4 or 5..%d (got %d; 3 has no shrink step in the reference)",
+              AA_MAX_F, f);
+}
+
 int mtb_crop_setup(const mtb_crop_setup_args* a, void* stream) {
   if (!a || !a->boxes || !a->intrinsics || !a->camspace_up || !a->aug_rotflipmat || !a->aug_scales || !a->new_intrinsics ||
       !a->rotations || !a->inv_projections || !a->pyramid_levels || (a->n_dist > 0 && !a->distortion))
@@ -2299,8 +2308,7 @@ int mtb_crop_setup(const mtb_crop_setup_args* a, void* stream) {
   if (a->n_boxes <= 0 || a->num_aug <= 0 || a->num_aug > MP_MAX_AUG || a->box_stride < 4 || a->n_dist < 0 || a->n_dist > MP_NDIST ||
       a->resolution <= 0)
     return fail(nullptr, MTB_ERR_INVALID_ARG, "invalid crop-setup sizes (n_boxes=%d num_aug=%d n_dist=%d)", a->n_boxes, a->num_aug, a->n_dist);
-  if (a->antialias_factor != 1 && a->antialias_factor != 2 && a->antialias_factor != 4)
-    return fail(nullptr, MTB_ERR_UNSUPPORTED, "antialias_factor must be 1, 2 or 4 (got %d)", a->antialias_factor);
+  if (!antialias_supported(a->antialias_factor)) return antialias_refusal(a->antialias_factor);
   CropSetupParams p;
   p.boxes = a->boxes; p.box_stride = a->box_stride; p.K = a->intrinsics; p.dist = a->distortion; p.ncoef = a->n_dist;
   p.up = a->camspace_up; p.rotflip = a->aug_rotflipmat; p.aug_scales = a->aug_scales;
@@ -2319,16 +2327,20 @@ int mtb_warp_crops(const mtb_warp_args* a, void* stream) {
   if (a->n_boxes <= 0 || a->num_aug <= 0 || a->num_aug > MP_MAX_AUG || a->n_dist < 0 || a->n_dist > MP_NDIST || a->resolution <= 0 ||
       a->height < 4 || a->width < 4 || a->n_images <= 0)
     return fail(nullptr, MTB_ERR_INVALID_ARG, "invalid warp sizes");
-  if (a->antialias_factor != 1 && a->antialias_factor != 2 && a->antialias_factor != 4)
-    return fail(nullptr, MTB_ERR_UNSUPPORTED, "antialias_factor must be 1, 2 or 4 (got %d)", a->antialias_factor);
+  if (!antialias_supported(a->antialias_factor)) return antialias_refusal(a->antialias_factor);
   if ((long long)a->n_boxes * a->num_aug > 65535) return fail(nullptr, MTB_ERR_UNSUPPORTED, "more than 65535 crops per call");
   WarpParams p;
   p.img = a->images; p.l1 = a->level1; p.l2 = a->level2; p.N = a->n_images; p.H = a->height; p.W = a->width;
   p.K = a->intrinsics; p.dist = a->distortion; p.ncoef = a->n_dist; p.image_ids = a->image_ids; p.invproj = a->inv_projections;
   p.level = a->pyramid_levels; p.gamma_exp = a->gamma_exponents; p.n_box = a->n_boxes; p.num_aug = a->num_aug;
   p.res = a->resolution; p.antialias = a->antialias_factor; p.crops = a->crops;
-  const int npix = a->resolution * a->resolution;
-  launch_k(warp_crops_kernel, dim3((npix + 255) / 256, a->n_boxes * a->num_aug), dim3(256), 0, (cudaStream_t)stream, p);
+  if (a->antialias_factor <= 4) {
+    const int npix = a->resolution * a->resolution;
+    launch_k(warp_crops_kernel, dim3((npix + 255) / 256, a->n_boxes * a->num_aug), dim3(256), 0, (cudaStream_t)stream, p);
+  } else {
+    const int tiles = (a->resolution + AA_TILE - 1) / AA_TILE;
+    launch_k(warp_crops_aa_kernel, dim3(tiles * tiles, a->n_boxes * a->num_aug), dim3(256), 0, (cudaStream_t)stream, p);
+  }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(nullptr, MTB_ERR_CUDA, "warp launch: %s", cudaGetErrorString(e));
   return MTB_OK;

@@ -5,8 +5,10 @@
 //                         R = rotflip[aug] @ R_noaug, inverse projection, pyramid level
 //                                                                           (multiperson_model.py:264-293, 321-355; warping.py:20-21)
 //   warp_crops_kernel     ALL num_aug x n_boxes crops in one launch: homography, 12-coefficient lens distortion, pyramid
-//                         level select, bilinear gather with zero padding, antialias supersampling, gamma
+//                         level select, bilinear gather with zero padding, antialias 1 / 2 / 4 supersampling, gamma
 //                                                                           (warping.py:6-107, multiperson_model.py:295-319)
+//   warp_crops_aa_kernel  the same render at antialias 5..16, shrunk by the antialiased bilinear resize per output tile
+//                         without the render reaching global memory      (multiperson_model.py:311-314)
 //   tta_merge_kernel      mirror joint swap, poses @ R, joint_transform_matrix, 2D projection with distortion and the
 //                         image intrinsics, inverse extrinsics, skeleton gather, mean over augmentations
 //                                                                           (multiperson_model.py:143-178, 246-259)
@@ -224,11 +226,10 @@ __device__ __forceinline__ float tap(const T* __restrict__ plane, int W, int xi,
   else return (float)plane[(size_t)yi * W + xi];
 }
 
-__global__ void __launch_bounds__(256) warp_crops_kernel(const WarpParams p) {
-  __shared__ float lut[256];
-  __shared__ float sp[9 + 6 + MP_NDIST];
-  const int crop = blockIdx.y;
-  const int a = crop / p.n_box, b = crop - a * p.n_box;
+// Block-wide (256 threads): the decode table into `lut`; into `sp` the inverse projection (9), the level intrinsics (6)
+// and the distortion (12) of crop `crop` (box b); then a barrier.  -> the crop's pyramid level.  The kernels derive the
+// level image themselves: returning it from here as well changes the code ptxas generates for warp_crops_kernel.
+__device__ __forceinline__ int warp_load_crop(const WarpParams& p, int crop, int b, float* lut, float* sp) {
   lut[threadIdx.x] = powf((float)threadIdx.x / 255.f, 2.2f);
   const int lv = p.level[crop];
   if (threadIdx.x < 9) sp[threadIdx.x] = p.invproj[(size_t)crop * 9 + threadIdx.x];
@@ -243,6 +244,55 @@ __global__ void __launch_bounds__(256) warp_crops_kernel(const WarpParams p) {
     sp[15 + i] = i < p.ncoef ? p.dist[(size_t)b * p.ncoef + i] : 0.f;
   }
   __syncthreads();
+  return lv;
+}
+
+// Sample (nx, ny) of the crop's render grid: adds the bilinear blend of each channel to acc, nothing when all four taps
+// are outside the level image.
+__device__ __forceinline__ void warp_sample(const float* sp, const Dist12& dk, int lv, int Wl, int Hl, size_t plane_sz,
+                                            const uint8_t* im0, const float* imf, const float* lut, float nx, float ny, float acc[3]) {
+  // old = invproj @ (x, y, 1); project; distort; K_level @ (q, 1)   (warping.py:41-47)
+  const float hx = sp[0] * nx + sp[1] * ny + sp[2];
+  const float hy = sp[3] * nx + sp[4] * ny + sp[5];
+  const float hz = sp[6] * nx + sp[7] * ny + sp[8];
+  float qx = hx / hz, qy = hy / hz;
+  distort_point(qx, qy, dk);
+  const float u = sp[9] * qx + sp[10] * qy + sp[11];
+  const float v = sp[12] * qx + sp[13] * qy + sp[14];
+  // grid_sample(align_corners=True, bilinear, zeros) on coordinates normalised by (size - 1) (warping.py:48-52)
+  const float gx = ((u / (float)(Wl - 1) * 2.f - 1.f) + 1.f) * 0.5f * (float)(Wl - 1);
+  const float gy = ((v / (float)(Hl - 1) * 2.f - 1.f) + 1.f) * 0.5f * (float)(Hl - 1);
+  if (!(gx > -1.f && gx < (float)Wl && gy > -1.f && gy < (float)Hl)) return;  // all four taps outside (also NaN)
+  const float fx0 = floorf(gx), fy0 = floorf(gy);
+  const int x0 = (int)fx0, y0 = (int)fy0;
+  const float wx1 = gx - fx0, wx0 = (fx0 + 1.f) - gx, wy1 = gy - fy0, wy0 = (fy0 + 1.f) - gy;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    float v00, v01, v10, v11;
+    if (lv == 0) {
+      const uint8_t* pl = im0 + (size_t)c * plane_sz;
+      v00 = tap<uint8_t, true>(pl, Wl, x0, y0, Wl, Hl, lut);
+      v01 = tap<uint8_t, true>(pl, Wl, x0 + 1, y0, Wl, Hl, lut);
+      v10 = tap<uint8_t, true>(pl, Wl, x0, y0 + 1, Wl, Hl, lut);
+      v11 = tap<uint8_t, true>(pl, Wl, x0 + 1, y0 + 1, Wl, Hl, lut);
+    } else {
+      const float* pl = imf + (size_t)c * plane_sz;
+      v00 = tap<float, false>(pl, Wl, x0, y0, Wl, Hl, nullptr);
+      v01 = tap<float, false>(pl, Wl, x0 + 1, y0, Wl, Hl, nullptr);
+      v10 = tap<float, false>(pl, Wl, x0, y0 + 1, Wl, Hl, nullptr);
+      v11 = tap<float, false>(pl, Wl, x0 + 1, y0 + 1, Wl, Hl, nullptr);
+    }
+    acc[c] += v00 * (wx0 * wy0) + v01 * (wx1 * wy0) + v10 * (wx0 * wy1) + v11 * (wx1 * wy1);
+  }
+}
+
+// antialias 1, 2 and 4: the af x af supersamples of each output pixel, averaged (the reference's avg_pool2d(af))
+__global__ void __launch_bounds__(256) warp_crops_kernel(const WarpParams p) {
+  __shared__ float lut[256];
+  __shared__ float sp[9 + 6 + MP_NDIST];
+  const int crop = blockIdx.y;
+  const int a = crop / p.n_box, b = crop - a * p.n_box;
+  const int lv = warp_load_crop(p, crop, b, lut, sp);
   Dist12 dk;
 #pragma unroll
   for (int i = 0; i < MP_NDIST; ++i) dk.d[i] = sp[15 + i];
@@ -259,45 +309,113 @@ __global__ void __launch_bounds__(256) warp_crops_kernel(const WarpParams p) {
     const int oy = pix / p.res, ox = pix - oy * p.res;
     float acc[3] = {0.f, 0.f, 0.f};
     for (int sy = 0; sy < af; ++sy)
-      for (int sx = 0; sx < af; ++sx) {
-        const float nx = (float)(ox * af + sx), ny = (float)(oy * af + sy);
-        // old = invproj @ (x, y, 1); project; distort; K_level @ (q, 1)   (warping.py:41-47)
-        const float hx = sp[0] * nx + sp[1] * ny + sp[2];
-        const float hy = sp[3] * nx + sp[4] * ny + sp[5];
-        const float hz = sp[6] * nx + sp[7] * ny + sp[8];
-        float qx = hx / hz, qy = hy / hz;
-        distort_point(qx, qy, dk);
-        const float u = sp[9] * qx + sp[10] * qy + sp[11];
-        const float v = sp[12] * qx + sp[13] * qy + sp[14];
-        // grid_sample(align_corners=True, bilinear, zeros) on coordinates normalised by (size - 1) (warping.py:48-52)
-        const float gx = ((u / (float)(Wl - 1) * 2.f - 1.f) + 1.f) * 0.5f * (float)(Wl - 1);
-        const float gy = ((v / (float)(Hl - 1) * 2.f - 1.f) + 1.f) * 0.5f * (float)(Hl - 1);
-        if (!(gx > -1.f && gx < (float)Wl && gy > -1.f && gy < (float)Hl)) continue;  // all four taps outside (also NaN)
-        const float fx0 = floorf(gx), fy0 = floorf(gy);
-        const int x0 = (int)fx0, y0 = (int)fy0;
-        const float wx1 = gx - fx0, wx0 = (fx0 + 1.f) - gx, wy1 = gy - fy0, wy0 = (fy0 + 1.f) - gy;
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-          float v00, v01, v10, v11;
-          if (lv == 0) {
-            const uint8_t* pl = im0 + (size_t)c * plane_sz;
-            v00 = tap<uint8_t, true>(pl, Wl, x0, y0, Wl, Hl, lut);
-            v01 = tap<uint8_t, true>(pl, Wl, x0 + 1, y0, Wl, Hl, lut);
-            v10 = tap<uint8_t, true>(pl, Wl, x0, y0 + 1, Wl, Hl, lut);
-            v11 = tap<uint8_t, true>(pl, Wl, x0 + 1, y0 + 1, Wl, Hl, lut);
-          } else {
-            const float* pl = imf + (size_t)c * plane_sz;
-            v00 = tap<float, false>(pl, Wl, x0, y0, Wl, Hl, nullptr);
-            v01 = tap<float, false>(pl, Wl, x0 + 1, y0, Wl, Hl, nullptr);
-            v10 = tap<float, false>(pl, Wl, x0, y0 + 1, Wl, Hl, nullptr);
-            v11 = tap<float, false>(pl, Wl, x0 + 1, y0 + 1, Wl, Hl, nullptr);
-          }
-          acc[c] += v00 * (wx0 * wy0) + v01 * (wx1 * wy0) + v10 * (wx0 * wy1) + v11 * (wx1 * wy1);
-        }
-      }
+      for (int sx = 0; sx < af; ++sx)
+        warp_sample(sp, dk, lv, Wl, Hl, plane_sz, im0, imf, lut, (float)(ox * af + sx), (float)(oy * af + sy), acc);
     float* o = p.crops + (size_t)crop * 3 * npix + pix;
 #pragma unroll
     for (int c = 0; c < 3; ++c) o[(size_t)c * npix] = powf(acc[c] * inv_n, gexp);  // crops **= aug_gammas / 2.2 (:318)
+  }
+}
+
+// ------------------------------------------------------------------------------------------ warp, antialias 5..16
+// The reference renders res*f and shrinks it with torchvision's resize(BILINEAR, antialias=True) (multiperson_model.py:
+// 311-314), i.e. F.interpolate(bilinear, align_corners=False, antialias=True): per axis, output i takes the render taps
+// j in [lo, lo + n) around center f (i + 0.5) with weight max(0, 1 - |j - center + 0.5| / f), clipped to the render and
+// renormalised over the taps that remain; the width pass runs first, then the height pass (ATen's separable CPU kernel).
+// One CTA per (crop, AA_TILE x AA_TILE output tile): it computes each supersample of the tile's footprint once, in chunks
+// of rows held in shared memory, reduces every chunk row by the width pass into a strip of [rows][AA_TILE][3], then runs
+// the height pass and the gamma.  Sums run in ascending tap order without atomics: a crop's output does not depend on
+// the launch it is part of.
+constexpr int AA_TILE = 8;
+constexpr int AA_MAX_F = 16;
+constexpr int AA_SPAN = (AA_TILE + 1) * AA_MAX_F;  // footprint of a tile, supersamples per axis, at most
+constexpr int AA_TAPS = 2 * AA_MAX_F;               // taps per output and axis, at most
+constexpr int AA_RAW = 2304;                        // supersamples per row chunk: 16 rows of the widest footprint
+
+// Taps [lo, lo + n) of output i (ATen's _compute_weights_aa, scale and support f, no align-corners shift)
+__device__ __forceinline__ void aa_range(int i, int f, int n_in, int& lo, int& n) {
+  const float center = (float)f * ((float)i + 0.5f);
+  lo = max((int)(center - (float)f + 0.5f), 0);
+  n = min((int)(center + (float)f + 0.5f), n_in) - lo;
+}
+
+// The renormalised fp32 weights of output i, in ATen's operations: |t| * fl(1 / f), 1 - x, the running total, w / total
+__device__ __forceinline__ void aa_weights(int i, int f, int n_in, float* w, int* range) {
+  int lo, n;
+  aa_range(i, f, n_in, lo, n);
+  const float center = (float)f * ((float)i + 0.5f), invscale = 1.f / (float)f;
+  float total = 0.f;
+  for (int j = 0; j < n; ++j) {
+    const float x = fabsf(((float)(j + lo) - center + 0.5f) * invscale);
+    w[j] = x < 1.f ? 1.f - x : 0.f;
+    total += w[j];
+  }
+  for (int j = 0; j < n; ++j) w[j] /= total;  // the tap nearest the center has weight >= 1/2
+  range[0] = lo;
+  range[1] = n;
+}
+
+__global__ void __launch_bounds__(256) warp_crops_aa_kernel(const WarpParams p) {
+  __shared__ float lut[256];
+  __shared__ float sp[9 + 6 + MP_NDIST];
+  __shared__ float raw[3][AA_RAW];                 // one chunk of footprint rows, per channel
+  __shared__ float strip[AA_SPAN][AA_TILE][3];     // width-pass output of every footprint row
+  __shared__ float wx[AA_TILE][AA_TAPS + 1], wy[AA_TILE][AA_TAPS + 1];
+  __shared__ int rx[AA_TILE][2], ry[AA_TILE][2];
+  const int crop = blockIdx.y;
+  const int a = crop / p.n_box, b = crop - a * p.n_box;
+  const int f = p.antialias, n_in = p.res * f;
+  const int tiles_x = (p.res + AA_TILE - 1) / AA_TILE;
+  const int ty = blockIdx.x / tiles_x, tx = blockIdx.x - ty * tiles_x;
+  const int ox0 = tx * AA_TILE, oy0 = ty * AA_TILE;
+  const int nox = min(AA_TILE, p.res - ox0), noy = min(AA_TILE, p.res - oy0);
+  const int t = threadIdx.x;
+  if (t >= 128 && t < 128 + nox) aa_weights(ox0 + t - 128, f, n_in, wx[t - 128], rx[t - 128]);
+  if (t >= 160 && t < 160 + noy) aa_weights(oy0 + t - 160, f, n_in, wy[t - 160], ry[t - 160]);
+  const int lv = warp_load_crop(p, crop, b, lut, sp);  // its barrier also publishes the weights
+  Dist12 dk;
+#pragma unroll
+  for (int i = 0; i < MP_NDIST; ++i) dk.d[i] = sp[15 + i];
+  const int Hl = p.H >> lv, Wl = p.W >> lv;
+  const int img_id = p.image_ids[b];
+  const size_t plane_sz = (size_t)Hl * Wl;
+  const uint8_t* im0 = p.img + (size_t)img_id * 3 * plane_sz;
+  const float* imf = (lv == 1 ? p.l1 : p.l2) + (size_t)img_id * 3 * plane_sz;
+  const int x_lo = rx[0][0], nx = rx[nox - 1][0] + rx[nox - 1][1] - x_lo;  // the tile's footprint
+  const int y_lo = ry[0][0], ny = ry[noy - 1][0] + ry[noy - 1][1] - y_lo;
+  const int chunk = AA_RAW / nx;
+  for (int r0 = 0; r0 < ny; r0 += chunk) {
+    const int nr = min(chunk, ny - r0);
+    for (int k = t; k < nr * nx; k += blockDim.x) {
+      const int r = k / nx, x = k - r * nx;
+      float acc[3] = {0.f, 0.f, 0.f};
+      warp_sample(sp, dk, lv, Wl, Hl, plane_sz, im0, imf, lut, (float)(x_lo + x), (float)(y_lo + r0 + r), acc);
+      raw[0][k] = acc[0];
+      raw[1][k] = acc[1];
+      raw[2][k] = acc[2];
+    }
+    __syncthreads();
+    for (int k = t; k < nr * AA_TILE * 3; k += blockDim.x) {  // width pass: (row, channel, output column)
+      const int ox = k % AA_TILE, c = (k / AA_TILE) % 3, r = k / (AA_TILE * 3);
+      if (ox >= nox) continue;
+      const float* row = raw[c] + r * nx + (rx[ox][0] - x_lo);
+      const float* w = wx[ox];
+      float s = 0.f;
+      for (int j = 0; j < rx[ox][1]; ++j) s += row[j] * w[j];
+      strip[r0 + r][ox][c] = s;
+    }
+    __syncthreads();
+  }
+  const float gexp = p.gamma_exp[a];
+  const int npix = p.res * p.res;
+  for (int k = t; k < AA_TILE * AA_TILE * 3; k += blockDim.x) {  // height pass and gamma: (channel, row, column)
+    const int ox = k % AA_TILE, oy = (k / AA_TILE) % AA_TILE, c = k / (AA_TILE * AA_TILE);
+    if (ox >= nox || oy >= noy) continue;
+    const int lo = ry[oy][0] - y_lo;
+    const float* w = wy[oy];
+    float s = 0.f;
+    for (int j = 0; j < ry[oy][1]; ++j) s += strip[lo + j][ox][c] * w[j];
+    p.crops[(size_t)crop * 3 * npix + (size_t)c * npix + (size_t)(oy0 + oy) * p.res + ox0 + ox] = powf(s, gexp);  // (:318)
   }
 }
 

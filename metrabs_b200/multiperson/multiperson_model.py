@@ -10,7 +10,11 @@ Differences from the reference, all deliberate: the person detector is third-par
 and out of scope, so ``detect_poses*`` take a ``detector`` callable; ``JointInfo`` comes from the un-vendored posepile
 (stand-in in joint_info.py); the public ``estimate_poses*`` of the reference crash on their tuple defaults (SURVEY.md 3.4)
 - here they work; the plausibility filter, commented out in the PyTorch reference (:158-163), runs when bone statistics
-are supplied."""
+are supplied.
+
+``antialias_factor`` (every public method): 1, 2, 4 or 5..16, the factors the reference accepts except 3, for which it
+has no shrink step (:309-315).  At 2 and 4 the res*f render is box-averaged, above 4 it is shrunk with the antialiased
+bilinear resize, as in the reference; other factors raise MetrabsB200Error."""
 import ctypes as C
 
 import numpy as np

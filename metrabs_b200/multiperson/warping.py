@@ -37,7 +37,8 @@ def build_pyramid(images):
 def crop_setup(boxes, intrinsic_matrix, distortion_coeffs, camspace_up, aug_rotflipmat, aug_scales, resolution,
                antialias_factor=1):
     """_get_new_rotation_and_scale + the matrices of _get_crops (multiperson_model.py:264-293, :321-355).
-    -> new_intrinsic_matrix [A,n,3,3], R [A,n,3,3], new_invprojmat [A*n,3,3], pyramid levels [A*n] (device tensors)."""
+    -> new_intrinsic_matrix [A,n,3,3], R [A,n,3,3], new_invprojmat [A*n,3,3], pyramid levels [A*n] (device tensors).
+    ``antialias_factor``: 1, 2, 4 or 5..16, as for warp_images_with_pyramid; others raise MetrabsB200Error."""
     dev = boxes.device
     n, a = boxes.shape[0], aug_scales.shape[0]
     boxes = boxes.float().contiguous()
@@ -61,7 +62,12 @@ def warp_images_with_pyramid(images, pyramid, intrinsic_matrix, new_invprojmats,
                              gamma_exponents, resolution, image_ids, num_aug, antialias_factor=1, out=None):
     """All ``num_aug * n_boxes`` crops in one launch (warping.py:6-52 + the gamma of multiperson_model.py:318), as the fp32
     NCHW tensor the crop model reads.  ``intrinsic_matrix`` / ``distortion_coeffs`` / ``image_ids`` are per BOX (the
-    reference tiles them over the augmentations, multiperson_model.py:299-305)."""
+    reference tiles them over the augmentations, multiperson_model.py:299-305).
+
+    ``antialias_factor`` f renders each crop at res * f: at 2 and 4 it is box-averaged (the reference's avg_pool2d), at
+    5..16 shrunk with the antialiased bilinear resize (torchvision's resize(BILINEAR, antialias=True), :311-314) inside the
+    kernel, without the render reaching device memory.  3 (the reference has no shrink for it), 0 and above 16 raise
+    MetrabsB200Error."""
     dev = images.device
     n = intrinsic_matrix.shape[0]
     images = images.contiguous()
